@@ -43,7 +43,7 @@
 #define EF_K1A_PF_L2 1           // K1a: prefetch.global.L2 128 bytes ahead of a slice's read position (besides the cp.async ring)
 #endif
 #ifndef EF_K1A_HDR_BATCH
-#define EF_K1A_HDR_BATCH 32      // waiting lanes that end a symbol loop early; 32 = the loop runs until no lane is busy
+#define EF_K1A_HDR_BATCH 24      // K1a: waiting lanes that end a symbol loop early (32: the loop runs until no lane is busy); 24 measured fastest of 8-32
 #endif
 #ifndef EF_K1A_V3
 #define EF_K1A_V3 1              // K1a: one symbol per step through the clz-indexed table, a following end of block folded in (0: the two-symbol table step)
@@ -54,14 +54,8 @@
 #ifndef EF_K1A_ES16
 #define EF_K1A_ES16 1            // K1a: the bitstream comes in through 16-byte cp.async.cg chunks (4 per lane in flight) instead of 4-byte words: a quarter of the
 #endif                           //      scattered-address global-memory instructions, and no reliance on L1 hits
-#ifndef EF_K1A_STAGE
-#define EF_K1A_STAGE 32          // K1a: the first N list entries of a macroblock are staged in shared memory and written out by the whole warp, coalesced, when the
-#endif                           //      macroblock is complete (0: every entry is its own scattered 4-byte store)
 #ifndef EF_K1A_UNROLL
 #define EF_K1A_UNROLL 3          // K1a v3: symbol steps per pass of the loop (one vote + branch per pass)
-#endif
-#ifndef EF_K1A_FLUSH_UNROLL
-#define EF_K1A_FLUSH_UNROLL 4    // K1a: source lanes per pass of the staged-list flush
 #endif
 #ifndef EF_PROBE_NOSTORE
 #define EF_PROBE_NOSTORE 0       // measurement probe only: K1a drops its coefficient stores (output wrong)

@@ -20,9 +20,9 @@
 //       can never run into each other and no allocation or prefix sum is needed.
 //       A global-memory instruction whose lanes point into 32 different slices costs the load/store
 //       unit a cycle per lane, and the round-1 parser issued two of them per symbol step; so the
-//       bitstream comes in as 16-byte cp.async.cg chunks (one per lane per 128 bits) and the first 32
-//       list entries of a macroblock are staged in shared memory and written out by the whole warp,
-//       one list per store instruction, when the macroblock is complete (DESIGN.md 4).
+//       bitstream comes in as 16-byte cp.async.cg chunks (one per lane per 128 bits) and list entries
+//       are staged in a per-lane ring in shared memory and written out by the whole warp, one list run
+//       per store instruction, independently of macroblock boundaries (DESIGN.md 4).
 //   K1b ef_recon_kernel   records -> pixels, one launch per picture index (P pictures read the
 //       previous picture of their stream). One HALF-WARP per macroblock record (a warp = two
 //       consecutive slots), all 1,081,344 of a BASELINE picture batch independent: scatter the list
@@ -89,13 +89,17 @@ constexpr int kRingBytes = 4 * kRingStride;
 constexpr int kRingStride = kParseThreads * 4;          // bytes between ring slots of one lane: slot-major, conflict-free
 constexpr int kRingBytes = 8 * kRingStride;
 #endif
-constexpr int kFlushUnroll = EF_K1A_FLUSH_UNROLL;
-constexpr int kStage = EF_K1A_STAGE;                    // list entries of the macroblock in flight staged per lane
+// List entries not yet written to HBM: a ring of kStage words per lane in shared memory (entry e of the slice's list in
+// word e % kStage). They go out coalesced, one list run per store instruction, before any lane's ring could overflow:
+// the symbol loop flushes when a lane holds more than kStageHigh entries, which leaves room for one pass of steps.
+constexpr int kStage = 32;
+constexpr int kStageHigh = kStage - (EF_K1A_V3 ? EF_K1A_UNROLL : 2);   // a pass adds at most one entry per step (v3) or two (one two-symbol step)
+static_assert(kStageHigh > 0, "a pass of the symbol loop must fit in the staging ring");
 // bytes per staging row: with the 16-byte bitstream slots a multiple of 16 (36 words for 32 entries), so that a lane's row
 // address is a multiple of its ring address (one IMAD where the compiler otherwise re-derives it from the thread index at
 // every store); else an odd number of words
 constexpr int kStageRow = EF_K1A_ES16 ? ((kStage * 4 + 16 + 15) & ~15) : (kStage + 1) * 4;
-constexpr int kStageBytesA = kStage > 0 ? kParseThreads * kStageRow : 0;
+constexpr int kStageBytesA = kParseThreads * kStageRow;
 
 struct BitReader {
     const uint32_t* words;   // the whole ES blob as aligned 32-bit words (cudaMalloc alignment)
@@ -197,7 +201,7 @@ struct BitReader {
 // per-lane slice parser state
 struct SliceState {
     BitReader br;
-    uint32_t* wptr;          // coefficient list of the macroblock in flight (HBM); entries are stored at wptr[cnt]
+    uint32_t* list;          // the slice's coefficient list in HBM (entry 3 x byte offset of the slice)
     uint32_t slot_base;      // record slot of macroblock (0,0) of this slice's picture | destination frame store << 31
     uint32_t seqi;           // index of the slice's sequence state in the stream's EfSeq table (K1a v3: handed to K1b for streams with their own matrices)
     const uint32_t* qzp;     // generic pointer to the table words in use: T.qz in shared memory (default matrices) or the stream's own in HBM
@@ -540,9 +544,9 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
     const uint32_t n_slots = (uint32_t)D.n_streams * (EF_MBW_MAX * EF_MBH_MAX);
 
     SliceState s;
-    s.first = 0; s.wptr = nullptr; s.slot_base = 0; s.qz = nullptr; s.mbw = 0; s.mb_x = s.mb_y = 0;
+    s.first = 0; s.list = D.coef; s.slot_base = 0; s.qz = nullptr; s.mbw = 0; s.mb_x = s.mb_y = 0;
     s.br.sring = smem_u32(smem + kTableBytes + kLutBytes) + threadIdx.x * (EF_K1A_ES16 ? 16 : 4);
-    // staged list entries: one row per lane
+    // staged list entries: one ring row per lane
     const uint32_t sstage_warp = smem_u32(smem + kTableBytes + kLutBytes + kRingBytes) + (threadIdx.x & ~31u) * kStageRow;
 #if EF_K1A_ES16
     const uint32_t sstage_bias = smem_u32(smem + kTableBytes + kLutBytes + kRingBytes) - (kStageRow / 16) * smem_u32(smem + kTableBytes + kLutBytes);
@@ -552,9 +556,11 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
 #define EF_SSTAGE sstage
 #endif
     bool active = false, exhausted = false, busy = false;
-    // the macroblock in flight: info word under construction (bit 0 set = a record is owed), entry count |
-    // skip run << 16, motion vector, record slot
-    uint32_t info_acc = 0, cnt = 0, skipw = 0, mvw = 0, slot = 0;
+    // the slice's list: `tot` entries so far, the first `done` of them in HBM, the rest in the lane's ring.
+    // The macroblock in flight: info word under construction (bit 0 set = a record is owed), its first list entry,
+    // skip run, motion vector, record slot
+    uint32_t tot = 0, done = 0;
+    uint32_t info_acc = 0, mb0 = 0, skipw = 0, mvw = 0, slot = 0;
     uint32_t blk24 = 0, blkbit = 0;                           // current block: number << 24 (v3: token head = number << 27 | quantiser_scale << 16), 0x100 << number
     int cbp_rem = 0, n = 0, intra = 0, ctx = 0;               // n = scan position of the block in flight; ctx = 1: the next symbol is the first coefficient of a non-intra block
     // next coded block of the macroblock in flight (cbp_rem != 0): block number, contexts, intra DC
@@ -570,15 +576,34 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
         n = 0; ctx = 1;                                       // dct_coeff_first: no end of block, '1s' = (0, 1)
         if (intra) { D.mb_rec[slot].dc[blk] = parse_dc(s, blk); n = 1; ctx = 0; }
     };
-    // list entry `cnt` of the macroblock in flight: staged in shared memory while it fits, else straight to the list in HBM
+    // next list entry of the slice: into the lane's ring
     auto put_entry = [&](uint32_t ent) {
-#if EF_PROBE_NOSTORE                                                  /* bottleneck probe (wrong output): only entries nobody produces are stored */
-        if (ent == 0x12345678u) s.wptr[cnt] = ent;
-#else
-        if (kStage > 0 && cnt < (uint32_t)kStage) asm volatile("st.shared.u32 [%0], %1;" ::"r"(EF_SSTAGE + cnt * 4), "r"(ent) : "memory");
-        else s.wptr[cnt] = ent;
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(EF_SSTAGE + (tot % kStage) * 4), "r"(ent) : "memory");
+        tot++;
+    };
+    // warp-wide (all lanes converged): every lane's entries still in its ring go to the list in HBM. Lane j stores
+    // entry j of one lane's pending run, so each store instruction writes one contiguous run of one list
+    auto flush = [&]() {
+        __syncwarp();                                                 // the ring words of other lanes are read below, and rewritten after
+#if !EF_PROBE_NOSTORE                                                 /* bottleneck probe (wrong output): no list stores */
+        const uint32_t pend = tot - done;                             // <= kStage
+        const uint64_t dst = (uint64_t)(s.list + done);
+        const uint32_t key = pend | (done << 8);                      // run length | ring position of its first entry
+        unsigned owed = __ballot_sync(0xFFFFFFFFu, pend != 0);
+        while (owed) {
+            const int src = __ffs(owed) - 1;
+            owed &= owed - 1;
+            const uint32_t k = __shfl_sync(0xFFFFFFFFu, key, src);
+            uint32_t* const d = (uint32_t*)((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)dst, src) | ((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)(dst >> 32), src) << 32));
+            if ((uint32_t)lane < (k & 255u)) {
+                uint32_t v;
+                asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(sstage_warp + (uint32_t)src * kStageRow + (((k >> 8) + lane) % kStage) * 4) : "memory");
+                d[lane] = v;
+            }
+        }
 #endif
-        cnt++;
+        __syncwarp();
+        done = tot;
     };
     // first round: thread t takes slice t; afterwards lanes whose slice ended pull from the cursor
     const uint32_t first_round = gridDim.x * blockDim.x;
@@ -586,46 +611,9 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
 
     for (;;) {
         // ---- header phase: records of finished macroblocks ------------------------------------------
-        if (kStage > 0) {
-            // the staged head of every finished list goes out coalesced: lane j writes entry j of the list of lane `src`
-            __syncwarp();
-            const uint64_t li_mine = (uint64_t)(s.wptr - D.coef);
-            if (kStage <= 32 && kHdrBatch == 32) {
-                // every lane is between macroblocks: a fixed walk over the 32 lists, the source lane an immediate
-                const uint32_t c_mine = (!busy && (info_acc & 1u)) ? min(cnt, (uint32_t)kStage) : 0u;
-                if (__any_sync(0xFFFFFFFFu, c_mine != 0)) {
-                    const uint32_t srow = sstage_warp + lane * 4;
-#pragma unroll (kFlushUnroll)
-                    for (int src = 0; src < 32; src++) {
-                        const uint32_t c = __shfl_sync(0xFFFFFFFFu, c_mine, src);
-                        const uint64_t lb = (uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)li_mine, src) | ((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)(li_mine >> 32), src) << 32);
-                        if (lane < c) {
-                            uint32_t v;
-                            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(srow + (uint32_t)src * kStageRow) : "memory");
-                            D.coef[lb + lane] = v;
-                        }
-                    }
-                }
-            } else {
-                unsigned owed = __ballot_sync(0xFFFFFFFFu, !busy && (info_acc & 1u) && cnt != 0);
-                while (owed) {
-                    const int src = __ffs(owed) - 1;
-                    owed &= owed - 1;
-                    const uint32_t c = min(__shfl_sync(0xFFFFFFFFu, cnt, src), (uint32_t)kStage);
-                    const uint64_t lb = (uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)li_mine, src) | ((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)(li_mine >> 32), src) << 32);
-                    for (uint32_t j = lane; j < c; j += 32) {
-                        uint32_t v;
-                        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(sstage_warp + (uint32_t)src * kStageRow + j * 4) : "memory");
-                        D.coef[lb + j] = v;
-                    }
-                }
-            }
-            __syncwarp();
-        }
         if (!busy && (info_acc & 1u)) {
-            const uint64_t li = (uint64_t)(s.wptr - D.coef);
-            *(uint4*)(D.mb_rec + slot) = make_uint4(cnt | (skipw << 16), mvw, (uint32_t)li, (uint32_t)(li >> 32));
-            s.wptr += cnt;
+            const uint64_t li = (uint64_t)(s.list - D.coef) + mb0;
+            *(uint4*)(D.mb_rec + slot) = make_uint4((tot - mb0) | (skipw << 16), mvw, (uint32_t)li, (uint32_t)(li >> 32));
 #if EF_K1B_DEQUANT
             if (s.qz) { info_acc |= 1u << 26; D.mb_rec[slot].pad[0] = s.seqi; }     // K1b dequantises with the stream's own matrices
 #endif
@@ -634,6 +622,7 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
         }
         // ---- refill lanes without a slice, parse the header of every waiting lane -------------------
         do {
+            if (__any_sync(0xFFFFFFFFu, !active && tot != done)) flush();   // a lane's ring is emptied before it takes its next slice
             unsigned need = __ballot_sync(0xFFFFFFFFu, !active && !exhausted);
             if (need) {
                 uint32_t base;
@@ -662,7 +651,8 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                         const uint64_t byte_off = D.es_off[w.stream] + w.es_off;
                         s.slot_base = (w.pic - (uint32_t)pic0) * n_slots + w.stream * (uint32_t)(EF_MBW_MAX * EF_MBH_MAX);
                         s.slot_base |= ((D.base_pics[w.stream] + w.pic + 1u) & 1u) << 31;      // destination frame store: flush_picture(), player.cpp:692
-                        s.wptr = D.coef + 3 * byte_off;          // >= 3 bits of bitstream per coefficient: lists cannot collide
+                        s.list = D.coef + 3 * byte_off;          // >= 3 bits of bitstream per coefficient: lists cannot collide
+                        tot = done = 0;
                         s.br.init(D.es, byte_off);
                         s.mb_y = code - 2; s.mb_x = s.mbw - 1;   // slice(), player.cpp:1255: the first increment lands on column 0 of row code-1
                         s.first = 1;
@@ -679,29 +669,34 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                 if (parse_header(s, T, cbp_rem, intra, skipw, mvw)) {
                     slot = (s.slot_base & 0x7FFFFFFFu) + (uint32_t)(s.mb_y * EF_MBW_MAX + s.mb_x);
                     info_acc = 1u | ((uint32_t)intra << 1) | ((uint32_t)cbp_rem << 2);
-                    cnt = 0;
+                    mb0 = tot;
                     busy = cbp_rem != 0;
                     if (busy) start_block();
                 } else active = false;
             }
         } while (__any_sync(0xFFFFFFFFu, !active && !exhausted));
-        if (!__any_sync(0xFFFFFFFFu, active)) break;
+        const unsigned amask = __ballot_sync(0xFFFFFFFFu, active);
+        if (!amask) break;
 
-        // ---- symbol loop: per busy lane and step, up to two coefficients and an end of block -------------
-        // Fast path: the next kLutBits bits index the two-symbol table; everything that lies wholly inside them
-        // (one or two run/level codes with their sign bits, a closing '10') is taken in one step. Long codes,
-        // the escape, invalid prefixes and symbols that would run past scan position 63 decode one symbol
-        // through the clz-indexed table (and fold a following end of block in).
-#if EF_K1A_V3
-        // ---- symbol loop, v3: per busy lane and step ONE run/level symbol through the clz-indexed table, a following
-        // end of block folded in; dequantised on the spot (table word of the scan position: shared memory for the default
-        // matrices, the stream's own table in HBM otherwise) or, with EF_K1B_DEQUANT, stored as a raw token
+        // ---- symbol loop: each lane runs through its own macroblock; a lane whose macroblock is complete waits (its
+        // record is owed) until the loop ends, when no lane is busy or when kHdrBatch lanes are waiting. Per pass, every
+        // busy lane takes EF_K1A_UNROLL steps (v3) or one two-symbol step
         const int qoff = intra ? 0 : 64, kq = intra ? 0 : 1;
+#if EF_K1A_V3
         const uint32_t* const qrow = s.qzp + qoff;               // table words of this macroblock's matrix, by scan position
+#else
+        // table word of scan position n: shared memory for the default matrices (no global-load latency in the symbol
+        // chain), the stream's own table in HBM otherwise (sequence headers that load matrices are rare)
+        auto qword = [&](int pos) -> uint32_t { return s.qz ? __ldg(s.qz + qoff + pos) : T.qz[qoff + pos]; };
+#endif
         for (;;) {
             const unsigned bmask = __ballot_sync(0xFFFFFFFFu, busy);
-            if (!bmask) break;
-            if (kHdrBatch < 32 && __popc(__ballot_sync(0xFFFFFFFFu, active && !busy)) >= kHdrBatch) break;
+            if (!bmask || __popc(amask & ~bmask) >= kHdrBatch) break;
+            if (__any_sync(0xFFFFFFFFu, tot - done > (uint32_t)kStageHigh)) flush();
+#if EF_K1A_V3
+            // per step ONE run/level symbol through the clz-indexed table, a following end of block folded in;
+            // dequantised on the spot (table word of the scan position: shared memory for the default matrices, the
+            // stream's own table in HBM otherwise) or, with EF_K1B_DEQUANT, stored as a raw token
 #pragma unroll
             for (int u_ = 0; u_ < EF_K1A_UNROLL; u_++)
             if (busy) {
@@ -737,17 +732,12 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                     }
                 }
             }
-        }
 #else
-        const int qoff = intra ? 0 : 64;
-        const int kq = intra ? 0 : 1;
-        // table word of scan position n: shared memory for the default matrices (no global-load latency in the symbol
-        // chain), the stream's own table in HBM otherwise (sequence headers that load matrices are rare)
-        auto qword = [&](int pos) -> uint32_t { return s.qz ? __ldg(s.qz + qoff + pos) : T.qz[qoff + pos]; };
-        for (;;) {
-            const unsigned bmask = __ballot_sync(0xFFFFFFFFu, busy);
-            if (!bmask) break;
-            if (kHdrBatch < 32 && __popc(__ballot_sync(0xFFFFFFFFu, active && !busy)) >= kHdrBatch) break;
+            // per step up to two coefficients and an end of block. Fast path: the next kLutBits bits index the
+            // two-symbol table; everything that lies wholly inside them (one or two run/level codes with their sign
+            // bits, a closing '10') is taken in one step. Long codes, the escape, invalid prefixes and symbols that
+            // would run past scan position 63 decode one symbol through the clz-indexed table (and fold a following
+            // end of block in).
             if (busy) {
                 BitReader& br = s.br;
                 const uint32_t w = br.peek();
@@ -771,9 +761,10 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                     }
                 }
             }
-        }
 #endif
+        }
     }
+#undef EF_SSTAGE
 }
 
 // =================================================================================================
