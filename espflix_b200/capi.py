@@ -75,6 +75,8 @@ _SIGNATURES = {
     "ef_idct_tc_run": (_I, [_I, _VP, _I, _VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), _I]),
     "ef_audio_demux_ts": (_I, [_I, _VP, _VP, _I, _VP, ctypes.c_uint64, _VP]),
     "ef_audio_decode": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
+    "ef_audio_enable": (_I, [_VP]),
+    "ef_decode_audio": (_I, [_VP, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -263,6 +265,38 @@ class Context:
             dst = np.zeros(2 * 352 + 160, dtype=np.uint16)
         self._check(self.lib.ef_blit(self._h, s, fb, dst.ctypes.data, line, x, width, frame_counter))
         return dst
+
+    # -- audio ------------------------------------------------------------------------------
+    def enable_audio(self):
+        """from now on every TS submit also demuxes the stream's audio (PID 0x101 / 0x102)"""
+        self._check(self.lib.ef_audio_enable(self._h))
+
+    def decode_audio(self, end=None, pdm=True, pcm_out=None, pdm_out=None, stream=0):
+        """ef_decode_audio: the frames of every stream that became decodable with the current submit -> list of dicts as
+        audio_decode() (frame_size, n_frames, pcm, pdm). end: per-stream flags (or True for all) that end the stream after
+        this call. pcm_out / pdm_out: preallocated (pinned) int16 / uint16 arrays large enough for the call; without them
+        a sizing call comes first."""
+        n = self.n_streams
+        if end is True:
+            end = np.ones(n, dtype=np.uint8)
+        elif end is not None:
+            end = np.ascontiguousarray(end, dtype=np.uint8)
+            assert end.size == n
+        info = np.zeros(n, dtype=_AUDIO_INFO)
+        if pcm_out is None:
+            self._check(self.lib.ef_decode_audio(self._h, _ptr(end), info.ctypes.data, None, 0, None, stream))
+            total = int(info["n_frames"].sum()) * 128
+            pcm_out = np.zeros(max(total, 1), dtype=np.int16)
+            pdm_out = np.zeros(max(2 * total, 1), dtype=np.uint16) if pdm else None
+        elif not pdm:
+            pdm_out = None
+        self._check(self.lib.ef_decode_audio(self._h, _ptr(end), info.ctypes.data, _ptr(pcm_out), pcm_out.size, _ptr(pdm_out), stream))
+        out = []
+        for i in info:
+            a, k = int(i["pcm_offset"]), int(i["n_frames"]) * 128
+            out.append({"frame_size": int(i["frame_size"]), "n_frames": int(i["n_frames"]), "pcm": pcm_out[a:a + k].copy(),
+                        "pdm": None if pdm_out is None else pdm_out[2 * a:2 * (a + k)].copy()})
+        return out
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

@@ -30,13 +30,20 @@ int ef_decode_resident_ctas(int which);
 __global__ void ef_tsidx_packet_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, int64_t* pkt_pts, uint8_t* pkt_kind);
 __global__ void ef_tsidx_compact_kernel(const uint64_t* pkt_off, const int64_t* pkt_pts, const uint8_t* pkt_kind, int64_t* seq_pts, uint32_t* seq_pos, int64_t* info);
 __global__ void ef_tsidx_sample_kernel(const int64_t* seq_pts, const uint32_t* seq_pos, int n, int64_t first_pts, uint32_t bin_size, uint32_t n_samples, uint32_t* samples);
-__global__ void ef_sbc_probe_kernel(const uint8_t* es, const uint64_t* off, int n_streams, int* frame_size);
-__global__ void ef_sbc_matrix_kernel(const uint8_t* es, const uint64_t* off, const int* frame_size, const uint64_t* slot_base, int n_streams, int32_t* vrows);
+__global__ void ef_audio_len_kernel(const EfAudioState* st, const uint64_t* new_off, const uint32_t* lead, const uint8_t* skip, int n_streams, uint64_t* len);
+__global__ void ef_audio_assemble_kernel(const EfAudioState* st, const uint8_t* src, const uint64_t* new_off, const uint32_t* lead, const uint8_t* skip, const uint64_t* blob_off, uint8_t* blob);
+__global__ void ef_sbc_probe_kernel(const uint8_t* es, const uint64_t* off, const EfAudioState* st, const uint8_t* ended, int n_streams, int4* plan);
+__global__ void ef_sbc_count_kernel(const uint8_t* es, const uint64_t* off, const uint8_t* ended, int n_streams, int4* plan);
+__global__ void ef_sbc_matrix_kernel(const uint8_t* es, const uint64_t* off, const int4* plan, const EfAudioState* st, const uint64_t* slot_base, int n_streams, int32_t* vrows, int32_t* sb_last);
 __global__ void ef_sbc_window_kernel(const int32_t* vrows, const uint64_t* slot_base, const uint64_t* pcm_off, int n_streams, int16_t* pcm);
-__global__ void ef_pdm_kernel(const int16_t* pcm, const uint64_t* pcm_off, int n_streams, uint16_t* pdm);
+__global__ void ef_pdm_kernel(const int16_t* pcm, const uint64_t* pcm_off, int n_streams, EfAudioState* st, uint16_t* pdm);
+__global__ void ef_audio_commit_kernel(EfAudioState* st, const uint8_t* blob, const uint64_t* blob_off, const int4* plan, const uint64_t* slot_base, const int32_t* vrows,
+                                       const int32_t* sb_last, const uint8_t* ended, int n_streams);
 __global__ void ef_audio_ts_packet_kernel(const uint8_t* ts, uint64_t n_packets, uint8_t* start, uint8_t* kind);
-__global__ void ef_audio_ts_scan_kernel(const uint64_t* pkt_off, int n_files, const uint8_t* start, const uint8_t* kind, uint32_t* out_pos, uint64_t* es_len);
-__global__ void ef_audio_ts_copy_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, const uint8_t* start, const uint32_t* out_pos, const uint64_t* es_off, uint8_t* es);
+__global__ void ef_audio_ts_scan_kernel(const uint64_t* ts_off, int n_files, const uint8_t* start, const uint8_t* kind, const uint8_t* gate_in, uint8_t* gate_out,
+                                        uint32_t* lead, uint8_t* skip, uint32_t* out_pos, uint64_t* es_len);
+__global__ void ef_audio_ts_copy_kernel(const uint8_t* ts, const uint64_t* ts_off, int n_files, uint64_t n_packets, const uint8_t* start, const uint32_t* out_pos, const uint64_t* es_off, uint8_t* es);
+__global__ void ef_audio_end_kernel(const uint8_t* ended, int n_streams, uint8_t* gate_cur, uint8_t* gate_next, uint8_t* skip_next, int next_is_ts);
 cudaError_t ef_audio_upload_constants();
 cudaError_t ef_launch_parse(const EfDev& dev, int pic0, int n_pics, int sm_count, size_t max_slices, cudaStream_t stream);
 cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t n_slots, cudaStream_t stream);
@@ -168,6 +175,48 @@ struct ef_ctx {
     bool profiling = false;                       // ef_set_profiling: CUDA events around K0 / K1a / K1b
     cudaEvent_t ev_prof[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };
     bool prof_index = false, prof_decode = false;
+    // audio (ef_audio_enable): every TS submit also demuxes PID 0x101 / 0x102 into the audio staging of its ES buffer;
+    // ef_decode_audio continues every stream's SBC decode from d_aud_state
+    bool audio = false;
+    bool aud_ts[2] = { false, false };            // ES buffer b holds the demuxed audio of a TS submit
+    bool aud_unconsumed = false;                  // the current submit's audio has not been through ef_decode_audio yet
+    EfAudioState* d_aud_state = nullptr;          // [n_streams]
+    uint8_t* d_aud2[2] = { nullptr, nullptr };    // per ES buffer: audio bytes of its submit, back to back
+    uint64_t* d_aud_off2[2] = { nullptr, nullptr };
+    uint8_t* d_gate2[2] = { nullptr, nullptr };   // per ES buffer: demux gate of every stream after its submit
+    uint32_t* d_lead2[2] = { nullptr, nullptr };  // per ES buffer: audio bytes before the first PES start
+    uint8_t* d_skip2[2] = { nullptr, nullptr };   // per ES buffer: drop those (the stream ended after the scan)
+    uint8_t* d_aud_start = nullptr;               // per TS packet: payload start, kind, output position
+    uint8_t* d_aud_kind = nullptr;
+    uint32_t* d_aud_pos = nullptr;
+    uint64_t* d_aud_len = nullptr;                // [n_streams + 1]
+    uint8_t* d_blob = nullptr;                    // one call's input: held-back bytes + new bytes of every stream
+    uint64_t* d_blob_len = nullptr;
+    uint64_t* d_blob_off = nullptr;
+    uint8_t* d_ended = nullptr;
+    uint8_t* h_ended = nullptr;                   // pinned
+    struct AudioScratch* aud_scratch = nullptr;
+};
+
+// Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
+// use a scratch of their own, a context keeps one.
+struct AudioScratch {
+    enum { PLAN, SB_LAST, SLOT, POFF, VROWS, PCM, PDM, N };
+    void* p[N] = {};
+    size_t cap[N] = {};
+    ~AudioScratch() { for (void* q : p) if (q) cudaFree(q); }
+    cudaError_t get(int k, size_t bytes, void** out)
+    {
+        if (cap[k] < bytes) {
+            if (p[k]) cudaFree(p[k]);
+            p[k] = nullptr; cap[k] = 0;
+            const cudaError_t e = cudaMalloc(&p[k], bytes);
+            if (e != cudaSuccess) return e;
+            cap[k] = bytes;
+        }
+        *out = p[k];
+        return cudaSuccess;
+    }
 };
 
 namespace {
@@ -330,6 +379,8 @@ void ef_destroy(ef_ctx* c)
     if (!c) return;
     cudaDeviceSynchronize();
     for (void* p : c->allocs) cudaFree(p);
+    delete c->aud_scratch;
+    if (c->h_ended) cudaFreeHost(c->h_ended);
     for (int b = 0; b < 2; b++) {
         if (c->h_off[b]) cudaFreeHost(c->h_off[b]);
         if (c->ev_up_done[b]) cudaEventDestroy(c->ev_up_done[b]);
@@ -362,6 +413,12 @@ int ef_reset(ef_ctx* c)
     CK(cudaGetLastError());
     c->launches++;
     CK(cudaMemset(c->h.info, 0, 32));
+    if (c->audio) {                                       // every stream's audio starts over; audio stays enabled
+        CK(cudaStreamSynchronize(c->up_stream));          // a queued submit's demux may still read a gate
+        CK(cudaMemset(c->d_aud_state, 0, (size_t)c->cfg.n_streams * sizeof(EfAudioState)));
+        for (int b = 0; b < 2; b++) { CK(cudaMemset(c->d_gate2[b], 0, (size_t)c->cfg.n_streams)); c->aud_ts[b] = false; }
+        c->aud_unconsumed = false;
+    }
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
     return EF_OK;
@@ -423,6 +480,32 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
             c->launches += 4;
         } else CK(cudaMemsetAsync(d_es_off, 0, ((size_t)n + 1) * 8, up));
     }
+    if (c->audio) {
+        // The demux gate of every stream continues from the submit that is current now (the front buffer): submits are
+        // demuxed in submit order on this stream, and a submit that replaces a queued one starts from the same gate.
+        const uint8_t* gate_in = c->d_gate2[c->active];
+        if (ts) {
+            const uint64_t n_packets = total / 188;
+            if (n_packets) {
+                ef_audio_ts_packet_kernel<<<(unsigned)((n_packets + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_aud_start, c->d_aud_kind);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
+            ef_audio_ts_scan_kernel<<<(n + 63) / 64, 64, 0, up>>>(c->d_ts_off, n, c->d_aud_start, c->d_aud_kind, gate_in, c->d_gate2[b], c->d_lead2[b], c->d_skip2[b],
+                                                                  c->d_aud_pos, c->d_aud_len);
+            CK(cudaGetLastError());
+            ef_ts_offsets_kernel<<<1, 1024, 0, up>>>(c->d_aud_len, n, c->d_aud_off2[b], c->d_aud2[b]);
+            CK(cudaGetLastError());
+            c->launches += 2;
+            if (n_packets) {
+                ef_audio_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, up>>>(c->d_ts, c->d_ts_off, n, n_packets, c->d_aud_start, c->d_aud_pos,
+                                                                                                  c->d_aud_off2[b], c->d_aud2[b]);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
+        } else CK(cudaMemcpyAsync(c->d_gate2[b], gate_in, (size_t)n, cudaMemcpyDeviceToDevice, up));   // ES submits carry no audio
+        c->aud_ts[b] = ts;
+    }
     CK(cudaEventRecord(c->ev_up_done[b], up));
     c->es_bytes = total;                        // for TS input an upper bound; the exact ES size is on the device
     c->pending = b;
@@ -443,9 +526,12 @@ int ef_index(ef_ctx* c, void* stream)
     cudaStream_t st = (cudaStream_t)stream;
     const int n = c->cfg.n_streams;
     if (c->pending >= 0) {                       // a fresh submit: wait for its upload, make it the front buffer
+        if (c->audio && c->aud_unconsumed)       // the audio of a TS submit is delivered exactly once
+            return fail(EF_ESTATE, "ef_index of a new submit before ef_decode_audio consumed the current submit's audio");
         CK(cudaStreamWaitEvent(st, c->ev_up_done[c->pending], 0));
         c->active = c->pending; c->pending = -1;
         c->d = c->dd[c->active];
+        c->aud_unconsumed = c->audio && c->aud_ts[c->active];
     }                                            // else: index the front buffer again (same input, next GOP period)
     if (c->profiling) { CK(cudaEventRecord(c->ev_prof[0], st)); c->prof_index = true; }
     CK(cudaMemsetAsync(c->h.info, 0, 32, st));
@@ -922,12 +1008,81 @@ int ef_tsidx_samples(int device, const int64_t* seq_pts, const uint32_t* seq_pos
     return EF_OK;
 }
 
-// ---- audio (SURVEY.md 8f-3): SBC decode + PDM, stateless --------------------------------------------------------
+// ---- audio (SURVEY.md 8f-3): SBC decode + PDM ---------------------------------------------------------------------
 static int audio_device(int device)
 {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || device < 0 || ndev <= device) return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", device, cudaGetErrorString(e));
+    return EF_OK;
+}
+
+static int audio_constants(int device)
+{
+    static bool constants = false;                       // per process; every device gets its copy on first use
+    static int constants_dev = -1;
+    if (!constants || constants_dev != device) { CK(ef_audio_upload_constants()); constants = true; constants_dev = device; }
+    return EF_OK;
+}
+
+// One decode call once its input is in HBM (blob + blob_off[n + 1]: every stream's held-back bytes followed by its new
+// bytes): probe and count, then - unless pcm is NULL (sizing: info[] only, no state changes) - SBC -> PCM (-> PDM) and
+// the update of the per-stream state. Synchronous on `cs`.
+static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w,
+                             ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, cudaStream_t cs, uint64_t* launches)
+{
+    int4* plan = nullptr;
+    CK(w.get(AudioScratch::PLAN, (size_t)n * sizeof(int4), (void**)&plan));
+    ef_sbc_probe_kernel<<<(n + 127) / 128, 128, 0, cs>>>(blob, blob_off, st, ended, n, plan);
+    CK(cudaGetLastError());
+    ef_sbc_count_kernel<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, cs>>>(blob, blob_off, ended, n, plan);
+    CK(cudaGetLastError());
+    *launches += 2;
+    std::vector<int4> hp((size_t)n);
+    CK(cudaMemcpyAsync(hp.data(), plan, (size_t)n * sizeof(int4), cudaMemcpyDeviceToHost, cs));
+    CK(cudaStreamSynchronize(cs));
+    std::vector<uint64_t> slot((size_t)n + 1, 0), poff((size_t)n + 1, 0);
+    for (int s = 0; s < n; s++) {
+        const uint32_t frames = (uint32_t)hp[s].z;
+        info[s].frame_size = hp[s].x; info[s].n_frames = frames; info[s].pcm_offset = poff[s];
+        slot[s + 1] = slot[s] + (frames ? 1 + (uint64_t)hp[s].y + frames : 0);   // history rows (+ the probe decode of frame 0) + frames
+        poff[s + 1] = poff[s] + (uint64_t)frames * 128;
+    }
+    const uint64_t n_pcm = poff[n];
+    if (!pcm) return EF_OK;                                  // sizing call
+    if (n_pcm > pcm_cap) return fail(EF_ENOMEM, "%llu PCM samples, capacity %llu", (unsigned long long)n_pcm, (unsigned long long)pcm_cap);
+    uint64_t *d_slot = nullptr, *d_poff = nullptr;
+    int32_t *sb_last = nullptr, *vrows = nullptr;
+    int16_t* d_pcm = nullptr;
+    uint16_t* d_pdm = nullptr;
+    CK(w.get(AudioScratch::SLOT, slot.size() * 8, (void**)&d_slot));
+    CK(w.get(AudioScratch::POFF, poff.size() * 8, (void**)&d_poff));
+    CK(w.get(AudioScratch::SB_LAST, (size_t)n * 128 * 4, (void**)&sb_last));
+    CK(cudaMemcpyAsync(d_slot, slot.data(), slot.size() * 8, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(d_poff, poff.data(), poff.size() * 8, cudaMemcpyHostToDevice, cs));
+    if (n_pcm) {
+        CK(w.get(AudioScratch::VROWS, slot[n] * 16 * 16 * 4, (void**)&vrows));
+        CK(w.get(AudioScratch::PCM, n_pcm * 2, (void**)&d_pcm));
+        ef_sbc_matrix_kernel<<<(unsigned)((slot[n] + 3) / 4), 128, 0, cs>>>(blob, blob_off, plan, st, d_slot, n, vrows, sb_last);
+        CK(cudaGetLastError());
+        ef_sbc_window_kernel<<<(unsigned)((n_pcm + 255) / 256), 256, 0, cs>>>(vrows, d_slot, d_poff, n, d_pcm);
+        CK(cudaGetLastError());
+        *launches += 2;
+        if (pdm) {
+            CK(w.get(AudioScratch::PDM, n_pcm * 4, (void**)&d_pdm));
+            ef_pdm_kernel<<<(n + 31) / 32, 32, 0, cs>>>(d_pcm, d_poff, n, st, d_pdm);
+            CK(cudaGetLastError());
+            *launches += 1;
+        }
+    }
+    ef_audio_commit_kernel<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, cs>>>(st, blob, blob_off, plan, d_slot, vrows, sb_last, ended, n);
+    CK(cudaGetLastError());
+    *launches += 1;
+    if (n_pcm) {
+        CK(cudaMemcpyAsync(pcm, d_pcm, n_pcm * 2, cudaMemcpyDeviceToHost, cs));
+        if (pdm) CK(cudaMemcpyAsync(pdm, d_pdm, n_pcm * 4, cudaMemcpyDeviceToHost, cs));
+    }
+    CK(cudaStreamSynchronize(cs));
     return EF_OK;
 }
 
@@ -939,18 +1094,22 @@ int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_
     DeviceScope scope_(device);
     for (int f = 0; f <= n_files; f++) if (off[f] % 188 || (f && off[f] < off[f - 1])) return fail(EF_EINVAL, "offsets must be non-decreasing multiples of 188");
     const uint64_t total = off[n_files] - off[0], n_packets = total / 188;
-    std::vector<uint64_t> poff((size_t)n_files + 1);
-    for (int f = 0; f <= n_files; f++) poff[f] = (off[f] - off[0]) / 188;
-    DevBuf d_ts, d_start, d_kind, d_off, d_pos, d_len, d_esoff, d_es;
-    CK(d_ts.alloc(total)); CK(d_start.alloc(n_packets)); CK(d_kind.alloc(n_packets)); CK(d_off.alloc(poff.size() * 8));
-    CK(d_pos.alloc(n_packets * 4)); CK(d_len.alloc((size_t)n_files * 8)); CK(d_esoff.alloc(poff.size() * 8));
+    std::vector<uint64_t> roff((size_t)n_files + 1);
+    for (int f = 0; f <= n_files; f++) roff[f] = off[f] - off[0];
+    DevBuf d_ts, d_start, d_kind, d_off, d_pos, d_len, d_esoff, d_es, d_gate, d_lead, d_skip;
+    CK(d_ts.alloc(total)); CK(d_start.alloc(n_packets)); CK(d_kind.alloc(n_packets)); CK(d_off.alloc(roff.size() * 8));
+    CK(d_pos.alloc(n_packets * 4)); CK(d_len.alloc((size_t)n_files * 8)); CK(d_esoff.alloc(roff.size() * 8));
+    CK(d_gate.alloc((size_t)n_files * 2)); CK(d_lead.alloc((size_t)n_files * 4)); CK(d_skip.alloc((size_t)n_files));
     CK(cudaMemcpy(d_ts.p, ts + off[0], total, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(d_off.p, poff.data(), poff.size() * 8, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_off.p, roff.data(), roff.size() * 8, cudaMemcpyHostToDevice));
+    CK(cudaMemset(d_gate.p, 0, (size_t)n_files));                       // every file starts with the gate shut (MpegDecoder::reset())
     if (n_packets) {
         ef_audio_ts_packet_kernel<<<(unsigned)((n_packets + 255) / 256), 256>>>((const uint8_t*)d_ts.p, n_packets, (uint8_t*)d_start.p, (uint8_t*)d_kind.p);
         CK(cudaGetLastError());
     }
-    ef_audio_ts_scan_kernel<<<(n_files + 63) / 64, 64>>>((const uint64_t*)d_off.p, n_files, (const uint8_t*)d_start.p, (const uint8_t*)d_kind.p, (uint32_t*)d_pos.p, (uint64_t*)d_len.p);
+    uint8_t* gate = (uint8_t*)d_gate.p;
+    ef_audio_ts_scan_kernel<<<(n_files + 63) / 64, 64>>>((const uint64_t*)d_off.p, n_files, (const uint8_t*)d_start.p, (const uint8_t*)d_kind.p, gate, gate + n_files,
+                                                         (uint32_t*)d_lead.p, (uint8_t*)d_skip.p, (uint32_t*)d_pos.p, (uint64_t*)d_len.p);
     CK(cudaGetLastError());
     std::vector<uint64_t> len((size_t)n_files);
     CK(cudaMemcpy(len.data(), d_len.p, len.size() * 8, cudaMemcpyDeviceToHost));
@@ -959,7 +1118,7 @@ int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_
     if (es_off[n_files] > es_cap || (!es && es_off[n_files])) return fail(EF_ENOMEM, "%llu audio bytes, capacity %llu", (unsigned long long)es_off[n_files], (unsigned long long)es_cap);
     if (es_off[n_files]) {
         CK(d_es.alloc(es_off[n_files]));
-        CK(cudaMemcpy(d_esoff.p, es_off, poff.size() * 8, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d_esoff.p, es_off, roff.size() * 8, cudaMemcpyHostToDevice));
         ef_audio_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256>>>((const uint8_t*)d_ts.p, (const uint64_t*)d_off.p, n_files, n_packets,
                                                                                    (const uint8_t*)d_start.p, (const uint32_t*)d_pos.p, (const uint64_t*)d_esoff.p, (uint8_t*)d_es.p);
         CK(cudaGetLastError());
@@ -968,6 +1127,7 @@ int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_
     return EF_OK;
 }
 
+// the whole-stream call: the context's kernels with a fresh state for every stream, every stream ending in this call
 int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_streams, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm)
 {
     if (!sbc || !off || !info || n_streams < 1) return fail(EF_EINVAL, "null argument");
@@ -975,46 +1135,88 @@ int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_s
     if (rc != EF_OK) return rc;
     DeviceScope scope_(device);
     for (int s = 0; s < n_streams; s++) if (off[s] > off[s + 1]) return fail(EF_EINVAL, "stream offsets must be non-decreasing");
-    static bool constants = false;                       // per process; every device gets its copy on first use
-    static int constants_dev = -1;
-    if (!constants || constants_dev != device) { CK(ef_audio_upload_constants()); constants = true; constants_dev = device; }
+    if ((rc = audio_constants(device)) != EF_OK) return rc;
     const uint64_t total = off[n_streams] - off[0];
     std::vector<uint64_t> roff((size_t)n_streams + 1);
     for (int s = 0; s <= n_streams; s++) roff[s] = off[s] - off[0];
-    DevBuf d_es, d_off, d_fs, d_slot, d_poff, d_v, d_pcm, d_pdm;
-    CK(d_es.alloc(total + 16)); CK(d_off.alloc(roff.size() * 8)); CK(d_fs.alloc((size_t)n_streams * 4));
+    DevBuf d_es, d_off, d_st, d_end;
+    CK(d_es.alloc(total + 16)); CK(d_off.alloc(roff.size() * 8));
+    CK(d_st.alloc((size_t)n_streams * sizeof(EfAudioState))); CK(d_end.alloc((size_t)n_streams));
     CK(cudaMemcpy(d_es.p, sbc + off[0], total, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(d_off.p, roff.data(), roff.size() * 8, cudaMemcpyHostToDevice));
-    ef_sbc_probe_kernel<<<(n_streams + 127) / 128, 128>>>((const uint8_t*)d_es.p, (const uint64_t*)d_off.p, n_streams, (int*)d_fs.p);
-    CK(cudaGetLastError());
-    std::vector<int> fs((size_t)n_streams);
-    CK(cudaMemcpy(fs.data(), d_fs.p, fs.size() * 4, cudaMemcpyDeviceToHost));
-    std::vector<uint64_t> slot((size_t)n_streams + 1, 0), poff((size_t)n_streams + 1, 0);
-    for (int s = 0; s < n_streams; s++) {
-        const uint64_t len = roff[s + 1] - roff[s];
-        const uint32_t frames = fs[s] > 0 ? (uint32_t)(len / (uint64_t)fs[s]) : 0u;
-        info[s].frame_size = fs[s]; info[s].n_frames = frames; info[s].pcm_offset = poff[s];
-        slot[s + 1] = slot[s] + (fs[s] > 0 ? (uint64_t)frames + 1 : 0);      // + the probe decode of frame 0
-        poff[s + 1] = poff[s] + (uint64_t)frames * 128;
+    CK(cudaMemset(d_st.p, 0, (size_t)n_streams * sizeof(EfAudioState)));
+    CK(cudaMemset(d_end.p, 1, (size_t)n_streams));
+    AudioScratch w;
+    uint64_t launches = 0;
+    return audio_decode_blob((const uint8_t*)d_es.p, (const uint64_t*)d_off.p, (EfAudioState*)d_st.p, (const uint8_t*)d_end.p, n_streams, w,
+                             info, pcm, pcm_cap, pdm, 0, &launches);
+}
+
+int ef_audio_enable(ef_ctx* c)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (c->audio) return EF_OK;
+    int rc = audio_constants(c->cfg.device);
+    if (rc != EF_OK) return rc;
+    const int n = c->cfg.n_streams;
+    const size_t cap = c->cfg.es_capacity, packets = cap / 188 + 1;
+#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
+    A(c->d_aud_state, (size_t)n);
+    for (int b = 0; b < 2; b++) {
+        A(c->d_aud2[b], cap + 1024);                      // a submit's audio is never longer than its transport stream
+        A(c->d_aud_off2[b], (size_t)n + 1);
+        A(c->d_gate2[b], (size_t)n); A(c->d_lead2[b], (size_t)n); A(c->d_skip2[b], (size_t)n);
     }
-    const uint64_t n_pcm = poff[n_streams];
-    if (!pcm) return EF_OK;                                  // sizing call
-    if (n_pcm > pcm_cap) return fail(EF_ENOMEM, "%llu PCM samples, capacity %llu", (unsigned long long)n_pcm, (unsigned long long)pcm_cap);
-    if (!n_pcm) return EF_OK;
-    CK(d_slot.alloc(slot.size() * 8)); CK(d_poff.alloc(poff.size() * 8));
-    CK(d_v.alloc(slot[n_streams] * 16 * 16 * 4)); CK(d_pcm.alloc(n_pcm * 2));
-    CK(cudaMemcpy(d_slot.p, slot.data(), slot.size() * 8, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(d_poff.p, poff.data(), poff.size() * 8, cudaMemcpyHostToDevice));
-    ef_sbc_matrix_kernel<<<(unsigned)((slot[n_streams] + 3) / 4), 128>>>((const uint8_t*)d_es.p, (const uint64_t*)d_off.p, (const int*)d_fs.p, (const uint64_t*)d_slot.p, n_streams, (int32_t*)d_v.p);
+    A(c->d_aud_start, packets); A(c->d_aud_kind, packets); A(c->d_aud_pos, packets); A(c->d_aud_len, (size_t)n + 1);
+    A(c->d_blob, cap + (size_t)n * EF_AUDIO_CARRY + 1024); A(c->d_blob_len, (size_t)n + 1); A(c->d_blob_off, (size_t)n + 1);
+    A(c->d_ended, (size_t)n);
+#undef A
+    if (!c->h_ended) CK(cudaHostAlloc((void**)&c->h_ended, (size_t)n, cudaHostAllocDefault));
+    if (!c->aud_scratch) c->aud_scratch = new AudioScratch();
+    CK(cudaMemset(c->d_aud_state, 0, (size_t)n * sizeof(EfAudioState)));
+    for (int b = 0; b < 2; b++) {
+        CK(cudaMemset(c->d_gate2[b], 0, (size_t)n)); CK(cudaMemset(c->d_skip2[b], 0, (size_t)n)); CK(cudaMemset(c->d_lead2[b], 0, (size_t)n * 4));
+        CK(cudaMemset(c->d_aud_off2[b], 0, ((size_t)n + 1) * 8));
+        c->aud_ts[b] = false;
+    }
+    CK(cudaDeviceSynchronize());
+    c->aud_unconsumed = false;
+    c->audio = true;
+    return EF_OK;
+}
+
+int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !info) return fail(EF_EINVAL, "null argument");
+    if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio before ef_audio_enable");
+    int rc = audio_constants(c->cfg.device);
+    if (rc != EF_OK) return rc;
+    const int n = c->cfg.n_streams, a = c->active, p = c->pending;
+    cudaStream_t cs = (cudaStream_t)stream;
+    bool any_end = false;
+    for (int s = 0; s < n; s++) { c->h_ended[s] = end_of_stream && end_of_stream[s] ? 1 : 0; any_end |= c->h_ended[s] != 0; }
+    CK(cudaStreamWaitEvent(cs, c->ev_up_done[a], 0));        // the demux of the current submit has finished
+    if (p >= 0) CK(cudaStreamWaitEvent(cs, c->ev_up_done[p], 0));   // and that of a submit queued behind it (ef_audio_end_kernel)
+    CK(cudaMemcpyAsync(c->d_ended, c->h_ended, (size_t)n, cudaMemcpyHostToDevice, cs));
+    const uint64_t* new_off = c->aud_unconsumed ? c->d_aud_off2[a] : nullptr;
+    ef_audio_len_kernel<<<(n + 255) / 256, 256, 0, cs>>>(c->d_aud_state, new_off, c->d_lead2[a], c->d_skip2[a], n, c->d_blob_len);
     CK(cudaGetLastError());
-    ef_sbc_window_kernel<<<(unsigned)((n_pcm + 255) / 256), 256>>>((const int32_t*)d_v.p, (const uint64_t*)d_slot.p, (const uint64_t*)d_poff.p, n_streams, (int16_t*)d_pcm.p);
+    ef_ts_offsets_kernel<<<1, 1024, 0, cs>>>(c->d_blob_len, n, c->d_blob_off, c->d_blob);
     CK(cudaGetLastError());
-    CK(cudaMemcpy(pcm, d_pcm.p, n_pcm * 2, cudaMemcpyDeviceToHost));
-    if (pdm) {
-        CK(d_pdm.alloc(n_pcm * 4));
-        ef_pdm_kernel<<<(n_streams + 31) / 32, 32>>>((const int16_t*)d_pcm.p, (const uint64_t*)d_poff.p, n_streams, (uint16_t*)d_pdm.p);
+    ef_audio_assemble_kernel<<<n, 256, 0, cs>>>(c->d_aud_state, c->d_aud2[a], new_off, c->d_lead2[a], c->d_skip2[a], c->d_blob_off, c->d_blob);
+    CK(cudaGetLastError());
+    c->launches += 3;
+    rc = audio_decode_blob(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, *c->aud_scratch, info, pcm, pcm_cap, pdm, cs, &c->launches);
+    if (rc != EF_OK || !pcm) return rc;
+    c->aud_unconsumed = false;
+    if (any_end) {
+        ef_audio_end_kernel<<<(n + 255) / 256, 256, 0, cs>>>(c->d_ended, n, c->d_gate2[a], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
+                                                             p >= 0 && c->aud_ts[p]);
         CK(cudaGetLastError());
-        CK(cudaMemcpy(pdm, d_pdm.p, n_pcm * 4, cudaMemcpyDeviceToHost));
+        c->launches++;
+        CK(cudaStreamSynchronize(cs));
     }
     return EF_OK;
 }

@@ -197,6 +197,18 @@ struct EfDev {               // device-visible context (lives in device memory)
     EfGeometry geo;
 };
 
+// Per-stream audio state that one ef_decode_audio call hands to the next (ef_audio.cu). All zero = a fresh stream.
+#define EF_AUDIO_CARRY 264       // most bytes one SBC frame's bit loader reads: header + scale factors 8 + 16 blocks x 128 bits
+struct __align__(16) EfAudioState {
+    int32_t frame_size;      // 0 not learned yet, > 0 learned by the probe, -1 / -2 first frame rejected / outside the domain
+    int32_t carry_len;       // bytes held back: [0, EF_AUDIO_CARRY)
+    int32_t i0, i1, i2;      // delta-sigma modulator of pdm_second_order()
+    int32_t pad[3];
+    int32_t sb[16][8];       // subband samples of the last accepted frame (a rejected frame re-synthesises them)
+    int32_t vhist[9][16];    // V rows of the last 9 blocks (the window reaches 9 blocks back)
+    uint8_t carry[EF_AUDIO_CARRY];
+};
+
 static inline __host__ __device__ size_t ef_frame_offset(int stream, int fb) { return ((size_t)stream * 2 + (size_t)fb) * EF_FRAME; }
 static inline __host__ __device__ int ef_tile_offset(int mx, int my) { return (my * EF_MBW_MAX + mx) * EF_TILE; }
 // byte offset inside a tiled frame of luma pixel (x,y) / of chroma plane p (0 = block 4, 1 = block 5) pixel (x,y)

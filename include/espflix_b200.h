@@ -41,6 +41,7 @@
  *   ef_audio_demux_ts             MpegDecoder::demux() for the audio PIDs -> push_audio() player.cpp:381-432, video.cpp:1007
  *   ef_audio_decode               decode_audio() video.cpp:964, sbc_decoder() sbc_decoder.cpp:343, pdm_second_order()
  *                                 espflix.ino:73
+ *   ef_audio_enable / ef_decode_audio  the same audio path fed by the context's TS submits, one submit at a time
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -208,6 +209,28 @@ typedef struct { int32_t frame_size; uint32_t n_frames; uint64_t pcm_offset; } e
 int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_files, uint8_t* es, uint64_t es_cap, uint64_t* es_off);
 int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_streams, ef_audio_info* info,
                     int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm);
+
+/* ---- audio through a context: the same decode, continued submit after submit ------------------------------------
+ * ef_audio_enable  from now on every ef_submit_ts_* of this context also demuxes PID 0x101 / 0x102 of every stream
+ *                  (MpegDecoder::demux() -> push_audio(), player.cpp:381-432); the demux gate of a stream carries from
+ *                  one submit to the next. Audio state lives in the context until ef_reset, which clears it and keeps
+ *                  audio enabled. ES submits carry no audio.
+ * ef_decode_audio  decode_audio() (video.cpp:964-986) + sbc_decoder() + pdm_second_order() for every stream, continuing
+ *                  where the previous call stopped: consumes the audio of the TS submit the last ef_index made current,
+ *                  appended to the bytes each stream still holds, and emits every frame that has become decodable (all
+ *                  the bytes its bit loader reads are present). Output and info[] as ef_audio_decode: info[s].n_frames /
+ *                  pcm_offset = this call's frames, frame_size = the stream's learned size or 0 / -1 / -2.
+ *                  end_of_stream[n_streams] (may be NULL): the stream ends after this call; its held-back frames are
+ *                  decoded as the whole-stream call decodes them, then its audio state and demux gate start over (also
+ *                  for a TS submit already queued behind the current one). pcm == NULL: sizing call, fills info[] and
+ *                  changes no state. pdm == NULL: no PDM, and the modulator state stays where it is. Synchronous.
+ *                  Concatenated over the calls, PCM and PDM equal ef_audio_decode on the stream's whole audio.
+ *                  Errors: EF_ESTATE before ef_audio_enable; EF_ENOMEM when pcm_cap is too small (state untouched).
+ *                  On an audio-enabled context, ef_index of a new submit returns EF_ESTATE while the current TS submit's
+ *                  audio has not been consumed; indexing the same submit again adds no audio. */
+int ef_audio_enable(ef_ctx* ctx);
+int ef_decode_audio(ef_ctx* ctx, const uint8_t* end_of_stream, ef_audio_info* info,
+                    int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
