@@ -77,6 +77,8 @@ _SIGNATURES = {
     "ef_audio_decode": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_audio_enable": (_I, [_VP]),
     "ef_decode_audio": (_I, [_VP, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_pts_enable": (_I, [_VP]),
+    "ef_picture_pts": (_I, [_VP, _I, _I, _I, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -297,6 +299,21 @@ class Context:
             out.append({"frame_size": int(i["frame_size"]), "n_frames": int(i["n_frames"]), "pcm": pcm_out[a:a + k].copy(),
                         "pdm": None if pdm_out is None else pdm_out[2 * a:2 * (a + k)].copy()})
         return out
+
+    # -- presentation timestamps -----------------------------------------------------------------
+    def enable_pts(self):
+        """from now on every TS submit also lists its video PES starts, and every index() resolves the pts of every picture"""
+        self._check(self.lib.ef_pts_enable(self._h))
+
+    def picture_pts(self, first=0, count=None, n_pictures=None):
+        """ef_picture_pts for the submit the last index() made current -> (int64[count, n_pictures] pts of every picture, -1
+        past a stream's pictures; int64[count] pts of every stream's most recent picture over all submits, get_pts())"""
+        count = self.n_streams - first if count is None else count
+        n_pictures = self.max_pictures if n_pictures is None else n_pictures
+        pic = np.full((max(count, 0), n_pictures), -1, dtype=np.int64)
+        last = np.full(max(count, 0), -1, dtype=np.int64)
+        self._check(self.lib.ef_picture_pts(self._h, first, count, n_pictures, _ptr(pic) if pic.size else None, _ptr(last) if last.size else None))
+        return pic, last
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

@@ -24,6 +24,9 @@ __global__ void ef_ts_len_kernel(const uint8_t* ts, uint64_t n_packets, uint32_t
 __global__ void ef_ts_copy_kernel(const uint8_t* ts, uint64_t n_packets, const uint32_t* local_off, const uint16_t* pkt_stream, const uint64_t* es_off, uint8_t* es);
 __global__ void ef_ts_scan_kernel(const uint32_t* len, const uint64_t* ts_off, uint32_t* local_off, uint16_t* pkt_stream, uint64_t* stream_total);
 __global__ void ef_ts_offsets_kernel(const uint64_t* stream_total, int n_streams, uint64_t* es_off, uint8_t* es);
+__global__ void ef_pts_packet_kernel(const uint8_t* ts, const uint64_t* ts_off, const uint32_t* local_off, uint32_t* list_off, int64_t* list_pts, uint2* span);
+__global__ void ef_pts_resolve_kernel(const EfDev* Dp, const uint2* span, const uint32_t* list_off, const int64_t* list_pts, int64_t* carry, int64_t* last,
+                                      int64_t* pic_pts);
 size_t ef_recon_smem_bytes();
 cudaError_t ef_decode_configure();
 int ef_decode_resident_ctas(int which);
@@ -196,6 +199,16 @@ struct ef_ctx {
     uint8_t* d_ended = nullptr;
     uint8_t* h_ended = nullptr;                   // pinned
     struct AudioScratch* aud_scratch = nullptr;
+    // presentation timestamps (ef_pts_enable): every TS submit also lists the video PES starts with a valid PTS of every
+    // stream in its ES buffer's list; ef_index resolves the PTS of every picture from it
+    bool pts = false;
+    bool pts_resolved = false;                    // the last ef_index ran the resolve pass (ef_picture_pts has something to report)
+    uint32_t* d_pts_off2[2] = { nullptr, nullptr };   // per ES buffer, one entry per packet: stream-local ES offset of the PES payload
+    int64_t* d_pts_val2[2] = { nullptr, nullptr };    // ... and its PTS
+    uint2* d_pts_span2[2] = { nullptr, nullptr };     // per ES buffer: (first entry, entries) of every stream
+    int64_t* d_pts_carry = nullptr;               // [n_streams] the last valid PTS of all submits so far (the reference's _pts)
+    int64_t* d_pts_last = nullptr;                // [n_streams] PTS of the most recent picture (get_pts())
+    int64_t* d_pic_pts = nullptr;                 // [n_streams][max_pictures] PTS of every picture of the current submit
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -419,6 +432,12 @@ int ef_reset(ef_ctx* c)
         for (int b = 0; b < 2; b++) { CK(cudaMemset(c->d_gate2[b], 0, (size_t)c->cfg.n_streams)); c->aud_ts[b] = false; }
         c->aud_unconsumed = false;
     }
+    if (c->pts) {                                         // every stream's PTS starts over at -1; PTS stays enabled
+        CK(cudaDeviceSynchronize());                      // a resolve pass on a caller's stream may still write them
+        CK(cudaMemset(c->d_pts_carry, 0xFF, (size_t)c->cfg.n_streams * 8));
+        CK(cudaMemset(c->d_pts_last, 0xFF, (size_t)c->cfg.n_streams * 8));
+        c->pts_resolved = false;
+    }
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
     return EF_OK;
@@ -479,6 +498,13 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
             CK(cudaGetLastError());
             c->launches += 4;
         } else CK(cudaMemsetAsync(d_es_off, 0, ((size_t)n + 1) * 8, up));
+    }
+    if (c->pts) {                                         // the video PES starts of this submit, into its ES buffer's list
+        if (ts) {
+            ef_pts_packet_kernel<<<n, 256, 0, up>>>(c->d_ts, c->d_ts_off, c->d_pkt_off, c->d_pts_off2[b], c->d_pts_val2[b], c->d_pts_span2[b]);
+            CK(cudaGetLastError());
+            c->launches++;
+        } else CK(cudaMemsetAsync(c->d_pts_span2[b], 0, (size_t)n * sizeof(uint2), up));   // ES submits carry no PES
     }
     if (c->audio) {
         // The demux gate of every stream continues from the submit that is current now (the front buffer): submits are
@@ -544,6 +570,14 @@ int ef_index(ef_ctx* c, void* stream)
     CK(cudaGetLastError());
     c->launches += 3;
     if (c->profiling) CK(cudaEventRecord(c->ev_prof[1], st));
+    if (c->pts) {
+        const int a = c->active;
+        ef_pts_resolve_kernel<<<(n * 32 + 127) / 128, 128, 0, st>>>(c->d, c->d_pts_span2[a], c->d_pts_off2[a], c->d_pts_val2[a], c->d_pts_carry, c->d_pts_last,
+                                                                    c->d_pic_pts);
+        CK(cudaGetLastError());
+        c->launches++;
+        c->pts_resolved = true;
+    }
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));
     c->indexed = true;
     return EF_OK;
@@ -1218,6 +1252,46 @@ int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info
         c->launches++;
         CK(cudaStreamSynchronize(cs));
     }
+    return EF_OK;
+}
+
+// ---- presentation timestamps: push_video(frame, front, _last_pts, mode) player.cpp:692-702, get_pts() player.cpp:653-656 ----
+int ef_pts_enable(ef_ctx* c)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (c->pts) return EF_OK;
+    const int n = c->cfg.n_streams;
+    const size_t packets = c->cfg.es_capacity / 188 + 1;
+    int rc;
+#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
+    for (int b = 0; b < 2; b++) { A(c->d_pts_off2[b], packets); A(c->d_pts_val2[b], packets); A(c->d_pts_span2[b], (size_t)n); }
+    A(c->d_pts_carry, (size_t)n); A(c->d_pts_last, (size_t)n); A(c->d_pic_pts, (size_t)n * c->cfg.max_pictures);
+#undef A
+    CK(cudaDeviceSynchronize());                          // a queued TS submit was demuxed without PES lists: it carries none
+    for (int b = 0; b < 2; b++) CK(cudaMemset(c->d_pts_span2[b], 0, (size_t)n * sizeof(uint2)));
+    CK(cudaMemset(c->d_pts_carry, 0xFF, (size_t)n * 8));
+    CK(cudaMemset(c->d_pts_last, 0xFF, (size_t)n * 8));
+    CK(cudaMemset(c->d_pic_pts, 0xFF, (size_t)n * c->cfg.max_pictures * 8));
+    CK(cudaDeviceSynchronize());
+    c->pts = true;
+    c->pts_resolved = false;
+    return EF_OK;
+}
+
+int ef_picture_pts(ef_ctx* c, int first, int count, int n_pictures, int64_t* pic_pts, int64_t* last_pts)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->pts) return fail(EF_ESTATE, "ef_picture_pts before ef_pts_enable");
+    if (!c->pts_resolved) return fail(EF_ESTATE, "ef_picture_pts before ef_index");
+    if (first < 0 || count < 1 || first > c->cfg.n_streams - count) return fail(EF_EINVAL, "stream range out of bounds");
+    if (n_pictures < 0 || n_pictures > c->cfg.max_pictures) return fail(EF_EINVAL, "n_pictures %d out of range", n_pictures);
+    CK(cudaDeviceSynchronize());
+    const size_t mp = (size_t)c->cfg.max_pictures;
+    if (pic_pts && n_pictures)
+        CK(cudaMemcpy2D(pic_pts, (size_t)n_pictures * 8, c->d_pic_pts + (size_t)first * mp, mp * 8, (size_t)n_pictures * 8, (size_t)count, cudaMemcpyDeviceToHost));
+    if (last_pts) CK(cudaMemcpy(last_pts, c->d_pts_last + first, (size_t)count * 8, cudaMemcpyDeviceToHost));
     return EF_OK;
 }
 

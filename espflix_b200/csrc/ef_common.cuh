@@ -134,7 +134,7 @@ struct __align__(16) EfPic {
     uint16_t seq;           // index into the stream's EfSeq table (0 = state carried over from the previous submit)
     uint8_t type;           // picture_coding_type 1..4 (0 = none)
     uint8_t fp_rsize;       // bit0 full_pel_forward, bits1-3 forward_r_size, as slice() will see them
-    uint32_t pad;
+    uint32_t code_off;      // stream-relative offset of the picture start code's code byte (0x00), for the PTS latch
 };
 
 struct __align__(16) EfWork {   // one slice of one stream for one picture index

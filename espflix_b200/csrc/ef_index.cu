@@ -13,6 +13,8 @@
 // TS input (the reference's wire format) is first compacted to an elementary stream by
 //   ef_ts_len_kernel / ef_ts_copy_kernel    one thread per 188-byte packet (more()/demux(),
 //                                           player.cpp:381-493)
+// and, after ef_pts_enable, the presentation timestamp of every picture by
+//   ef_pts_packet_kernel (per TS submit, one CTA per stream) / ef_pts_resolve_kernel (per ef_index, one warp per stream)
 #include "ef_common.cuh"
 #include "ef_iso11172_tables.h"
 
@@ -140,7 +142,7 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
                     if (idx < (uint32_t)D.max_pictures && lane == 0) {
                         EfPic p;
                         p.first_slice = n_slice; p.n_slices = 0; p.type = (uint8_t)type; p.fp_rsize = (uint8_t)fp_rs;
-                        p.seq = (uint16_t)min(n_seq, (uint32_t)D.max_seq); p.pad = 0;
+                        p.seq = (uint16_t)min(n_seq, (uint32_t)D.max_seq); p.code_off = (uint32_t)(pos + 3);
                         pics[idx] = p;
                     }
                 } else if (code >= 0x01 && code <= 0xAF) {                    // slice start code
@@ -377,4 +379,105 @@ ef_ts_offsets_kernel(const uint64_t* __restrict__ stream_total, int n_streams, u
     if (threadIdx.x == 0) es_off[n_streams] = carry;
     // K1's bit reader runs a few bytes past the last slice: zero the 256 bytes behind the elementary stream
     if (threadIdx.x < 256) es[carry + threadIdx.x] = 0;
+}
+
+// ---- presentation timestamps of the pictures of TS submits (ef_pts_enable) ------------------------------------------
+// The reference latches _pts in demux() when a video PES start carries a valid PTS (player.cpp:399-419; parse_pts()'s prefix
+// check, player.cpp:299-306) and hands it to the picture whose header is parsed next: picture() -> flush_picture() sets
+// _last_pts = _pts (player.cpp:692-702) and pushes it with that picture one header later. demux() runs when the bit reader
+// fetches the packet's first payload byte (more(), player.cpp:459-493), and FILL_BITS keeps 24 bits buffered (player.cpp:348-352),
+// so when picture() runs after the 24-bit prefix and the 8-bit code (player.cpp:1360-1363) the reader has fetched the code byte
+// and the 2 bytes after it. Hence: pts(picture) = PTS of the last valid video PES start whose first payload byte lies at ES
+// offset <= code byte + 2, else the value carried from earlier submits (-1 if none; reset() does not clear _pts).
+
+// PTS of a video (PID 0x100) packet that starts a PES with a non-empty payload and a PTS with the right prefix; -1 otherwise
+__device__ __forceinline__ int64_t ts_video_pes_pts(const uint8_t* d)
+{
+    if (d[0] != 0x47 || !(d[1] & 0x40) || !(d[3] & 0x10)) return -1;
+    if ((((d[1] << 8) | d[2]) & 0x1FFF) != 0x100) return -1;
+    const int o = (d[3] & 0x20) ? 5 + d[4] : 4;
+    if (o + 9 > 188 || o + 9 + d[o + 8] >= 188) return -1;        // no PES payload reaches the ES (as ts_payload())
+    const int flags = (d[o + 6] << 8) | d[o + 7];
+    if (!(flags & 0x0080) || o + 14 > 188) return -1;             // PES_PTS
+    const uint8_t* q = d + o + 9;
+    if ((q[0] & 0xF0) != ((flags >> 2) & 0x30)) return -1;        // parse_pts(): '0010' for PTS only, '0011' with DTS
+    int64_t n = ((int64_t)(q[0] & 0x0E)) << 29;
+    n += (int64_t)((((uint32_t)q[1] << 8) | q[2]) >> 1) << 15;
+    return n + ((((uint32_t)q[3] << 8) | q[4]) >> 1);
+}
+
+// Packet pass, one CTA per stream, one thread per packet: the stream's video PES starts with a valid PTS, in packet order, as
+// (stream-local ES offset of the first payload byte, pts) at list_*[first packet of the stream ...]; span[s] = (that index, count).
+// local_off comes from ef_ts_scan_kernel. The lists belong to one ES buffer: the shared packet tables are overwritten by the next
+// submit while the compute stream may still resolve this one.
+__global__ void __launch_bounds__(256)
+ef_pts_packet_kernel(const uint8_t* __restrict__ ts, const uint64_t* __restrict__ ts_off, const uint32_t* __restrict__ local_off,
+                     uint32_t* __restrict__ list_off, int64_t* __restrict__ list_pts, uint2* __restrict__ span)
+{
+    __shared__ uint32_t warp_cnt[8];
+    __shared__ uint32_t carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, s = blockIdx.x;
+    const uint64_t p0 = ts_off[s] / 188, p1 = ts_off[s + 1] / 188;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (uint64_t base = p0; base < p1; base += 256) {
+        const uint64_t k = base + threadIdx.x;
+        const int64_t pts = k < p1 ? ts_video_pes_pts(ts + k * 188) : -1;
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, pts >= 0);
+        if (lane == 0) warp_cnt[warp] = __popc(m);
+        __syncthreads();
+        uint32_t before = carry;
+        for (int w = 0; w < warp; w++) before += warp_cnt[w];
+        if (pts >= 0) {
+            const uint64_t j = p0 + before + __popc(m & ((1u << lane) - 1u));
+            list_off[j] = local_off[k];
+            list_pts[j] = pts;
+        }
+        __syncthreads();
+        if (threadIdx.x == 255) carry = before + __popc(m);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) span[s] = make_uint2((uint32_t)p0, carry);
+}
+
+// Resolve pass after ef_fill_kernel, one warp per stream, lanes over pictures: upper-bound search for code byte + 2 in the
+// stream's list, else the carried PTS. pic_pts[s][p] (-1 past the stream's pictures); carry[s] becomes the submit's last valid
+// PTS and last[s] the PTS of its most recent picture (get_pts(), player.cpp:653-656). Indexing the same submit again rolls
+// both as if the input followed itself.
+__global__ void __launch_bounds__(128)
+ef_pts_resolve_kernel(const EfDev* __restrict__ Dp, const uint2* __restrict__ span, const uint32_t* __restrict__ list_off,
+                      const int64_t* __restrict__ list_pts, int64_t* __restrict__ carry, int64_t* __restrict__ last, int64_t* __restrict__ pic_pts)
+{
+    const EfDev& D = *Dp;
+    const int lane = threadIdx.x & 31;
+    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (s >= D.n_streams) return;
+    const uint2 sp = span[s];
+    const uint32_t* lo = list_off + sp.x;
+    const int64_t* lp = list_pts + sp.x;
+    const int64_t carried = carry[s];
+    const uint32_t np = D.n_pics[s];
+    const EfPic* pics = D.pics + (size_t)s * D.max_pictures;
+    int64_t* out = pic_pts + (size_t)s * D.max_pictures;
+    int64_t newest = last[s];
+    for (uint32_t p0 = 0; p0 < (uint32_t)D.max_pictures; p0 += 32) {
+        const uint32_t p = p0 + lane;
+        int64_t v = -1;
+        if (p < np) {
+            const uint64_t latch = (uint64_t)pics[p].code_off + 2;
+            uint32_t a = 0, b = sp.y;                                  // first entry with offset > latch
+            while (a < b) {
+                const uint32_t m = (a + b) >> 1;
+                if (lo[m] <= latch) a = m + 1; else b = m;
+            }
+            v = a ? lp[a - 1] : carried;
+        }
+        if (p < (uint32_t)D.max_pictures) out[p] = v;
+        const int64_t at_last = __shfl_sync(0xFFFFFFFFu, v, (np - 1) & 31);
+        if (np && (np - 1) / 32 == p0 / 32) newest = at_last;
+    }
+    if (lane == 0) {
+        carry[s] = sp.y ? lp[sp.y - 1] : carried;
+        last[s] = newest;
+    }
 }

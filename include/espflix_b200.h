@@ -42,6 +42,9 @@
  *   ef_audio_decode               decode_audio() video.cpp:964, sbc_decoder() sbc_decoder.cpp:343, pdm_second_order()
  *                                 espflix.ino:73
  *   ef_audio_enable / ef_decode_audio  the same audio path fed by the context's TS submits, one submit at a time
+ *   ef_pts_enable / ef_picture_pts     the pts push_video(frame, front, _last_pts, mode) hands over with every picture
+ *                                 (flush_picture() player.cpp:692-702, latched from demux() player.cpp:399-419) and
+ *                                 get_pts() player.cpp:653-656, for every stream of a TS submit
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -231,6 +234,30 @@ int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_s
 int ef_audio_enable(ef_ctx* ctx);
 int ef_decode_audio(ef_ctx* ctx, const uint8_t* end_of_stream, ef_audio_info* info,
                     int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream);
+
+/* ---- presentation timestamps of the pictures of TS submits -----------------------------------------------------
+ * The reference's decoder latches _pts when a video PES start carries a PTS with a valid prefix (demux(), parse_pts(),
+ * player.cpp:299-306, 399-419; a missing or malformed PTS keeps the previous value, reset() does not clear it) and pushes
+ * every picture with the value latched at its header (flush_picture(), player.cpp:692-702). Its bit reader keeps 24 bits
+ * buffered (player.cpp:348-352) and demuxes a packet when it fetches the packet's first payload byte (more(), player.cpp:
+ * 459-493), so at picture() (player.cpp:1360-1363) it has demuxed up to the code byte + 2. The rule, over the stream's
+ * whole video ES across submits:
+ *     pts(picture) = PTS of the last video PES start with a valid PTS whose first payload byte lies at ES offset
+ *                    <= (offset of the picture start code's 0x00 code byte) + 2; -1 if there is none.
+ * B/D picture headers latch like I/P headers. The reference pushes nothing while the first picture's pts is -1 (the
+ * frame buffers do not swap); the rule's value is reported there all the same.
+ * ef_pts_enable   from now on every ef_submit_ts_* also lists the video PES starts of every stream (one device pass on
+ *                 the upload stream) and every ef_index resolves the pts of every picture (one pass). A context that
+ *                 never calls it launches no extra kernel. ES submits, and TS submits made before enabling, carry no PES:
+ *                 their pictures get the carried value. ef_reset sets every stream back to -1 and keeps PTS enabled.
+ *                 Indexing the same submit again carries the state on as if the same input followed itself.
+ * ef_picture_pts  synchronous; about the submit made current by the last ef_index, streams [first, first + count):
+ *                 pic_pts[k * n_pictures + p] = pts of picture p of stream first + k (-1 for p >= its picture count),
+ *                 last_pts[k] = what get_pts() returns after that submit: the pts of the stream's most recent picture over
+ *                 all submits (-1 if none). Either pointer may be NULL. EF_ESTATE before ef_pts_enable or before an
+ *                 ef_index that followed it; EF_EINVAL for a bad stream range or n_pictures outside 0..max_pictures. */
+int ef_pts_enable(ef_ctx* ctx);
+int ef_picture_pts(ef_ctx* ctx, int first, int count, int n_pictures, int64_t* pic_pts, int64_t* last_pts);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
