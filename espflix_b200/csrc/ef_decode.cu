@@ -206,7 +206,7 @@ struct SliceState {
     uint32_t seqi;           // index of the slice's sequence state in the stream's EfSeq table (K1a v3: handed to K1b for streams with their own matrices)
     const uint32_t* qzp;     // generic pointer to the table words in use: T.qz in shared memory (default matrices) or the stream's own in HBM
     const uint32_t* qz;      // scan-order quantiser | prescale | raster index tables [intra 64 | non-intra 64] of a stream with its OWN matrices (global memory); nullptr = the defaults, served from shared memory
-    int mbw, mbh;
+    int mbw;
     int mb_x, mb_y;          // last macroblock handled
     int first;               // next macroblock is the first of the slice (Q6)
     int ptype, full_pel, r_size;
@@ -417,12 +417,12 @@ __device__ __forceinline__ bool parse_header(SliceState& s, const SharedTables& 
         uint32_t e = T.mba[lz * 32 + ((w << (lz + 1)) >> 27)];
         int len = e & 15, val = (int)(e >> 4);
         if (!len) return false;
-        if (val >= 34) {                            // 34 stuffing, 35 escape: consume and look again
+        if (val == 35 || (val == 34 && !increment)) {     // escape, or stuffing before the first escape: consume and look again
             br.skip(len);
             if (val == 35) increment += 33;
             continue;
         }
-        increment += val;
+        increment += val;                           // stuffing after an escape ends the address: + 34 (player.cpp:1269-1275)
         used = len;
         break;
     }
@@ -431,7 +431,7 @@ __device__ __forceinline__ bool parse_header(SliceState& s, const SharedTables& 
     else if (increment > 1) { s.dc_y = s.dc_cr = s.dc_cb = 128; s.mv_h = s.mv_v = 0; skip_before = increment - 1; }
     s.mb_x += increment;
     while (s.mb_x >= s.mbw) { s.mb_x -= s.mbw; s.mb_y++; }     // inc_mb(), player.cpp:823
-    if (s.mb_y >= s.mbh) return false;              // the reference would write past the frame here
+    if (s.mb_y >= EF_MBH_MAX) return false;         // past the frame's 12 strips: the reference would write out of bounds
 
     int mb_type;                                    // macroblock_type (player.cpp:1292)
     bits = w << used;
@@ -644,7 +644,6 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                         s.ptype = (w.info >> 8) & 7; s.full_pel = (w.info >> 11) & 1; s.r_size = (w.info >> 12) & 7;
                         const EfSeq* seq = D.seq + (size_t)w.stream * (D.max_seq + 1) + (w.info >> 16);
                         s.mbw = min((int)seq->mb_width, EF_MBW_MAX);
-                        s.mbh = min((int)seq->mb_height, EF_MBH_MAX);
                         s.qz = seq->custom ? (const uint32_t*)seq->qz : nullptr;
                         s.seqi = w.info >> 16;
                         s.qzp = s.qz ? s.qz : T.qz;
@@ -657,7 +656,7 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                         s.mb_y = code - 2; s.mb_x = s.mbw - 1;   // slice(), player.cpp:1255: the first increment lands on column 0 of row code-1
                         s.first = 1;
                         s.dc_y = s.dc_cr = s.dc_cb = 128; s.mv_h = s.mv_v = 0;
-                        active = code >= 1 && code <= s.mbh && s.mbw > 0 && seq->valid;
+                        active = code >= 1 && code - 2 < (int)seq->mb_height && s.mbw > 0 && seq->valid;     // player.cpp:1257
                         if (active) {
                             s.qscale = (int)s.br.get(5);
                             while (s.br.get(1)) s.br.skip(8);    // extra_information_slice
@@ -708,7 +707,7 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                 bool block_done = sy.kind == EF_SYM_EOB;
                 if (sy.kind == EF_SYM_DERAIL) {                  // give up on this and the remaining blocks, end the slice
                     info_acc |= (blkbit << 6) | ((uint32_t)cbp_rem << 14);
-                    s.mb_y = s.mbh;
+                    s.mb_y = EF_MBH_MAX;
                     busy = false;
                 } else {
                     if (sy.kind == EF_SYM_COEF) {
@@ -749,7 +748,7 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                 if (fl & EF_STEP_COEF2) { n += st.run2; put_entry(ef_coef_entry(qword(n), st.lvl2, s.qscale, kq, blk24)); n++; }
                 if (fl & 16u) {                                // give up on this and the remaining blocks, end the slice
                     info_acc |= (blkbit << 6) | ((uint32_t)cbp_rem << 14);
-                    s.mb_y = s.mbh;
+                    s.mb_y = EF_MBH_MAX;
                     busy = false;
                 } else {
                     br.skip(len);

@@ -463,7 +463,7 @@ static int slice(dec_t* d, int s)
 {
     d->mb_y = s - 2;
     d->mb_x = d->mb_width - 1;
-    if (d->mb_y >= d->mb_height - 1) return -1;        /* reference tests >= mb_height and then writes out of bounds for s == 13 */
+    if (d->mb_y >= d->mb_height) return -1;            /* player.cpp:1257 */
     reset_predictors(d);
     d->quantizer_scale = (int)get_bits(d, 5);
     while (get_bit(d)) get_bits(d, 8);
@@ -481,14 +481,14 @@ static int slice(dec_t* d, int s)
             if (increment > 1) reset_predictors(d);
             while (increment > 1) {
                 inc_mb(d);
-                if (d->mb_y >= d->mb_height) return -1;   /* reference: out-of-bounds write */
+                if (d->mb_y >= 12) return -1;             /* past the frame's 12 strips: the reference writes out of bounds */
                 g_stats.skipped++;
                 predict_zero(d);
                 increment--;
             }
             inc_mb(d);
         }
-        if (d->mb_y >= d->mb_height) return -1;        /* reference: out-of-bounds write */
+        if (d->mb_y >= 12) return -1;                  /* past the frame's 12 strips: the reference writes out of bounds */
 
         int mb_type = get_vlc(d, d->picture_coding_type == 1 ? &T_type_i : &T_type_p);
         int intra = mb_type & 0x01;

@@ -4,7 +4,7 @@
   here (no GPU):   python tools/sweep_variants.py build  tag1="-DEF_K1A_HDR_BATCH=8" tag2="..."
                    cross-compiles espflix_b200/libespflix_b200.<tag>.so for every tag (they travel to the GPU box)
   under gpurun:    python tools/sweep_variants.py run [--check] [--bench-args "..."] tag1 tag2 ...
-                   per tag: optional quick parity check (a subset of tests/test_decode_gpu.py against the oracle),
+                   per tag: optional quick parity check (a subset of tests/test_decode_gpu.py, then tests/test_syntax_gpu.py),
                    then bench.py --no-cpu; one line per tag in gpurun_out/sweep_variants.txt
 The product library (tag "base" = libespflix_b200.so) is never replaced by a variant."""
 import json
@@ -45,6 +45,9 @@ def main():
         if check:
             r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_decode_gpu.py", "-x", "-q", "-m", "gpu", "-k",
                                 "coverage or mixed or outside or multi_picture"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
+            if r.returncode == 0:       # the syntax-level streams reach the header and K1b paths the coverage streams do not
+                r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_syntax_gpu.py", "-x", "-q", "-m", "gpu"],
+                                   cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
             status = "parity " + ("ok" if r.returncode == 0 else "FAILED " + r.stdout[-400:].replace("\n", " | "))
         r = subprocess.run([sys.executable, "bench.py"] + bench_args.split(), cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
         try:
