@@ -79,6 +79,9 @@ _SIGNATURES = {
     "ef_decode_audio": (_I, [_VP, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_pts_enable": (_I, [_VP]),
     "ef_picture_pts": (_I, [_VP, _I, _I, _I, _VP, _VP]),
+    "ef_present_enable": (_I, [_VP, _VP]),
+    "ef_present_picture": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_present_idle": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -315,6 +318,34 @@ class Context:
         self._check(self.lib.ef_picture_pts(self._h, first, count, n_pictures, _ptr(pic) if pic.size else None, _ptr(last) if last.size else None))
         return pic, last
 
+    # -- paced presentation ---------------------------------------------------------------------
+    def enable_present(self, frame_counter0=None):
+        """every stream gets its own display, starting at line 0 of field frame_counter0[s] (default 0); needs enable_pts()"""
+        fc = None if frame_counter0 is None else np.ascontiguousarray(np.broadcast_to(frame_counter0, (self.n_streams,)), dtype=np.uint32)
+        self._check(self.lib.ef_present_enable(self._h, _ptr(fc)))
+
+    def _present(self, call, out, stream):
+        info = np.zeros(self.n_streams, dtype=PRESENT_INFO)
+        if out is None:
+            dst, cap = None, 0
+        else:
+            assert out.is_cuda and str(out.dtype) == "torch.uint16" and out.is_contiguous()
+            w, n = self.geometry()
+            dst, cap = out.data_ptr(), out.numel() // (w * n)       # whole fields only
+        self._check(call(dst, cap, info.ctypes.data, stream))
+        return info
+
+    def present_picture(self, pic, modes=None, out=None, stream=0):
+        """ef_present_picture: decode picture index `pic` and push it on every stream that has it. out: CUDA uint16 tensor of
+        whole fields (None: sizing call). Returns info (PRESENT_INFO per stream)."""
+        md = None if modes is None else np.ascontiguousarray(np.broadcast_to(modes, (self.n_streams,)), dtype=np.uint8)
+        return self._present(lambda d, c, i, st: self.lib.ef_present_picture(self._h, pic, _ptr(md), d, c, i, st), out, stream)
+
+    def present_idle(self, n_fields, out=None, stream=0):
+        """ef_present_idle: every display runs on until it has emitted n_fields[s] more fields"""
+        nf = np.ascontiguousarray(np.broadcast_to(n_fields, (self.n_streams,)), dtype=np.uint32)
+        return self._present(lambda d, c, i, st: self.lib.ef_present_idle(self._h, nf.ctypes.data, d, c, i, st), out, stream)
+
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))
 
@@ -326,6 +357,10 @@ class Context:
         a, b, c = ctypes.c_float(), ctypes.c_float(), ctypes.c_float()
         self._check(self.lib.ef_stage_ms(self._h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)))
         return a.value, b.value, c.value
+
+
+PRESENT_INFO = np.dtype([("first", "<u8"), ("n_fields", "<u4"), ("frame_counter", "<u4"), ("flip_field", "<u4"), ("flip_line", "<i4"),
+                         ("flags", "<i4"), ("pad", "<i4")])
 
 
 # -- trick-mode index (indexer/indexer.cpp; SURVEY.md 8f-4) ---------------------------------------------

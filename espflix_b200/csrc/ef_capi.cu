@@ -52,6 +52,12 @@ cudaError_t ef_launch_parse(const EfDev& dev, int pic0, int n_pics, int sm_count
 cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t n_slots, cudaStream_t stream);
 cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometry& g, int fb, int frame_counter, const EfPresent& pr, cudaStream_t stream);
 cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line, int x, int width, int frame_counter, uint16_t* dst, cudaStream_t stream);
+cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
+                                      uint64_t* launches);
+__global__ void ef_pace_kernel(const EfPaceState* st, EfPaceState* next, EfPaceRun* run, EfPaceOut* out, const int64_t* pic_pts, const uint32_t* n_pics,
+                               const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc);
+__global__ void ef_pace_fill_kernel(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc);
+static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
 
 namespace {
 
@@ -143,6 +149,7 @@ struct ef_ctx {
     EfDev h;                   // host copy of the device context
     EfDev* d = nullptr;           // = dd[active]
     std::vector<void*> allocs;
+    std::vector<void*> allocs_host;               // pinned
     // Two elementary-stream buffers: a submit uploads into the back one on an internal stream while
     // the kernels of the previous submit still read the front one; ef_index flips them.
     uint8_t* d_es2[2] = { nullptr, nullptr };
@@ -209,6 +216,24 @@ struct ef_ctx {
     int64_t* d_pts_carry = nullptr;               // [n_streams] the last valid PTS of all submits so far (the reference's _pts)
     int64_t* d_pts_last = nullptr;                // [n_streams] PTS of the most recent picture (get_pts())
     int64_t* d_pic_pts = nullptr;                 // [n_streams][max_pictures] PTS of every picture of the current submit
+    // paced presentation (ef_present_enable): every stream's display, advanced by ef_present_picture / ef_present_idle
+    bool paced = false;
+    bool pace_indexed = false;                    // an ef_index followed ef_present_enable: its pictures are to be presented
+    int pace_ntsc = 1;                            // the standard, fixed at ef_present_enable
+    int pace_next = 0;                            // the picture index ef_present_picture takes next
+    int pace_npics = -1;                          // picture indices of the current submit (-1: not read yet)
+    int pace_p0 = 0;                              // first picture index of the current K1a range
+    EfPaceState* d_pace = nullptr;                // [n_streams]
+    EfPaceState* d_pace_next = nullptr;           // [n_streams] the state after the call being made
+    EfPaceRun* d_pace_run = nullptr;              // [n_streams]
+    EfPaceOut* d_pace_out = nullptr;              // [n_streams]
+    EfPaceOut* h_pace_out = nullptr;              // pinned
+    uint64_t* d_pace_first = nullptr;             // [n_streams] output offset of every stream's fields
+    uint64_t* h_pace_first = nullptr;             // pinned
+    uint32_t* d_pace_arg = nullptr;               // [n_streams] modes (bytes) or idle field counts
+    uint32_t* h_pace_arg = nullptr;               // pinned
+    EfFieldDesc* d_desc = nullptr;                // one per emitted field, grown on demand
+    uint64_t desc_cap = 0;
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -275,6 +300,17 @@ int resolve_fb(ef_ctx* c, int stream_index, int fb, int* out)
     CK(cudaMemcpy(&a, c->h.base_pics + stream_index, 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&b, c->h.n_pics + stream_index, 4, cudaMemcpyDeviceToHost));
     *out = (int)((a + b) & 1u);
+    return EF_OK;
+}
+
+// picture indices of the submit the last ef_index made current (synchronous the first time per submit)
+int pace_pictures(ef_ctx* c)
+{
+    if (c->pace_npics >= 0) return EF_OK;
+    uint32_t mp = 0;
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(&mp, c->h.info, 4, cudaMemcpyDeviceToHost));
+    c->pace_npics = (int)mp;
     return EF_OK;
 }
 
@@ -392,6 +428,8 @@ void ef_destroy(ef_ctx* c)
     if (!c) return;
     cudaDeviceSynchronize();
     for (void* p : c->allocs) cudaFree(p);
+    for (void* p : c->allocs_host) cudaFreeHost(p);
+    if (c->d_desc) cudaFree(c->d_desc);
     delete c->aud_scratch;
     if (c->h_ended) cudaFreeHost(c->h_ended);
     for (int b = 0; b < 2; b++) {
@@ -438,8 +476,11 @@ int ef_reset(ef_ctx* c)
         CK(cudaMemset(c->d_pts_last, 0xFF, (size_t)c->cfg.n_streams * 8));
         c->pts_resolved = false;
     }
+    if (c->paced)                                         // video_reset() (video.cpp:1070-1074): every display latches a new origin
+        CK(cudaMemset2D((uint8_t*)c->d_pace + offsetof(EfPaceState, fc_origin), sizeof(EfPaceState), 0, 4, (size_t)c->cfg.n_streams));
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
+    c->pace_indexed = false;
     return EF_OK;
 }
 
@@ -551,6 +592,11 @@ int ef_index(ef_ctx* c, void* stream)
     if (!c->submitted) return fail(EF_ESTATE, "ef_index before any submit");
     cudaStream_t st = (cudaStream_t)stream;
     const int n = c->cfg.n_streams;
+    if (c->paced && c->pace_indexed) {                    // the schedule needs every picture of the current submit
+        int rc = pace_pictures(c);
+        if (rc != EF_OK) return rc;
+        if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_index while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
+    }
     if (c->pending >= 0) {                       // a fresh submit: wait for its upload, make it the front buffer
         if (c->audio && c->aud_unconsumed)       // the audio of a TS submit is delivered exactly once
             return fail(EF_ESTATE, "ef_index of a new submit before ef_decode_audio consumed the current submit's audio");
@@ -580,6 +626,7 @@ int ef_index(ef_ctx* c, void* stream)
     }
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));
     c->indexed = true;
+    if (c->paced) { c->pace_indexed = true; c->pace_next = 0; c->pace_npics = -1; }
     return EF_OK;
 }
 
@@ -628,28 +675,49 @@ static int ensure_stage2(ef_ctx* c, int k, size_t bytes)
     return EF_OK;
 }
 
+static EfDev decode_dev(ef_ctx* c)                      // K1 takes the context by value (kernel parameter space)
+{
+    EfDev dev = c->h;
+    dev.es = c->d_es2[c->active]; dev.es_off = c->d_es_off2[c->active];
+    return dev;
+}
+
+// K1a over picture indices [p0, p0 + k): their macroblock records for decode_recon
+static int decode_parse(ef_ctx* c, int p0, int k, cudaStream_t st)
+{
+    const size_t slots = (size_t)k * c->cfg.n_streams * EF_MBW_MAX * EF_MBH_MAX;
+    CK(cudaMemsetAsync(c->h.mb_info, 0, slots * 4, st));
+    CK(cudaMemsetAsync(c->h.parse_cursor, 0, ((size_t)k + 1) * 4, st));
+    if (c->profiling) { CK(cudaEventRecord(c->ev_prof[2], st)); c->prof_decode = true; }
+    CK(ef_launch_parse(decode_dev(c), p0, k, c->sm_count, (size_t)k * c->cfg.n_streams * c->cfg.max_slices_per_picture, st));
+    if (c->profiling) CK(cudaEventRecord(c->ev_prof[3], st));
+    if (c->frames_read_pending) { CK(cudaStreamWaitEvent(st, c->ev_frames_read, 0)); c->frames_read_pending = false; }   // an asynchronous read-back still reads the frame stores
+    c->launches++;
+    return EF_OK;
+}
+
+// K1b of record picture i of the last decode_parse into the frame stores
+static int decode_recon(ef_ctx* c, int i, cudaStream_t st)
+{
+    CK(ef_launch_recon(decode_dev(c), i, c->sm_count, (size_t)c->cfg.n_streams * EF_MBW_MAX * EF_MBH_MAX, st));
+    c->launches++;
+    return EF_OK;
+}
+
 // K1a over picture indices [p0, p0 + k), then K1b once per picture index. host_dst != nullptr: every picture index
 // is exported (I420) straight after its K1b launch and copied to host_dst[p][stream] on the read-back stream while
 // the next picture index is being rebuilt - what push_video() sees, picture by picture (video.h:49).
 static int decode_range(ef_ctx* c, int p0, int k, cudaStream_t st, uint8_t* host_dst = nullptr, int layout = 0)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
-    const size_t slots = (size_t)k * c->cfg.n_streams * EF_MBW_MAX * EF_MBH_MAX;
-    CK(cudaMemsetAsync(c->h.mb_info, 0, slots * 4, st));
-    CK(cudaMemsetAsync(c->h.parse_cursor, 0, ((size_t)k + 1) * 4, st));
-    if (c->profiling) { CK(cudaEventRecord(c->ev_prof[2], st)); c->prof_decode = true; }
-    EfDev dev = c->h;                                       // K1 takes the context by value (kernel parameter space)
-    dev.es = c->d_es2[c->active]; dev.es_off = c->d_es_off2[c->active];
-    CK(ef_launch_parse(dev, p0, k, c->sm_count, (size_t)k * c->cfg.n_streams * c->cfg.max_slices_per_picture, st));
-    if (c->profiling) CK(cudaEventRecord(c->ev_prof[3], st));
+    int rc = decode_parse(c, p0, k, st);
+    if (rc != EF_OK) return rc;
     const size_t batch_bytes = (size_t)c->cfg.n_streams * EF_FRAME;
-    if (c->frames_read_pending) { CK(cudaStreamWaitEvent(st, c->ev_frames_read, 0)); c->frames_read_pending = false; }   // an asynchronous read-back still reads the frame stores
     for (int i = 0; i < k; i++) {
-        CK(ef_launch_recon(dev, i, c->sm_count, (size_t)c->cfg.n_streams * EF_MBW_MAX * EF_MBH_MAX, st));
+        if ((rc = decode_recon(c, i, st)) != EF_OK) return rc;
         if (host_dst) {
             const int b = c->stage_idx ^= 1;
-            int rc = ensure_stage2(c, b, batch_bytes);
-            if (rc != EF_OK) return rc;
+            if ((rc = ensure_stage2(c, b, batch_bytes)) != EF_OK) return rc;
             CK(cudaStreamWaitEvent(st, c->ev_down_done[b], 0));            // the previous copy out of this staging buffer has finished
             const uint64_t threads = (uint64_t)c->cfg.n_streams * (EF_FRAME / 8);
             ef_export_frames_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(c->h.frames, c->h.base_pics, c->h.n_pics, 0, c->cfg.n_streams, -2 - (p0 + i), layout, c->d_stage2[b]);
@@ -663,7 +731,6 @@ static int decode_range(ef_ctx* c, int p0, int k, cudaStream_t st, uint8_t* host
     }
     if (c->profiling) CK(cudaEventRecord(c->ev_prof[4], st));
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));     // the front ES buffer is in use until here
-    c->launches += 1 + (uint64_t)k;
     return EF_OK;
 }
 
@@ -671,6 +738,7 @@ int ef_decode_picture(ef_ctx* c, int pic, void* stream)
 {
     if (!c) return fail(EF_EINVAL, "null context");
     if (!c->indexed) return fail(EF_ESTATE, "ef_decode_picture before ef_index");
+    if (c->paced) return fail(EF_ESTATE, "ef_decode_picture on a presenting context: ef_present_picture decodes");
     if (pic < 0 || pic >= c->cfg.max_pictures) return fail(EF_EINVAL, "picture index %d out of range", pic);
     return decode_range(c, pic, 1, (cudaStream_t)stream);
 }
@@ -679,6 +747,7 @@ int ef_decode_all(ef_ctx* c, int n_pictures, void* stream)
 {
     if (!c) return fail(EF_EINVAL, "null context");
     if (!c->indexed) return fail(EF_ESTATE, "ef_decode_all before ef_index");
+    if (c->paced) return fail(EF_ESTATE, "ef_decode_all on a presenting context: ef_present_picture decodes");
     if (n_pictures < 0 || n_pictures > c->cfg.max_pictures) return fail(EF_EINVAL, "n_pictures %d out of range", n_pictures);
     for (int p = 0; p < n_pictures; p += c->h.rec_pics) {
         const int k = n_pictures - p < c->h.rec_pics ? n_pictures - p : c->h.rec_pics;
@@ -693,6 +762,7 @@ int ef_decode_all_to_host(ef_ctx* c, int n_pictures, uint8_t* dst, int layout, v
     if (!c || !dst) return fail(EF_EINVAL, "null argument");
     if (layout != 0 && layout != 1) return fail(EF_EINVAL, "layout must be 0 (I420) or 1 (strips)");
     if (!c->indexed) return fail(EF_ESTATE, "ef_decode_all_to_host before ef_index");
+    if (c->paced) return fail(EF_ESTATE, "ef_decode_all_to_host on a presenting context: ef_present_picture decodes");
     if (n_pictures < 0 || n_pictures > c->cfg.max_pictures) return fail(EF_EINVAL, "n_pictures %d out of range", n_pictures);
     for (int p = 0; p < n_pictures; p += c->h.rec_pics) {
         const int k = n_pictures - p < c->h.rec_pics ? n_pictures - p : c->h.rec_pics;
@@ -826,6 +896,7 @@ int ef_video_init(ef_ctx* c, int ntsc)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
+    if (c->paced && (ntsc ? 1 : 0) != c->pace_ntsc) return fail(EF_ESTATE, "the standard of a presenting context is fixed by ef_present_enable");
     EfGeometry g;
     memset(&g, 0, sizeof(g));
     g.ntsc = ntsc ? 1 : 0;
@@ -1293,6 +1364,114 @@ int ef_picture_pts(ef_ctx* c, int first, int count, int n_pictures, int64_t* pic
         CK(cudaMemcpy2D(pic_pts, (size_t)n_pictures * 8, c->d_pic_pts + (size_t)first * mp, mp * 8, (size_t)n_pictures * 8, (size_t)count, cudaMemcpyDeviceToHost));
     if (last_pts) CK(cudaMemcpy(last_pts, c->d_pts_last + first, (size_t)count * 8, cudaMemcpyDeviceToHost));
     return EF_OK;
+}
+
+// ---- paced presentation: push_video(frame, front, pts, mode) video.cpp:1023-1057 + video_isr video.cpp:1122-1198 per stream ----
+int ef_present_enable(ef_ctx* c, const uint32_t* frame_counter0)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (c->paced) return fail(EF_ESTATE, "ef_present_enable: already enabled");
+    if (!c->pts || !c->video) return fail(EF_ESTATE, "ef_present_enable needs ef_pts_enable and ef_video_init first");
+    const int n = c->cfg.n_streams;
+    int rc;
+#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
+    if (!c->d_pace) {
+        A(c->d_pace, (size_t)n); A(c->d_pace_next, (size_t)n); A(c->d_pace_run, (size_t)n); A(c->d_pace_out, (size_t)n);
+        A(c->d_pace_first, (size_t)n); A(c->d_pace_arg, (size_t)n);
+        CK(cudaHostAlloc((void**)&c->h_pace_out, (size_t)n * sizeof(EfPaceOut), cudaHostAllocDefault));
+        CK(cudaHostAlloc((void**)&c->h_pace_first, (size_t)n * 8, cudaHostAllocDefault));
+        CK(cudaHostAlloc((void**)&c->h_pace_arg, (size_t)n * 4, cudaHostAllocDefault));
+        c->allocs_host.push_back(c->h_pace_out); c->allocs_host.push_back(c->h_pace_first); c->allocs_host.push_back(c->h_pace_arg);
+    }
+#undef A
+    std::vector<EfPaceState> st((size_t)n);
+    for (int s = 0; s < n; s++) {                         // line 0 of field frame_counter0[s], no frame presented, no origin
+        memset(&st[s], 0, sizeof(EfPaceState));
+        st[s].fc = frame_counter0 ? frame_counter0[s] : 0u;
+        st[s].cur = -1;
+    }
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(c->d_pace, st.data(), st.size() * sizeof(EfPaceState), cudaMemcpyHostToDevice));
+    c->paced = true;
+    c->pace_ntsc = c->h.geo.ntsc;
+    c->pace_indexed = false;
+    return EF_OK;
+}
+
+// One presentation call: schedule (one thread per stream, into scratch), one read of the counts, then - unless this is a sizing
+// call or dst is too small - the decode of picture index `pic`, the descriptors and state commit, and the paced K2.
+static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
+                          cudaStream_t st)
+{
+    const int n = c->cfg.n_streams;
+    if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
+    if (pic >= 0) for (int s = 0; modes && s < n; s++) if (modes[s] > 3) return fail(EF_EINVAL, "mode %d of stream %d is not 0..3", modes[s], s);
+    if (pic >= 0 && modes) memcpy(c->h_pace_arg, modes, (size_t)n);
+    if (pic < 0) memcpy(c->h_pace_arg, idle_n, (size_t)n * 4);
+    const bool arg = pic < 0 || modes;
+    if (arg) CK(cudaMemcpyAsync(c->d_pace_arg, c->h_pace_arg, pic < 0 ? (size_t)n * 4 : (size_t)n, cudaMemcpyHostToDevice, st));
+    ef_pace_kernel<<<(n + 127) / 128, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_out, c->d_pic_pts, c->h.n_pics, c->h.base_pics,
+                                                   pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, (const uint32_t*)c->d_pace_arg, pic,
+                                                   c->cfg.max_pictures, n, c->pace_ntsc);
+    CK(cudaGetLastError());
+    c->launches++;
+    CK(cudaMemcpyAsync(c->h_pace_out, c->d_pace_out, (size_t)n * sizeof(EfPaceOut), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    uint64_t total = 0;
+    for (int s = 0; s < n; s++) {
+        c->h_pace_out[s].first = c->h_pace_first[s] = total;
+        total += c->h_pace_out[s].n_fields;
+    }
+    memcpy(info, c->h_pace_out, (size_t)n * sizeof(EfPaceOut));
+    if (!dst) return EF_OK;                                // sizing call: nothing decoded, no state changed
+    if (total > dst_fields) return fail(EF_ENOMEM, "%llu fields, capacity %llu", (unsigned long long)total, (unsigned long long)dst_fields);
+    int rc;
+    if (pic >= 0) {
+        if (pic % c->h.rec_pics == 0) {                    // K1a once per rec_pics picture indices, as ef_decode_all
+            c->pace_p0 = pic;
+            const int k = c->pace_npics - pic < c->h.rec_pics ? c->pace_npics - pic : c->h.rec_pics;
+            if ((rc = decode_parse(c, pic, k, st)) != EF_OK) return rc;
+        }
+        if ((rc = decode_recon(c, pic - c->pace_p0, st)) != EF_OK) return rc;
+        CK(cudaEventRecord(c->ev_buf_free[c->active], st));   // the front ES buffer is in use until here
+        c->pace_next = pic + 1;
+    }
+    if (total > c->desc_cap) {
+        CK(cudaStreamSynchronize(st));
+        if (c->d_desc) CK(cudaFree(c->d_desc));
+        c->d_desc = nullptr; c->desc_cap = 0;
+        CK(cudaMalloc(&c->d_desc, total * sizeof(EfFieldDesc)));
+        c->desc_cap = total;
+    }
+    CK(cudaMemcpyAsync(c->d_pace_first, c->h_pace_first, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    ef_pace_fill_kernel<<<n, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc);
+    CK(cudaGetLastError());
+    c->launches++;
+    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, total, dst, st, &c->launches));
+    CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
+    return EF_OK;
+}
+
+int ef_present_picture(ef_ctx* c, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !info) return fail(EF_EINVAL, "null argument");
+    if (!c->paced) return fail(EF_ESTATE, "ef_present_picture before ef_present_enable");
+    if (!c->pace_indexed) return fail(EF_ESTATE, "ef_present_picture before an ef_index that followed ef_present_enable");
+    int rc = pace_pictures(c);
+    if (rc != EF_OK) return rc;
+    if (pic != c->pace_next || pic >= c->pace_npics)
+        return fail(EF_ESTATE, "ef_present_picture(%d): the next picture index is %d of %d", pic, c->pace_next, c->pace_npics);
+    return present_common(c, pic, modes, nullptr, dst, dst_fields, info, (cudaStream_t)stream);
+}
+
+int ef_present_idle(ef_ctx* c, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !info || !n_fields) return fail(EF_EINVAL, "null argument");
+    if (!c->paced) return fail(EF_ESTATE, "ef_present_idle before ef_present_enable");
+    return present_common(c, -1, nullptr, n_fields, dst, dst_fields, info, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -209,6 +209,35 @@ struct __align__(16) EfAudioState {
     uint8_t carry[EF_AUDIO_CARRY];
 };
 
+// Paced presentation (ef_present_*, ef_composite.cu): one stream's display under the instant-decoder model. Between calls
+// nothing is pending (every push runs to its flip), so push_video's _next_frame / _next_frame_time and _animate need no
+// slot; _hscroll is a function of _animate_index after every animate() call.
+struct __align__(16) EfPaceState {
+    uint32_t fc, line;           // position: _frame_counter of the field being drawn, next line to draw
+    uint32_t pts_origin, fc_origin;   // _pts_origin, _video_frame_counter_origin (0 = latch at the next push)
+    int32_t cur;                 // current frame store, -1 before the first flip
+    int32_t ai;                  // _animate_index
+    uint32_t flags;              // bit 0: a picture was not pushed (pts -1, mode 0): outside the domain
+    uint32_t pad;
+};
+struct __align__(16) EfPaceRun {     // what one call emits for a stream: fields fc0, fc0 + 1, ... n of them
+    uint32_t fc0;
+    int32_t cur;                 // current frame store while they are drawn (-1: blank fields)
+    int32_t ai;                  // _animate_index on the first one's active lines
+    uint32_t n;
+};
+struct EfPaceOut {               // layout of ef_present_info (include/espflix_b200.h)
+    uint64_t first;
+    uint32_t n_fields, frame_counter, flip_field;
+    int32_t flip_line, flags;
+};
+struct __align__(16) EfFieldDesc {   // one paced K2 field; its output slot is its index
+    uint32_t stream;
+    int32_t fb;                  // frame store, -2 = no frame presented yet
+    uint32_t frame_counter;
+    int32_t hscroll;
+};
+
 static inline __host__ __device__ size_t ef_frame_offset(int stream, int fb) { return ((size_t)stream * 2 + (size_t)fb) * EF_FRAME; }
 static inline __host__ __device__ int ef_tile_offset(int mx, int my) { return (my * EF_MBW_MAX + mx) * EF_TILE; }
 // byte offset inside a tiled frame of luma pixel (x,y) / of chroma plane p (0 = block 4, 1 = block 5) pixel (x,y)

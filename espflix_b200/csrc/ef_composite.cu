@@ -169,9 +169,12 @@ __device__ __forceinline__ int blank_class(const EfPresent& pr, int line)
     return kNtsc ? 0 : ((line + 1) & 1) + 2;                              // PAL: the burst table alternates (burst_pal())
 }
 
-template <bool kNtsc>
+// kPaced (ef_present_*): y = the field's slot; stream, frame store, frame counter and hscroll come from desc[y], the field goes
+// to dst + y * LINES * W, and the overlay is off. Otherwise y = stream and the field goes to the stream's field buffer.
+template <bool kNtsc, bool kPaced>
 __global__ void __launch_bounds__(kK2Threads)
-ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr)
+ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr, const EfFieldDesc* __restrict__ desc,
+                    uint16_t* __restrict__ dst)
 {
     using G = Geo<kNtsc>;
     constexpr int CPL = G::W / 8;                                          // 16-byte chunks per line
@@ -182,21 +185,29 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
     __shared__ int s_src[16], s_distinct[16], s_n;
     const EfDev& D = *Dp;
     const uint32_t* tab = D.color_tab;                                     // 3 KB chroma LUT through L1
-    const int stream = (int)blockIdx.y;
     const int line0 = (int)blockIdx.x * 16;
+    int stream = (int)blockIdx.y;
+    EfPresent p = pr;
+    uint16_t* out0;
+    if constexpr (kPaced) {
+        const EfFieldDesc f = desc[blockIdx.y];
+        stream = (int)f.stream; fb_sel = f.fb; frame_counter = (int)f.frame_counter; p.hscroll = f.hscroll; p.blend = 0;
+        out0 = dst + (size_t)blockIdx.y * (G::LINES * G::W) + (size_t)line0 * G::W;
+    } else {
+        out0 = D.fields + (size_t)stream * D.field_stride + (size_t)line0 * G::W;
+    }
     const int nlines = min(16, G::LINES - line0);
     const int fl0 = line0 - G::TOP;                                        // frame line of the band's first line (bands = macroblock rows)
     const bool active = fl0 >= 0 && fl0 < EF_H && fb_sel != -2;            // -2: no frame presented yet (video.cpp:1140)
-    uint16_t* out0 = D.fields + (size_t)stream * D.field_stride + (size_t)line0 * G::W;
 
     if (!active) {
         // ---- blank band: every distinct line once ------------------------------------------------------------------
         if (threadIdx.x == 0) {
             int n = 0;
             for (int l = 0; l < nlines; l++) {
-                const int c = blank_class<kNtsc>(pr, line0 + l);
+                const int c = blank_class<kNtsc>(p, line0 + l);
                 int src = l;
-                for (int k = 0; k < l; k++) if (blank_class<kNtsc>(pr, line0 + k) == c) { src = k; break; }
+                for (int k = 0; k < l; k++) if (blank_class<kNtsc>(p, line0 + k) == c) { src = k; break; }
                 s_src[l] = src;
                 if (src == l) s_distinct[n++] = l;
             }
@@ -206,7 +217,7 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
         const int n = s_n;
         for (int i = (int)threadIdx.x; i < n * CPL; i += kK2Threads) {
             const int l = s_distinct[i / CPL], c = i % CPL;
-            *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, pr, line0 + l, c * 8);
+            *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> async proxy
         __syncthreads();
@@ -222,14 +233,14 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
     for (int i = (int)threadIdx.x; i < 2 * MARGIN_N; i += kK2Threads) {
         const int l = i / MARGIN_N, k = i % MARGIN_N;
         const int c = k >= BLIT_C ? k + BLIT_N : k;
-        *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, pr, line0 + l, c * 8);
+        *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
     }
     {
         const int lane = (int)threadIdx.x & 31, warp = (int)threadIdx.x >> 5;
         const int row = lane & 15, fl = fl0 + row;                         // frame line 0..191
         int fb0 = fb_sel >= 0 ? fb_sel : (int)((D.base_pics[stream] + D.n_pics[stream]) & 1u);
         // two-frame horizontal scroll (video.cpp:1146-1154): blit(f, dst, i, h, 352-h) then blit(f^1, dst + (352-h)*2, i, 0, h)
-        int h = pr.hscroll;
+        int h = p.hscroll;
         if (h < 0) { h += EF_W; fb0 ^= 1; }
         const int split = (EF_W - h) >> 3;                                 // first 8-pixel group drawn by the second blit
         const uint32_t dither = c_dither[(fl & 3) + ((frame_counter & 1) << 2)];
@@ -421,8 +432,8 @@ cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometr
 {
 #ifndef EF_K2_LEGACY
     const dim3 bands((unsigned)(g.line_count + 15) / 16, (unsigned)n_streams);
-    if (g.ntsc) ef_composite_kernel<true><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr);
-    else ef_composite_kernel<false><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr);
+    if (g.ntsc) ef_composite_kernel<true, false><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr, nullptr, nullptr);
+    else ef_composite_kernel<false, false><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr, nullptr, nullptr);
     return cudaGetLastError();
 #else
     const unsigned items = (unsigned)(g.line_width >> 4) + (((unsigned)g.blit_start >> 3) & 1u);   // 32-byte work items per line (see the kernel)
@@ -432,6 +443,110 @@ cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometr
     if (g.ntsc) ef_composite_kernel<true><<<grid, 256, 0, stream>>>(dev, fb, frame_counter, pr);
     else ef_composite_kernel<false><<<grid, 256, 0, stream>>>(dev, fb, frame_counter, pr);
     return cudaGetLastError();
+#endif
+}
+
+// ---- paced presentation (ef_present_*): push_video's PTS -> field schedule (video.cpp:1023-1057) against the flip of video_isr
+// (video.cpp:1122-1198), instant-decoder model, one thread per stream. A push runs push_video's arithmetic at the display's
+// position, then "draws" lines up to the flip: the first line below vsync_start that is not an active line of a presented
+// frame, once the frame counter has reached _next_frame_time. Closed form: the flip is in the current field or at line 0 of a
+// later one, so no loop walks lines or fields (a PTS jump of 2^33 ticks costs nothing here; the caller then lacks the room).
+// The fields a call emits are those whose line active_bottom - 1 it draws; animate() (video.cpp:1076-1088) runs at every field
+// end and at the flip. The state is written to `next` and committed by ef_pace_fill_kernel once the output fits.
+namespace {
+__constant__ int16_t c_easd[16] = { 0, 8, 16, 24, 48, 72, 104, 136, 176, 216, 248, 280, 304, 328, 336, 344 };   // _easd, video.cpp:1077
+
+__device__ __forceinline__ int pace_animate(int ai, uint64_t n)            // _animate_index after n animate() calls
+{
+    const uint64_t a = (uint64_t)abs(ai);
+    return a <= n ? 0 : ai > 0 ? ai - (int)n : ai + (int)n;
+}
+__device__ __forceinline__ int pace_hscroll(int ai) { return ai < 0 ? -c_easd[-ai] : c_easd[ai]; }   // _hscroll once animate() left ai
+}  // namespace
+
+// pic >= 0: every stream with a picture `pic` pushes it (pts from pic_pts, modes[s] or 0); pic < 0: every stream idles until
+// it has emitted idle_n[s] fields
+__global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* __restrict__ next, EfPaceRun* __restrict__ run, EfPaceOut* __restrict__ out,
+                               const int64_t* __restrict__ pic_pts, const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ base_pics,
+                               const uint8_t* __restrict__ modes, const uint32_t* __restrict__ idle_n, int pic, int max_pictures, int n_streams, int ntsc)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_streams) return;
+    const uint32_t top = ntsc ? 32 : 64, bottom = top + EF_H, vsync = ntsc ? 259 : 304;   // video.cpp:1135-1137
+    EfPaceState q = st[s];
+    const uint32_t F = q.fc;
+    const uint32_t first = q.line <= bottom - 1 ? 0u : 1u;                 // does this call draw line active_bottom - 1 of field F?
+    EfPaceRun r = { F + first, q.cur, pace_animate(q.ai, first), 0 };
+    EfPaceOut o = { 0, 0, F + first, 0, -1, 0 };
+    uint64_t n = 0;
+    if (pic < 0) {
+        n = idle_n[s];
+        if (n) {
+            const uint64_t end = first + n - 1;                            // stop right after line active_bottom - 1 of the last field
+            q.ai = pace_animate(q.ai, end);
+            q.fc = F + (uint32_t)end; q.line = bottom;
+        }
+    } else if ((uint32_t)pic < n_pics[s]) {
+        const int64_t pts = pic_pts[(size_t)s * max_pictures + pic];
+        const int mode = modes ? modes[s] : 0;
+        if (pts == -1 && mode == 0) q.flags |= 1u;                         // flush_picture() pushes nothing (player.cpp:692-702)
+        else {
+            const uint32_t vp = (uint32_t)(pts / (ntsc ? 1500 : 1800));
+            if (q.fc_origin == 0) { q.pts_origin = vp; q.fc_origin = F; }
+            uint32_t d = vp - q.pts_origin + q.fc_origin;
+            if (mode) d = F;                                               // due now (video.cpp:1039-1042)
+            if (d < F && (int)(F - d) > 2) q.fc_origin = 0;                // late by more than two fields: re-latch at the next push
+            uint32_t ff = 0, fl = 0;                                       // fields from F to the flip, flip line
+            if (d <= F) {
+                uint32_t l = q.line;
+                if (q.cur >= 0 && l >= top && l < bottom) l = bottom;      // not on an active line of a presented frame
+                if (l < vsync) fl = l; else ff = 1;
+            } else ff = d - F;
+            const int64_t last = (int64_t)ff - (fl >= bottom - 1 ? 0 : 1);
+            n = last >= (int64_t)first ? (uint64_t)(last - (int64_t)first + 1) : 0;
+            int ai = pace_animate(q.ai, ff);
+            if (mode == 2) ai = -16; else if (mode == 3) ai = 16;          // load_poster: the scroll starts at the flip (video.cpp:1168-1171)
+            q.ai = pace_animate(ai, 1);
+            q.fc = F + ff; q.line = fl + 1;
+            q.cur = (int)((base_pics[s] + (uint32_t)pic + 1u) & 1u);       // the store flush_picture() gave picture `pic` (player.cpp:692)
+            o.flip_field = q.fc; o.flip_line = (int)fl;
+        }
+    }
+    r.n = o.n_fields = n > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)n;
+    o.flags = (int)q.flags;
+    next[s] = q; run[s] = r; out[s] = o;
+}
+
+// once the fields fit: one descriptor per emitted field, at the stream's offset `first` in the output; commits the state
+__global__ void ef_pace_fill_kernel(EfPaceState* __restrict__ st, const EfPaceState* __restrict__ next, const EfPaceRun* __restrict__ run,
+                                    const uint64_t* __restrict__ first, EfFieldDesc* __restrict__ desc)
+{
+    const int s = blockIdx.x;
+    const EfPaceRun r = run[s];
+    const uint64_t base = first[s];
+    for (uint32_t j = threadIdx.x; j < r.n; j += blockDim.x)
+        desc[base + j] = { (uint32_t)s, r.cur < 0 ? -2 : r.cur, r.fc0 + j, pace_hscroll(pace_animate(r.ai, j)) };
+    if (threadIdx.x == 0) st[s] = next[s];
+}
+
+// the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y)
+cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
+                                      uint64_t* launches)
+{
+#ifndef EF_K2_LEGACY
+    const size_t per = (size_t)g.line_count * g.line_width;
+    for (uint64_t f0 = 0; f0 < n_fields; f0 += 65535) {
+        const dim3 grid((unsigned)(g.line_count + 15) / 16, (unsigned)(n_fields - f0 < 65535 ? n_fields - f0 : 65535));
+        if (g.ntsc) ef_composite_kernel<true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
+        else ef_composite_kernel<false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+#else
+    (void)dev; (void)g; (void)desc; (void)n_fields; (void)dst; (void)stream; (void)launches;
+    return cudaErrorNotSupported;                                          // the band kernel is the only one with a paced form
 #endif
 }
 

@@ -45,6 +45,8 @@
  *   ef_pts_enable / ef_picture_pts     the pts push_video(frame, front, _last_pts, mode) hands over with every picture
  *                                 (flush_picture() player.cpp:692-702, latched from demux() player.cpp:399-419) and
  *                                 get_pts() player.cpp:653-656, for every stream of a TS submit
+ *   ef_present_enable / _picture / _idle  push_video(frame, front, pts, mode) video.cpp:1023-1057 against the frame flip
+ *                                 of video_isr video.cpp:1122-1198: every stream's paced composite fields, in HBM
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -258,6 +260,43 @@ int ef_decode_audio(ef_ctx* ctx, const uint8_t* end_of_stream, ef_audio_info* in
  *                 ef_index that followed it; EF_EINVAL for a bad stream range or n_pictures outside 0..max_pictures. */
 int ef_pts_enable(ef_ctx* ctx);
 int ef_picture_pts(ef_ctx* ctx, int first, int count, int n_pictures, int64_t* pic_pts, int64_t* last_pts);
+
+/* Paced presentation: the composite fields each stream's TV shows. Every stream has its own display under the instant-decoder
+ * model (time passes only while push_video waits): position (frame counter F, last line drawn), _pts_origin and
+ * _video_frame_counter_origin, the current frame store and the poster scroll (_animate_index / _hscroll). Pushing picture k
+ * runs push_video's arithmetic at the current F (video.cpp:1023-1057: pts / 1500 NTSC or / 1800 PAL, the origin latch, mode != 0
+ * due now, more than two fields late re-latches), then draws lines until the flip (video_isr, video.cpp:1122-1198): the first
+ * line below vsync_start that is not an active line of a presented frame, once F >= _next_frame_time. animate() runs at the
+ * flip and at every field end (video.cpp:1076-1088). A push emits the fields whose line active_bottom - 1 it draws, each as
+ * K2 draws it from the current store (picture k - 1), the other store (picture k), the hscroll of its active lines and its
+ * F. The overlay is not drawn (blend 0). Fields are line_count x line_width uint16 samples.
+ * ef_present_enable   needs ef_pts_enable and ef_video_init first (else EF_ESTATE) and fixes the standard: a later
+ *                     ef_video_init that changes it returns EF_ESTATE. Each display starts at line 0 of field
+ *                     frame_counter0[s] (NULL: 0) with no frame presented. Presentation starts with the next ef_index. From
+ *                     then on ef_decode_picture / ef_decode_all / ef_decode_all_to_host return EF_ESTATE (frames decoded
+ *                     outside the schedule would desynchronise it), and ef_index returns EF_ESTATE while picture indices
+ *                     of the current submit are unpresented. ef_reset does video_reset() (video.cpp:1070-1074) on every
+ *                     display: the next push latches a new origin; position, current store and scroll stay.
+ * ef_present_picture  pic = 0, 1, ... of the current submit, in order (else EF_ESTATE). Decodes picture index `pic` of every
+ *                     stream (K1a once per rec_pics indices and K1b, as ef_decode_all) and pushes it, with its pts
+ *                     (ef_picture_pts) and modes[s] (NULL: 0; 1 = flush_picture(1) at the end of a stream, 2 / 3 =
+ *                     load_poster's scroll; > 3: EF_EINVAL), on every stream that has it. A picture with pts -1 and mode 0
+ *                     is not pushed (player.cpp:692-702): flags |= 1 (outside the domain), later fields unspecified.
+ * ef_present_idle     every display runs on with nothing pending until it has emitted n_fields[s] more fields (the tail
+ *                     after a stream's last flip; fields before any flip are blank).
+ * Both write every stream's emitted fields, packed in stream order, to dst (device, 16-byte aligned): stream s's
+ * info[s].n_fields fields start at dst + info[s].first x line_count x line_width and carry frame counters
+ * info[s].frame_counter, + 1, ... flip_field / flip_line: where the pushed picture flipped (-1: no picture pushed). flags:
+ * bit 0 = outside the domain. dst == NULL is a sizing call: info only, nothing changes. dst_fields below the total:
+ * EF_ENOMEM, nothing decoded and nothing changed. Synchronous on `stream`. */
+typedef struct {
+    uint64_t first;
+    uint32_t n_fields, frame_counter, flip_field;
+    int32_t flip_line, flags;
+} ef_present_info;
+int ef_present_enable(ef_ctx* ctx, const uint32_t* frame_counter0);
+int ef_present_picture(ef_ctx* ctx, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
+int ef_present_idle(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
