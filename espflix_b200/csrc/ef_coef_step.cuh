@@ -2,10 +2,10 @@
 // and by the host-side model test (tests/k1a_step_model.cpp), so the exact code the GPU runs is checked on the CPU
 // against a symbol-by-symbol restatement of get_vlc_dct()/block() (player.cpp:549-644, 1068-1121).
 //
-// A step looks at the next 32 bits of the slice (`w`, MSB first) and takes, in ONE table look-up, everything that
-// lies wholly inside the next EF_K1A_LUT_BITS bits: one or two (run, level) codes with their sign bits and a
-// closing end of block. Long codes, the escape, invalid prefixes and symbols that would pass scan position 63
-// decode a single symbol through the clz-indexed table (EfTables::dct) and fold a following '10' in.
+// ef_coef_sym decodes ONE symbol from the next 32 bits of the slice (`w`, MSB first) through the clz-indexed table
+// (EfTables::dct): a (run, level) code with its sign bit or escape payload, an end of block, or not a code. The kernel
+// folds a '10' that follows a coefficient into the same step. ef_coef_entry dequantises a coefficient and packs it into
+// its list entry.
 #pragma once
 #include "ef_common.cuh"
 
@@ -17,59 +17,6 @@
 #define EF_CLZ(x) ((x) ? __builtin_clz((unsigned)(x)) : 32)
 #endif
 #define EF_BYTE1(x) ((int)(((x) >> 8) & 255u))                    // bits 8-15, zero-extended
-#define EF_SBYTE2(x) ((int)(int8_t)(((x) >> 16) & 255u))          // bits 16-23, sign-extended
-
-// flags of a step
-#define EF_STEP_COEF1 1u      // (run1, lvl1) is a coefficient
-#define EF_STEP_COEF2 2u      // (run2, lvl2) is a second coefficient
-#define EF_STEP_EOB 4u        // the block ends after them ('10')
-#define EF_STEP_ABORT 8u      // scan position >= 64: block() returns -1, nothing of the block is stored; bits consumed
-#define EF_STEP_DERAIL 16u    // not a code: the reference derails here; nothing consumed
-
-struct EfCoefStep {
-    uint32_t fl;
-    int len;                  // bits consumed
-    int run1, lvl1, run2, lvl2;
-};
-
-// w = next 32 bits; first = dct_coeff_first context (no end of block, '1s' = (0, 1)); n = scan position reached in
-// the block (next coefficient lands at n + run). lut = EfTables::lut2, dct = EfTables::dct.
-static __host__ __device__ __forceinline__ EfCoefStep ef_coef_step(uint32_t w, bool first, int n, const uint2* __restrict__ lut, const uint16_t* __restrict__ dct)
-{
-    EfCoefStep r;
-#if EF_K1A_LUT_BITS > 0
-    const uint2 e = lut[(first ? (1 << EF_K1A_LUT_BITS) : 0) + (int)(w >> (32 - EF_K1A_LUT_BITS))];
-#else
-    const uint2 e = make_uint2(127u << 24, 0u);            // tuning variant: every symbol through the clz-indexed table
-    (void)lut;
-#endif
-    r.fl = e.y & 255u;
-    r.len = (int)(e.x & 255u);
-    r.run1 = EF_BYTE1(e.x); r.lvl1 = EF_SBYTE2(e.x);
-    r.run2 = EF_BYTE1(e.y); r.lvl2 = EF_SBYTE2(e.y);
-    if (n + (int)(e.x >> 24) > 63) {                       // not in the table (span 127), or the pair would pass position 63
-        const int lz = EF_CLZ(w);
-        uint32_t t = 0;                                    // >= 12 leading zeros: not a code
-        if (lz < 12) t = dct[(first ? 13 * 32 - 32 : -32) + lz * 32 + (int)((w << lz) >> 26)];
-        r.len = (int)(t & 31u); r.run1 = (int)((t >> 5) & 31u);
-        const int mag = (int)(t >> 10);
-        r.fl = EF_STEP_COEF1;
-        if (mag) r.lvl1 = ((w >> ((32 - r.len) & 31)) & 1u) ? -mag : mag;    // sign = last bit of a regular code
-        else if (r.len == 2) r.fl = EF_STEP_EOB;           // '10': end of block (player.cpp:1075)
-        else if (r.len == 6) {                             // escape: 6-bit run, 8- or 16-bit level (player.cpp:1092)
-            r.run1 = (int)((w >> 20) & 63u);
-            const int b = (int)((w >> 12) & 255u);
-            if (b == 0) { r.lvl1 = (int)((w >> 4) & 255u); r.len = 28; }
-            else if (b == 128) { r.lvl1 = (int)((w >> 4) & 255u) - 256; r.len = 28; }
-            else { r.lvl1 = (int)(int8_t)b; r.len = 20; }
-        } else r.fl = EF_STEP_DERAIL;
-        if (r.fl == EF_STEP_COEF1) {
-            if (n + r.run1 > 63) r.fl = EF_STEP_ABORT;
-            else if (r.len <= 30 && ((w << r.len) >> 30) == 2u) { r.fl = EF_STEP_COEF1 | EF_STEP_EOB; r.len += 2; }
-        }
-    }
-    return r;
-}
 
 // One coefficient of block(), player.cpp:1106-1121, from its signed level to its list entry. Dequantisation in
 // magnitude form: v = 2*level (+-1 when not intra, k = 1); v = (v * qscale * q) / 16 with C truncation, i.e. on the
@@ -89,13 +36,6 @@ static __host__ __device__ __forceinline__ uint32_t ef_coef_entry(uint32_t z, in
     return (uint32_t)(v * EF_BYTE1(z) + (int)((z & 0x00FC0000u) | blk24));
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// K1a v3 (EF_K1A_V3): one symbol per step through the clz-indexed table, a following '10' folded in, and NO
-// arithmetic on the level: the parser stores a raw token and K1b dequantises while it expands the list (the same
-// instructions run there for 32 entries at once instead of for the ~14 lanes of a parser warp that are in a
-// coefficient at the same time).
-//   token = block << 27 | scan position << 21 | quantiser_scale << 16 | (int16) level
-// ---------------------------------------------------------------------------------------------------------------
 #define EF_SYM_COEF 0u
 #define EF_SYM_EOB 1u         // '10' on its own (an intra block without AC coefficients)
 #define EF_SYM_DERAIL 2u      // not a code: nothing consumed
@@ -128,22 +68,4 @@ static __host__ __device__ __forceinline__ EfSym ef_coef_sym(uint32_t w, bool fi
         } else r.kind = EF_SYM_DERAIL;
     }
     return r;
-}
-
-static __host__ __device__ __forceinline__ uint32_t ef_token(uint32_t blk, int n, int qscale, int level)
-{
-    return (blk << 27) | ((uint32_t)n << 21) | ((uint32_t)qscale << 16) | ((uint32_t)level & 0xFFFFu);
-}
-
-// block(), player.cpp:1106-1121, for one token: the dequantised, AAN-prescaled coefficient b[zz]. Same arithmetic as
-// ef_coef_entry above; z = table word of the scan position (quantiser | prescale << 8 | zz << 18), k = 1 when not intra.
-static __host__ __device__ __forceinline__ int ef_dequant(uint32_t z, int level, int qscale, int k)
-{
-    const int mag = level < 0 ? -level : level;
-    int neg = level < 0;
-    int m = ((2 * mag + k) * (qscale * (int)(z & 255u))) >> 4;
-    if (m == 0) neg = 0;
-    m = ((m > 1 ? m : 1) - 1) | 1;
-    m = m < 2047 + neg ? m : 2047 + neg;
-    return (neg ? -m : m) * EF_BYTE1(z);
 }

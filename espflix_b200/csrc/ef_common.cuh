@@ -39,40 +39,11 @@
 #ifndef EF_K1A_CTAS
 #define EF_K1A_CTAS 4
 #endif
-#ifndef EF_K1A_PF_L2
-#define EF_K1A_PF_L2 1           // K1a: prefetch.global.L2 128 bytes ahead of a slice's read position (besides the cp.async ring)
-#endif
 #ifndef EF_K1A_HDR_BATCH
 #define EF_K1A_HDR_BATCH 24      // K1a: waiting lanes that end a symbol loop early (32: the loop runs until no lane is busy); 24 measured fastest of 8-32
 #endif
-#ifndef EF_K1A_V3
-#define EF_K1A_V3 1              // K1a: one symbol per step through the clz-indexed table, a following end of block folded in (0: the two-symbol table step)
-#endif
-#ifndef EF_K1B_DEQUANT
-#define EF_K1B_DEQUANT 0         // 1: K1a v3 stores raw tokens and K1b dequantises while it expands the list (measured: K1a -4 %, K1b +12 %: lost)
-#endif
-#ifndef EF_K1A_ES16
-#define EF_K1A_ES16 1            // K1a: the bitstream comes in through 16-byte cp.async.cg chunks (4 per lane in flight) instead of 4-byte words: a quarter of the
-#endif                           //      scattered-address global-memory instructions, and no reliance on L1 hits
 #ifndef EF_K1A_UNROLL
-#define EF_K1A_UNROLL 3          // K1a v3: symbol steps per pass of the loop (one vote + branch per pass)
-#endif
-#ifndef EF_PROBE_NOSTORE
-#define EF_PROBE_NOSTORE 0       // measurement probe only: K1a drops its coefficient stores (output wrong)
-#endif
-#ifndef EF_K1A_RING_AHEAD
-#define EF_K1A_RING_AHEAD 1      // K1a: the word after `lo` is already in a register when a refill needs it (its ring load was issued one refill earlier)
-#endif
-#ifndef EF_K1A_LUT_BITS
-#if EF_K1A_V3
-#define EF_K1A_LUT_BITS 0
-#else
-#define EF_K1A_LUT_BITS 10
-#endif
-#endif
-// EF_K1A_LUT_BITS (EF_K1A_V3 = 0 only): the two-symbol coefficient table is indexed by the next 2^K bits of the stream
-#ifndef EF_K1B_PIN16
-#define EF_K1B_PIN16 1           // K1b: clamp two pixels per DPX instruction (VIADDMNMX.S16x2) instead of one
+#define EF_K1A_UNROLL 3          // K1a: symbol steps per pass of the loop (one vote + branch per pass)
 #endif
 #ifndef EF_K1B_WARPS
 #define EF_K1B_WARPS 7       // K1b (reconstruct): warps per CTA, CTAs per SM
@@ -94,13 +65,6 @@
 //   ptype:bits 0-2 length, 3-7 macroblock_type flags, indexed by next 6 bits     [64]     u8
 //   qz:   per scan position n: quantiser byte | AAN prescale << 8 | raster index zig_zag[n] << 18; [0..63] intra,
 //         [64..127] non-intra (the layout of a coefficient-list entry above bit 18)     [128]    u32
-//   lut2: the fast path of the coefficient parser, indexed by the next EF_K1A_LUT_BITS bits: up to two
-//         (run, level) symbols and a trailing end-of-block that lie wholly inside those bits.
-//         .x = bits consumed | run1 << 8 | (int8) level1 << 16 | span << 24, span = scan positions advanced before
-//              the last coefficient (run1, or run1 + 1 + run2); 127 = not decodable from these bits (long code,
-//              escape, invalid): the parser then decodes one symbol through `dct`
-//         .y = flags (1 first coefficient, 2 second coefficient, 4 end of block) | run2 << 8 | (int8) level2 << 16
-//         [0] = dct_coeff_next context, [1] = first coefficient of a non-intra block   [2][2^K]  u32 x 2
 struct EfTables {
     uint16_t dct[26 * 32];
     uint16_t mba[8 * 32];
@@ -113,7 +77,6 @@ struct EfTables {
     uint8_t izz[64];        // raster index -> zig-zag scan position
     uint8_t prescale[64];   // AAN prescale, raster (reference scale_dct_q, player.cpp:161)
     uint8_t zigzag[64];     // scan position -> raster index
-    uint2 lut2[(2 << EF_K1A_LUT_BITS) > 16 ? (2 << EF_K1A_LUT_BITS) : 16];
 };
 
 // sequence state as the decode kernel reads it: quantiser matrices in SCAN order (the parser

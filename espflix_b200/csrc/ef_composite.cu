@@ -23,26 +23,7 @@ __device__ __forceinline__ uint32_t chroma_word(const uint32_t* tab, uint32_t u,
 // both standards): the four subcarrier phases of a table entry are 48, 48 +- r(c) with
 //   r(c) = sgn(128 - c) * ((16 |128 - c| + 11) / 22)          [= round_half_away((128 - c) * 24 / 33), espflix.cpp:1091-1180]
 // clamped to [0, 127]: U rides on the sine phases (bytes 1, 0), V on the cosine phases (bytes 3, 2; swapped on the PAL
-// lines that use cos_v_neg). EF_K2_ARITH computes CHROMA_EVEN / CHROMA_ODD from that instead of two dependent gathers.
-#ifndef EF_K2_ARITH
-#define EF_K2_ARITH 0
-#endif
-__device__ __forceinline__ int chroma_r(uint32_t c)
-{
-    const int d = 128 - (int)(c & 255u);
-    const int q = ((16 * abs(d) + 11) * 745) >> 14;                       // / 22, exact for numerators <= 2059 (tests/test_tables.py)
-    return d < 0 ? -q : q;
-}
-__device__ __forceinline__ uint32_t chroma_word_arith(uint32_t u, uint32_t v, bool v_neg)
-{
-    const int ru = chroma_r(u);
-    int rv = chroma_r(v);
-    if (v_neg) rv = -rv;
-    const uint32_t b3 = (uint32_t)__viaddmin_s32_relu(48, rv, 127), b2 = (uint32_t)__viaddmin_s32_relu(48, -rv, 127);
-    const uint32_t b1 = (uint32_t)__viaddmin_s32_relu(48, ru, 127), b0 = (uint32_t)__viaddmin_s32_relu(48, -ru, 127);
-    const uint32_t w = (b3 << 24) + (b2 << 16) + (b1 << 8) + b0 + 0x30303030u;       // + the constant phase of the other table
-    return (w & 0xFCFCFCFCu) >> 2;
-}
+// lines that use cos_v_neg).
 
 // compile-time geometry of the two standards (video_init / pal_init, video.cpp:572-630; values
 // probe-verified against the reference in tests/golden/composite_pins.json)
@@ -130,7 +111,6 @@ __device__ __forceinline__ uint4 blit_quad(uint32_t y4, uint32_t dither, uint32_
                       ((p1 << 16) | (p0 >> 8)) + cb, (((p1 << 8) & 0xFF000000u) | (p0 >> 16)) + (cb << 8));
 }
 
-#ifndef EF_K2_LEGACY
 // ---- K2 v6: a CTA synthesises a BAND of 16 consecutive lines of one stream in shared memory and hands the finished
 // rows to the TMA engine (cp.async.bulk.global.shared::cta): the field leaves the SM as bulk stores instead of 16-byte
 // STG, which took the output off the L1/TEX pipe - the v4 kernel was bound there (86 % busy at 42 % DRAM throughput,
@@ -279,14 +259,8 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
                 v = ((v >> 1) & 0x7F7F7F7Fu) + ((vn[t] >> 1) & 0x7F7F7F7Fu);
             }
             uint32_t lum = cstart[t] ? 0u : ((((lumw[t] + dither) & 0xFCFCFCFCu) >> 2) >> 24);   // carry = last pixel of the previous group
-#if EF_K2_ARITH
-            const bool vneg = !kNtsc && vt == 512;                         // PAL odd lines: cos_v_neg (video.cpp:584-591)
-            const uint4 o0 = blit_quad(y8[t].x, dither, chroma_word_arith(u, v, vneg), chroma_word_arith(u >> 8, v >> 8, vneg), lum);
-            const uint4 o1 = blit_quad(y8[t].y, dither, chroma_word_arith(u >> 16, v >> 16, vneg), chroma_word_arith(u >> 24, v >> 24, vneg), lum);
-#else
             const uint4 o0 = blit_quad(y8[t].x, dither, chroma_word(tab, u, v, vt), chroma_word(tab, u >> 8, v >> 8, vt), lum);
             const uint4 o1 = blit_quad(y8[t].y, dither, chroma_word(tab, u >> 16, v >> 16, vt), chroma_word(tab, u >> 24, v >> 24, vt), lum);
-#endif
             uint8_t* o = sm + row * LS + (G::BLIT + gd * 16) * 2;
             *(uint4*)o = o0;
             *(uint4*)(o + 16) = o1;
@@ -305,87 +279,6 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
     }
 }
-#else
-// grid: x = threads of one field / 256, y = stream. One thread = two adjacent 16-byte chunks (32 bytes out,
-// 8 luma pixels in: one 8-byte luma load, one 4-byte load per chroma plane). The pairing is phased so that
-// the blit span starts on a pair boundary (NTSC chunk 20: pairs (2j, 2j+1); PAL chunk 35: pairs (2j-1, 2j)).
-// A warp covers 16 consecutive pairs of TWO consecutive lines (lanes 0-15 the even line, lanes 16-31 the
-// odd one): in the tiled frame the two luma rows of a tile share 32-byte sectors and both lines read the same
-// chroma row, so every sector the warp fetches is used whole. Stores are 512 contiguous bytes per half-warp.
-template <bool kNtsc>
-__global__ void __launch_bounds__(256)
-ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr)
-{
-    using G = Geo<kNtsc>;
-    constexpr int CPL = G::W / 8;                                          // 16-byte chunks per line (even)
-    constexpr int PHASE = (G::BLIT / 8) & 1;                               // 0: pairs (2j, 2j+1); 1: pairs (2j-1, 2j), single chunks at both ends
-    constexpr int ITEMS = CPL / 2 + PHASE;                                 // work items per line
-    constexpr int GROUPS = (ITEMS + 15) / 16;                              // warps per line pair
-    const EfDev& D = *Dp;
-#ifndef EF_K2_LUT_SMEM
-    const uint32_t* tab = D.color_tab;                                     // 3 KB chroma LUT through L1 (measured faster than a shared-memory copy per CTA)
-#else
-    __shared__ uint32_t tab[768];
-    for (int i = threadIdx.x; i < 768; i += 256) tab[i] = D.color_tab[i];
-    __syncthreads();
-#endif
-    const uint32_t t = blockIdx.x * 256u + threadIdx.x;
-    const uint32_t stream = blockIdx.y;
-    const int pair = (int)(t / (GROUPS * 32)), r = (int)(t - (uint32_t)pair * (GROUPS * 32));
-    const int lane = r & 31;
-    const int line = 2 * pair + (lane >> 4), j = (r >> 5) * 16 + (lane & 15);
-    if (pair >= G::LINES / 2 || j >= ITEMS) return;
-    const int c0 = 2 * j - PHASE;                                          // first chunk of the item; c0 == -1 / c0 + 1 == CPL: single chunk
-    uint16_t* out = D.fields + (size_t)stream * D.field_stride + (size_t)line * G::W;
-
-    const int fl = line - G::TOP;                                          // frame line 0..191 on active lines
-    const bool active = fl >= 0 && fl < EF_H && fb_sel != -2;              // -2: no frame presented yet (video.cpp:1140)
-    const int x0 = c0 * 8;
-    if (active && x0 >= G::BLIT && x0 < G::BLIT + 2 * EF_W) {
-        int fb = fb_sel >= 0 ? fb_sel : (int)((D.base_pics[stream] + D.n_pics[stream]) & 1u);
-        // two-frame horizontal scroll (video.cpp:1146-1154): blit(f, dst, i, h, 352-h) then blit(f^1, dst + (352-h)*2, i, 0, h)
-        int h = pr.hscroll;
-        if (h < 0) { h += EF_W; fb ^= 1; }
-        const int gd = (x0 - G::BLIT) >> 4;                                // 8-pixel group of the destination, 0..43
-        const int split = (EF_W - h) >> 3;                                 // first group drawn by the second blit
-        const bool second = gd >= split;
-        if (second) fb ^= 1;
-        const int g = second ? gd - split : gd + (h >> 3);                 // 8-pixel group of the source frame
-        const bool call_start = second ? g == 0 : gd == 0;                 // blit() starts its luma carry at 0
-        const uint8_t* f = D.frames + ef_frame_offset((int)stream, fb);
-        const uint32_t dither = c_dither[(fl & 3) + ((frame_counter & 1) << 2)];
-        // tiled frame (ef_common.cuh): the 8 luma pixels of group g are half a tile row, the 4 chroma samples half a chroma tile row
-        const int cy = fl >> 1;
-        const int tcol = (g >> 1) * EF_TILE;
-        const uint8_t* yrow = f + (fl >> 4) * EF_MBW_MAX * EF_TILE + (fl & 15) * 16;
-        const uint8_t* crow = f + (cy >> 3) * EF_MBW_MAX * EF_TILE + (cy & 7) * 8 + 256 + (g & 1) * 4;   // get_cr(line>>1); get_cb is the next 64-byte plane
-        uint32_t u4 = *(const uint32_t*)(crow + tcol);
-        uint32_t v4 = *(const uint32_t*)(crow + tcol + 64);
-        int vt = 256;
-        if (fl & 1) {                                                      // odd lines average with the next chroma row (video.cpp:704-716)
-            const int n = cy + (fl == 191 ? 0 : 1);
-            const uint8_t* nrow = f + (n >> 3) * EF_MBW_MAX * EF_TILE + (n & 7) * 8 + 256 + (g & 1) * 4;
-            u4 = ((u4 >> 1) & 0x7F7F7F7Fu) + ((*(const uint32_t*)(nrow + tcol) >> 1) & 0x7F7F7F7Fu);
-            v4 = ((v4 >> 1) & 0x7F7F7F7Fu) + ((*(const uint32_t*)(nrow + tcol + 64) >> 1) & 0x7F7F7F7Fu);
-            vt = 512;
-        }
-        const uint2 y8 = *(const uint2*)(yrow + tcol + (g & 1) * 8);
-        uint32_t lum = 0;                                                  // carry = last pixel of the previous group, 0 at the start of a blit() call
-        if (!call_start) {
-            const int q = 2 * g - 1;                                       // previous 4-pixel group
-            lum = ((((*(const uint32_t*)(yrow + (q >> 2) * EF_TILE + (q & 3) * 4) + dither) & 0xFCFCFCFCu) >> 2) >> 24);
-        }
-        const uint4 o0 = blit_quad(y8.x, dither, chroma_word(tab, u4, v4, vt), chroma_word(tab, u4 >> 8, v4 >> 8, vt), lum);
-        const uint4 o1 = blit_quad(y8.y, dither, chroma_word(tab, u4 >> 16, v4 >> 16, vt), chroma_word(tab, u4 >> 24, v4 >> 24, vt), lum);
-        __stcs((uint4*)(out + x0), o0);                                    // streaming stores: the field is not re-read by this kernel
-        __stcs((uint4*)(out + x0 + 8), o1);
-    } else {
-        if (c0 >= 0) __stcs((uint4*)(out + x0), blank_chunk<kNtsc>(D, pr, line, x0));
-        if (c0 + 1 < CPL) __stcs((uint4*)(out + x0 + 8), blank_chunk<kNtsc>(D, pr, line, x0 + 8));
-    }
-}
-
-#endif
 
 // single blit() call into a device buffer (line-blit entry point; used by ef_blit): one thread per 4 luma pixels
 __global__ void ef_blit_kernel(const EfDev* __restrict__ Dp, int stream, int fb, int fl, int x, int width, int frame_counter, uint16_t* __restrict__ dst)
@@ -430,20 +323,10 @@ __global__ void ef_blit_kernel(const EfDev* __restrict__ Dp, int stream, int fb,
 
 cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometry& g, int fb, int frame_counter, const EfPresent& pr, cudaStream_t stream)
 {
-#ifndef EF_K2_LEGACY
     const dim3 bands((unsigned)(g.line_count + 15) / 16, (unsigned)n_streams);
     if (g.ntsc) ef_composite_kernel<true, false><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr, nullptr, nullptr);
     else ef_composite_kernel<false, false><<<bands, kK2Threads, 0, stream>>>(dev, fb, frame_counter, pr, nullptr, nullptr);
     return cudaGetLastError();
-#else
-    const unsigned items = (unsigned)(g.line_width >> 4) + (((unsigned)g.blit_start >> 3) & 1u);   // 32-byte work items per line (see the kernel)
-    const unsigned groups = (items + 15) / 16;
-    const unsigned threads = groups * 32 * (unsigned)(g.line_count / 2);   // both standards have an even line count
-    const dim3 grid((threads + 255) / 256, (unsigned)n_streams);
-    if (g.ntsc) ef_composite_kernel<true><<<grid, 256, 0, stream>>>(dev, fb, frame_counter, pr);
-    else ef_composite_kernel<false><<<grid, 256, 0, stream>>>(dev, fb, frame_counter, pr);
-    return cudaGetLastError();
-#endif
 }
 
 // ---- paced presentation (ef_present_*): push_video's PTS -> field schedule (video.cpp:1023-1057) against the flip of video_isr
@@ -533,7 +416,6 @@ __global__ void ef_pace_fill_kernel(EfPaceState* __restrict__ st, const EfPaceSt
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
                                       uint64_t* launches)
 {
-#ifndef EF_K2_LEGACY
     const size_t per = (size_t)g.line_count * g.line_width;
     for (uint64_t f0 = 0; f0 < n_fields; f0 += 65535) {
         const dim3 grid((unsigned)(g.line_count + 15) / 16, (unsigned)(n_fields - f0 < 65535 ? n_fields - f0 : 65535));
@@ -544,10 +426,6 @@ cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, con
         ++*launches;
     }
     return cudaSuccess;
-#else
-    (void)dev; (void)g; (void)desc; (void)n_fields; (void)dst; (void)stream; (void)launches;
-    return cudaErrorNotSupported;                                          // the band kernel is the only one with a paced form
-#endif
 }
 
 cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line, int x, int width, int frame_counter, uint16_t* dst, cudaStream_t stream)

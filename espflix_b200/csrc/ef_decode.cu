@@ -56,7 +56,6 @@ constexpr int kDenseWords = 6 * kDenseStride;   // int32 [6][72] prescaled coeff
 constexpr int kDenseBytes = kDenseWords * 4;
 constexpr int kStageBytes = 4 * EF_TILE;        // motion-compensation staging: up to 2 x 2 reference tiles per macroblock
 constexpr int kWarpBytes = 2 * (kDenseBytes + kStageBytes) + 16;   // two macroblocks per warp + their mbarriers
-constexpr int kReconQzBytes = EF_K1B_DEQUANT ? 128 * 4 : 0;             // K1b dequantises (v3): the default matrices' table words, once per CTA
 
 struct SharedTables {                           // same layout as the head of EfTables
     uint16_t dct[26 * 32];
@@ -69,36 +68,27 @@ struct SharedTables {                           // same layout as the head of Ef
     uint32_t qz[128];                           // default matrices: quantiser | prescale << 8 | raster index << 18
 };
 constexpr int kTableBytes = (sizeof(SharedTables) + 15) & ~15;
-constexpr int kLutBits = EF_K1A_LUT_BITS;       // the two-symbol table (EfTables::lut2) is indexed by the next kLutBits bits
-constexpr int kLutSize = 1 << kLutBits;         // entries per context
-constexpr int kLutBytes = kLutBits > 0 ? 2 * kLutSize * (int)sizeof(uint2) : 0;
 
 // ---------------------------------------------------------------------------------------------
 // bit reader (FILL_BITS/peek_bits/get_bits, player.cpp:348-352, 495-514): MSB-first. `hi` holds the
 // current 32-bit word, `lo` the next one, pos = bits of `hi` already consumed; peek() is a single funnel
-// shift. The words after `lo` come through a per-lane ring of 8 words in shared memory filled by 4-byte
-// cp.async copies issued 7 words ahead: a register scoreboard is warp-wide, so a plain look-ahead load
+// shift. The words after `lo` come through a per-lane ring of four 16-byte chunks in shared memory filled by
+// cp.async.cg copies issued three chunks ahead: a register scoreboard is warp-wide, so a plain look-ahead load
 // into a register stalls ALL lanes at the next refill of ANY lane (that was 1/3 of K1a's stall samples);
-// the asynchronous copies involve no register. Reads run at most 12 bytes past the slice plus the 28
-// prefetched ones (into the next start code); the ES blob carries 256 bytes of zero padding at its end.
+// the asynchronous copies involve no register. Reads reach at most 76 bytes from the start of the word being parsed
+// (into the next start code); the ES blob carries 256 bytes of zero padding at its end.
 // ---------------------------------------------------------------------------------------------
-#if EF_K1A_ES16
 constexpr int kRingStride = kParseThreads * 16;         // bytes between the 16-byte chunk slots of one lane (4 slots)
 constexpr int kRingBytes = 4 * kRingStride;
-#else
-constexpr int kRingStride = kParseThreads * 4;          // bytes between ring slots of one lane: slot-major, conflict-free
-constexpr int kRingBytes = 8 * kRingStride;
-#endif
 // List entries not yet written to HBM: a ring of kStage words per lane in shared memory (entry e of the slice's list in
 // word e % kStage). They go out coalesced, one list run per store instruction, before any lane's ring could overflow:
 // the symbol loop flushes when a lane holds more than kStageHigh entries, which leaves room for one pass of steps.
 constexpr int kStage = 32;
-constexpr int kStageHigh = kStage - (EF_K1A_V3 ? EF_K1A_UNROLL : 2);   // a pass adds at most one entry per step (v3) or two (one two-symbol step)
+constexpr int kStageHigh = kStage - EF_K1A_UNROLL;   // a pass adds at most one entry per step
 static_assert(kStageHigh > 0, "a pass of the symbol loop must fit in the staging ring");
-// bytes per staging row: with the 16-byte bitstream slots a multiple of 16 (36 words for 32 entries), so that a lane's row
-// address is a multiple of its ring address (one IMAD where the compiler otherwise re-derives it from the thread index at
-// every store); else an odd number of words
-constexpr int kStageRow = EF_K1A_ES16 ? ((kStage * 4 + 16 + 15) & ~15) : (kStage + 1) * 4;
+// bytes per staging row: a multiple of the 16-byte bitstream slot (36 words for 32 entries), so that a lane's row address
+// is a multiple of its ring address (one IMAD where the compiler otherwise re-derives it from the thread index at every store)
+constexpr int kStageRow = (kStage * 4 + 16 + 15) & ~15;
 constexpr int kStageBytesA = kParseThreads * kStageRow;
 
 struct BitReader {
@@ -106,12 +96,9 @@ struct BitReader {
     uint32_t rp;             // index of the next word to take from the ring
     uint32_t sring;          // shared-window address of this lane's ring slot 0
     uint32_t hi, lo;
-#if EF_K1A_RING_AHEAD || EF_K1A_ES16
     uint32_t nx;             // raw word after `lo` (its ring load is issued one refill before it is needed: off the dependent chain)
-#endif
     int pos;
 
-#if EF_K1A_ES16
     // 16-byte chunks: chunk c of the blob lives in slot c & 3. hi, lo, nx = words rp - 2, rp - 1, rp; the next word taken
     // from the ring is rp + 1, in chunk (rp + 1) >> 2, and the chunks in flight always reach 3 past that one.
     __device__ __forceinline__ void copy_chunk(uint32_t cidx)
@@ -145,51 +132,6 @@ struct BitReader {
             if ((rp & 3u) == 3u) copy_chunk((rp >> 2) + 4);               // its last word: the slot takes the chunk 4 further on
         }
     }
-#else
-    __device__ __forceinline__ void copy_in(uint32_t widx)
-    {
-        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(sring + (widx & 7u) * kRingStride), "l"(words + widx) : "memory");
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-    __device__ __forceinline__ void init(const uint8_t* blob, uint64_t byte_off)
-    {
-        words = (const uint32_t*)blob;
-        const uint32_t w0 = (uint32_t)(byte_off >> 2);
-        pos = (int)(byte_off & 3) * 8;
-        asm volatile("cp.async.wait_all;" ::: "memory");      // copies of the previous slice must not land in the new ring
-        rp = w0 + 2;
-#pragma unroll
-        for (int k = 0; k < 7; k++) copy_in(rp + k);
-        hi = __byte_perm(__ldg(words + w0), 0, 0x0123); lo = __byte_perm(__ldg(words + w0 + 1), 0, 0x0123);
-#if EF_K1A_RING_AHEAD
-        nx = __ldg(words + w0 + 2);
-#endif
-    }
-    __device__ __forceinline__ uint32_t peek() const { return __funnelshift_l(lo, hi, pos); }
-    __device__ __forceinline__ void skip(int n)
-    {
-        pos += n;
-        if (pos >= 32) {
-            pos -= 32; hi = lo;
-#if EF_K1A_RING_AHEAD
-            lo = __byte_perm(nx, 0, 0x0123);
-            asm volatile("cp.async.wait_group 5;" ::: "memory");          // word rp + 1 has landed (7 copies in flight, one group each)
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(nx) : "r"(sring + ((rp + 1) & 7u) * kRingStride) : "memory");
-            copy_in(rp + 7);                                              // slot (rp - 1) & 7: read one refill ago
-#else
-            asm volatile("cp.async.wait_group 6;" ::: "memory");          // word rp has landed (7 copies in flight, one group each)
-            uint32_t raw;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(raw) : "r"(sring + (rp & 7u) * kRingStride) : "memory");
-            lo = __byte_perm(raw, 0, 0x0123);
-            copy_in(rp + 7);                                              // into the slot that was read one refill ago
-#endif
-#if EF_K1A_PF_L2
-            if ((rp & 7u) == 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(words + rp + 32));   // 128 bytes ahead of this slice's read position
-#endif
-            rp++;
-        }
-    }
-#endif
     __device__ __forceinline__ uint32_t get(int n)     // 1 <= n <= 32
     {
         uint32_t v = peek() >> (32 - n);
@@ -203,7 +145,6 @@ struct SliceState {
     BitReader br;
     uint32_t* list;          // the slice's coefficient list in HBM (entry 3 x byte offset of the slice)
     uint32_t slot_base;      // record slot of macroblock (0,0) of this slice's picture | destination frame store << 31
-    uint32_t seqi;           // index of the slice's sequence state in the stream's EfSeq table (K1a v3: handed to K1b for streams with their own matrices)
     const uint32_t* qzp;     // generic pointer to the table words in use: T.qz in shared memory (default matrices) or the stream's own in HBM
     const uint32_t* qz;      // scan-order quantiser | prescale | raster index tables [intra 64 | non-intra 64] of a stream with its OWN matrices (global memory); nullptr = the defaults, served from shared memory
     int mbw;
@@ -272,18 +213,9 @@ __device__ __forceinline__ uint32_t pin4(uint32_t pred, int r0, int r1, int r2, 
     // still scaled by 256. Two pixels per DPX instruction: PRMT cuts (r >> 8) out of bytes 1-2 of two residuals as a pair
     // of int16 (|r >> 8| < 30,500 for any coefficients within +-2048: the 64 basis amplitudes sum to 14.85), another PRMT
     // spreads two prediction bytes to halfwords, VIADDMNMX.S16x2.RELU computes max(min(pred + res, 248), 0) on both.
-#if EF_K1B_PIN16
     const uint32_t s01 = __viaddmin_s16x2_relu(__byte_perm(pred, 0, 0x4140), __byte_perm((uint32_t)r0, (uint32_t)r1, 0x6521), 0x00F800F8u);
     const uint32_t s23 = __viaddmin_s16x2_relu(__byte_perm(pred, 0, 0x4342), __byte_perm((uint32_t)r2, (uint32_t)r3, 0x6521), 0x00F800F8u);
     return __byte_perm(s01, s23, 0x6420);
-#else
-    // one pixel per instruction: t = max(min(pred * 256 + r, 248 * 256 + 255), 0), floor(t / 256) = its byte 1
-    const int p0 = __viaddmin_s32_relu((int)__byte_perm(pred, 0, 0x4404), r0, 0xF8FF);
-    const int p1 = __viaddmin_s32_relu((int)__byte_perm(pred, 0, 0x4414), r1, 0xF8FF);
-    const int p2 = __viaddmin_s32_relu((int)__byte_perm(pred, 0, 0x4424), r2, 0xF8FF);
-    const int p3 = __viaddmin_s32_relu((int)__byte_perm(pred, 0, 0x4434), r3, 0xF8FF);
-    return __byte_perm(__byte_perm(p0, p1, 0x0051), __byte_perm(p2, p3, 0x0051), 0x5410);
-#endif
 }
 
 // (a+b+1)>>1 on four packed bytes (mocomp cases 1 and 2, player.cpp:777-805)
@@ -516,23 +448,18 @@ __device__ __forceinline__ int parse_dc(SliceState& s, int blk)
 //
 // Lane states: no slice (idle / exhausted), WAITING for the header of its next macroblock, BUSY in the
 // coefficient state machine. Header phases (flush finished records, refill idle lanes, parse headers)
-// alternate with symbol loops (per busy lane and step: one run/level symbol with a following end of block folded in -
-// or, with EF_K1A_V3 = 0, up to two coefficients and an end of block from one look-up in the two-symbol table); a
+// alternate with symbol loops (per busy lane and step: one run/level symbol with a following end of block folded in); a
 // symbol loop ends when no lane is busy or when kHdrBatch lanes are waiting.
 // =================================================================================================
 __global__ void __launch_bounds__(kParseThreads, kParseCtasPerSm)
 ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the context by value: every D.field is a constant-bank operand (no register, no load)
 {
-    extern __shared__ __align__(16) uint8_t smem[];           // tables | two-symbol table | bitstream rings | staged list entries
+    extern __shared__ __align__(16) uint8_t smem[];           // tables | bitstream rings | staged list entries
     SharedTables& T = *(SharedTables*)smem;
-    const uint2* lut = (const uint2*)(smem + kTableBytes);
     {   // stage the tables (the first sizeof(SharedTables) bytes of EfTables have the same layout)
         const uint32_t* src = (const uint32_t*)D.tables;
         uint32_t* dst = (uint32_t*)smem;
         for (int i = threadIdx.x; i < (int)(sizeof(SharedTables) / 4); i += blockDim.x) dst[i] = src[i];
-        const uint4* lsrc = (const uint4*)D.tables->lut2;
-        uint4* ldst = (uint4*)(smem + kTableBytes);
-        for (int i = threadIdx.x; i < kLutBytes / 16; i += blockDim.x) ldst[i] = lsrc[i];
     }
     __syncthreads();
     const int lane = threadIdx.x & 31;
@@ -545,47 +472,37 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
 
     SliceState s;
     s.first = 0; s.list = D.coef; s.slot_base = 0; s.qz = nullptr; s.mbw = 0; s.mb_x = s.mb_y = 0;
-    s.br.sring = smem_u32(smem + kTableBytes + kLutBytes) + threadIdx.x * (EF_K1A_ES16 ? 16 : 4);
+    s.br.sring = smem_u32(smem + kTableBytes) + threadIdx.x * 16;
     // staged list entries: one ring row per lane
-    const uint32_t sstage_warp = smem_u32(smem + kTableBytes + kLutBytes + kRingBytes) + (threadIdx.x & ~31u) * kStageRow;
-#if EF_K1A_ES16
-    const uint32_t sstage_bias = smem_u32(smem + kTableBytes + kLutBytes + kRingBytes) - (kStageRow / 16) * smem_u32(smem + kTableBytes + kLutBytes);
-#define EF_SSTAGE (s.br.sring * (kStageRow / 16) + sstage_bias)      /* = stage base + thread * kStageRow (sring = ring base + thread * 16) */
-#else
-    const uint32_t sstage = sstage_warp + lane * kStageRow;
-#define EF_SSTAGE sstage
-#endif
+    const uint32_t sstage_warp = smem_u32(smem + kTableBytes + kRingBytes) + (threadIdx.x & ~31u) * kStageRow;
+    const uint32_t sstage_bias = smem_u32(smem + kTableBytes + kRingBytes) - (kStageRow / 16) * smem_u32(smem + kTableBytes);
     bool active = false, exhausted = false, busy = false;
     // the slice's list: `tot` entries so far, the first `done` of them in HBM, the rest in the lane's ring.
     // The macroblock in flight: info word under construction (bit 0 set = a record is owed), its first list entry,
     // skip run, motion vector, record slot
     uint32_t tot = 0, done = 0;
     uint32_t info_acc = 0, mb0 = 0, skipw = 0, mvw = 0, slot = 0;
-    uint32_t blk24 = 0, blkbit = 0;                           // current block: number << 24 (v3: token head = number << 27 | quantiser_scale << 16), 0x100 << number
+    uint32_t blk24 = 0, blkbit = 0;                           // current block: number << 24, 0x100 << number
     int cbp_rem = 0, n = 0, intra = 0, ctx = 0;               // n = scan position of the block in flight; ctx = 1: the next symbol is the first coefficient of a non-intra block
     // next coded block of the macroblock in flight (cbp_rem != 0): block number, contexts, intra DC
     auto start_block = [&]() {
         const int blk = __ffs(cbp_rem) - 1;
-#if EF_K1B_DEQUANT
-        blk24 = ((uint32_t)blk << 27) | ((uint32_t)s.qscale << 16);
-#else
         blk24 = (uint32_t)blk << 24;
-#endif
         blkbit = 0x100u << blk;
         cbp_rem &= cbp_rem - 1;
         n = 0; ctx = 1;                                       // dct_coeff_first: no end of block, '1s' = (0, 1)
         if (intra) { D.mb_rec[slot].dc[blk] = parse_dc(s, blk); n = 1; ctx = 0; }
     };
-    // next list entry of the slice: into the lane's ring
+    // next list entry of the slice: into the lane's ring. Its row address is stage base + thread * kStageRow, derived from
+    // sring = ring base + thread * 16
     auto put_entry = [&](uint32_t ent) {
-        asm volatile("st.shared.u32 [%0], %1;" ::"r"(EF_SSTAGE + (tot % kStage) * 4), "r"(ent) : "memory");
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(s.br.sring * (kStageRow / 16) + sstage_bias + (tot % kStage) * 4), "r"(ent) : "memory");
         tot++;
     };
     // warp-wide (all lanes converged): every lane's entries still in its ring go to the list in HBM. Lane j stores
     // entry j of one lane's pending run, so each store instruction writes one contiguous run of one list
     auto flush = [&]() {
         __syncwarp();                                                 // the ring words of other lanes are read below, and rewritten after
-#if !EF_PROBE_NOSTORE                                                 /* bottleneck probe (wrong output): no list stores */
         const uint32_t pend = tot - done;                             // <= kStage
         const uint64_t dst = (uint64_t)(s.list + done);
         const uint32_t key = pend | (done << 8);                      // run length | ring position of its first entry
@@ -601,7 +518,6 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                 d[lane] = v;
             }
         }
-#endif
         __syncwarp();
         done = tot;
     };
@@ -614,9 +530,6 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
         if (!busy && (info_acc & 1u)) {
             const uint64_t li = (uint64_t)(s.list - D.coef) + mb0;
             *(uint4*)(D.mb_rec + slot) = make_uint4((tot - mb0) | (skipw << 16), mvw, (uint32_t)li, (uint32_t)(li >> 32));
-#if EF_K1B_DEQUANT
-            if (s.qz) { info_acc |= 1u << 26; D.mb_rec[slot].pad[0] = s.seqi; }     // K1b dequantises with the stream's own matrices
-#endif
             D.mb_info[slot] = info_acc | ((uint32_t)s.mbw << 20) | ((s.slot_base >> 31) << 25);
             info_acc = 0;
         }
@@ -645,7 +558,6 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                         const EfSeq* seq = D.seq + (size_t)w.stream * (D.max_seq + 1) + (w.info >> 16);
                         s.mbw = min((int)seq->mb_width, EF_MBW_MAX);
                         s.qz = seq->custom ? (const uint32_t*)seq->qz : nullptr;
-                        s.seqi = w.info >> 16;
                         s.qzp = s.qz ? s.qz : T.qz;
                         const uint64_t byte_off = D.es_off[w.stream] + w.es_off;
                         s.slot_base = (w.pic - (uint32_t)pic0) * n_slots + w.stream * (uint32_t)(EF_MBW_MAX * EF_MBH_MAX);
@@ -679,23 +591,16 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
 
         // ---- symbol loop: each lane runs through its own macroblock; a lane whose macroblock is complete waits (its
         // record is owed) until the loop ends, when no lane is busy or when kHdrBatch lanes are waiting. Per pass, every
-        // busy lane takes EF_K1A_UNROLL steps (v3) or one two-symbol step
+        // busy lane takes EF_K1A_UNROLL steps
         const int qoff = intra ? 0 : 64, kq = intra ? 0 : 1;
-#if EF_K1A_V3
         const uint32_t* const qrow = s.qzp + qoff;               // table words of this macroblock's matrix, by scan position
-#else
-        // table word of scan position n: shared memory for the default matrices (no global-load latency in the symbol
-        // chain), the stream's own table in HBM otherwise (sequence headers that load matrices are rare)
-        auto qword = [&](int pos) -> uint32_t { return s.qz ? __ldg(s.qz + qoff + pos) : T.qz[qoff + pos]; };
-#endif
         for (;;) {
             const unsigned bmask = __ballot_sync(0xFFFFFFFFu, busy);
             if (!bmask || __popc(amask & ~bmask) >= kHdrBatch) break;
             if (__any_sync(0xFFFFFFFFu, tot - done > (uint32_t)kStageHigh)) flush();
-#if EF_K1A_V3
             // per step ONE run/level symbol through the clz-indexed table, a following end of block folded in;
             // dequantised on the spot (table word of the scan position: shared memory for the default matrices, the
-            // stream's own table in HBM otherwise) or, with EF_K1B_DEQUANT, stored as a raw token
+            // stream's own table in HBM otherwise)
 #pragma unroll
             for (int u_ = 0; u_ < EF_K1A_UNROLL; u_++)
             if (busy) {
@@ -714,11 +619,7 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                         n += sy.run;
                         if (n > 63) { info_acc |= blkbit << 6; block_done = true; }      // block() returns -1: nothing of the block is stored; the symbol is consumed
                         else {
-#if EF_K1B_DEQUANT
-                            put_entry(blk24 | ((uint32_t)n << 21) | ((uint32_t)sy.lvl & 0xFFFFu));
-#else
                             put_entry(ef_coef_entry(qrow[n], sy.lvl, s.qscale, kq, blk24));
-#endif
                             n++;
                             if (len <= 30 && ((w << len) >> 30) == 2u) { len += 2; block_done = true; }   // '10' follows: end of block
                         }
@@ -731,39 +632,8 @@ ef_parse_kernel(const __grid_constant__ EfDev D, int pic0, int n_pics)   // the 
                     }
                 }
             }
-#else
-            // per step up to two coefficients and an end of block. Fast path: the next kLutBits bits index the
-            // two-symbol table; everything that lies wholly inside them (one or two run/level codes with their sign
-            // bits, a closing '10') is taken in one step. Long codes, the escape, invalid prefixes and symbols that
-            // would run past scan position 63 decode one symbol through the clz-indexed table (and fold a following
-            // end of block in).
-            if (busy) {
-                BitReader& br = s.br;
-                const uint32_t w = br.peek();
-                const EfCoefStep st = ef_coef_step(w, ctx != 0, n, lut, T.dct);
-                const uint32_t fl = st.fl;
-                const int len = st.len;
-                ctx = 0;
-                if (fl & EF_STEP_COEF1) { n += st.run1; put_entry(ef_coef_entry(qword(n), st.lvl1, s.qscale, kq, blk24)); n++; }
-                if (fl & EF_STEP_COEF2) { n += st.run2; put_entry(ef_coef_entry(qword(n), st.lvl2, s.qscale, kq, blk24)); n++; }
-                if (fl & 16u) {                                // give up on this and the remaining blocks, end the slice
-                    info_acc |= (blkbit << 6) | ((uint32_t)cbp_rem << 14);
-                    s.mb_y = EF_MBH_MAX;
-                    busy = false;
-                } else {
-                    br.skip(len);
-                    if (fl & 12u) {
-                        if (fl & 8u) info_acc |= blkbit << 6;
-                        else if (n == 1) info_acc |= blkbit;   // Q5
-                        busy = cbp_rem != 0;
-                        if (busy) start_block();
-                    }
-                }
-            }
-#endif
         }
     }
-#undef EF_SSTAGE
 }
 
 // =================================================================================================
@@ -789,11 +659,6 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
     uint32_t bar_phase = 0;
     if (hl == 0) mbar_init(bar, 1);
     for (int i = hl; i < kDenseWords; i += 16) dense[i] = 0;
-#if EF_K1B_DEQUANT
-    const uint32_t* qzs = (const uint32_t*)(smem + (size_t)kReconWarps * kWarpBytes);   // default matrices: quantiser | prescale << 8 | raster index << 18 per scan position
-    for (int i = threadIdx.x; i < 128; i += blockDim.x) ((uint32_t*)qzs)[i] = D.tables->qz[i];
-    __syncthreads();
-#endif
     __syncwarp();
 
     constexpr uint32_t kMbs = EF_MBW_MAX * EF_MBH_MAX;
@@ -808,7 +673,7 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
     // one load per lane fetches a record: lanes 0-9 of the half its words, lane 12 the info word
     auto fetch = [&](uint32_t slot) -> uint32_t {
         uint32_t v = 0;
-        if (slot < n_slots && (hl < (EF_K1B_DEQUANT ? 11 : 10) || hl == 12)) v = __ldg(hl == 12 ? infos + slot : recs + (size_t)slot * (sizeof(EfMbRec) / 4) + hl);
+        if (slot < n_slots && (hl < 10 || hl == 12)) v = __ldg(hl == 12 ? infos + slot : recs + (size_t)slot * (sizeof(EfMbRec) / 4) + hl);
         return v;
     };
 
@@ -883,20 +748,8 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
         }
 
         // expand the coefficient list into the dense scratch (entries of aborted blocks are dropped)
-#if EF_K1B_DEQUANT
-        // token = block << 27 | scan position << 21 | quantiser_scale << 16 | (int16) level: dequantise here (block(),
-        // player.cpp:1106-1121), with the table word of the scan position from shared memory (default matrices) or from
-        // the stream's sequence state (info bit 26; record word 10 = its index)
-        const int qoff = intra_r ? 0 : 64, kq = intra_r ? 0 : 1;
-        const uint32_t seqi = __shfl_sync(0xFFFFFFFFu, recw, hb + 10);
-        const uint32_t* cqz = nullptr;
-        if (valid && ((info >> 26) & 1u)) cqz = D.seq[(size_t)stream * (D.max_seq + 1) + min(seqi, (uint32_t)D.max_seq)].qz;
-#define EF_EXPAND(ent) { const uint32_t t_ = (ent); const int eb = (t_ >> 27) & 7; if (!((abm >> eb) & 1)) { const int n_ = qoff + ((t_ >> 21) & 63); \
-            const uint32_t z_ = cqz ? __ldg(cqz + n_) : qzs[n_]; dense[eb * kDenseStride + ((z_ >> 18) & 63)] = ef_dequant(z_, (int)(int16_t)(t_ & 0xFFFFu), (int)((t_ >> 16) & 31u), kq); } }
-#else
         // entry = (block << 24 | raster position << 18) + value, |value| < 2^17: adding 2^17 undoes the borrow of a negative value
 #define EF_EXPAND(ent) { const uint32_t hi_ = (ent) + 0x20000u; const int eb = (hi_ >> 24) & 7; if (!((abm >> eb) & 1)) dense[eb * kDenseStride + ((hi_ >> 18) & 63)] = ((int)((ent) << 14)) >> 14; }
-#endif
         if (hl < entries) EF_EXPAND(e0)
         if (hl + 16 < entries) EF_EXPAND(e1)
         if (hl + 32 < entries) EF_EXPAND(e2)
@@ -986,8 +839,8 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
 }
 
 // host-side launch helpers -----------------------------------------------------------------------
-size_t ef_recon_smem_bytes() { return (size_t)kReconWarps * kWarpBytes + kReconQzBytes; }
-static constexpr size_t kParseSmemBytes = (size_t)kTableBytes + kLutBytes + kRingBytes + kStageBytesA;
+size_t ef_recon_smem_bytes() { return (size_t)kReconWarps * kWarpBytes; }
+static constexpr size_t kParseSmemBytes = (size_t)kTableBytes + kRingBytes + kStageBytesA;
 
 static int g_parse_ctas = kParseCtasPerSm, g_recon_ctas = kReconCtasPerSm;   // resident CTAs per SM, measured by the occupancy API
 

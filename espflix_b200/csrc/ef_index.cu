@@ -90,7 +90,6 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
     load_chunk(0, v, nxt);
     load_chunk(512, v1, nxt1);
     for (uint64_t chunk = 0; chunk < span && !stop; chunk += 512, v = v1, nxt = nxt1, v1 = v2, nxt1 = nxt2) {
-        const uint64_t o = chunk + (uint64_t)lane * 16;
         load_chunk(chunk + 1024, v2, nxt2);
         const uint32_t w[5] = { v.x, v.y, v.z, v.w, nxt };
         // "00 00 01" at byte i of the lane's 20-byte window, all 16 positions at once: exact per-byte masks of the zero

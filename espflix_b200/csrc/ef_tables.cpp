@@ -30,67 +30,7 @@ bool place(uint16_t* tab, int max_lz, const char* code, uint16_t entry)
     return true;
 }
 
-// one coefficient symbol (code + sign bit, or end of block) read from the first `avail` bits of `bits`
-// (MSB first, `avail` <= 32). first = dct_coeff_first context. Returns the length, 0 if no symbol lies wholly
-// inside the available bits (long codes, the escape, invalid prefixes).
-int match_symbol(uint32_t bits, int avail, bool first, int& run, int& level, bool& eob)
-{
-    auto starts = [&](const char* code, int len) {
-        if (len > avail) return false;
-        for (int i = 0; i < len; i++) if ((int)((bits >> (31 - i)) & 1) != (code[i] == '1')) return false;
-        return true;
-    };
-    eob = false;
-    if (first) {
-        if (avail >= 2 && (bits >> 31)) { run = 0; level = (bits >> 30) & 1 ? -1 : 1; return 2; }      // "1s"
-    } else {
-        if (starts("10", 2)) { eob = true; run = level = 0; return 2; }
-    }
-    for (int i = 0; i < EF_VLC_DCT_COUNT; i++) {
-        const char* c = ef_vlc_dct[i].code;
-        const int len = (int)strlen(c);
-        if (first && len == 2) continue;                                // "11s" does not exist as a first coefficient
-        if (!starts(c, len) || len + 1 > avail) continue;
-        run = ef_vlc_dct[i].value >> 8;
-        level = ef_vlc_dct[i].value & 0xFF;
-        if ((bits >> (31 - len)) & 1) level = -level;
-        return len + 1;
-    }
-    return 0;
-}
-
 }  // namespace
-
-// The two-symbol table of the coefficient parser (EfTables::lut2): for every K-bit window, the symbols that
-// lie wholly inside it - one or two coefficients and a closing end of block - or "decode the slow way".
-static void build_lut2(uint2* lut, int kbits)
-{
-    for (int ctx = 0; ctx < 2; ctx++) {
-        for (uint32_t p = 0; p < (1u << kbits); p++) {
-            const uint32_t bits = p << (32 - kbits);
-            uint2 e = make_uint2(127u << 24, 0u);
-            int run1, lvl1, run2, lvl2, used = 0;
-            bool eob;
-            int l = match_symbol(bits, kbits, ctx == 1, run1, lvl1, eob);
-            if (l && eob) e = make_uint2(2u, 4u);
-            else if (l) {
-                used = l;
-                uint32_t flags = 1, span = (uint32_t)run1, r2 = 0, v2 = 0;
-                l = match_symbol(bits << used, kbits - used, false, run2, lvl2, eob);
-                if (l && !eob) {
-                    used += l; flags |= 2; span += 1u + (uint32_t)run2; r2 = (uint32_t)run2; v2 = (uint32_t)lvl2 & 255u;
-                    int r3, v3;
-                    l = match_symbol(bits << used, kbits - used, false, r3, v3, eob);
-                    if (!(l && eob)) l = 0;
-                }
-                if (l && eob) { used += 2; flags |= 4; }
-                if (span < 64)
-                    e = make_uint2((uint32_t)used | ((uint32_t)run1 << 8) | (((uint32_t)lvl1 & 255u) << 16) | (span << 24), flags | (r2 << 8) | (v2 << 16));
-            }
-            lut[((size_t)ctx << kbits) + p] = e;
-        }
-    }
-}
 
 const unsigned char* ef_default_intra_ptr() { return ef_default_intra_q; }
 
@@ -147,7 +87,6 @@ int ef_build_tables(EfTables* t)
     for (int n = 0; n < 64; n++) { t->qdef[n] = ef_default_intra_q[ef_zigzag[n]]; t->qdef[64 + n] = 16; }
     for (int n = 0; n < 64; n++) t->zp[n] = (uint16_t)(ef_zigzag[n] | (ef_aan_prescale[ef_zigzag[n]] << 8));
     for (int n = 0; n < 128; n++) t->qz[n] = ef_qz_entry(t->qdef[n], n & 63);
-    if (EF_K1A_LUT_BITS > 0) build_lut2(t->lut2, EF_K1A_LUT_BITS);
     return 0;
 }
 

@@ -1,7 +1,7 @@
 // tests/k1a_step_model.cpp — CPU model test of K1a's coefficient step (espflix_b200/csrc/ef_coef_step.cuh): the
 // SAME header the kernel compiles is driven here on the host over encoded and random bit strings and compared,
 // block by block, with a symbol-by-symbol restatement of the reference's block() loop (player.cpp:1068-1121) that
-// reads the ISO code list directly (independent of both lookup tables). Built and run by tests/test_k1a_step_model.py.
+// reads the ISO code list directly (independent of the lookup table). Built and run by tests/test_k1a_step_model.py.
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -67,27 +67,8 @@ static Result ref_block(const Bits& B, size_t pos, bool nonintra)
     return r;
 }
 
+// K1a: one symbol per step (ef_coef_sym), a following '10' folded in by the caller exactly as the kernel does
 static Result model_block(const EfTables& T, const Bits& B, size_t pos, bool nonintra)
-{
-    Result r; r.end = 2;
-    int n = nonintra ? 0 : 1;
-    bool first = nonintra;
-    for (int guard = 0; guard < 200; guard++) {
-        const EfCoefStep s = ef_coef_step(B.window(pos), first, n, T.lut2, T.dct);
-        first = false;
-        if (s.fl & EF_STEP_COEF1) { n += s.run1; r.c.push_back({ n, s.lvl1 }); n++; }
-        if (s.fl & EF_STEP_COEF2) { n += s.run2; r.c.push_back({ n, s.lvl2 }); n++; }
-        if (s.fl & EF_STEP_DERAIL) { r.end = 2; break; }
-        pos += s.len;
-        if (s.fl & EF_STEP_ABORT) { r.end = 1; break; }
-        if (s.fl & EF_STEP_EOB) { r.end = 0; break; }
-    }
-    r.bits = pos;
-    return r;
-}
-
-// K1a v3: one symbol per step (ef_coef_sym), a following '10' folded in by the caller exactly as the kernel does
-static Result model_block_v3(const EfTables& T, const Bits& B, size_t pos, bool nonintra)
 {
     Result r; r.end = 2;
     int n = nonintra ? 0 : 1;
@@ -102,9 +83,7 @@ static Result model_block_v3(const EfTables& T, const Bits& B, size_t pos, bool 
         if (s.kind == EF_SYM_COEF) {
             n += s.run;
             if (n > 63) { pos += len; r.end = 1; break; }
-            // through the token, as K1b reads it back
-            const uint32_t tok = ef_token(5u, n, 31, s.lvl);
-            r.c.push_back({ (int)((tok >> 21) & 63u), (int)(int16_t)(tok & 0xFFFFu) });
+            r.c.push_back({ n, s.lvl });
             n++;
             if (len <= 30 && ((w << len) >> 30) == 2u) { len += 2; done = true; }
         }
@@ -115,21 +94,13 @@ static Result model_block_v3(const EfTables& T, const Bits& B, size_t pos, bool 
     return r;
 }
 
-static long n_blocks = 0, n_coefs = 0, n_steps_saved = 0;
+static long n_blocks = 0, n_coefs = 0;
 static int compare(const EfTables& T, const Bits& B, size_t pos, bool nonintra, const char* what)
 {
     const Result a = ref_block(B, pos, nonintra), m = model_block(T, B, pos, nonintra);
     n_blocks++; n_coefs += (long)a.c.size();
     bool ok = a.end == m.end && a.c.size() == m.c.size() && (a.end == 2 || a.bits == m.bits);
     for (size_t i = 0; ok && i < a.c.size(); i++) ok = a.c[i].pos == m.c[i].pos && a.c[i].level == m.c[i].level;
-    const Result v3 = model_block_v3(T, B, pos, nonintra);
-    bool ok3 = a.end == v3.end && a.c.size() == v3.c.size() && (a.end == 2 || a.bits == v3.bits);
-    for (size_t i = 0; ok3 && i < a.c.size(); i++) ok3 = a.c[i].pos == v3.c[i].pos && a.c[i].level == v3.c[i].level;
-    if (!ok3) {
-        fprintf(stderr, "V3 MISMATCH (%s, %s): ref end %d coefs %zu bits %zu / v3 end %d coefs %zu bits %zu\n", what, nonintra ? "non-intra" : "intra",
-                a.end, a.c.size(), a.bits - pos, v3.end, v3.c.size(), v3.bits - pos);
-        return 1;
-    }
     if (!ok) {
         fprintf(stderr, "MISMATCH (%s, %s): ref end %d coefs %zu bits %zu / model end %d coefs %zu bits %zu\n", what, nonintra ? "non-intra" : "intra",
                 a.end, a.c.size(), a.bits - pos, m.end, m.c.size(), m.bits - pos);
@@ -181,12 +152,11 @@ int main()
         for (int k = 0; k < 12; k++) B.put((rnd() % 7 == 0) ? 0u : rnd(), 32);
         bad += compare(T, B, rnd() % 32, rnd() & 1, "random");
     }
-    // 3. every 10-bit prefix at every scan position, both contexts (exercises the position-63 guard of the pairs)
+    // 3. every 10-bit prefix, both contexts, followed by zeros, ones or random bits
     for (int ctx = 0; ctx < 2 && bad < 5; ctx++)
         for (uint32_t p = 0; p < 1024 && bad < 5; p++)
             for (int fill = 0; fill < 4 && bad < 5; fill++) {
                 Bits B; B.put(p, 10); B.put(fill == 0 ? 0u : fill == 1 ? 0xFFFFFFFFu : rnd(), 32); B.put(rnd(), 32); B.put(rnd(), 32);
-                // prefix some coefficients so that the block is already at position `at`
                 bad += compare(T, B, 0, ctx == 1, "prefix");
             }
     // 4. list entry: pack/unpack round trip over the whole value range, as K1b reads it
@@ -206,9 +176,6 @@ int main()
                 const uint32_t ent = ef_coef_entry(z, level, qs, k, blk << 24);
                 const uint32_t hi = ent + 0x20000u;
                 const int got = ((int)(ent << 14)) >> 14, gb = (hi >> 24) & 7, gp = (hi >> 18) & 63;
-                const uint32_t tok = ef_token(blk, n & 63, qs, level);               // v3: token -> K1b's dequantisation
-                const int got3 = ef_dequant(T.qz[(intra ? 0 : 64) + (int)((tok >> 21) & 63u)], (int)(int16_t)(tok & 0xFFFFu), (int)((tok >> 16) & 31u), k);
-                if (got3 != want || (tok >> 27) != blk) { fprintf(stderr, "TOKEN MISMATCH n %d level %d qs %d: want %d got %d\n", n, level, qs, want, got3); bad++; }
                 if (got != want || gb != (int)blk || gp != zz) {
                     fprintf(stderr, "ENTRY MISMATCH n %d level %d qs %d: want %d blk %u pos %d, got %d blk %d pos %d\n", n, level, qs, want, blk, zz, got, gb, gp);
                     bad++;

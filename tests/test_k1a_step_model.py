@@ -1,7 +1,7 @@
 """CPU model test of K1a's coefficient step: tests/k1a_step_model.cpp compiles the SAME header the kernel uses
-(espflix_b200/csrc/ef_coef_step.cuh: two-symbol table look-up, slow path, list-entry packing) for the host and holds
-it to a symbol-by-symbol restatement of block() (player.cpp:1068-1121) over ~400,000 encoded, random and exhaustive
-prefix blocks. Runs without a GPU."""
+(espflix_b200/csrc/ef_coef_step.cuh: one symbol per step through the clz-indexed table, the end-of-block fold, list-entry
+packing) for the host and holds it to a symbol-by-symbol restatement of block() (player.cpp:1068-1121) over ~400,000
+encoded, random and exhaustive prefix blocks. Runs without a GPU."""
 import json
 import os
 import subprocess
@@ -9,7 +9,7 @@ import subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_coefficient_step_matches_the_symbol_by_symbol_parser(tmp_path):
+def test_one_symbol_step_matches_the_symbol_by_symbol_parser(tmp_path):
     exe = str(tmp_path / "k1a_step_model")
     cuda_inc = "/usr/local/cuda/include"
     subprocess.run(["g++", "-O2", "-std=c++17", "-I", cuda_inc, "-x", "c++", os.path.join(ROOT, "tests", "k1a_step_model.cpp"),
