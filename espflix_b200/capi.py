@@ -82,6 +82,7 @@ _SIGNATURES = {
     "ef_present_enable": (_I, [_VP, _VP]),
     "ef_present_picture": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_idle": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -345,6 +346,18 @@ class Context:
         """ef_present_idle: every display runs on until it has emitted n_fields[s] more fields"""
         nf = np.ascontiguousarray(np.broadcast_to(n_fields, (self.n_streams,)), dtype=np.uint32)
         return self._present(lambda d, c, i, st: self.lib.ef_present_idle(self._h, nf.ctypes.data, d, c, i, st), out, stream)
+
+    def present_overlay(self, bitmaps=None, blend=None, progress=None, set=None, first=0, count=None):
+        """ef_present_overlay: stage overlay changes for streams [first, first + count); they latch at line 0 of the first field
+        the next present call reaches. bitmaps: [count, 16, 80] uint8 (or one bitmap for all), blend / progress: int32 per stream or
+        one for all, set: per-stream bits (1 bitmap, 2 blend, 4 progress; None = all three). None leaves that attribute unset."""
+        count = self.n_streams - first if count is None else count
+
+        bm = None if bitmaps is None else np.asarray(bitmaps, dtype=np.uint8).reshape(-1, 1280)
+        keep = [None if a is None else np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=dt), shape))
+                for a, dt, shape in ((bm, np.uint8, (count, 1280)), (blend, np.int32, (count,)), (progress, np.int32, (count,)), (set, np.uint8, (count,)))]
+        ptrs = [None if a is None or a.size == 0 else a.ctypes.data for a in keep]
+        self._check(self.lib.ef_present_overlay(self._h, first, count, *ptrs))
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

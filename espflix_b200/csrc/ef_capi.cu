@@ -53,10 +53,13 @@ cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t 
 cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometry& g, int fb, int frame_counter, const EfPresent& pr, cudaStream_t stream);
 cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line, int x, int width, int frame_counter, uint16_t* dst, cudaStream_t stream);
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches);
+                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps);
 __global__ void ef_pace_kernel(const EfPaceState* st, EfPaceState* next, EfPaceRun* run, EfPaceOut* out, const int64_t* pic_pts, const uint32_t* n_pics,
-                               const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc);
-__global__ void ef_pace_fill_kernel(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc);
+                               const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc,
+                               const EfOverlayState* ovl, EfOverlayState* ovl_next);
+__global__ void ef_pace_fill_kernel(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc,
+                                    EfOverlayState* ovl, const EfOverlayState* ovl_next, EfFieldOverlay* fovl);
+__global__ void ef_overlay_stage_kernel(EfOverlayState* ovl, uint8_t* slots, const EfOverlayCmd* cmd, const uint8_t* bitmaps, int first);
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
 
 namespace {
@@ -234,6 +237,15 @@ struct ef_ctx {
     uint32_t* h_pace_arg = nullptr;               // pinned
     EfFieldDesc* d_desc = nullptr;                // one per emitted field, grown on demand
     uint64_t desc_cap = 0;
+    // overlay of paced presentation (ef_present_overlay): allocated by its first call; until then the present calls run the
+    // kernels they ran before
+    EfOverlayState* d_ovl = nullptr;              // [n_streams]
+    EfOverlayState* d_ovl_next = nullptr;         // [n_streams] the state after the call being made
+    uint8_t* d_ovl_slots = nullptr;               // [n_streams][2][1280] latched and staged bitmap
+    uint8_t* d_ovl_in = nullptr;                  // [n_streams][1280] the bitmaps of one ef_present_overlay call
+    EfOverlayCmd* d_ovl_cmd = nullptr;            // [n_streams]
+    EfFieldOverlay* d_fovl = nullptr;             // one per emitted field, beside d_desc
+    uint64_t fovl_cap = 0;
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -430,6 +442,7 @@ void ef_destroy(ef_ctx* c)
     for (void* p : c->allocs) cudaFree(p);
     for (void* p : c->allocs_host) cudaFreeHost(p);
     if (c->d_desc) cudaFree(c->d_desc);
+    if (c->d_fovl) cudaFree(c->d_fovl);
     delete c->aud_scratch;
     if (c->h_ended) cudaFreeHost(c->h_ended);
     for (int b = 0; b < 2; b++) {
@@ -1413,7 +1426,7 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
     if (arg) CK(cudaMemcpyAsync(c->d_pace_arg, c->h_pace_arg, pic < 0 ? (size_t)n * 4 : (size_t)n, cudaMemcpyHostToDevice, st));
     ef_pace_kernel<<<(n + 127) / 128, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_out, c->d_pic_pts, c->h.n_pics, c->h.base_pics,
                                                    pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, (const uint32_t*)c->d_pace_arg, pic,
-                                                   c->cfg.max_pictures, n, c->pace_ntsc);
+                                                   c->cfg.max_pictures, n, c->pace_ntsc, c->d_ovl, c->d_ovl_next);
     CK(cudaGetLastError());
     c->launches++;
     CK(cudaMemcpyAsync(c->h_pace_out, c->d_pace_out, (size_t)n * sizeof(EfPaceOut), cudaMemcpyDeviceToHost, st));
@@ -1444,11 +1457,19 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
         CK(cudaMalloc(&c->d_desc, total * sizeof(EfFieldDesc)));
         c->desc_cap = total;
     }
+    if (c->d_ovl && total > c->fovl_cap) {
+        CK(cudaStreamSynchronize(st));
+        if (c->d_fovl) CK(cudaFree(c->d_fovl));
+        c->d_fovl = nullptr; c->fovl_cap = 0;
+        CK(cudaMalloc(&c->d_fovl, total * sizeof(EfFieldOverlay)));
+        c->fovl_cap = total;
+    }
     CK(cudaMemcpyAsync(c->d_pace_first, c->h_pace_first, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    ef_pace_fill_kernel<<<n, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc);
+    ef_pace_fill_kernel<<<n, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc, c->d_ovl, c->d_ovl_next,
+                                           c->d_ovl ? c->d_fovl : nullptr);
     CK(cudaGetLastError());
     c->launches++;
-    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, total, dst, st, &c->launches));
+    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, total, dst, st, &c->launches, c->d_ovl ? c->d_fovl : nullptr, c->d_ovl_slots));
     CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
     return EF_OK;
 }
@@ -1472,6 +1493,43 @@ int ef_present_idle(ef_ctx* c, const uint32_t* n_fields, uint16_t* dst, uint64_t
     if (!c || !info || !n_fields) return fail(EF_EINVAL, "null argument");
     if (!c->paced) return fail(EF_ESTATE, "ef_present_idle before ef_present_enable");
     return present_common(c, -1, nullptr, n_fields, dst, dst_fields, info, (cudaStream_t)stream);
+}
+
+// ---- overlay of paced presentation: _video_composite, _video_composite_blend, _video_composite_progress per stream (video.cpp:839-887) ----
+int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, const int32_t* blend, const int32_t* progress, const uint8_t* set)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->paced) return fail(EF_ESTATE, "ef_present_overlay before ef_present_enable");
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    std::vector<EfOverlayCmd> cmd((size_t)count);
+    for (int i = 0; i < count; i++) {
+        uint32_t m = set ? set[i] & 7u : 7u;
+        if (!bitmaps) m &= ~1u;
+        if (!blend) m &= ~2u;
+        if (!progress) m &= ~4u;
+        if ((m & 2u) && blend[i] < -1) return fail(EF_EINVAL, "blend %d of stream %d is below -1", blend[i], first + i);
+        cmd[i] = { (m & 2u) ? blend[i] : 0, (m & 4u) ? progress[i] : 0, m, 0u };
+    }
+    int rc;
+#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
+    if (!c->d_ovl) {
+        A(c->d_ovl, (size_t)n); A(c->d_ovl_next, (size_t)n); A(c->d_ovl_cmd, (size_t)n);
+        A(c->d_ovl_slots, (size_t)n * 2 * EF_OVERLAY_BYTES); A(c->d_ovl_in, (size_t)n * EF_OVERLAY_BYTES);
+        CK(cudaMemset(c->d_ovl, 0, (size_t)n * sizeof(EfOverlayState)));   // blend 0: nothing drawn
+        CK(cudaMemset(c->d_ovl_slots, 0, (size_t)n * 2 * EF_OVERLAY_BYTES));
+    }
+#undef A
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(c->d_ovl_cmd, cmd.data(), cmd.size() * sizeof(EfOverlayCmd), cudaMemcpyHostToDevice));
+    if (bitmaps) CK(cudaMemcpy(c->d_ovl_in, bitmaps, (size_t)count * EF_OVERLAY_BYTES, cudaMemcpyHostToDevice));
+    ef_overlay_stage_kernel<<<count, 96>>>(c->d_ovl, c->d_ovl_slots, c->d_ovl_cmd, c->d_ovl_in, first);
+    CK(cudaGetLastError());
+    c->launches++;
+    CK(cudaDeviceSynchronize());
+    return EF_OK;
 }
 
 }  // extern "C"

@@ -200,6 +200,34 @@ struct __align__(16) EfFieldDesc {   // one paced K2 field; its output slot is i
     uint32_t frame_counter;
     int32_t hscroll;
 };
+// The overlay of paced presentation (ef_present_overlay): composite()'s bitmap, blend and progress per stream (video.cpp:839-887).
+// Staged changes wait in `pending` (the bitmap in slot ^ 1) and latch at line 0 of the first field that starts at or after the
+// position where the next present call begins. A latched blend b > 0 counts down once per field end (video.cpp:1193-1194): field
+// G shows max(0, b - (G - blend_fc)).
+#define EF_OVERLAY_BYTES 1280    // _video_composite[16][80]
+struct __align__(16) EfOverlayState {
+    int32_t blend;               // latched _video_composite_blend
+    uint32_t blend_fc;           // the field it was latched at
+    int32_t progress;            // latched _video_composite_progress
+    uint32_t slot;               // the stream's bitmap slot (0 / 1) the latched bitmap is in
+    uint32_t pending;            // staged and not latched yet: bit 0 bitmap (in slot ^ 1), bit 1 p_blend, bit 2 p_progress
+    int32_t p_blend, p_progress;
+    uint32_t latch_fc;           // scratch copy of a call only: the field its staged changes latch at
+};
+struct __align__(16) EfOverlayCmd {  // one stream's change of one ef_present_overlay call
+    int32_t blend, progress;
+    uint32_t set;                // bit 0 bitmap, bit 1 blend, bit 2 progress
+    uint32_t pad;
+};
+struct __align__(16) EfFieldOverlay {    // the overlay one paced K2 field is drawn with, beside its EfFieldDesc
+    int32_t blend, progress;
+    uint32_t slot, pad;
+};
+static inline __host__ __device__ int ef_overlay_blend(int32_t b, uint32_t blend_fc, uint32_t fc)
+{
+    const uint32_t d = fc - blend_fc;    // fields since the latch, modulo 2^32
+    return b <= 0 ? b : d >= (uint32_t)b ? 0 : b - (int)d;
+}
 
 static inline __host__ __device__ size_t ef_frame_offset(int stream, int fb) { return ((size_t)stream * 2 + (size_t)fb) * EF_FRAME; }
 static inline __host__ __device__ int ef_tile_offset(int mx, int my) { return (my * EF_MBW_MAX + mx) * EF_TILE; }

@@ -151,11 +151,14 @@ __device__ __forceinline__ int blank_class(const EfPresent& pr, int line)
 
 // kPaced (ef_present_*): y = the field's slot; stream, frame store, frame counter and hscroll come from desc[y], the field goes
 // to dst + y * LINES * W, and the overlay is off. Otherwise y = stream and the field goes to the stream's field buffer.
-template <bool kNtsc, bool kPaced>
+// kOverlay (paced only): the overlay is on, with blend, progress and bitmap slot from fovl[y]; pr.bitmap is the base of the
+// bitmap slots, two per stream.
+template <bool kNtsc, bool kPaced, bool kOverlay = false>
 __global__ void __launch_bounds__(kK2Threads)
 ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr, const EfFieldDesc* __restrict__ desc,
-                    uint16_t* __restrict__ dst)
+                    uint16_t* __restrict__ dst, const EfFieldOverlay* __restrict__ fovl = nullptr)
 {
+    static_assert(kPaced || !kOverlay, "the per-field overlay is a paced variant");
     using G = Geo<kNtsc>;
     constexpr int CPL = G::W / 8;                                          // 16-byte chunks per line
     constexpr int LB = G::W * 2, LS = LB + 16;                             // bytes per line in the field / in shared memory
@@ -171,7 +174,14 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
     uint16_t* out0;
     if constexpr (kPaced) {
         const EfFieldDesc f = desc[blockIdx.y];
-        stream = (int)f.stream; fb_sel = f.fb; frame_counter = (int)f.frame_counter; p.hscroll = f.hscroll; p.blend = 0;
+        stream = (int)f.stream; fb_sel = f.fb; frame_counter = (int)f.frame_counter; p.hscroll = f.hscroll;
+        if constexpr (kOverlay) {
+            const EfFieldOverlay v = fovl[blockIdx.y];
+            p.blend = v.blend; p.progress = v.progress;
+            p.bitmap = pr.bitmap + ((size_t)stream * 2 + v.slot) * EF_OVERLAY_BYTES;
+        } else {
+            p.blend = 0;
+        }
         out0 = dst + (size_t)blockIdx.y * (G::LINES * G::W) + (size_t)line0 * G::W;
     } else {
         out0 = D.fields + (size_t)stream * D.field_stride + (size_t)line0 * G::W;
@@ -348,10 +358,12 @@ __device__ __forceinline__ int pace_hscroll(int ai) { return ai < 0 ? -c_easd[-a
 }  // namespace
 
 // pic >= 0: every stream with a picture `pic` pushes it (pts from pic_pts, modes[s] or 0); pic < 0: every stream idles until
-// it has emitted idle_n[s] fields
+// it has emitted idle_n[s] fields. ovl (NULL unless the context stages overlays): the staged overlay changes latch, into
+// ovl_next, when the call draws line 0 of their latch field
 __global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* __restrict__ next, EfPaceRun* __restrict__ run, EfPaceOut* __restrict__ out,
                                const int64_t* __restrict__ pic_pts, const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ base_pics,
-                               const uint8_t* __restrict__ modes, const uint32_t* __restrict__ idle_n, int pic, int max_pictures, int n_streams, int ntsc)
+                               const uint8_t* __restrict__ modes, const uint32_t* __restrict__ idle_n, int pic, int max_pictures, int n_streams, int ntsc,
+                               const EfOverlayState* __restrict__ ovl, EfOverlayState* __restrict__ ovl_next)
 {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_streams) return;
@@ -398,28 +410,81 @@ __global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* 
     r.n = o.n_fields = n > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)n;
     o.flags = (int)q.flags;
     next[s] = q; run[s] = r; out[s] = o;
+    if (ovl) {
+        // latch field G: F when the call starts at line 0, else F + 1. The changes latch if the call draws line 0 of G, i.e. it
+        // ends past (G, 0); otherwise they stay pending and latch at the same field with the next call's.
+        EfOverlayState v = ovl[s];
+        const uint32_t need = st[s].line == 0 ? 0u : 1u, adv = q.fc - F;
+        v.latch_fc = F + need;
+        if (v.pending && (adv > need || (adv == need && q.line > 0))) {
+            if (v.pending & 1u) v.slot ^= 1u;
+            if (v.pending & 2u) { v.blend = v.p_blend; v.blend_fc = v.latch_fc; }
+            if (v.pending & 4u) v.progress = v.p_progress;
+            v.pending = 0;
+        }
+        ovl_next[s] = v;
+    }
 }
 
-// once the fields fit: one descriptor per emitted field, at the stream's offset `first` in the output; commits the state
+// once the fields fit: one descriptor per emitted field, at the stream's offset `first` in the output; commits the state. ovl: also
+// the overlay each field is drawn with (fields before the latch field show the state latched before this call), and its commit
 __global__ void ef_pace_fill_kernel(EfPaceState* __restrict__ st, const EfPaceState* __restrict__ next, const EfPaceRun* __restrict__ run,
-                                    const uint64_t* __restrict__ first, EfFieldDesc* __restrict__ desc)
+                                    const uint64_t* __restrict__ first, EfFieldDesc* __restrict__ desc,
+                                    EfOverlayState* __restrict__ ovl, const EfOverlayState* __restrict__ ovl_next, EfFieldOverlay* __restrict__ fovl)
 {
     const int s = blockIdx.x;
     const EfPaceRun r = run[s];
     const uint64_t base = first[s];
     for (uint32_t j = threadIdx.x; j < r.n; j += blockDim.x)
         desc[base + j] = { (uint32_t)s, r.cur < 0 ? -2 : r.cur, r.fc0 + j, pace_hscroll(pace_animate(r.ai, j)) };
+    if (ovl) {
+        const EfOverlayState a = ovl[s], b = ovl_next[s];
+        const uint32_t k = b.latch_fc - r.fc0;                             // 0 or 1 fields drawn before the latch
+        for (uint32_t j = threadIdx.x; j < r.n; j += blockDim.x) {
+            const bool old = j < k;
+            fovl[base + j] = { ef_overlay_blend(old ? a.blend : b.blend, old ? a.blend_fc : b.blend_fc, r.fc0 + j), old ? a.progress : b.progress,
+                               old ? a.slot : b.slot, 0u };
+        }
+        __syncthreads();                                                   // every thread has read ovl[s]
+        if (threadIdx.x == 0) ovl[s] = b;
+    }
     if (threadIdx.x == 0) st[s] = next[s];
 }
 
-// the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y)
+// ef_present_overlay: stream first + i takes cmd[i]; a bitmap goes to the slot that is not latched. One CTA per stream.
+__global__ void ef_overlay_stage_kernel(EfOverlayState* __restrict__ ovl, uint8_t* __restrict__ slots, const EfOverlayCmd* __restrict__ cmd,
+                                        const uint8_t* __restrict__ bitmaps, int first)
+{
+    const int i = blockIdx.x, s = first + i;
+    const EfOverlayCmd c = cmd[i];
+    if (c.set & 1u) {
+        uint4* d = (uint4*)(slots + ((size_t)s * 2 + (ovl[s].slot ^ 1u)) * EF_OVERLAY_BYTES);
+        const uint4* src = (const uint4*)(bitmaps + (size_t)i * EF_OVERLAY_BYTES);
+        for (int k = (int)threadIdx.x; k < EF_OVERLAY_BYTES / 16; k += blockDim.x) d[k] = src[k];
+    }
+    __syncthreads();                                                       // every thread has read ovl[s].slot
+    if (threadIdx.x == 0) {
+        EfOverlayState v = ovl[s];
+        if (c.set & 2u) v.p_blend = c.blend;
+        if (c.set & 4u) v.p_progress = c.progress;
+        v.pending |= c.set;
+        ovl[s] = v;
+    }
+}
+
+// the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y). fovl != NULL: the overlay variant, with
+// the per-field overlay fovl and the bitmap slots `bitmaps`
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches)
+                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps)
 {
     const size_t per = (size_t)g.line_count * g.line_width;
     for (uint64_t f0 = 0; f0 < n_fields; f0 += 65535) {
         const dim3 grid((unsigned)(g.line_count + 15) / 16, (unsigned)(n_fields - f0 < 65535 ? n_fields - f0 : 65535));
-        if (g.ntsc) ef_composite_kernel<true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
+        if (fovl) {
+            const EfPresent pr = { 0, 0, 0, bitmaps };
+            if (g.ntsc) ef_composite_kernel<true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);
+            else ef_composite_kernel<false, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);
+        } else if (g.ntsc) ef_composite_kernel<true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
         else ef_composite_kernel<false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;

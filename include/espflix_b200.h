@@ -268,8 +268,8 @@ int ef_picture_pts(ef_ctx* ctx, int first, int count, int n_pictures, int64_t* p
  * due now, more than two fields late re-latches), then draws lines until the flip (video_isr, video.cpp:1122-1198): the first
  * line below vsync_start that is not an active line of a presented frame, once F >= _next_frame_time. animate() runs at the
  * flip and at every field end (video.cpp:1076-1088). A push emits the fields whose line active_bottom - 1 it draws, each as
- * K2 draws it from the current store (picture k - 1), the other store (picture k), the hscroll of its active lines and its
- * F. The overlay is not drawn (blend 0). Fields are line_count x line_width uint16 samples.
+ * K2 draws it from the current store (picture k - 1), the other store (picture k), the hscroll of its active lines, its F and
+ * the stream's overlay (ef_present_overlay; none until it is called). Fields are line_count x line_width uint16 samples.
  * ef_present_enable   needs ef_pts_enable and ef_video_init first (else EF_ESTATE) and fixes the standard: a later
  *                     ef_video_init that changes it returns EF_ESTATE. Each display starts at line 0 of field
  *                     frame_counter0[s] (NULL: 0) with no frame presented. Presentation starts with the next ef_index. From
@@ -297,6 +297,23 @@ typedef struct {
 int ef_present_enable(ef_ctx* ctx, const uint32_t* frame_counter0);
 int ef_present_picture(ef_ctx* ctx, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
 int ef_present_idle(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
+
+/* ef_present_overlay  composite() of every paced field (video.cpp:839-887, 1181-1194): the 80 x 16 bitmap and the progress bar
+ *                     on the 16 lines from active_bottom + 2, faded by the blend. Stages changes for streams [first, first +
+ *                     count): bitmaps = count x 1280 bytes (_video_composite[16][80] of each stream), blend and progress (int32
+ *                     each) and set[i] (bit 0 bitmap, bit 1 blend, bit 2 progress; set NULL = all three; a NULL array = that
+ *                     attribute is not set). Staged changes merge, the last write winning per attribute, and latch at line 0
+ *                     of the first field that starts at or after the position where the next ef_present_picture /
+ *                     ef_present_idle call begins: field F at (F, line 0), F + 1 otherwise. A call that does not draw that
+ *                     line (it emits no field past it) leaves them pending, as do a sizing call and EF_ENOMEM. Every field is
+ *                     drawn with the state latched at its line 0; a latched blend b > 0 counts down at every field end, so
+ *                     field G shows max(0, b - (G - G_latch)) (frame counters modulo 2^32); -1 and >= 32 are full strength,
+ *                     0 draws nothing. The bar fills step i = 0, 2, ..., 238 where i < progress. Every stream starts with
+ *                     blend 0; ef_reset keeps latched and staged overlays (video_reset() leaves them alone). Synchronous,
+ *                     host memory. EF_ESTATE before ef_present_enable; EF_EINVAL for a bad stream range or a blend below -1
+ *                     (the reference's fade arithmetic wraps there). */
+int ef_present_overlay(ef_ctx* ctx, int first, int count, const uint8_t* bitmaps, const int32_t* blend, const int32_t* progress,
+                       const uint8_t* set);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
