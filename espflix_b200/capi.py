@@ -83,6 +83,7 @@ _SIGNATURES = {
     "ef_present_picture": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_idle": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
+    "ef_restart_streams": (_I, [_VP, _I, _I, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -358,6 +359,13 @@ class Context:
                 for a, dt, shape in ((bm, np.uint8, (count, 1280)), (blend, np.int32, (count,)), (progress, np.int32, (count,)), (set, np.uint8, (count,)))]
         ptrs = [None if a is None or a.size == 0 else a.ctypes.data for a in keep]
         self._check(self.lib.ef_present_overlay(self._h, first, count, *ptrs))
+
+    # -- per-stream restart ----------------------------------------------------------------------
+    def restart_streams(self, ops, first=0):
+        """ef_restart_streams: ops[i] for stream first + i, between the current submit and the next one. 0 nothing, 1 the
+        reference's MpegDecoder::reset() + video_reset() (a new title or a seek), 2 video_pause(0) (resume after a pause)."""
+        ops = np.ascontiguousarray(ops, dtype=np.uint8).reshape(-1)
+        self._check(self.lib.ef_restart_streams(self._h, first, ops.size, ops.ctypes.data if ops.size else None))
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

@@ -145,6 +145,9 @@ __global__ void ef_sbc_probe_kernel(const uint8_t* __restrict__ es, const uint64
         const int total = sbc_frame_bits(es + off[s], len < 64 ? len : 64, bits, sf);   // decode_audio() hands sbc_decoder 64 bytes
         const int f = total < 0 ? total : 8 + 2 * total;  // the lazy byte loader has consumed header + scale factors + 16 * total bits
         if (f < 0 || ended[s] || len >= (uint64_t)f) { fs = f; probe = f > 0; }
+        // a probe that fails the sync byte still synthesises the decoder's last subband samples into its filter memory (nothing
+        // reaches the PCM): only a stream restarted after it decoded frames has any (a fresh stream's are zero)
+        if (f == -1 && st[s].synced && es[off[s]] != 0x9C) probe = 1;
     }
     plan[s] = make_int4(fs, probe, 0, 0);
 }
@@ -218,7 +221,7 @@ ef_sbc_matrix_kernel(const uint8_t* __restrict__ es, const uint64_t* __restrict_
             }
             // lane -> block lane/2, subbands 4 (lane & 1) .. + 3
             const int blk = lane >> 1, sb0 = (lane & 1) * 4;
-            if (total < 0 && !probe) {
+            if (total < 0 && (!probe || fs < 0)) {         // (a rejected probe: ef_sbc_probe_kernel)
 #pragma unroll
                 for (int k = 0; k < 4; k++) sb_s[w][blk][sb0 + k] = st[s].sb[blk][sb0 + k];
             } else {
@@ -343,12 +346,12 @@ __global__ void ef_audio_commit_kernel(EfAudioState* __restrict__ st, const uint
     const uint64_t used = p.x > 0 ? (uint64_t)p.z * (uint64_t)p.x : p.x < 0 ? len : 0;
     const int keep = (int)(len - used);                    // < EF_AUDIO_CARRY (ef_sbc_count_kernel, ef_sbc_probe_kernel)
     for (int i = lane; i < keep; i += 32) a.carry[i] = blob[blob_off[s] + used + i];
-    if (p.z) {
+    if (p.z || (p.y && p.x < 0)) {                         // frames decoded, or a rejected probe re-synthesised (ef_sbc_probe_kernel)
         for (int i = lane; i < 128; i += 32) a.sb[i >> 3][i & 7] = sb_last[(size_t)s * 128 + i];
         const int32_t* rows = vrows + (slot_base[s + 1] * 16 - 9) * 16;
         for (int i = lane; i < 9 * 16; i += 32) a.vhist[i >> 4][i & 15] = rows[i];
     }
-    if (lane == 0) { a.frame_size = p.x; a.carry_len = keep; }
+    if (lane == 0) { a.frame_size = p.x; a.carry_len = keep; if (p.z) a.synced = 1; }
 }
 
 // ---- TS -> audio bytes --------------------------------------------------------------------------------------

@@ -144,6 +144,25 @@ __global__ void ef_reset_seq_kernel(EfDev* Dp, const uint8_t* default_intra)
     D.n_pics[s] = 0; D.base_pics[s] = 0; D.n_seq[s] = 0;
 }
 
+// ef_restart_streams: one thread per stream of [first, first + count). op 1 = MpegDecoder::reset() + video_reset()
+// (player.cpp:439-453, video.cpp:1070-1074): get_pts() back to -1 (the carried _pts stays), the SBC ring and the learned
+// frame size cleared (the filter memory, the last subband samples and the modulator stay), the display latches a new
+// origin; ended[s] marks the stream for ef_audio_end_kernel, which shuts its demux gate. op 2 = video_pause(0)
+// (video.cpp:1060-1068): the new origin only. Null arrays belong to subsystems that were never enabled.
+__global__ void ef_restart_kernel(const uint8_t* __restrict__ ops, int first, int count, EfPaceState* __restrict__ pace, int64_t* __restrict__ pts_last,
+                                  EfAudioState* __restrict__ aud, uint8_t* __restrict__ ended)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const int s = first + k, op = ops[k];
+    if (ended) ended[s] = op == 1;
+    if (!op) return;
+    if (pace) pace[s].fc_origin = 0;
+    if (op != 1) return;
+    if (pts_last) pts_last[s] = -1;
+    if (aud) { aud[s].frame_size = 0; aud[s].carry_len = 0; }
+}
+
 }  // namespace
 
 struct ef_ctx {
@@ -246,6 +265,7 @@ struct ef_ctx {
     EfOverlayCmd* d_ovl_cmd = nullptr;            // [n_streams]
     EfFieldOverlay* d_fovl = nullptr;             // one per emitted field, beside d_desc
     uint64_t fovl_cap = 0;
+    uint8_t* d_restart_ops = nullptr;             // [n_streams] the ops of one ef_restart_streams call, allocated by its first call
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -494,6 +514,47 @@ int ef_reset(ef_ctx* c)
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
     c->pace_indexed = false;
+    return EF_OK;
+}
+
+// Per-stream restart between the current submit and the next one (queued or not). Synchronous: everything already
+// queued on the device (a resolve pass, a queued submit's demux) has finished before the state changes.
+int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first || (count && !ops))
+        return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    bool any_reset = false;
+    for (int i = 0; i < count; i++) {
+        if (ops[i] > 2) return fail(EF_EINVAL, "op %d of stream %d is not 0..2", ops[i], first + i);
+        any_reset |= ops[i] == 1;
+    }
+    if (c->paced && c->pace_indexed) {                    // the schedule of the current submit must be complete
+        int rc = pace_pictures(c);
+        if (rc != EF_OK) return rc;
+        if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_restart_streams while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
+    }
+    if (c->audio && c->aud_unconsumed) return fail(EF_ESTATE, "ef_restart_streams before ef_decode_audio consumed the current submit's audio");
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());
+    const bool audio = c->audio && any_reset;
+    if (!c->d_restart_ops) { int rc = dev_alloc(c, &c->d_restart_ops, (size_t)n); if (rc != EF_OK) return rc; }
+    CK(cudaMemcpy(c->d_restart_ops, ops, (size_t)count, cudaMemcpyHostToDevice));
+    if (audio) CK(cudaMemset(c->d_ended, 0, (size_t)n));
+    ef_restart_kernel<<<(count + 127) / 128, 128>>>(c->d_restart_ops, first, count, c->paced ? c->d_pace : nullptr, c->pts ? c->d_pts_last : nullptr,
+                                                     audio ? c->d_aud_state : nullptr, audio ? c->d_ended : nullptr);
+    CK(cudaGetLastError());
+    c->launches++;
+    if (audio) {                                          // the demux gates: the current one, and that of a submit queued behind it
+        const int p = c->pending;
+        ef_audio_end_kernel<<<(n + 255) / 256, 256>>>(c->d_ended, n, c->d_gate2[c->active], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
+                                                       p >= 0 && c->aud_ts[p]);
+        CK(cudaGetLastError());
+        c->launches++;
+    }
+    CK(cudaDeviceSynchronize());
     return EF_OK;
 }
 
@@ -1163,7 +1224,9 @@ static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAu
     for (int s = 0; s < n; s++) {
         const uint32_t frames = (uint32_t)hp[s].z;
         info[s].frame_size = hp[s].x; info[s].n_frames = frames; info[s].pcm_offset = poff[s];
-        slot[s + 1] = slot[s] + (frames ? 1 + (uint64_t)hp[s].y + frames : 0);   // history rows (+ the probe decode of frame 0) + frames
+        // history rows (+ the probe decode of frame 0) + frames; a rejected probe of a restarted stream (y set, size < 0) its two rows
+        const bool resynth = hp[s].y && hp[s].x < 0;
+        slot[s + 1] = slot[s] + (frames || resynth ? 1 + (uint64_t)hp[s].y + frames : 0);
         poff[s + 1] = poff[s] + (uint64_t)frames * 128;
     }
     const uint64_t n_pcm = poff[n];
@@ -1178,6 +1241,12 @@ static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAu
     CK(w.get(AudioScratch::SB_LAST, (size_t)n * 128 * 4, (void**)&sb_last));
     CK(cudaMemcpyAsync(d_slot, slot.data(), slot.size() * 8, cudaMemcpyHostToDevice, cs));
     CK(cudaMemcpyAsync(d_poff, poff.data(), poff.size() * 8, cudaMemcpyHostToDevice, cs));
+    if (slot[n] && !n_pcm) {                                 // only rejected probes of restarted streams: their filter memory moves on
+        CK(w.get(AudioScratch::VROWS, slot[n] * 16 * 16 * 4, (void**)&vrows));
+        ef_sbc_matrix_kernel<<<(unsigned)((slot[n] + 3) / 4), 128, 0, cs>>>(blob, blob_off, plan, st, d_slot, n, vrows, sb_last);
+        CK(cudaGetLastError());
+        *launches += 1;
+    }
     if (n_pcm) {
         CK(w.get(AudioScratch::VROWS, slot[n] * 16 * 16 * 4, (void**)&vrows));
         CK(w.get(AudioScratch::PCM, n_pcm * 2, (void**)&d_pcm));

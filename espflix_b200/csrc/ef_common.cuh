@@ -166,7 +166,8 @@ struct __align__(16) EfAudioState {
     int32_t frame_size;      // 0 not learned yet, > 0 learned by the probe, -1 / -2 first frame rejected / outside the domain
     int32_t carry_len;       // bytes held back: [0, EF_AUDIO_CARRY)
     int32_t i0, i1, i2;      // delta-sigma modulator of pdm_second_order()
-    int32_t pad[3];
+    int32_t synced;          // a frame was decoded: a probe that fails the sync byte re-synthesises sb (sbc_decoder.cpp:343-372)
+    int32_t pad[2];
     int32_t sb[16][8];       // subband samples of the last accepted frame (a rejected frame re-synthesises them)
     int32_t vhist[9][16];    // V rows of the last 9 blocks (the window reaches 9 blocks back)
     uint8_t carry[EF_AUDIO_CARRY];

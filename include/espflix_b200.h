@@ -47,6 +47,8 @@
  *                                 get_pts() player.cpp:653-656, for every stream of a TS submit
  *   ef_present_enable / _picture / _idle  push_video(frame, front, pts, mode) video.cpp:1023-1057 against the frame flip
  *                                 of video_isr video.cpp:1122-1198: every stream's paced composite fields, in HBM
+ *   ef_restart_streams            MpegDecoder::reset() + video_reset() (player.cpp:439, video.cpp:1070) or video_pause(0)
+ *                                 (video.cpp:1060) for chosen streams of the batch
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -314,6 +316,22 @@ int ef_present_idle(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64
  *                     (the reference's fade arithmetic wraps there). */
 int ef_present_overlay(ef_ctx* ctx, int first, int count, const uint8_t* bitmaps, const int32_t* blend, const int32_t* progress,
                        const uint8_t* set);
+
+/* ---- per-stream restart: what the reference's player does on play / skip / fast_forward / rewind / load_poster / play_pause --
+ * ef_restart_streams  ops[i] for stream first + i: 0 = nothing; 1 = MpegDecoder::reset() with its video_reset() (player.cpp:439-453,
+ *                     video.cpp:1070-1074); 2 = video_pause(0) (video.cpp:1060-1068). The restart falls between the current submit
+ *                     and the next one, whether that one is already queued or not. Op 1: get_pts() reads -1 until the next picture
+ *                     (the carried _pts stays, so a program whose first video PES has no PTS takes the old one); the audio demux
+ *                     gate shuts (the next submit's audio bytes before its first PES start are dropped, also for a TS submit
+ *                     already queued); the SBC bytes held back and the learned frame size are dropped (the next frame is probed
+ *                     and decoded twice) while the filter memory, the last subband samples and the delta-sigma modulator
+ *                     carry on; the display latches a new origin at the next push. Ops 1 and 2 both clear the display origin;
+ *                     frame stores, sequence state, display position, current store, scroll and overlay stay. Streams with op 0
+ *                     and all other streams do not change; subsystems never enabled are not touched. Synchronous, host memory.
+ *                     EF_EINVAL for a bad stream range or an op above 2; EF_ESTATE (as ef_index) on a presenting context while
+ *                     picture indices of the current submit are unpresented, or on an audio context while the current TS
+ *                     submit's audio has not been through ef_decode_audio. */
+int ef_restart_streams(ef_ctx* ctx, int first, int count, const uint8_t* ops);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
