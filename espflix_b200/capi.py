@@ -77,6 +77,8 @@ _SIGNATURES = {
     "ef_audio_decode": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_audio_enable": (_I, [_VP]),
     "ef_decode_audio": (_I, [_VP, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_decode_audio_async": (_I, [_VP, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_audio_wait": (_I, [_VP]),
     "ef_pts_enable": (_I, [_VP]),
     "ef_picture_pts": (_I, [_VP, _I, _I, _I, _VP, _VP]),
     "ef_present_enable": (_I, [_VP, _VP]),
@@ -304,6 +306,43 @@ class Context:
             out.append({"frame_size": int(i["frame_size"]), "n_frames": int(i["n_frames"]), "pcm": pcm_out[a:a + k].copy(),
                         "pdm": None if pdm_out is None else pdm_out[2 * a:2 * (a + k)].copy()})
         return out
+
+    def decode_audio_async(self, pcm, pdm=None, info=None, end=None, stream=0):
+        """ef_decode_audio_async: decode_audio() into CUDA tensors, returning once the work is enqueued on `stream` (a
+        torch.cuda.Stream or a raw handle). pcm: int16 tensor of pcm_cap samples; pdm: None or uint16 tensor of 2 * pcm_cap
+        words; info: None or an int32 tensor [n_streams, 4] that receives the ef_audio_info rows (see audio_info()).
+        Returns info. audio_wait() says whether the call fit."""
+        import torch
+        n = self.n_streams
+        if info is None:
+            info = torch.zeros((n, 4), dtype=torch.int32, device=pcm.device)
+        for t, dt, what in ((pcm, torch.int16, "pcm"), (pdm, torch.uint16, "pdm"), (info, torch.int32, "info")):
+            if t is not None and not (t.is_cuda and t.dtype == dt and t.is_contiguous()):
+                raise TypeError("%s must be a contiguous CUDA %s tensor" % (what, dt))
+        assert info.numel() == 4 * n
+        if end is True:
+            end = np.ones(n, dtype=np.uint8)
+        elif end is not None:
+            end = np.ascontiguousarray(end, dtype=np.uint8)
+            assert end.size == n
+        cap = pcm.numel() if pdm is None else min(pcm.numel(), pdm.numel() // 2)
+        st = getattr(stream, "cuda_stream", stream)
+        self._check(self.lib.ef_decode_audio_async(self._h, _ptr(end), info.data_ptr(), pcm.data_ptr(), cap,
+                                                   None if pdm is None else pdm.data_ptr(), st))
+        return info
+
+    def audio_wait(self):
+        """ef_audio_wait: waits for the last decode_audio_async -> EF_OK, or EF_ENOMEM when its samples exceeded pcm_cap
+        (nothing decoded, no state changed)"""
+        rc = self.lib.ef_audio_wait(self._h)
+        if rc not in (EF_OK, EF_ENOMEM):
+            self._check(rc)
+        return rc
+
+    @staticmethod
+    def audio_info(info):
+        """the int32 [n_streams, 4] info tensor of decode_audio_async -> numpy array of the ef_audio_info rows"""
+        return np.ascontiguousarray(info.cpu().numpy()).view(_AUDIO_INFO).reshape(-1)
 
     # -- presentation timestamps -----------------------------------------------------------------
     def enable_pts(self):

@@ -12,6 +12,8 @@
 //   ef_sbc_probe_kernel   one thread per stream: the frame size decode_audio() learns from the first 64 bytes
 //   ef_sbc_matrix_kernel  one warp per frame: header, scale factors, bit allocation (12.6.3), 128 samples cut out of
 //                         the bit field at computed offsets (no serial bit reader), IQUANT, matrixing -> V[16][16]
+//   ef_audio_size_kernel  one CTA: slot and PCM offsets, info[] and the capacity verdict, so that a call needs no read-back
+//                         to size itself (ef_decode_audio_async); the kernels after it read their totals from HBM
 //   ef_sbc_window_kernel  one thread per PCM sample: 10 taps over the V rows of this and the nine blocks before
 //   ef_pdm_kernel         one thread per stream: the second-order delta-sigma modulator is a serial non-linear
 //                         recurrence (32 one-bit samples per PCM sample); streams run side by side
@@ -27,6 +29,7 @@
 // 8 subbands, 16 blocks (write_pcm_16(mono,128,1) passes 128 samples whatever the header says); a frame size that
 // does not divide the reference's 4 KB ring makes it read past the ring on the straddling frame (undefined there;
 // here the stream is simply linear).
+#include "../../include/espflix_b200.h"
 #include "ef_common.cuh"
 #include "ef_sbc_tables.h"
 
@@ -182,6 +185,59 @@ __global__ void ef_sbc_count_kernel(const uint8_t* __restrict__ es, const uint64
     if (lane == 0) plan[s].z = (int)n;
 }
 
+// One CTA of 1,024 threads: the slot and PCM offsets of every stream from plan[] (exclusive prefix sums, tile by tile
+// with the carry of the tiles before), the call's info[] rows and the capacity verdict. A call whose samples exceed
+// pcm_cap publishes zero offsets throughout: the matrix, window and PDM kernels then find nothing to do (their grids
+// come from a bound, not from these totals), and the gated commit and end kernels leave every stream as it was.
+// info[] keeps the counts either way.
+__global__ void __launch_bounds__(1024)
+ef_audio_size_kernel(const int4* __restrict__ plan, int n_streams, uint64_t pcm_cap, uint64_t* __restrict__ slot_base, uint64_t* __restrict__ pcm_off,
+                     ef_audio_info* __restrict__ info, int* __restrict__ verdict)
+{
+    __shared__ uint64_t warp_sum[2][32];
+    __shared__ uint64_t carry[2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry[0] = carry[1] = 0;
+    __syncthreads();
+    for (int base = 0; base < n_streams; base += 1024) {
+        const int k = base + threadIdx.x;
+        const int4 p = k < n_streams ? plan[k] : make_int4(0, 0, 0, 0);
+        const uint32_t frames = (uint32_t)p.z;
+        // history rows (+ the probe decode of frame 0) + frames; a rejected probe of a restarted stream (y set, size < 0) its two rows
+        const uint64_t v0 = frames || (p.y && p.x < 0) ? 1 + (uint64_t)p.y + frames : 0, v1 = (uint64_t)frames * 128;
+        uint64_t x0 = v0, x1 = v1;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y0 = __shfl_up_sync(0xFFFFFFFFu, x0, d), y1 = __shfl_up_sync(0xFFFFFFFFu, x1, d);
+            if (lane >= d) { x0 += y0; x1 += y1; }
+        }
+        if (lane == 31) { warp_sum[0][warp] = x0; warp_sum[1][warp] = x1; }
+        __syncthreads();
+        if (warp < 2) {                                    // warp 0 scans the slot sums, warp 1 the sample sums
+            const uint64_t t = warp_sum[warp][lane];
+            uint64_t z = t;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
+            warp_sum[warp][lane] = z - t;
+        }
+        __syncthreads();
+        const uint64_t e0 = carry[0] + warp_sum[0][warp] + x0 - v0, e1 = carry[1] + warp_sum[1][warp] + x1 - v1;
+        if (k < n_streams) {
+            slot_base[k] = e0;
+            pcm_off[k] = e1;
+            info[k].frame_size = p.x; info[k].n_frames = frames; info[k].pcm_offset = e1;
+        }
+        __syncthreads();
+        if (threadIdx.x == 1023) { carry[0] = e0 + v0; carry[1] = e1 + v1; }
+        __syncthreads();
+    }
+    const bool over = carry[1] > pcm_cap;
+    if (over)                                              // the same thread wrote these entries above
+        for (int i = threadIdx.x; i <= n_streams; i += 1024) { slot_base[i] = 0; pcm_off[i] = 0; }
+    else if (threadIdx.x == 0) { slot_base[n_streams] = carry[0]; pcm_off[n_streams] = carry[1]; }
+    if (threadIdx.x == 0) *verdict = over;
+}
+
 // One warp per frame slot. Slots of stream s (slot_base[s] ..): 0 = the V rows of its last 9 blocks before this call
 // (rows 7..15), then, when plan[s].y, the probe decode of frame 0 (video.cpp:971), then frame f of this call at slot
 // f + 1 + plan[s].y. V rows go to vrows[(16 slot + blk) * 16 + i]. The last slot of a stream also leaves its subband
@@ -329,12 +385,15 @@ __global__ void ef_pdm_kernel(const int16_t* __restrict__ pcm, const uint64_t* _
 // one warp per stream, after the call's kernels: hold back the bytes of the first frame not decoded (all bytes while
 // the frame size is unknown, none once the first frame was rejected), keep the last accepted frame's subband samples
 // and the last 9 V rows. An ended stream starts over from zero (MpegDecoder::reset(), player.cpp:439).
+// kGated: the call may have exceeded its capacity (ef_audio_size_kernel's verdict); then nothing changes.
+template <bool kGated>
 __global__ void ef_audio_commit_kernel(EfAudioState* __restrict__ st, const uint8_t* __restrict__ blob, const uint64_t* __restrict__ blob_off,
                                        const int4* __restrict__ plan, const uint64_t* __restrict__ slot_base, const int32_t* __restrict__ vrows,
-                                       const int32_t* __restrict__ sb_last, const uint8_t* __restrict__ ended, int n_streams)
+                                       const int32_t* __restrict__ sb_last, const uint8_t* __restrict__ ended, int n_streams, const int* __restrict__ verdict)
 {
     const int s = (int)(((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
     if (s >= n_streams) return;
+    if (kGated && *verdict) return;
     EfAudioState& a = st[s];
     if (ended[s]) {
         int32_t* w = (int32_t*)&a;
@@ -423,14 +482,35 @@ __global__ void ef_audio_ts_copy_kernel(const uint8_t* __restrict__ ts, const ui
 // ef_decode_audio ended these streams: their demux gate shuts (MpegDecoder::reset()). A TS submit already demuxed
 // behind the current one saw the gate open: its bytes before its first PES start are dropped (skip) and a gate it only
 // inherited shuts. An ES submit queued there copied the gate: it shuts too.
+template <bool kGated>
 __global__ void ef_audio_end_kernel(const uint8_t* __restrict__ ended, int n_streams, uint8_t* __restrict__ gate_cur, uint8_t* __restrict__ gate_next,
-                                    uint8_t* __restrict__ skip_next, int next_is_ts)
+                                    uint8_t* __restrict__ skip_next, int next_is_ts, const int* __restrict__ verdict)
 {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_streams || !ended[s]) return;
+    if (kGated && *verdict) return;
     gate_cur[s] = 0;
     if (!gate_next) return;
     if (!next_is_ts) gate_next[s] = 0;
     else { if (gate_next[s] == 2) gate_next[s] = 0; skip_next[s] = 1; }
 }
 
+// The commit and end kernels of a call, gated on `verdict` when it is not NULL (a call that checks its capacity on the
+// device); the ungated instantiations are what the synchronous call has always run.
+cudaError_t ef_launch_audio_commit(EfAudioState* st, const uint8_t* blob, const uint64_t* blob_off, const int4* plan, const uint64_t* slot_base,
+                                   const int32_t* vrows, const int32_t* sb_last, const uint8_t* ended, int n_streams, const int* verdict, cudaStream_t cs)
+{
+    const unsigned grid = (unsigned)(((size_t)n_streams * 32 + 255) / 256);
+    if (verdict) ef_audio_commit_kernel<true><<<grid, 256, 0, cs>>>(st, blob, blob_off, plan, slot_base, vrows, sb_last, ended, n_streams, verdict);
+    else ef_audio_commit_kernel<false><<<grid, 256, 0, cs>>>(st, blob, blob_off, plan, slot_base, vrows, sb_last, ended, n_streams, nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_launch_audio_end(const uint8_t* ended, int n_streams, uint8_t* gate_cur, uint8_t* gate_next, uint8_t* skip_next, int next_is_ts,
+                                const int* verdict, cudaStream_t cs)
+{
+    const unsigned grid = (unsigned)((n_streams + 255) / 256);
+    if (verdict) ef_audio_end_kernel<true><<<grid, 256, 0, cs>>>(ended, n_streams, gate_cur, gate_next, skip_next, next_is_ts, verdict);
+    else ef_audio_end_kernel<false><<<grid, 256, 0, cs>>>(ended, n_streams, gate_cur, gate_next, skip_next, next_is_ts, nullptr);
+    return cudaGetLastError();
+}

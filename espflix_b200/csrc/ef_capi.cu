@@ -40,13 +40,15 @@ __global__ void ef_sbc_count_kernel(const uint8_t* es, const uint64_t* off, cons
 __global__ void ef_sbc_matrix_kernel(const uint8_t* es, const uint64_t* off, const int4* plan, const EfAudioState* st, const uint64_t* slot_base, int n_streams, int32_t* vrows, int32_t* sb_last);
 __global__ void ef_sbc_window_kernel(const int32_t* vrows, const uint64_t* slot_base, const uint64_t* pcm_off, int n_streams, int16_t* pcm);
 __global__ void ef_pdm_kernel(const int16_t* pcm, const uint64_t* pcm_off, int n_streams, EfAudioState* st, uint16_t* pdm);
-__global__ void ef_audio_commit_kernel(EfAudioState* st, const uint8_t* blob, const uint64_t* blob_off, const int4* plan, const uint64_t* slot_base, const int32_t* vrows,
-                                       const int32_t* sb_last, const uint8_t* ended, int n_streams);
+__global__ void ef_audio_size_kernel(const int4* plan, int n_streams, uint64_t pcm_cap, uint64_t* slot_base, uint64_t* pcm_off, ef_audio_info* info, int* verdict);
+cudaError_t ef_launch_audio_commit(EfAudioState* st, const uint8_t* blob, const uint64_t* blob_off, const int4* plan, const uint64_t* slot_base,
+                                   const int32_t* vrows, const int32_t* sb_last, const uint8_t* ended, int n_streams, const int* verdict, cudaStream_t cs);
+cudaError_t ef_launch_audio_end(const uint8_t* ended, int n_streams, uint8_t* gate_cur, uint8_t* gate_next, uint8_t* skip_next, int next_is_ts,
+                                const int* verdict, cudaStream_t cs);
 __global__ void ef_audio_ts_packet_kernel(const uint8_t* ts, uint64_t n_packets, uint8_t* start, uint8_t* kind);
 __global__ void ef_audio_ts_scan_kernel(const uint64_t* ts_off, int n_files, const uint8_t* start, const uint8_t* kind, const uint8_t* gate_in, uint8_t* gate_out,
                                         uint32_t* lead, uint8_t* skip, uint32_t* out_pos, uint64_t* es_len);
 __global__ void ef_audio_ts_copy_kernel(const uint8_t* ts, const uint64_t* ts_off, int n_files, uint64_t n_packets, const uint8_t* start, const uint32_t* out_pos, const uint64_t* es_off, uint8_t* es);
-__global__ void ef_audio_end_kernel(const uint8_t* ended, int n_streams, uint8_t* gate_cur, uint8_t* gate_next, uint8_t* skip_next, int next_is_ts);
 cudaError_t ef_audio_upload_constants();
 cudaError_t ef_launch_parse(const EfDev& dev, int pic0, int n_pics, int sm_count, size_t max_slices, cudaStream_t stream);
 cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t n_slots, cudaStream_t stream);
@@ -228,6 +230,12 @@ struct ef_ctx {
     uint8_t* d_ended = nullptr;
     uint8_t* h_ended = nullptr;                   // pinned
     struct AudioScratch* aud_scratch = nullptr;
+    // ef_decode_audio_async: whether a call is outstanding, whether it took the current submit's audio, and its verdict
+    // (pinned, written by the call's stream). ev_aud_done follows every audio call; ev_ended_free the upload of h_ended.
+    bool aud_async = false, aud_async_new = false;
+    int aud_async_rc = EF_OK;
+    int* h_aud_verdict = nullptr;                 // pinned
+    cudaEvent_t ev_aud_done = nullptr, ev_ended_free = nullptr;
     // presentation timestamps (ef_pts_enable): every TS submit also lists the video PES starts with a valid PTS of every
     // stream in its ES buffer's list; ef_index resolves the PTS of every picture from it
     bool pts = false;
@@ -250,6 +258,8 @@ struct ef_ctx {
     EfPaceRun* d_pace_run = nullptr;              // [n_streams]
     EfPaceOut* d_pace_out = nullptr;              // [n_streams]
     EfPaceOut* h_pace_out = nullptr;              // pinned
+    uint32_t* h_pace_npics = nullptr;             // pinned: the picture indices of the submit, copied by ef_index
+    cudaEvent_t ev_indexed = nullptr;             // ef_index has finished (its stream)
     uint64_t* d_pace_first = nullptr;             // [n_streams] output offset of every stream's fields
     uint64_t* h_pace_first = nullptr;             // pinned
     uint32_t* d_pace_arg = nullptr;               // [n_streams] modes (bytes) or idle field counts
@@ -271,7 +281,7 @@ struct ef_ctx {
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
 // use a scratch of their own, a context keeps one.
 struct AudioScratch {
-    enum { PLAN, SB_LAST, SLOT, POFF, VROWS, PCM, PDM, N };
+    enum { PLAN, SB_LAST, SLOT, POFF, VROWS, PCM, PDM, INFO, VERDICT, N };
     void* p[N] = {};
     size_t cap[N] = {};
     ~AudioScratch() { for (void* q : p) if (q) cudaFree(q); }
@@ -287,6 +297,7 @@ struct AudioScratch {
         *out = p[k];
         return cudaSuccess;
     }
+    bool fits(int k, size_t bytes) const { return cap[k] >= bytes; }
 };
 
 namespace {
@@ -335,14 +346,13 @@ int resolve_fb(ef_ctx* c, int stream_index, int fb, int* out)
     return EF_OK;
 }
 
-// picture indices of the submit the last ef_index made current (synchronous the first time per submit)
+// picture indices of the submit the last ef_index made current (waits for that ef_index the first time per submit; work
+// on other streams, such as an audio decode, runs on)
 int pace_pictures(ef_ctx* c)
 {
     if (c->pace_npics >= 0) return EF_OK;
-    uint32_t mp = 0;
-    CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(&mp, c->h.info, 4, cudaMemcpyDeviceToHost));
-    c->pace_npics = (int)mp;
+    CK(cudaEventSynchronize(c->ev_indexed));
+    c->pace_npics = (int)*c->h_pace_npics;
     return EF_OK;
 }
 
@@ -401,6 +411,9 @@ int ef_create(ef_ctx** out, const ef_config* cfg)
     CK(cudaEventCreateWithFlags(&c->ev_user, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&c->ev_export, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&c->ev_frames_read, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&c->ev_indexed, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&c->ev_aud_done, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&c->ev_ended_free, cudaEventDisableTiming));
     CK(cudaStreamCreateWithFlags(&c->up_stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&c->down_stream, cudaStreamNonBlocking));
     A(h.frames, (size_t)n * 2 * EF_FRAME + 1024);
@@ -475,6 +488,10 @@ void ef_destroy(ef_ctx* c)
     if (c->ev_user) cudaEventDestroy(c->ev_user);
     if (c->ev_export) cudaEventDestroy(c->ev_export);
     if (c->ev_frames_read) cudaEventDestroy(c->ev_frames_read);
+    if (c->ev_indexed) cudaEventDestroy(c->ev_indexed);
+    if (c->ev_aud_done) cudaEventDestroy(c->ev_aud_done);
+    if (c->ev_ended_free) cudaEventDestroy(c->ev_ended_free);
+    if (c->h_aud_verdict) cudaFreeHost(c->h_aud_verdict);
     if (c->up_stream) cudaStreamDestroy(c->up_stream);
     if (c->down_stream) cudaStreamDestroy(c->down_stream);
     delete c;
@@ -487,11 +504,24 @@ static int wait_frames_read(ef_ctx* c)
     return EF_OK;
 }
 
+// An outstanding ef_decode_audio_async: wait for it and settle the bookkeeping only the host keeps (whether the current
+// submit's audio has been consumed). Every call whose outcome depends on that resolves first.
+static int audio_resolve(ef_ctx* c)
+{
+    if (!c->aud_async) return EF_OK;
+    CK(cudaEventSynchronize(c->ev_aud_done));
+    c->aud_async = false;
+    c->aud_async_rc = *c->h_aud_verdict ? EF_ENOMEM : EF_OK;
+    if (c->aud_async_rc == EF_OK && c->aud_async_new) c->aud_unconsumed = false;
+    return EF_OK;
+}
+
 int ef_reset(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     { int rcw = wait_frames_read(c); if (rcw != EF_OK) return rcw; }
+    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
     CK(cudaMemset(c->h.frames, 0, (size_t)c->cfg.n_streams * 2 * EF_FRAME + 1024));     // Frame::init zero-fills (player.cpp:25)
     ef_reset_seq_kernel<<<(c->cfg.n_streams + 127) / 128, 128>>>(c->d, c->d_default_intra);
     CK(cudaGetLastError());
@@ -536,6 +566,7 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
         if (rc != EF_OK) return rc;
         if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_restart_streams while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
     }
+    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
     if (c->audio && c->aud_unconsumed) return fail(EF_ESTATE, "ef_restart_streams before ef_decode_audio consumed the current submit's audio");
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
@@ -549,9 +580,8 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
     c->launches++;
     if (audio) {                                          // the demux gates: the current one, and that of a submit queued behind it
         const int p = c->pending;
-        ef_audio_end_kernel<<<(n + 255) / 256, 256>>>(c->d_ended, n, c->d_gate2[c->active], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
-                                                       p >= 0 && c->aud_ts[p]);
-        CK(cudaGetLastError());
+        CK(ef_launch_audio_end(c->d_ended, n, c->d_gate2[c->active], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
+                               p >= 0 && c->aud_ts[p], nullptr, 0));
         c->launches++;
     }
     CK(cudaDeviceSynchronize());
@@ -583,6 +613,8 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
         CK(cudaStreamWaitEvent(up, c->ev_user, 0));
     }
     CK(cudaStreamWaitEvent(up, c->ev_buf_free[b], 0));    // kernels of the submit that last used this buffer are done
+    if (c->audio) CK(cudaStreamWaitEvent(up, c->ev_aud_done, 0));   // and the last audio call: it reads this buffer's audio, or
+                                                                     // shuts demux gates the demux below reads
     uint8_t* d_es = c->d_es2[b];
     uint64_t* d_es_off = c->d_es_off2[b];
     if (!ts) {
@@ -672,6 +704,7 @@ int ef_index(ef_ctx* c, void* stream)
         if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_index while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
     }
     if (c->pending >= 0) {                       // a fresh submit: wait for its upload, make it the front buffer
+        { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
         if (c->audio && c->aud_unconsumed)       // the audio of a TS submit is delivered exactly once
             return fail(EF_ESTATE, "ef_index of a new submit before ef_decode_audio consumed the current submit's audio");
         CK(cudaStreamWaitEvent(st, c->ev_up_done[c->pending], 0));
@@ -699,6 +732,10 @@ int ef_index(ef_ctx* c, void* stream)
         c->pts_resolved = true;
     }
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));
+    if (c->paced) {                              // the picture indices the present calls need, without a device-wide wait
+        CK(cudaMemcpyAsync(c->h_pace_npics, c->h.info, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaEventRecord(c->ev_indexed, st));
+    }
     c->indexed = true;
     if (c->paced) { c->pace_indexed = true; c->pace_next = 0; c->pace_npics = -1; }
     return EF_OK;
@@ -1205,66 +1242,95 @@ static int audio_constants(int device)
 }
 
 // One decode call once its input is in HBM (blob + blob_off[n + 1]: every stream's held-back bytes followed by its new
-// bytes): probe and count, then - unless pcm is NULL (sizing: info[] only, no state changes) - SBC -> PCM (-> PDM) and
-// the update of the per-stream state. Synchronous on `cs`.
-static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w,
-                             ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, cudaStream_t cs, uint64_t* launches)
+// bytes), in two halves on `cs`, neither of which waits for the device:
+//   audio_plan  probe, count, and ef_audio_size_kernel: slot and PCM offsets, info[] (device) and the verdict against pcm_cap
+//   audio_run   SBC -> PCM (-> PDM) into pcm / pdm (device) and the update of the per-stream state
+// The grids of audio_run come from a bound on the call's samples (bound_pcm), not from its totals, which only the device
+// knows: a stream has at most 2 + frames slots (history, probe, frames), so slots <= 2 n + bound_pcm / 128. Blocks past
+// the totals return at once (the kernels read their totals from HBM); when the caller sizes pcm_cap to its call, as a
+// sizing call lets it, the bound is the need and few blocks are idle. The V-row scratch follows the same bound.
+static size_t audio_vrow_bytes(int n, uint64_t bound_pcm) { return (2 * (size_t)n + bound_pcm / 128) * 16 * 16 * 4; }
+
+static int audio_scratch(AudioScratch& w, int n, uint64_t bound_pcm)
 {
-    int4* plan = nullptr;
-    CK(w.get(AudioScratch::PLAN, (size_t)n * sizeof(int4), (void**)&plan));
+    void* q;
+    CK(w.get(AudioScratch::PLAN, (size_t)n * sizeof(int4), &q));
+    CK(w.get(AudioScratch::SLOT, ((size_t)n + 1) * 8, &q));
+    CK(w.get(AudioScratch::POFF, ((size_t)n + 1) * 8, &q));
+    CK(w.get(AudioScratch::SB_LAST, (size_t)n * 128 * 4, &q));
+    CK(w.get(AudioScratch::INFO, (size_t)n * sizeof(ef_audio_info), &q));
+    CK(w.get(AudioScratch::VERDICT, sizeof(int), &q));
+    CK(w.get(AudioScratch::VROWS, audio_vrow_bytes(n, bound_pcm), &q));
+    return EF_OK;
+}
+
+static int audio_plan(const uint8_t* blob, const uint64_t* blob_off, const EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w,
+                      uint64_t pcm_cap, ef_audio_info* d_info, cudaStream_t cs, uint64_t* launches)
+{
+    int4* plan = (int4*)w.p[AudioScratch::PLAN];
     ef_sbc_probe_kernel<<<(n + 127) / 128, 128, 0, cs>>>(blob, blob_off, st, ended, n, plan);
     CK(cudaGetLastError());
     ef_sbc_count_kernel<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, cs>>>(blob, blob_off, ended, n, plan);
     CK(cudaGetLastError());
-    *launches += 2;
-    std::vector<int4> hp((size_t)n);
-    CK(cudaMemcpyAsync(hp.data(), plan, (size_t)n * sizeof(int4), cudaMemcpyDeviceToHost, cs));
-    CK(cudaStreamSynchronize(cs));
-    std::vector<uint64_t> slot((size_t)n + 1, 0), poff((size_t)n + 1, 0);
-    for (int s = 0; s < n; s++) {
-        const uint32_t frames = (uint32_t)hp[s].z;
-        info[s].frame_size = hp[s].x; info[s].n_frames = frames; info[s].pcm_offset = poff[s];
-        // history rows (+ the probe decode of frame 0) + frames; a rejected probe of a restarted stream (y set, size < 0) its two rows
-        const bool resynth = hp[s].y && hp[s].x < 0;
-        slot[s + 1] = slot[s] + (frames || resynth ? 1 + (uint64_t)hp[s].y + frames : 0);
-        poff[s + 1] = poff[s] + (uint64_t)frames * 128;
-    }
-    const uint64_t n_pcm = poff[n];
-    if (!pcm) return EF_OK;                                  // sizing call
-    if (n_pcm > pcm_cap) return fail(EF_ENOMEM, "%llu PCM samples, capacity %llu", (unsigned long long)n_pcm, (unsigned long long)pcm_cap);
-    uint64_t *d_slot = nullptr, *d_poff = nullptr;
-    int32_t *sb_last = nullptr, *vrows = nullptr;
-    int16_t* d_pcm = nullptr;
-    uint16_t* d_pdm = nullptr;
-    CK(w.get(AudioScratch::SLOT, slot.size() * 8, (void**)&d_slot));
-    CK(w.get(AudioScratch::POFF, poff.size() * 8, (void**)&d_poff));
-    CK(w.get(AudioScratch::SB_LAST, (size_t)n * 128 * 4, (void**)&sb_last));
-    CK(cudaMemcpyAsync(d_slot, slot.data(), slot.size() * 8, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(d_poff, poff.data(), poff.size() * 8, cudaMemcpyHostToDevice, cs));
-    if (slot[n] && !n_pcm) {                                 // only rejected probes of restarted streams: their filter memory moves on
-        CK(w.get(AudioScratch::VROWS, slot[n] * 16 * 16 * 4, (void**)&vrows));
-        ef_sbc_matrix_kernel<<<(unsigned)((slot[n] + 3) / 4), 128, 0, cs>>>(blob, blob_off, plan, st, d_slot, n, vrows, sb_last);
+    ef_audio_size_kernel<<<1, 1024, 0, cs>>>(plan, n, pcm_cap, (uint64_t*)w.p[AudioScratch::SLOT], (uint64_t*)w.p[AudioScratch::POFF], d_info,
+                                             (int*)w.p[AudioScratch::VERDICT]);
+    CK(cudaGetLastError());
+    *launches += 3;
+    return EF_OK;
+}
+
+// gated: the commit is skipped on the device when the call exceeded its capacity (the caller has not checked it)
+static int audio_run(const uint8_t* blob, const uint64_t* blob_off, EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w, uint64_t bound_pcm,
+                     int16_t* pcm, uint16_t* pdm, bool gated, cudaStream_t cs, uint64_t* launches)
+{
+    const int4* plan = (const int4*)w.p[AudioScratch::PLAN];
+    const uint64_t* d_slot = (const uint64_t*)w.p[AudioScratch::SLOT];
+    const uint64_t* d_poff = (const uint64_t*)w.p[AudioScratch::POFF];
+    int32_t* sb_last = (int32_t*)w.p[AudioScratch::SB_LAST];
+    int32_t* vrows = (int32_t*)w.p[AudioScratch::VROWS];
+    const uint64_t slots = 2 * (uint64_t)n + bound_pcm / 128;
+    ef_sbc_matrix_kernel<<<(unsigned)((slots + 3) / 4), 128, 0, cs>>>(blob, blob_off, plan, st, d_slot, n, vrows, sb_last);
+    CK(cudaGetLastError());
+    *launches += 1;
+    if (bound_pcm) {
+        ef_sbc_window_kernel<<<(unsigned)((bound_pcm + 255) / 256), 256, 0, cs>>>(vrows, d_slot, d_poff, n, pcm);
         CK(cudaGetLastError());
         *launches += 1;
-    }
-    if (n_pcm) {
-        CK(w.get(AudioScratch::VROWS, slot[n] * 16 * 16 * 4, (void**)&vrows));
-        CK(w.get(AudioScratch::PCM, n_pcm * 2, (void**)&d_pcm));
-        ef_sbc_matrix_kernel<<<(unsigned)((slot[n] + 3) / 4), 128, 0, cs>>>(blob, blob_off, plan, st, d_slot, n, vrows, sb_last);
-        CK(cudaGetLastError());
-        ef_sbc_window_kernel<<<(unsigned)((n_pcm + 255) / 256), 256, 0, cs>>>(vrows, d_slot, d_poff, n, d_pcm);
-        CK(cudaGetLastError());
-        *launches += 2;
         if (pdm) {
-            CK(w.get(AudioScratch::PDM, n_pcm * 4, (void**)&d_pdm));
-            ef_pdm_kernel<<<(n + 31) / 32, 32, 0, cs>>>(d_pcm, d_poff, n, st, d_pdm);
+            ef_pdm_kernel<<<(n + 31) / 32, 32, 0, cs>>>(pcm, d_poff, n, st, pdm);
             CK(cudaGetLastError());
             *launches += 1;
         }
     }
-    ef_audio_commit_kernel<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, cs>>>(st, blob, blob_off, plan, d_slot, vrows, sb_last, ended, n);
-    CK(cudaGetLastError());
+    CK(ef_launch_audio_commit(st, blob, blob_off, plan, d_slot, vrows, sb_last, ended, n, gated ? (const int*)w.p[AudioScratch::VERDICT] : nullptr, cs));
     *launches += 1;
+    return EF_OK;
+}
+
+// The synchronous call: the plan, one read of info[], then - unless pcm is NULL (sizing: info[] only, no state changes) or
+// the call does not fit - the decode with the bound at the call's own samples, the copies to the host and a wait.
+// after(): launches that belong to the call once it decoded (the context's demux-gate kernel).
+extern "C++" {
+template <typename After>
+static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w,
+                             ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, cudaStream_t cs, uint64_t* launches, After after)
+{
+    int rc;
+    if ((rc = audio_scratch(w, n, 0)) != EF_OK) return rc;
+    ef_audio_info* d_info = (ef_audio_info*)w.p[AudioScratch::INFO];
+    if ((rc = audio_plan(blob, blob_off, st, ended, n, w, pcm ? pcm_cap : ~0ull, d_info, cs, launches)) != EF_OK) return rc;
+    CK(cudaMemcpyAsync(info, d_info, (size_t)n * sizeof(ef_audio_info), cudaMemcpyDeviceToHost, cs));
+    CK(cudaStreamSynchronize(cs));
+    const uint64_t n_pcm = info[n - 1].pcm_offset + (uint64_t)info[n - 1].n_frames * 128;
+    if (!pcm) return EF_OK;                                  // sizing call
+    if (n_pcm > pcm_cap) return fail(EF_ENOMEM, "%llu PCM samples, capacity %llu", (unsigned long long)n_pcm, (unsigned long long)pcm_cap);
+    int16_t* d_pcm = nullptr;
+    uint16_t* d_pdm = nullptr;
+    if ((rc = audio_scratch(w, n, n_pcm)) != EF_OK) return rc;
+    CK(w.get(AudioScratch::PCM, n_pcm * 2, (void**)&d_pcm));
+    if (pdm) CK(w.get(AudioScratch::PDM, n_pcm * 4, (void**)&d_pdm));
+    if ((rc = audio_run(blob, blob_off, st, ended, n, w, n_pcm, d_pcm, pdm ? d_pdm : nullptr, false, cs, launches)) != EF_OK) return rc;
+    if ((rc = after()) != EF_OK) return rc;
     if (n_pcm) {
         CK(cudaMemcpyAsync(pcm, d_pcm, n_pcm * 2, cudaMemcpyDeviceToHost, cs));
         if (pdm) CK(cudaMemcpyAsync(pdm, d_pdm, n_pcm * 4, cudaMemcpyDeviceToHost, cs));
@@ -1272,6 +1338,7 @@ static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAu
     CK(cudaStreamSynchronize(cs));
     return EF_OK;
 }
+}  // extern "C++"
 
 int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_files, uint8_t* es, uint64_t es_cap, uint64_t* es_off)
 {
@@ -1336,13 +1403,14 @@ int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_s
     AudioScratch w;
     uint64_t launches = 0;
     return audio_decode_blob((const uint8_t*)d_es.p, (const uint64_t*)d_off.p, (EfAudioState*)d_st.p, (const uint8_t*)d_end.p, n_streams, w,
-                             info, pcm, pcm_cap, pdm, 0, &launches);
+                             info, pcm, pcm_cap, pdm, 0, &launches, [] { return EF_OK; });
 }
 
 int ef_audio_enable(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
+    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
     if (c->audio) return EF_OK;
     int rc = audio_constants(c->cfg.device);
     if (rc != EF_OK) return rc;
@@ -1373,20 +1441,20 @@ int ef_audio_enable(ef_ctx* c)
     return EF_OK;
 }
 
-int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream)
+// The front half of a context's audio call on `cs`: after the demux of the current submit (and of one queued behind it, whose
+// gate ef_audio_end_kernel may shut) and after the previous audio call (it shares the blob, the scratch and h_ended), the
+// end flags go up and every stream's held-back bytes and new bytes are assembled into the blob. Returns whether any ends.
+static int audio_assemble(ef_ctx* c, const uint8_t* end_of_stream, cudaStream_t cs, bool* any_end)
 {
-    DeviceScope scope_(c ? c->cfg.device : -1);
-    if (!c || !info) return fail(EF_EINVAL, "null argument");
-    if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio before ef_audio_enable");
-    int rc = audio_constants(c->cfg.device);
-    if (rc != EF_OK) return rc;
     const int n = c->cfg.n_streams, a = c->active, p = c->pending;
-    cudaStream_t cs = (cudaStream_t)stream;
-    bool any_end = false;
-    for (int s = 0; s < n; s++) { c->h_ended[s] = end_of_stream && end_of_stream[s] ? 1 : 0; any_end |= c->h_ended[s] != 0; }
+    CK(cudaEventSynchronize(c->ev_ended_free));              // the previous call's upload of h_ended has left it
+    *any_end = false;
+    for (int s = 0; s < n; s++) { c->h_ended[s] = end_of_stream && end_of_stream[s] ? 1 : 0; *any_end |= c->h_ended[s] != 0; }
     CK(cudaStreamWaitEvent(cs, c->ev_up_done[a], 0));        // the demux of the current submit has finished
     if (p >= 0) CK(cudaStreamWaitEvent(cs, c->ev_up_done[p], 0));   // and that of a submit queued behind it (ef_audio_end_kernel)
+    CK(cudaStreamWaitEvent(cs, c->ev_aud_done, 0));
     CK(cudaMemcpyAsync(c->d_ended, c->h_ended, (size_t)n, cudaMemcpyHostToDevice, cs));
+    CK(cudaEventRecord(c->ev_ended_free, cs));
     const uint64_t* new_off = c->aud_unconsumed ? c->d_aud_off2[a] : nullptr;
     ef_audio_len_kernel<<<(n + 255) / 256, 256, 0, cs>>>(c->d_aud_state, new_off, c->d_lead2[a], c->d_skip2[a], n, c->d_blob_len);
     CK(cudaGetLastError());
@@ -1395,17 +1463,84 @@ int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info
     ef_audio_assemble_kernel<<<n, 256, 0, cs>>>(c->d_aud_state, c->d_aud2[a], new_off, c->d_lead2[a], c->d_skip2[a], c->d_blob_off, c->d_blob);
     CK(cudaGetLastError());
     c->launches += 3;
-    rc = audio_decode_blob(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, *c->aud_scratch, info, pcm, pcm_cap, pdm, cs, &c->launches);
+    return EF_OK;
+}
+
+// ef_audio_end_kernel for the streams this call ends: the current demux gate, and that of a submit queued behind it
+static int audio_end(ef_ctx* c, const int* verdict, cudaStream_t cs)
+{
+    const int n = c->cfg.n_streams, a = c->active, p = c->pending;
+    CK(ef_launch_audio_end(c->d_ended, n, c->d_gate2[a], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr, p >= 0 && c->aud_ts[p], verdict, cs));
+    c->launches++;
+    return EF_OK;
+}
+
+int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !info) return fail(EF_EINVAL, "null argument");
+    if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio before ef_audio_enable");
+    int rc = audio_constants(c->cfg.device);
+    if (rc != EF_OK) return rc;
+    if ((rc = audio_resolve(c)) != EF_OK) return rc;
+    const int n = c->cfg.n_streams;
+    cudaStream_t cs = (cudaStream_t)stream;
+    bool any_end = false;
+    if ((rc = audio_assemble(c, end_of_stream, cs, &any_end)) != EF_OK) return rc;
+    rc = audio_decode_blob(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, *c->aud_scratch, info, pcm, pcm_cap, pdm, cs, &c->launches,
+                           [&] { return any_end ? audio_end(c, nullptr, cs) : EF_OK; });
+    CK(cudaEventRecord(c->ev_aud_done, cs));
     if (rc != EF_OK || !pcm) return rc;
     c->aud_unconsumed = false;
-    if (any_end) {
-        ef_audio_end_kernel<<<(n + 255) / 256, 256, 0, cs>>>(c->d_ended, n, c->d_gate2[a], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
-                                                             p >= 0 && c->aud_ts[p]);
-        CK(cudaGetLastError());
-        c->launches++;
-        CK(cudaStreamSynchronize(cs));
-    }
     return EF_OK;
+}
+
+static bool is_device_ptr(const void* p)
+{
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+}
+
+int ef_decode_audio_async(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !info || !pcm) return fail(EF_EINVAL, "null argument");
+    if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio_async before ef_audio_enable");
+    if (!is_device_ptr(info) || !is_device_ptr(pcm) || (pdm && !is_device_ptr(pdm)))
+        return fail(EF_EINVAL, "ef_decode_audio_async takes device memory for info, pcm and pdm");
+    int rc = audio_constants(c->cfg.device);
+    if (rc != EF_OK) return rc;
+    // whether this call takes the current submit's audio depends on the outstanding call only when that one took it
+    if (c->aud_async && c->aud_async_new && (rc = audio_resolve(c)) != EF_OK) return rc;
+    const int n = c->cfg.n_streams;
+    AudioScratch& w = *c->aud_scratch;
+    if (!w.fits(AudioScratch::VROWS, audio_vrow_bytes(n, pcm_cap)) || !w.fits(AudioScratch::VERDICT, sizeof(int))) {
+        CK(cudaEventSynchronize(c->ev_aud_done));            // the scratch grows: no earlier call may still use it
+        if ((rc = audio_scratch(w, n, pcm_cap)) != EF_OK) return rc;
+    }
+    if (!c->h_aud_verdict) CK(cudaHostAlloc((void**)&c->h_aud_verdict, sizeof(int), cudaHostAllocDefault));
+    cudaStream_t cs = (cudaStream_t)stream;
+    bool any_end = false;
+    if ((rc = audio_assemble(c, end_of_stream, cs, &any_end)) != EF_OK) return rc;
+    if ((rc = audio_plan(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, info, cs, &c->launches)) != EF_OK) return rc;
+    if ((rc = audio_run(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, pcm, pdm, true, cs, &c->launches)) != EF_OK) return rc;
+    if (any_end && (rc = audio_end(c, (const int*)w.p[AudioScratch::VERDICT], cs)) != EF_OK) return rc;
+    CK(cudaMemcpyAsync(c->h_aud_verdict, w.p[AudioScratch::VERDICT], sizeof(int), cudaMemcpyDeviceToHost, cs));
+    CK(cudaEventRecord(c->ev_aud_done, cs));
+    c->aud_async = true;
+    c->aud_async_new = c->aud_unconsumed;
+    return EF_OK;
+}
+
+int ef_audio_wait(ef_ctx* c)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    int rc = audio_resolve(c);
+    if (rc != EF_OK) return rc;
+    if (c->aud_async_rc == EF_ENOMEM) return fail(EF_ENOMEM, "the last ef_decode_audio_async exceeded its pcm_cap: nothing was decoded, no state changed");
+    return c->aud_async_rc;
 }
 
 // ---- presentation timestamps: push_video(frame, front, _last_pts, mode) player.cpp:692-702, get_pts() player.cpp:653-656 ----
@@ -1464,7 +1599,9 @@ int ef_present_enable(ef_ctx* c, const uint32_t* frame_counter0)
         CK(cudaHostAlloc((void**)&c->h_pace_out, (size_t)n * sizeof(EfPaceOut), cudaHostAllocDefault));
         CK(cudaHostAlloc((void**)&c->h_pace_first, (size_t)n * 8, cudaHostAllocDefault));
         CK(cudaHostAlloc((void**)&c->h_pace_arg, (size_t)n * 4, cudaHostAllocDefault));
+        CK(cudaHostAlloc((void**)&c->h_pace_npics, 4, cudaHostAllocDefault));
         c->allocs_host.push_back(c->h_pace_out); c->allocs_host.push_back(c->h_pace_first); c->allocs_host.push_back(c->h_pace_arg);
+        c->allocs_host.push_back(c->h_pace_npics);
     }
 #undef A
     std::vector<EfPaceState> st((size_t)n);

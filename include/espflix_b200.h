@@ -42,6 +42,8 @@
  *   ef_audio_decode               decode_audio() video.cpp:964, sbc_decoder() sbc_decoder.cpp:343, pdm_second_order()
  *                                 espflix.ino:73
  *   ef_audio_enable / ef_decode_audio  the same audio path fed by the context's TS submits, one submit at a time
+ *   ef_decode_audio_async / ef_audio_wait  the same into device memory, returning before the decode is done: the
+ *                                 reference's audio thread decoding on its own core beside video_isr (espflix.cpp:658)
  *   ef_pts_enable / ef_picture_pts     the pts push_video(frame, front, _last_pts, mode) hands over with every picture
  *                                 (flush_picture() player.cpp:692-702, latched from demux() player.cpp:399-419) and
  *                                 get_pts() player.cpp:653-656, for every stream of a TS submit
@@ -238,6 +240,27 @@ int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_s
 int ef_audio_enable(ef_ctx* ctx);
 int ef_decode_audio(ef_ctx* ctx, const uint8_t* end_of_stream, ef_audio_info* info,
                     int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream);
+
+/* ef_decode_audio_async  the same decode as ef_decode_audio, with its output in device memory: info[n_streams], pcm[pcm_cap]
+ *                  and pdm[2 * pcm_cap] (may be NULL) are device pointers. Every size is computed on the device and the call
+ *                  returns once its work is enqueued on `stream`, without waiting for the device, so the decode runs beside
+ *                  whatever the caller runs on other streams (paced presentation). info[] is written on the device, in stream
+ *                  order, before the samples. Sync and async calls may be mixed in any order; concatenated, their output
+ *                  equals ef_audio_decode on the whole stream.
+ *                  Capacity is checked on the device: when the call's samples exceed pcm_cap, nothing is written but
+ *                  info[] (the counts, so the call doubles as an asynchronous sizing call), no stream state changes,
+ *                  end_of_stream has no effect, the submit's audio stays unconsumed, and ef_audio_wait returns EF_ENOMEM;
+ *                  a call with a larger buffer may follow before the next ef_index. The kernels' grids follow pcm_cap, so
+ *                  size it to the call (an asynchronous sizing call, or the previous submit's need plus a margin).
+ *                  Errors: EF_EINVAL for a NULL pcm or a host pointer; EF_ESTATE before ef_audio_enable.
+ * ef_audio_wait    waits for the last ef_decode_audio_async of the context: EF_OK, or EF_ENOMEM when it did not fit.
+ *                  ef_index of a new submit, ef_decode_audio, ef_restart_streams, ef_reset and ef_audio_enable wait for
+ *                  an outstanding call themselves (only the host knows whether it consumed the submit's audio); an async
+ *                  call waits for the one before it only when that one consumed the submit's audio. Everything else is
+ *                  ordered on the device: a later submit's upload and demux wait for the call with an event. */
+int ef_decode_audio_async(ef_ctx* ctx, const uint8_t* end_of_stream, ef_audio_info* info,
+                          int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, void* stream);
+int ef_audio_wait(ef_ctx* ctx);
 
 /* ---- presentation timestamps of the pictures of TS submits -----------------------------------------------------
  * The reference's decoder latches _pts when a video PES start carries a PTS with a valid prefix (demux(), parse_pts(),
