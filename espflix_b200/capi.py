@@ -84,6 +84,9 @@ _SIGNATURES = {
     "ef_present_enable": (_I, [_VP, _VP]),
     "ef_present_picture": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_idle": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_present_picture_async": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_present_idle_async": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
+    "ef_present_wait": (_I, [_VP, ctypes.POINTER(_I)]),
     "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ef_restart_streams": (_I, [_VP, _I, _I, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
@@ -386,6 +389,46 @@ class Context:
         """ef_present_idle: every display runs on until it has emitted n_fields[s] more fields"""
         nf = np.ascontiguousarray(np.broadcast_to(n_fields, (self.n_streams,)), dtype=np.uint32)
         return self._present(lambda d, c, i, st: self.lib.ef_present_idle(self._h, nf.ctypes.data, d, c, i, st), out, stream)
+
+    def _present_async(self, call, out, info):
+        import torch
+        if info is None:
+            info = torch.zeros((self.n_streams, 8), dtype=torch.int32, device=out.device)
+        for t, dt, what in ((out, torch.uint16, "out"), (info, torch.int32, "info")):
+            if not (t.is_cuda and t.dtype == dt and t.is_contiguous()):
+                raise TypeError("%s must be a contiguous CUDA %s tensor" % (what, dt))
+        assert info.numel() == 8 * self.n_streams
+        w, n = self.geometry()
+        self._check(call(out.data_ptr(), out.numel() // (w * n), info.data_ptr()))      # whole fields only
+        return info
+
+    def present_picture_async(self, pic, out, info=None, modes=None, stream=0):
+        """ef_present_picture_async: present_picture() into the CUDA uint16 tensor `out`, returning once the work is enqueued on
+        `stream` (a torch.cuda.Stream or a raw handle). info: None or an int32 tensor [n_streams, 8] that receives the
+        ef_present_info rows (see present_info()). Returns info. present_wait() says how far the chain of async calls got."""
+        md = None if modes is None else np.ascontiguousarray(np.broadcast_to(modes, (self.n_streams,)), dtype=np.uint8)
+        st = getattr(stream, "cuda_stream", stream)
+        return self._present_async(lambda d, c, i: self.lib.ef_present_picture_async(self._h, pic, _ptr(md), d, c, i, st), out, info)
+
+    def present_idle_async(self, n_fields, out, info=None, stream=0):
+        """ef_present_idle_async: present_idle() into the CUDA uint16 tensor `out`, enqueued on `stream`. Returns info."""
+        nf = np.ascontiguousarray(np.broadcast_to(n_fields, (self.n_streams,)), dtype=np.uint32)
+        st = getattr(stream, "cuda_stream", stream)
+        return self._present_async(lambda d, c, i: self.lib.ef_present_idle_async(self._h, nf.ctypes.data, d, c, i, st), out, info)
+
+    def present_wait(self):
+        """ef_present_wait: waits for the chain of async present calls -> (EF_OK, or EF_ENOMEM when a call exceeded its buffer;
+        the calls that took effect)"""
+        k = _I()
+        rc = self.lib.ef_present_wait(self._h, ctypes.byref(k))
+        if rc not in (EF_OK, EF_ENOMEM):
+            self._check(rc)
+        return rc, k.value
+
+    @staticmethod
+    def present_info(info):
+        """the int32 [n_streams, 8] info tensor of present_*_async -> numpy array of the PRESENT_INFO rows"""
+        return np.ascontiguousarray(info.cpu().numpy()).view(PRESENT_INFO).reshape(-1)
 
     def present_overlay(self, bitmaps=None, blend=None, progress=None, set=None, first=0, count=None):
         """ef_present_overlay: stage overlay changes for streams [first, first + count); they latch at line 0 of the first field

@@ -55,12 +55,14 @@ cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t 
 cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometry& g, int fb, int frame_counter, const EfPresent& pr, cudaStream_t stream);
 cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line, int x, int width, int frame_counter, uint16_t* dst, cudaStream_t stream);
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps);
+                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total);
 __global__ void ef_pace_kernel(const EfPaceState* st, EfPaceState* next, EfPaceRun* run, EfPaceOut* out, const int64_t* pic_pts, const uint32_t* n_pics,
                                const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc,
                                const EfOverlayState* ovl, EfOverlayState* ovl_next);
-__global__ void ef_pace_fill_kernel(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc,
-                                    EfOverlayState* ovl, const EfOverlayState* ovl_next, EfFieldOverlay* fovl);
+cudaError_t ef_launch_pace_fill(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc, EfOverlayState* ovl,
+                                const EfOverlayState* ovl_next, EfFieldOverlay* fovl, int n_streams, const int* chain, cudaStream_t stream);
+__global__ void ef_pace_size_kernel(const EfPaceOut* out, int n_streams, uint64_t cap, uint64_t* first, EfPaceOut* info, uint64_t* total, int* chain,
+                                    uint32_t* rec);
 __global__ void ef_overlay_stage_kernel(EfOverlayState* ovl, uint8_t* slots, const EfOverlayCmd* cmd, const uint8_t* bitmaps, int first);
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
 
@@ -253,6 +255,7 @@ struct ef_ctx {
     int pace_next = 0;                            // the picture index ef_present_picture takes next
     int pace_npics = -1;                          // picture indices of the current submit (-1: not read yet)
     int pace_p0 = 0;                              // first picture index of the current K1a range
+    int pace_parse_at = 0;                        // the picture index whose present call runs the next K1a
     EfPaceState* d_pace = nullptr;                // [n_streams]
     EfPaceState* d_pace_next = nullptr;           // [n_streams] the state after the call being made
     EfPaceRun* d_pace_run = nullptr;              // [n_streams]
@@ -276,6 +279,21 @@ struct ef_ctx {
     EfFieldOverlay* d_fovl = nullptr;             // one per emitted field, beside d_desc
     uint64_t fovl_cap = 0;
     uint8_t* d_restart_ops = nullptr;             // [n_streams] the ops of one ef_restart_streams call, allocated by its first call
+    // ef_present_*_async, allocated by the first call: the chain of calls since the last ef_present_wait (or the last call that
+    // resolved it) and its verdict. d_pace_chain = { a call did not fit, calls that took effect }, copied to h_pace_chain at the end
+    // of every call, which then records ev_pace_done. chain_next / chain_pic: pace_next before each call of the chain, and its pic.
+    bool pace_async = false;                      // a chain is outstanding
+    int pace_async_rc = EF_OK, pace_async_n = 0;  // the result of the last resolved chain
+    int* d_pace_chain = nullptr;
+    int* h_pace_chain = nullptr;                  // pinned
+    uint64_t* d_pace_total = nullptr;             // the fields of the call being made (0 when it does not take effect)
+    std::vector<int> chain_next, chain_pic;
+    cudaEvent_t ev_pace_done = nullptr;
+    // modes / idle field counts of async calls: a pinned ring, slot k free again once ev_pace_ring[k] has passed
+    enum { kPaceRing = 16 };
+    uint32_t* h_pace_ring = nullptr;              // pinned [kPaceRing][n_streams]
+    cudaEvent_t ev_pace_ring[kPaceRing] = {};
+    int pace_ring_i = 0;
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -491,6 +509,8 @@ void ef_destroy(ef_ctx* c)
     if (c->ev_indexed) cudaEventDestroy(c->ev_indexed);
     if (c->ev_aud_done) cudaEventDestroy(c->ev_aud_done);
     if (c->ev_ended_free) cudaEventDestroy(c->ev_ended_free);
+    if (c->ev_pace_done) cudaEventDestroy(c->ev_pace_done);
+    for (cudaEvent_t e : c->ev_pace_ring) if (e) cudaEventDestroy(e);
     if (c->h_aud_verdict) cudaFreeHost(c->h_aud_verdict);
     if (c->up_stream) cudaStreamDestroy(c->up_stream);
     if (c->down_stream) cudaStreamDestroy(c->down_stream);
@@ -516,12 +536,32 @@ static int audio_resolve(ef_ctx* c)
     return EF_OK;
 }
 
+// An outstanding chain of ef_present_*_async calls: wait for it and settle what only the host keeps. After a call that did not
+// fit, the next picture index rolls back to that call's, and when a picture call of the chain did not take effect its records
+// are gone (the size kernel zeroed them): the next picture call parses again from there.
+static int pace_resolve(ef_ctx* c)
+{
+    if (!c->pace_async) return EF_OK;
+    CK(cudaEventSynchronize(c->ev_pace_done));
+    c->pace_async = false;
+    const int failed = c->h_pace_chain[0], done = c->h_pace_chain[1];
+    c->pace_async_n = done;
+    c->pace_async_rc = failed ? EF_ENOMEM : EF_OK;
+    if (failed) {
+        c->pace_next = c->chain_next[(size_t)done];
+        for (size_t i = (size_t)done; i < c->chain_pic.size(); i++)
+            if (c->chain_pic[i] >= 0) { c->pace_parse_at = c->pace_next; break; }
+    }
+    return EF_OK;
+}
+
 int ef_reset(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     { int rcw = wait_frames_read(c); if (rcw != EF_OK) return rcw; }
     { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
     CK(cudaMemset(c->h.frames, 0, (size_t)c->cfg.n_streams * 2 * EF_FRAME + 1024));     // Frame::init zero-fills (player.cpp:25)
     ef_reset_seq_kernel<<<(c->cfg.n_streams + 127) / 128, 128>>>(c->d, c->d_default_intra);
     CK(cudaGetLastError());
@@ -561,6 +601,7 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
         if (ops[i] > 2) return fail(EF_EINVAL, "op %d of stream %d is not 0..2", ops[i], first + i);
         any_reset |= ops[i] == 1;
     }
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
     if (c->paced && c->pace_indexed) {                    // the schedule of the current submit must be complete
         int rc = pace_pictures(c);
         if (rc != EF_OK) return rc;
@@ -698,6 +739,7 @@ int ef_index(ef_ctx* c, void* stream)
     if (!c->submitted) return fail(EF_ESTATE, "ef_index before any submit");
     cudaStream_t st = (cudaStream_t)stream;
     const int n = c->cfg.n_streams;
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
     if (c->paced && c->pace_indexed) {                    // the schedule needs every picture of the current submit
         int rc = pace_pictures(c);
         if (rc != EF_OK) return rc;
@@ -737,7 +779,7 @@ int ef_index(ef_ctx* c, void* stream)
         CK(cudaEventRecord(c->ev_indexed, st));
     }
     c->indexed = true;
-    if (c->paced) { c->pace_indexed = true; c->pace_next = 0; c->pace_npics = -1; }
+    if (c->paced) { c->pace_indexed = true; c->pace_next = 0; c->pace_npics = -1; c->pace_parse_at = 0; }
     return EF_OK;
 }
 
@@ -1008,6 +1050,7 @@ int ef_video_init(ef_ctx* c, int ntsc)
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     if (c->paced && (ntsc ? 1 : 0) != c->pace_ntsc) return fail(EF_ESTATE, "the standard of a presenting context is fixed by ef_present_enable");
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
     EfGeometry g;
     memset(&g, 0, sizeof(g));
     g.ntsc = ntsc ? 1 : 0;
@@ -1618,23 +1661,94 @@ int ef_present_enable(ef_ctx* c, const uint32_t* frame_counter0)
     return EF_OK;
 }
 
-// One presentation call: schedule (one thread per stream, into scratch), one read of the counts, then - unless this is a sizing
-// call or dst is too small - the decode of picture index `pic`, the descriptors and state commit, and the paced K2.
-static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
-                          cudaStream_t st)
+// The halves of a presentation call that the synchronous and the asynchronous calls share, all on `st`:
+//   present_schedule  the call's modes / idle field counts (through the pinned buffer `pinned`) and the schedule, one thread per
+//                     stream, into scratch
+//   present_parse     K1a when `pic` starts a range: once per rec_pics picture indices, as ef_decode_all, and again from the index
+//                     an asynchronous chain failed at
+//   present_recon     K1b of picture index `pic`
+//   present_room      the descriptor and per-field overlay arrays grown to `fields` (waits for what may still read them)
+//   present_render    descriptors and state commit, then the paced K2 over `slots` output slots; gated: both decided on the device
+static int present_schedule(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, void* pinned, cudaStream_t st)
 {
     const int n = c->cfg.n_streams;
-    if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
-    if (pic >= 0) for (int s = 0; modes && s < n; s++) if (modes[s] > 3) return fail(EF_EINVAL, "mode %d of stream %d is not 0..3", modes[s], s);
-    if (pic >= 0 && modes) memcpy(c->h_pace_arg, modes, (size_t)n);
-    if (pic < 0) memcpy(c->h_pace_arg, idle_n, (size_t)n * 4);
+    if (pic >= 0 && modes) memcpy(pinned, modes, (size_t)n);
+    if (pic < 0) memcpy(pinned, idle_n, (size_t)n * 4);
     const bool arg = pic < 0 || modes;
-    if (arg) CK(cudaMemcpyAsync(c->d_pace_arg, c->h_pace_arg, pic < 0 ? (size_t)n * 4 : (size_t)n, cudaMemcpyHostToDevice, st));
+    if (arg) CK(cudaMemcpyAsync(c->d_pace_arg, pinned, pic < 0 ? (size_t)n * 4 : (size_t)n, cudaMemcpyHostToDevice, st));
     ef_pace_kernel<<<(n + 127) / 128, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_out, c->d_pic_pts, c->h.n_pics, c->h.base_pics,
                                                    pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, (const uint32_t*)c->d_pace_arg, pic,
                                                    c->cfg.max_pictures, n, c->pace_ntsc, c->d_ovl, c->d_ovl_next);
     CK(cudaGetLastError());
     c->launches++;
+    return EF_OK;
+}
+
+static int present_parse(ef_ctx* c, int pic, cudaStream_t st)
+{
+    if (pic != c->pace_parse_at) return EF_OK;
+    const int k = c->pace_npics - pic < c->h.rec_pics ? c->pace_npics - pic : c->h.rec_pics;
+    c->pace_p0 = pic;
+    c->pace_parse_at = pic + k;
+    return decode_parse(c, pic, k, st);
+}
+
+static int present_recon(ef_ctx* c, int pic, cudaStream_t st)
+{
+    int rc = decode_recon(c, pic - c->pace_p0, st);
+    if (rc != EF_OK) return rc;
+    CK(cudaEventRecord(c->ev_buf_free[c->active], st));   // the front ES buffer is in use until here
+    c->pace_next = pic + 1;
+    return EF_OK;
+}
+
+static int present_room(ef_ctx* c, uint64_t fields, cudaStream_t st)
+{
+    const bool desc = fields > c->desc_cap, fovl = c->d_ovl && fields > c->fovl_cap;
+    if (!desc && !fovl) return EF_OK;
+    CK(cudaStreamSynchronize(st));
+    if (c->pace_async) CK(cudaEventSynchronize(c->ev_pace_done));   // the calls of the outstanding chain, on whatever stream
+    if (desc) {
+        if (c->d_desc) CK(cudaFree(c->d_desc));
+        c->d_desc = nullptr; c->desc_cap = 0;
+        CK(cudaMalloc(&c->d_desc, fields * sizeof(EfFieldDesc)));
+        c->desc_cap = fields;
+    }
+    if (fovl) {
+        if (c->d_fovl) CK(cudaFree(c->d_fovl));
+        c->d_fovl = nullptr; c->fovl_cap = 0;
+        CK(cudaMalloc(&c->d_fovl, fields * sizeof(EfFieldOverlay)));
+        c->fovl_cap = fields;
+    }
+    return EF_OK;
+}
+
+static int present_render(ef_ctx* c, uint16_t* dst, uint64_t slots, bool gated, cudaStream_t st)
+{
+    EfFieldOverlay* fovl = c->d_ovl ? c->d_fovl : nullptr;
+    CK(ef_launch_pace_fill(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc, c->d_ovl, c->d_ovl_next, fovl, c->cfg.n_streams,
+                           gated ? c->d_pace_chain : nullptr, st));
+    c->launches++;
+    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, slots, dst, st, &c->launches, fovl, c->d_ovl_slots, gated ? c->d_pace_total : nullptr));
+    return EF_OK;
+}
+
+static int present_check_modes(ef_ctx* c, int pic, const uint8_t* modes)
+{
+    if (pic >= 0) for (int s = 0; modes && s < c->cfg.n_streams; s++) if (modes[s] > 3) return fail(EF_EINVAL, "mode %d of stream %d is not 0..3", modes[s], s);
+    return EF_OK;
+}
+
+// The synchronous call: the schedule, one read of the counts, then - unless this is a sizing call or dst is too small - the decode
+// of picture index `pic`, the descriptors and state commit, and the paced K2.
+static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
+                          cudaStream_t st)
+{
+    const int n = c->cfg.n_streams;
+    if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
+    int rc = present_check_modes(c, pic, modes);
+    if (rc != EF_OK) return rc;
+    if ((rc = present_schedule(c, pic, modes, idle_n, c->h_pace_arg, st)) != EF_OK) return rc;
     CK(cudaMemcpyAsync(c->h_pace_out, c->d_pace_out, (size_t)n * sizeof(EfPaceOut), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     uint64_t total = 0;
@@ -1645,38 +1759,73 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
     memcpy(info, c->h_pace_out, (size_t)n * sizeof(EfPaceOut));
     if (!dst) return EF_OK;                                // sizing call: nothing decoded, no state changed
     if (total > dst_fields) return fail(EF_ENOMEM, "%llu fields, capacity %llu", (unsigned long long)total, (unsigned long long)dst_fields);
-    int rc;
     if (pic >= 0) {
-        if (pic % c->h.rec_pics == 0) {                    // K1a once per rec_pics picture indices, as ef_decode_all
-            c->pace_p0 = pic;
-            const int k = c->pace_npics - pic < c->h.rec_pics ? c->pace_npics - pic : c->h.rec_pics;
-            if ((rc = decode_parse(c, pic, k, st)) != EF_OK) return rc;
-        }
-        if ((rc = decode_recon(c, pic - c->pace_p0, st)) != EF_OK) return rc;
-        CK(cudaEventRecord(c->ev_buf_free[c->active], st));   // the front ES buffer is in use until here
-        c->pace_next = pic + 1;
+        if ((rc = present_parse(c, pic, st)) != EF_OK) return rc;
+        if ((rc = present_recon(c, pic, st)) != EF_OK) return rc;
     }
-    if (total > c->desc_cap) {
-        CK(cudaStreamSynchronize(st));
-        if (c->d_desc) CK(cudaFree(c->d_desc));
-        c->d_desc = nullptr; c->desc_cap = 0;
-        CK(cudaMalloc(&c->d_desc, total * sizeof(EfFieldDesc)));
-        c->desc_cap = total;
-    }
-    if (c->d_ovl && total > c->fovl_cap) {
-        CK(cudaStreamSynchronize(st));
-        if (c->d_fovl) CK(cudaFree(c->d_fovl));
-        c->d_fovl = nullptr; c->fovl_cap = 0;
-        CK(cudaMalloc(&c->d_fovl, total * sizeof(EfFieldOverlay)));
-        c->fovl_cap = total;
-    }
+    if ((rc = present_room(c, total, st)) != EF_OK) return rc;
     CK(cudaMemcpyAsync(c->d_pace_first, c->h_pace_first, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    ef_pace_fill_kernel<<<n, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc, c->d_ovl, c->d_ovl_next,
-                                           c->d_ovl ? c->d_fovl : nullptr);
+    if ((rc = present_render(c, dst, total, false, st)) != EF_OK) return rc;
+    CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
+    return EF_OK;
+}
+
+// The asynchronous call: the same work, sized on the device (ef_pace_size_kernel) between the parse and the reconstruction, with
+// the fill and K2 gated on the chain's verdict. Waits for the host only when the descriptor arrays grow (dst_fields grew) and
+// when the ring slot of its arguments is still in use by the call kPaceRing calls back.
+static int present_async(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
+                         cudaStream_t st)
+{
+    const int n = c->cfg.n_streams;
+    if (!dst || !info || !is_device_ptr(dst) || !is_device_ptr(info)) return fail(EF_EINVAL, "the async present calls take device memory for dst and info");
+    if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
+    int rc = present_check_modes(c, pic, modes);
+    if (rc != EF_OK) return rc;
+    if (!c->d_pace_chain) {
+        if ((rc = dev_alloc(c, &c->d_pace_chain, 2)) != EF_OK) return rc;
+        if ((rc = dev_alloc(c, &c->d_pace_total, 1)) != EF_OK) return rc;
+        CK(cudaHostAlloc((void**)&c->h_pace_chain, 2 * sizeof(int), cudaHostAllocDefault));
+        c->allocs_host.push_back(c->h_pace_chain);
+        CK(cudaHostAlloc((void**)&c->h_pace_ring, (size_t)ef_ctx::kPaceRing * n * 4, cudaHostAllocDefault));
+        c->allocs_host.push_back(c->h_pace_ring);
+        CK(cudaEventCreateWithFlags(&c->ev_pace_done, cudaEventDisableTiming));
+        for (cudaEvent_t& e : c->ev_pace_ring) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    if ((rc = present_room(c, dst_fields, st)) != EF_OK) return rc;
+    if (!c->pace_async) {                                  // a new chain
+        CK(cudaMemsetAsync(c->d_pace_chain, 0, 2 * sizeof(int), st));
+        c->chain_next.clear(); c->chain_pic.clear();
+        c->pace_async = true;
+        c->pace_async_rc = EF_OK; c->pace_async_n = 0;
+    } else CK(cudaStreamWaitEvent(st, c->ev_pace_done, 0)); // after the chain's previous call, on whatever stream it ran
+    const int k = c->pace_ring_i;
+    c->pace_ring_i = (k + 1) % ef_ctx::kPaceRing;
+    CK(cudaEventSynchronize(c->ev_pace_ring[k]));
+    if ((rc = present_schedule(c, pic, modes, idle_n, c->h_pace_ring + (size_t)k * n, st)) != EF_OK) return rc;
+    CK(cudaEventRecord(c->ev_pace_ring[k], st));
+    c->chain_next.push_back(c->pace_next);
+    c->chain_pic.push_back(pic);
+    if (pic >= 0 && (rc = present_parse(c, pic, st)) != EF_OK) return rc;   // before the size kernel, which may zero its records
+    uint32_t* rec = pic >= 0 ? c->h.mb_info + (size_t)(pic - c->pace_p0) * n * EF_MBW_MAX * EF_MBH_MAX : nullptr;
+    ef_pace_size_kernel<<<1, 1024, 0, st>>>(c->d_pace_out, n, dst_fields, c->d_pace_first, (EfPaceOut*)info, c->d_pace_total, c->d_pace_chain, rec);
     CK(cudaGetLastError());
     c->launches++;
-    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, total, dst, st, &c->launches, c->d_ovl ? c->d_fovl : nullptr, c->d_ovl_slots));
-    CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
+    if (pic >= 0 && (rc = present_recon(c, pic, st)) != EF_OK) return rc;
+    if ((rc = present_render(c, dst, dst_fields, true, st)) != EF_OK) return rc;
+    CK(cudaMemcpyAsync(c->h_pace_chain, c->d_pace_chain, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(c->ev_pace_done, st));
+    return EF_OK;
+}
+
+// the checks of a picture call: order and state
+static int present_picture_check(ef_ctx* c, int pic, const char* what)
+{
+    if (!c->paced) return fail(EF_ESTATE, "%s before ef_present_enable", what);
+    if (!c->pace_indexed) return fail(EF_ESTATE, "%s before an ef_index that followed ef_present_enable", what);
+    int rc = pace_pictures(c);
+    if (rc != EF_OK) return rc;
+    if (pic != c->pace_next || pic >= c->pace_npics)
+        return fail(EF_ESTATE, "%s(%d): the next picture index is %d of %d", what, pic, c->pace_next, c->pace_npics);
     return EF_OK;
 }
 
@@ -1684,12 +1833,9 @@ int ef_present_picture(ef_ctx* c, int pic, const uint8_t* modes, uint16_t* dst, 
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !info) return fail(EF_EINVAL, "null argument");
-    if (!c->paced) return fail(EF_ESTATE, "ef_present_picture before ef_present_enable");
-    if (!c->pace_indexed) return fail(EF_ESTATE, "ef_present_picture before an ef_index that followed ef_present_enable");
-    int rc = pace_pictures(c);
+    int rc = pace_resolve(c);
     if (rc != EF_OK) return rc;
-    if (pic != c->pace_next || pic >= c->pace_npics)
-        return fail(EF_ESTATE, "ef_present_picture(%d): the next picture index is %d of %d", pic, c->pace_next, c->pace_npics);
+    if ((rc = present_picture_check(c, pic, "ef_present_picture")) != EF_OK) return rc;
     return present_common(c, pic, modes, nullptr, dst, dst_fields, info, (cudaStream_t)stream);
 }
 
@@ -1698,7 +1844,38 @@ int ef_present_idle(ef_ctx* c, const uint32_t* n_fields, uint16_t* dst, uint64_t
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !info || !n_fields) return fail(EF_EINVAL, "null argument");
     if (!c->paced) return fail(EF_ESTATE, "ef_present_idle before ef_present_enable");
+    int rc = pace_resolve(c);
+    if (rc != EF_OK) return rc;
     return present_common(c, -1, nullptr, n_fields, dst, dst_fields, info, (cudaStream_t)stream);
+}
+
+int ef_present_picture_async(ef_ctx* c, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    int rc = present_picture_check(c, pic, "ef_present_picture_async");
+    if (rc != EF_OK) return rc;
+    return present_async(c, pic, modes, nullptr, dst, dst_fields, info, (cudaStream_t)stream);
+}
+
+int ef_present_idle_async(ef_ctx* c, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !n_fields) return fail(EF_EINVAL, "null argument");
+    if (!c->paced) return fail(EF_ESTATE, "ef_present_idle_async before ef_present_enable");
+    return present_async(c, -1, nullptr, n_fields, dst, dst_fields, info, (cudaStream_t)stream);
+}
+
+int ef_present_wait(ef_ctx* c, int* n_presented)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    int rc = pace_resolve(c);
+    if (rc != EF_OK) return rc;
+    if (n_presented) *n_presented = c->pace_async_n;
+    if (c->pace_async_rc == EF_ENOMEM)
+        return fail(EF_ENOMEM, "call %d of the last ef_present_*_async chain exceeded its dst_fields: it and the calls after it changed nothing", c->pace_async_n);
+    return c->pace_async_rc;
 }
 
 // ---- overlay of paced presentation: _video_composite, _video_composite_blend, _video_composite_progress per stream (video.cpp:839-887) ----
@@ -1707,6 +1884,7 @@ int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, 
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     if (!c->paced) return fail(EF_ESTATE, "ef_present_overlay before ef_present_enable");
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
     const int n = c->cfg.n_streams;
     if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
     std::vector<EfOverlayCmd> cmd((size_t)count);

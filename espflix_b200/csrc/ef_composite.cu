@@ -153,12 +153,19 @@ __device__ __forceinline__ int blank_class(const EfPresent& pr, int line)
 // to dst + y * LINES * W, and the overlay is off. Otherwise y = stream and the field goes to the stream's field buffer.
 // kOverlay (paced only): the overlay is on, with blend, progress and bitmap slot from fovl[y]; pr.bitmap is the base of the
 // bitmap slots, two per stream.
-template <bool kNtsc, bool kPaced, bool kOverlay = false>
+// kGated (paced only, ef_present_*_async): the grid follows the caller's capacity, not the call's fields; a CTA whose output slot
+// slot0 + y is at or past *total (ef_pace_size_kernel: the call's fields, 0 when its chain failed) exits at once.
+template <bool kNtsc, bool kPaced, bool kOverlay = false, bool kGated = false>
 __global__ void __launch_bounds__(kK2Threads)
 ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr, const EfFieldDesc* __restrict__ desc,
-                    uint16_t* __restrict__ dst, const EfFieldOverlay* __restrict__ fovl = nullptr)
+                    uint16_t* __restrict__ dst, const EfFieldOverlay* __restrict__ fovl = nullptr, const uint64_t* __restrict__ total = nullptr,
+                    uint64_t slot0 = 0)
 {
     static_assert(kPaced || !kOverlay, "the per-field overlay is a paced variant");
+    static_assert(kPaced || !kGated, "the gate is on the paced variant");
+    if constexpr (kGated) {
+        if (slot0 + blockIdx.y >= *total) return;
+    }
     using G = Geo<kNtsc>;
     constexpr int CPL = G::W / 8;                                          // 16-byte chunks per line
     constexpr int LB = G::W * 2, LS = LB + 16;                             // bytes per line in the field / in shared memory
@@ -427,11 +434,16 @@ __global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* 
 }
 
 // once the fields fit: one descriptor per emitted field, at the stream's offset `first` in the output; commits the state. ovl: also
-// the overlay each field is drawn with (fields before the latch field show the state latched before this call), and its commit
+// the overlay each field is drawn with (fields before the latch field show the state latched before this call), and its commit.
+// kGated (ef_present_*_async, where only the device knows whether the fields fit): nothing at all once chain[0] says a call of the
+// chain did not fit.
+template <bool kGated>
 __global__ void ef_pace_fill_kernel(EfPaceState* __restrict__ st, const EfPaceState* __restrict__ next, const EfPaceRun* __restrict__ run,
                                     const uint64_t* __restrict__ first, EfFieldDesc* __restrict__ desc,
-                                    EfOverlayState* __restrict__ ovl, const EfOverlayState* __restrict__ ovl_next, EfFieldOverlay* __restrict__ fovl)
+                                    EfOverlayState* __restrict__ ovl, const EfOverlayState* __restrict__ ovl_next, EfFieldOverlay* __restrict__ fovl,
+                                    const int* __restrict__ chain)
 {
+    if (kGated && *chain) return;
     const int s = blockIdx.x;
     const EfPaceRun r = run[s];
     const uint64_t base = first[s];
@@ -449,6 +461,72 @@ __global__ void ef_pace_fill_kernel(EfPaceState* __restrict__ st, const EfPaceSt
         if (threadIdx.x == 0) ovl[s] = b;
     }
     if (threadIdx.x == 0) st[s] = next[s];
+}
+
+cudaError_t ef_launch_pace_fill(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc, EfOverlayState* ovl,
+                                const EfOverlayState* ovl_next, EfFieldOverlay* fovl, int n_streams, const int* chain, cudaStream_t stream)
+{
+    if (chain) ef_pace_fill_kernel<true><<<n_streams, 128, 0, stream>>>(st, next, run, first, desc, ovl, ovl_next, fovl, chain);
+    else ef_pace_fill_kernel<false><<<n_streams, 128, 0, stream>>>(st, next, run, first, desc, ovl, ovl_next, fovl, nullptr);
+    return cudaGetLastError();
+}
+
+// ef_present_*_async: one CTA of 1,024 threads sizes a call on the device. The output offset of every stream's fields (an exclusive
+// prefix of out[].n_fields, tile by tile with the carry of the tiles before) goes to first[] and, with the rest of the schedule's row,
+// to the caller's info[]; *total gets the call's fields, or 0 when they exceed cap or an earlier call of the chain did not fit. The
+// verdict is ANDed into the chain: chain[0] turns 1 at the first call that does not fit and stays so, chain[1] counts the calls that
+// took effect. A call that does not take effect marks its info rows with flag bit 1 (the failing call keeps its counts and offsets,
+// so it doubles as a sizing call; later calls carry none) and zeroes the mb_info slots `rec` of its record picture (NULL for an
+// idle call): K1b then leaves every macroblock, and so the frame stores, as they are.
+__global__ void __launch_bounds__(1024)
+ef_pace_size_kernel(const EfPaceOut* __restrict__ out, int n_streams, uint64_t cap, uint64_t* __restrict__ first, EfPaceOut* __restrict__ info,
+                    uint64_t* __restrict__ total, int* __restrict__ chain, uint32_t* __restrict__ rec)
+{
+    __shared__ uint64_t warp_sum[32];
+    __shared__ uint64_t carry;
+    __shared__ int skip;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) { carry = 0; skip = *chain; }
+    __syncthreads();
+    for (int base = 0; base < n_streams; base += 1024) {
+        const int k = base + threadIdx.x;
+        const uint64_t v = k < n_streams ? out[k].n_fields : 0;
+        uint64_t x = v;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
+        if (lane == 31) warp_sum[warp] = x;
+        __syncthreads();
+        if (warp == 0) {
+            const uint64_t t = warp_sum[lane];
+            uint64_t z = t;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
+            warp_sum[lane] = z - t;
+        }
+        __syncthreads();
+        const uint64_t e = carry + warp_sum[warp] + x - v;
+        if (k < n_streams) first[k] = e;
+        __syncthreads();
+        if (threadIdx.x == 1023) carry = e + v;
+        __syncthreads();
+    }
+    const bool fits = !skip && carry <= cap;
+    for (int k = threadIdx.x; k < n_streams; k += 1024) {   // the same thread wrote first[k] above
+        EfPaceOut o = out[k];
+        o.first = skip ? 0 : first[k];
+        if (skip) o.n_fields = 0;
+        if (!fits) o.flags |= 2;
+        info[k] = o;
+    }
+    if (!fits && rec) {
+        uint4* r = (uint4*)rec;
+        const size_t n = (size_t)n_streams * (EF_MBW_MAX * EF_MBH_MAX / 4);
+        for (size_t i = threadIdx.x; i < n; i += 1024) r[i] = make_uint4(0, 0, 0, 0);
+    }
+    if (threadIdx.x == 0) {
+        *total = fits ? carry : 0;
+        if (fits) chain[1] += 1; else chain[0] = 1;
+    }
 }
 
 // ef_present_overlay: stream first + i takes cmd[i]; a bitmap goes to the slot that is not latched. One CTA per stream.
@@ -473,14 +551,22 @@ __global__ void ef_overlay_stage_kernel(EfOverlayState* __restrict__ ovl, uint8_
 }
 
 // the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y). fovl != NULL: the overlay variant, with
-// the per-field overlay fovl and the bitmap slots `bitmaps`
+// the per-field overlay fovl and the bitmap slots `bitmaps`. total != NULL: the gated variant, n_fields is the capacity of dst and
+// only the slots below *total are drawn
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps)
+                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total)
 {
     const size_t per = (size_t)g.line_count * g.line_width;
     for (uint64_t f0 = 0; f0 < n_fields; f0 += 65535) {
         const dim3 grid((unsigned)(g.line_count + 15) / 16, (unsigned)(n_fields - f0 < 65535 ? n_fields - f0 : 65535));
-        if (fovl) {
+        if (total) {
+            const EfPresent pr = { 0, 0, 0, bitmaps };
+            const EfFieldOverlay* fo = fovl ? fovl + f0 : nullptr;
+            if (fovl && g.ntsc) ef_composite_kernel<true, true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
+            else if (fovl) ef_composite_kernel<false, true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
+            else if (g.ntsc) ef_composite_kernel<true, true, false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
+            else ef_composite_kernel<false, true, false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
+        } else if (fovl) {
             const EfPresent pr = { 0, 0, 0, bitmaps };
             if (g.ntsc) ef_composite_kernel<true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);
             else ef_composite_kernel<false, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);

@@ -49,7 +49,8 @@
  *                                 get_pts() player.cpp:653-656, for every stream of a TS submit
  *   ef_present_enable / _picture / _idle  push_video(frame, front, pts, mode) video.cpp:1023-1057 against the frame flip
  *                                 of video_isr video.cpp:1122-1198: every stream's paced composite fields, in HBM
- *   ef_restart_streams            MpegDecoder::reset() + video_reset() (player.cpp:439, video.cpp:1070) or video_pause(0)
+ *   ef_present_*_async / ef_present_wait  the same, enqueued without waiting for the device
+ *   ef_restart_streams           MpegDecoder::reset() + video_reset() (player.cpp:439, video.cpp:1070) or video_pause(0)
  *                                 (video.cpp:1060) for chosen streams of the batch
  * Calls run on the context's device and restore the caller's current device.
  */
@@ -322,6 +323,39 @@ typedef struct {
 int ef_present_enable(ef_ctx* ctx, const uint32_t* frame_counter0);
 int ef_present_picture(ef_ctx* ctx, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
 int ef_present_idle(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info, void* stream);
+
+/* ef_present_picture_async / ef_present_idle_async  the same work as ef_present_picture / ef_present_idle with the same arguments
+ *                     (schedule, decode, push and render; modes 0..3, the overlay latch, K1a once per rec_pics indices), returning
+ *                     once it is enqueued on `stream`: nothing is read back, so a player can enqueue a whole submit and prepare
+ *                     the next upload, or hand earlier fields to a device consumer, while the GPU renders. dst and info are device
+ *                     memory (NULL, a host pointer or an unaligned dst: EF_EINVAL); info[] gets the ef_present_info rows, written
+ *                     on the device in stream order before the fields, so every stream's fields can be located without a host
+ *                     read. modes / n_fields are host memory, read before the call returns. Order and EF_ESTATE as the
+ *                     synchronous calls; the next picture index advances when a call is enqueued. The host waits only for the
+ *                     picture count of a submit (once per submit, as the synchronous calls), when dst_fields grows past every
+ *                     earlier call's (the descriptor arrays grow), and when 16 calls are still queued ahead of this one.
+ *                     The async calls since the last ef_present_wait form a chain; the capacity is checked on the device. When a
+ *                     call's fields exceed dst_fields, its info[] carries the counts and offsets it would have needed (an
+ *                     asynchronous sizing call) and flags bit 1; nothing is decoded, no display or overlay state changes and dst
+ *                     is not written. Every later call of the chain then does nothing either: its info[] rows have n_fields 0
+ *                     and flags bit 1. Sync and async calls may be mixed in any order; concatenated, their fields and info[]
+ *                     equal an all-synchronous run.
+ *                     K2's grid follows dst_fields (its CTAs past the call's fields exit at once), so size dst_fields to the call:
+ *                     from an asynchronous sizing call, or the previous submit's need plus a margin.
+ *                     Launches per call: the schedule and the size kernel; K1a when `pic` starts a rec_pics range (and at the
+ *                     index a failed chain is retried from); K1b; the descriptors; ceil(dst_fields / 65,535) K2. An idle call
+ *                     launches the same without K1a and K1b.
+ * ef_present_wait     waits for the chain: EF_OK, or EF_ENOMEM when a call did not fit. *n_presented (may be NULL) = the calls of
+ *                     the chain that took effect. After EF_ENOMEM the next picture index rolls back to the failing call's, and
+ *                     a retry with a larger dst continues bit for bit as if the failed call had never been made. ef_index,
+ *                     ef_present_picture, ef_present_idle, ef_present_overlay, ef_restart_streams, ef_reset and ef_video_init
+ *                     wait for an outstanding chain themselves (only the host knows how far it got); its result stays
+ *                     available to ef_present_wait until the next async call. */
+int ef_present_picture_async(ef_ctx* ctx, int pic, const uint8_t* modes, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
+                             void* stream);
+int ef_present_idle_async(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
+                          void* stream);
+int ef_present_wait(ef_ctx* ctx, int* n_presented);
 
 /* ef_present_overlay  composite() of every paced field (video.cpp:839-887, 1181-1194): the 80 x 16 bitmap and the progress bar
  *                     on the 16 lines from active_bottom + 2, faded by the blend. Stages changes for streams [first, first +
