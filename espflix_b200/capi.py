@@ -89,6 +89,9 @@ _SIGNATURES = {
     "ef_present_wait": (_I, [_VP, ctypes.POINTER(_I)]),
     "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ef_restart_streams": (_I, [_VP, _I, _I, _VP]),
+    "ef_carry_enable": (_I, [_VP, ctypes.c_uint32]),
+    "ef_end_streams": (_I, [_VP, _I, _I, _VP]),
+    "ef_carry_info": (_I, [_VP, _I, _I, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
 }
 
@@ -448,6 +451,27 @@ class Context:
         reference's MpegDecoder::reset() + video_reset() (a new title or a seek), 2 video_pause(0) (resume after a pause)."""
         ops = np.ascontiguousarray(ops, dtype=np.uint8).reshape(-1)
         self._check(self.lib.ef_restart_streams(self._h, first, ops.size, ops.ctypes.data if ops.size else None))
+
+    # -- TS submits cut anywhere ------------------------------------------------------------------
+    def enable_carry(self, max_carry):
+        """ef_carry_enable: from the next submit, TS submits may be cut at any packet boundary; every stream holds up to
+        max_carry bytes of its unfinished access unit between submits"""
+        self._check(self.lib.ef_carry_enable(self._h, int(max_carry)))
+
+    def end_streams(self, ends, first=0):
+        """ef_end_streams: the streams first + i with ends[i] != 0 end with the pending submit (their last unit counts as
+        complete at its index())"""
+        ends = np.ascontiguousarray(ends, dtype=np.uint8).reshape(-1)
+        self._check(self.lib.ef_end_streams(self._h, first, ends.size, ends.ctypes.data if ends.size else None))
+
+    def carry_info(self, first=0, count=None):
+        """ef_carry_info -> (uint32[count] bytes each stream holds after the current submit, uint8[count] flags: bit 0 = its held
+        bytes exceeded max_carry)"""
+        count = self.n_streams - first if count is None else count
+        held = np.zeros(max(count, 1), dtype=np.uint32)
+        flags = np.zeros(max(count, 1), dtype=np.uint8)
+        self._check(self.lib.ef_carry_info(self._h, first, count, held.ctypes.data, flags.ctypes.data))
+        return held[:count], flags[:count]
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

@@ -17,7 +17,14 @@ void ef_build_color_tab(uint32_t* tab768, int ntsc);
 void ef_build_pal_burst(int16_t* b0, int16_t* b1, int width);
 cudaError_t ef_index_upload_constants();
 const unsigned char* ef_default_intra_ptr();
-__global__ void ef_scan_kernel(EfDev* Dp);
+cudaError_t ef_launch_scan(EfDev* Dp, const EfCarryArgs* carry, int n_streams, cudaStream_t st);
+cudaError_t ef_launch_pts_resolve(const EfDev* Dp, const uint2* span, const uint32_t* list_off, const int64_t* list_pts, int64_t* carry,
+                                  int64_t* last, int64_t* pic_pts, const EfCarryArgs* C, int n_streams, cudaStream_t st);
+__global__ void ef_carry_lead_kernel(const uint32_t* held, int n_streams, uint64_t* stream_total, uint32_t* held_in);
+__global__ void ef_carry_copy_kernel(const uint8_t* src_es, const uint64_t* src_off, const uint32_t* held, const uint64_t* es_off, uint8_t* es,
+                                     uint64_t* pay_off, int n_streams);
+__global__ void ef_carry_restart_kernel(const uint8_t* ops, int first, int count, EfCarryArgs C, int64_t* pts_carry, uint8_t* q_es,
+                                        const uint64_t* q_off, const uint32_t* q_held_in);
 __global__ void ef_prefix_kernel(EfDev* Dp);
 __global__ void ef_fill_kernel(EfDev* Dp);
 __global__ void ef_ts_len_kernel(const uint8_t* ts, uint64_t n_packets, uint32_t* out_len);
@@ -25,8 +32,6 @@ __global__ void ef_ts_copy_kernel(const uint8_t* ts, uint64_t n_packets, const u
 __global__ void ef_ts_scan_kernel(const uint32_t* len, const uint64_t* ts_off, uint32_t* local_off, uint16_t* pkt_stream, uint64_t* stream_total);
 __global__ void ef_ts_offsets_kernel(const uint64_t* stream_total, int n_streams, uint64_t* es_off, uint8_t* es);
 __global__ void ef_pts_packet_kernel(const uint8_t* ts, const uint64_t* ts_off, const uint32_t* local_off, uint32_t* list_off, int64_t* list_pts, uint2* span);
-__global__ void ef_pts_resolve_kernel(const EfDev* Dp, const uint2* span, const uint32_t* list_off, const int64_t* list_pts, int64_t* carry, int64_t* last,
-                                      int64_t* pic_pts);
 size_t ef_recon_smem_bytes();
 cudaError_t ef_decode_configure();
 int ef_decode_resident_ctas(int which);
@@ -294,6 +299,20 @@ struct ef_ctx {
     uint32_t* h_pace_ring = nullptr;              // pinned [kPaceRing][n_streams]
     cudaEvent_t ev_pace_ring[kPaceRing] = {};
     int pace_ring_i = 0;
+    // TS submits cut anywhere (ef_carry_enable): K0 leaves every stream's unfinished access unit in the front ES buffer and its
+    // length in d_held; the next upload copies it to the head of the stream's region once that ef_index has finished (ev_scanned)
+    bool carry = false;
+    uint32_t max_carry = 0;
+    uint32_t* d_held = nullptr;                   // [n_streams] EfCarryArgs::held
+    uint32_t* d_held_code = nullptr;              // [n_streams] EfCarryArgs::held_code
+    uint8_t* d_carry_flags = nullptr;             // [n_streams] EfCarryArgs::flags
+    uint32_t* d_held_in2[2] = { nullptr, nullptr };   // per ES buffer: held bytes at the head of each stream's region
+    uint8_t* d_end2[2] = { nullptr, nullptr };    // per ES buffer: ef_end_streams flags of its submit
+    std::vector<uint8_t> h_end2[2];               // their host copies (merged over the calls for one submit)
+    uint64_t* d_pay_off = nullptr;                // [n_streams + 1] where each stream's new payload starts in the back buffer
+    int64_t* d_pts_hold = nullptr;                // [n_streams] EfCarryArgs::pts_hold
+    int64_t* d_pts_pre = nullptr;                 // [n_streams] EfCarryArgs::pts_pre
+    cudaEvent_t ev_scanned = nullptr;             // the last ef_index has written d_held (and resolved the held picture's pts)
 };
 
 // Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
@@ -339,6 +358,47 @@ int push_dev(ef_ctx* c)
         t.es = c->d_es2[b]; t.es_off = c->d_es_off2[b];
         CK(cudaMemcpy(c->dd[b], &t, sizeof(EfDev), cudaMemcpyHostToDevice));
     }
+    return EF_OK;
+}
+
+// the carry state of a carrying context, as K0 and the PTS resolve pass of ES buffer b see it
+EfCarryArgs carry_args(ef_ctx* c, int b)
+{
+    EfCarryArgs a;
+    a.held = c->d_held; a.held_code = c->d_held_code; a.flags = c->d_carry_flags; a.end = c->d_end2[b]; a.held_in = c->d_held_in2[b];
+    a.pts_hold = c->d_pts_hold; a.pts_pre = c->d_pts_pre; a.max_carry = c->max_carry;
+    return a;
+}
+
+// every stream holds nothing (ef_carry_enable, ef_reset)
+int carry_clear(ef_ctx* c)
+{
+    const size_t n = (size_t)c->cfg.n_streams;
+    CK(cudaMemset(c->d_held, 0, n * 4));
+    CK(cudaMemset(c->d_held_code, 0xFF, n * 4));
+    CK(cudaMemset(c->d_carry_flags, 0, n));
+    CK(cudaMemset(c->d_pts_hold, 0xFF, n * 8));
+    CK(cudaMemset(c->d_pts_pre, 0xFF, n * 8));
+    for (int b = 0; b < 2; b++) {
+        CK(cudaMemset(c->d_held_in2[b], 0, n * 4));
+        CK(cudaMemset(c->d_end2[b], 0, n));
+        c->h_end2[b].assign(n, 0);
+    }
+    return EF_OK;
+}
+
+// replace a device allocation of old_n elements by one of new_n, keeping its contents
+template <typename T>
+int dev_grow(ef_ctx* c, T** p, size_t old_n, size_t new_n)
+{
+    T* q = nullptr;
+    int rc = dev_alloc(c, &q, new_n);
+    if (rc != EF_OK) return rc;
+    CK(cudaMemset(q, 0, new_n * sizeof(T)));
+    CK(cudaMemcpy(q, *p, old_n * sizeof(T), cudaMemcpyDeviceToDevice));
+    for (size_t i = 0; i < c->allocs.size(); i++)
+        if (c->allocs[i] == (void*)*p) { cudaFree(*p); c->allocs.erase(c->allocs.begin() + (long)i); break; }
+    *p = q;
     return EF_OK;
 }
 
@@ -510,6 +570,7 @@ void ef_destroy(ef_ctx* c)
     if (c->ev_aud_done) cudaEventDestroy(c->ev_aud_done);
     if (c->ev_ended_free) cudaEventDestroy(c->ev_ended_free);
     if (c->ev_pace_done) cudaEventDestroy(c->ev_pace_done);
+    if (c->ev_scanned) cudaEventDestroy(c->ev_scanned);
     for (cudaEvent_t e : c->ev_pace_ring) if (e) cudaEventDestroy(e);
     if (c->h_aud_verdict) cudaFreeHost(c->h_aud_verdict);
     if (c->up_stream) cudaStreamDestroy(c->up_stream);
@@ -581,6 +642,11 @@ int ef_reset(ef_ctx* c)
     }
     if (c->paced)                                         // video_reset() (video.cpp:1070-1074): every display latches a new origin
         CK(cudaMemset2D((uint8_t*)c->d_pace + offsetof(EfPaceState, fc_origin), sizeof(EfPaceState), 0, 4, (size_t)c->cfg.n_streams));
+    if (c->carry) {                                       // every stream's held bytes are dropped; carry stays enabled
+        CK(cudaDeviceSynchronize());
+        int rcc = carry_clear(c);
+        if (rcc != EF_OK) return rcc;
+    }
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
     c->pace_indexed = false;
@@ -625,6 +691,14 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
                                p >= 0 && c->aud_ts[p], nullptr, 0));
         c->launches++;
     }
+    if (c->carry && any_reset) {                          // MpegDecoder::reset() clears the bit reader (player.cpp:446-447)
+        const int p = c->pending;
+        ef_carry_restart_kernel<<<(count * 32 + 127) / 128, 128>>>(c->d_restart_ops, first, count, carry_args(c, c->active), c->pts ? c->d_pts_carry : nullptr,
+                                                                   p >= 0 ? c->d_es2[p] : nullptr, p >= 0 ? c->d_es_off2[p] : nullptr,
+                                                                   p >= 0 ? c->d_held_in2[p] : nullptr);
+        CK(cudaGetLastError());
+        c->launches++;
+    }
     CK(cudaDeviceSynchronize());
     return EF_OK;
 }
@@ -637,6 +711,7 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !src || !off) return fail(EF_EINVAL, "null argument");
+    if (c->carry && !ts) return fail(EF_ESTATE, "ES submits on a carrying context: submit transport streams");
     const int n = c->cfg.n_streams;
     const int b = c->pending >= 0 ? c->pending : (c->active ^ 1);
     CK(cudaEventSynchronize(c->ev_up_done[b]));          // the pinned offsets of the previous upload into this buffer are free again
@@ -675,7 +750,32 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
         }
         CK(cudaMemcpyAsync(c->d_ts, src, total, kind, up));
         CK(cudaMemcpyAsync(c->d_ts_off, hoff, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, up));
-        if (n_packets) {
+        if (c->carry) {
+            // every stream's region: its held bytes (known once the last ef_index has run), then the new payload
+            const int a = c->active;
+            if (n_packets) {
+                ef_ts_len_kernel<<<(unsigned)((n_packets + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_len);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
+            ef_ts_scan_kernel<<<n, 256, 0, up>>>(c->d_pkt_len, c->d_ts_off, c->d_pkt_off, c->d_pkt_stream, c->d_stream_total);
+            CK(cudaGetLastError());
+            CK(cudaStreamWaitEvent(up, c->ev_scanned, 0));
+            ef_carry_lead_kernel<<<(n + 255) / 256, 256, 0, up>>>(c->d_held, n, c->d_stream_total, c->d_held_in2[b]);
+            CK(cudaGetLastError());
+            ef_ts_offsets_kernel<<<1, 1024, 0, up>>>(c->d_stream_total, n, d_es_off, d_es);
+            CK(cudaGetLastError());
+            ef_carry_copy_kernel<<<(n * 32 + 127) / 128, 128, 0, up>>>(c->d_es2[a], c->d_es_off2[a], c->d_held, d_es_off, d_es, c->d_pay_off, n);
+            CK(cudaGetLastError());
+            c->launches += 4;
+            if (n_packets) {
+                ef_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_off, c->d_pkt_stream, c->d_pay_off, d_es);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
+            CK(cudaMemsetAsync(c->d_end2[b], 0, (size_t)n, up));
+            c->h_end2[b].assign((size_t)n, 0);
+        } else if (n_packets) {
             ef_ts_len_kernel<<<(unsigned)((n_packets + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_len);
             CK(cudaGetLastError());
             ef_ts_scan_kernel<<<n, 256, 0, up>>>(c->d_pkt_len, c->d_ts_off, c->d_pkt_off, c->d_pkt_stream, c->d_stream_total);
@@ -737,6 +837,7 @@ int ef_index(ef_ctx* c, void* stream)
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     if (!c->submitted) return fail(EF_ESTATE, "ef_index before any submit");
+    if (c->carry && c->pending < 0) return fail(EF_ESTATE, "ef_index without a fresh submit on a carrying context (its held bytes have moved on)");
     cudaStream_t st = (cudaStream_t)stream;
     const int n = c->cfg.n_streams;
     { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
@@ -756,8 +857,8 @@ int ef_index(ef_ctx* c, void* stream)
     }                                            // else: index the front buffer again (same input, next GOP period)
     if (c->profiling) { CK(cudaEventRecord(c->ev_prof[0], st)); c->prof_index = true; }
     CK(cudaMemsetAsync(c->h.info, 0, 32, st));
-    ef_scan_kernel<<<(n * 32 + 127) / 128, 128, 0, st>>>(c->d);
-    CK(cudaGetLastError());
+    const EfCarryArgs carry = c->carry ? carry_args(c, c->active) : EfCarryArgs{};
+    CK(ef_launch_scan(c->d, c->carry ? &carry : nullptr, n, st));
     ef_prefix_kernel<<<c->h.max_pictures, 1024, 0, st>>>(c->d);
     CK(cudaGetLastError());
     const size_t threads = (size_t)n * c->h.max_pictures;
@@ -767,12 +868,12 @@ int ef_index(ef_ctx* c, void* stream)
     if (c->profiling) CK(cudaEventRecord(c->ev_prof[1], st));
     if (c->pts) {
         const int a = c->active;
-        ef_pts_resolve_kernel<<<(n * 32 + 127) / 128, 128, 0, st>>>(c->d, c->d_pts_span2[a], c->d_pts_off2[a], c->d_pts_val2[a], c->d_pts_carry, c->d_pts_last,
-                                                                    c->d_pic_pts);
-        CK(cudaGetLastError());
+        CK(ef_launch_pts_resolve(c->d, c->d_pts_span2[a], c->d_pts_off2[a], c->d_pts_val2[a], c->d_pts_carry, c->d_pts_last, c->d_pic_pts,
+                                 c->carry ? &carry : nullptr, n, st));
         c->launches++;
         c->pts_resolved = true;
     }
+    if (c->carry) CK(cudaEventRecord(c->ev_scanned, st));   // the next upload copies the held bytes after this
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));
     if (c->paced) {                              // the picture indices the present calls need, without a device-wide wait
         CK(cudaMemcpyAsync(c->h_pace_npics, c->h.info, 4, cudaMemcpyDeviceToHost, st));
@@ -799,7 +900,77 @@ int ef_index_info(ef_ctx* c, int* max_pictures, uint64_t* total_pictures, uint64
         CK(cudaMemcpy(&last, c->d_es_off2[c->active] + c->cfg.n_streams, 8, cudaMemcpyDeviceToHost));
         *es_bytes = last;
     }
+    if ((info[3] & 4u) && (info[3] & 3u))
+        return fail(EF_ENOMEM, "index overflow (flags %u): raise max_pictures / max_slices_per_picture; and a stream's held bytes exceeded "
+                               "max_carry: see ef_carry_info", info[3]);
+    if (info[3] & 4u) return fail(EF_ENOMEM, "a stream's held bytes exceeded max_carry (flags %u): see ef_carry_info", info[3]);
     if (info[3]) return fail(EF_ENOMEM, "index overflow (flags %u): raise max_pictures / max_slices_per_picture", info[3]);
+    return EF_OK;
+}
+
+// ---- TS submits cut at any packet boundary: the reference's decoder pulls bytes on demand (FILL_BITS -> more(),
+// player.cpp:348-352, 459-493), so a picture may span any number of the producer's Buffers (espflix.cpp:723-737) ----------
+int ef_carry_enable(ef_ctx* c, uint32_t max_carry)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (c->carry) return fail(EF_ESTATE, "carry is already enabled");
+    if (c->pending >= 0) return fail(EF_ESTATE, "ef_carry_enable with a submit pending: enable it before the next submit");
+    if (max_carry < 4) return fail(EF_EINVAL, "max_carry %u must be at least 4 bytes", max_carry);
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+    const size_t n = (size_t)c->cfg.n_streams, extra = n * max_carry;
+    const size_t es_old = c->cfg.es_capacity + 1024, es_new = es_old + extra;
+    CK(cudaDeviceSynchronize());
+    int rc;
+    // both ES buffers and everything sized from them (the coefficient lists of K1a, 3 entries per ES byte) grow by n x max_carry;
+    // the front buffer keeps the current submit, which may still be decoded
+    for (int b = 0; b < 2; b++) if ((rc = dev_grow(c, &c->d_es2[b], es_old, es_new)) != EF_OK) return rc;
+    if ((rc = dev_grow(c, &c->h.coef, 3 * es_old + 1024, 3 * es_new + 1024)) != EF_OK) return rc;
+#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
+    A(c->d_held, n); A(c->d_held_code, n); A(c->d_carry_flags, n); A(c->d_pay_off, n + 1);
+    A(c->d_pts_hold, n); A(c->d_pts_pre, n);
+    for (int b = 0; b < 2; b++) { A(c->d_held_in2[b], n); A(c->d_end2[b], n); }
+#undef A
+    c->max_carry = max_carry;
+    if ((rc = carry_clear(c)) != EF_OK) return rc;
+    if ((rc = push_dev(c)) != EF_OK) return rc;
+    if (!c->ev_scanned) CK(cudaEventCreateWithFlags(&c->ev_scanned, cudaEventDisableTiming));
+    CK(cudaEventRecord(c->ev_scanned, 0));
+    CK(cudaDeviceSynchronize());
+    c->carry = true;
+    return EF_OK;
+}
+
+int ef_end_streams(ef_ctx* c, int first, int count, const uint8_t* ends)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first || (count && !ends))
+        return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    if (!c->carry) return fail(EF_ESTATE, "ef_end_streams before ef_carry_enable");
+    if (c->pending < 0) return fail(EF_ESTATE, "ef_end_streams with no submit pending");
+    if (!count) return EF_OK;
+    const int p = c->pending;
+    std::vector<uint8_t>& h = c->h_end2[p];
+    for (int i = 0; i < count; i++) h[(size_t)first + i] |= ends[i] ? 1 : 0;
+    // pageable source: the copy takes the flags before it returns; the upload stream orders it after the submit's own clear
+    CK(cudaMemcpyAsync(c->d_end2[p] + first, h.data() + first, (size_t)count, cudaMemcpyHostToDevice, c->up_stream));
+    CK(cudaEventRecord(c->ev_up_done[p], c->up_stream));
+    return EF_OK;
+}
+
+int ef_carry_info(ef_ctx* c, int first, int count, uint32_t* held_bytes, uint8_t* flags)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    if (!c->carry) return fail(EF_ESTATE, "ef_carry_info before ef_carry_enable");
+    CK(cudaDeviceSynchronize());
+    if (held_bytes && count) CK(cudaMemcpy(held_bytes, c->d_held + first, (size_t)count * 4, cudaMemcpyDeviceToHost));
+    if (flags && count) CK(cudaMemcpy(flags, c->d_carry_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
     return EF_OK;
 }
 

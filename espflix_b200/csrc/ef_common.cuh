@@ -160,6 +160,20 @@ struct EfDev {               // device-visible context (lives in device memory)
     EfGeometry geo;
 };
 
+// TS submits cut at any packet boundary (ef_carry_enable): what K0 and the PTS resolve pass keep per stream between submits.
+// A stream's region of a submit is its held bytes followed by the submit's new video ES.
+#define EF_NO_PICTURE 0xFFFFFFFFu
+struct EfCarryArgs {
+    uint32_t* held;          // [n_streams] bytes held after the submit (the unfinished access unit; written by K0)
+    uint32_t* held_code;     // [n_streams] offset of the held picture's code byte in the region, EF_NO_PICTURE when none
+    uint8_t* flags;          // [n_streams] bit 0: held bytes exceeded max_carry (sticky until op 1, end of stream or ef_reset)
+    const uint8_t* end;      // [n_streams] ef_end_streams flags of the submit
+    const uint32_t* held_in; // [n_streams] bytes at the head of the region that the previous submit held
+    int64_t* pts_hold;       // [n_streams] pts of the held picture, resolved over the bytes received so far
+    int64_t* pts_pre;        // [n_streams] last valid PTS before the held bytes
+    uint32_t max_carry;
+};
+
 // Per-stream audio state that one ef_decode_audio call hands to the next (ef_audio.cu). All zero = a fresh stream.
 #define EF_AUDIO_CARRY 264       // most bytes one SBC frame's bit loader reads: header + scale factors 8 + 16 blocks x 128 bits
 struct __align__(16) EfAudioState {

@@ -39,8 +39,13 @@ cudaError_t ef_index_upload_constants()
     return cudaMemcpyToSymbol(c_default_intra_q, ef_default_intra_q, 64);
 }
 
+// kCarry (ef_carry_enable): the submit may end inside an access unit (an optional sequence header, an optional GOP header, a
+// picture header and its slices). A unit is complete once all four bytes of a later sequence, GOP, picture or sequence-end
+// code are present; only complete units count, and the first incomplete one is held for the next submit (C.held / C.held_code),
+// with the rolled state (seqs[0], fp_rs, n_pics for base_pics) as if it had not been scanned. Without kCarry, C is unused.
+template <bool kCarry>
 __global__ void __launch_bounds__(128)
-ef_scan_kernel(EfDev* __restrict__ Dp)
+ef_scan_kernel(EfDev* __restrict__ Dp, EfCarryArgs C)
 {
     EfDev& D = *Dp;
     const int lane = threadIdx.x & 31;
@@ -76,6 +81,12 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
     uint32_t n_pic = 0, n_slice = 0, n_seq = 0;           // warp-uniform running counts
     // fp_rs: full_pel | r_size << 1 of the last P header (stale state a B/D picture would see)
     bool stop = false;
+    // kCarry: the open unit (0 none, 1 headers only, 2 with its picture header), where it starts, its picture's code byte,
+    // and the counts and P-vector state as of the last complete unit
+    int open = 0;
+    uint64_t unit = 0;
+    uint32_t unit_code = EF_NO_PICTURE;
+    uint32_t c_pic = 0, c_slice = 0, c_seq = 0, c_fp = fp_rs;
 
     // the sweep is latency bound (one warp per stream): keep the loads of the next two 512-byte chunks in flight
     auto load_chunk = [&](uint64_t chunk, uint4& v, uint32_t& nxt) {
@@ -129,6 +140,16 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
                 const int bi = i + 3;
                 const uint32_t wsel = bi < 4 ? w[0] : bi < 8 ? w[1] : bi < 12 ? w[2] : bi < 16 ? w[3] : w[4];
                 const uint32_t code = __shfl_sync(0xFFFFFFFFu, (wsel >> ((bi & 3) * 8)) & 0xFFu, src);
+                if constexpr (kCarry) {                                       // unit boundaries (marker dispatch, player.cpp:1318)
+                    if (code == 0x00 || code == 0xB3 || code == 0xB8 || code == 0xB7) {
+                        if (open == 2 || code == 0xB7) { c_pic = n_pic; c_slice = n_slice; c_seq = n_seq; c_fp = fp_rs; }
+                        if (code == 0xB7) open = 0;
+                        else {
+                            if (open != 1) unit = pos;                        // a new unit starts here (after headers it continues)
+                            if (code == 0x00) { open = 2; unit_code = (uint32_t)(pos + 3); } else open = 1;
+                        }
+                    }
+                }
                 if (code == 0x00) {                                           // picture(), player.cpp:704
                     const uint32_t idx = n_pic++;
                     const uint64_t hb = (pos + 4) * 8;
@@ -183,6 +204,26 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
     }
     __syncwarp();
 
+    if constexpr (kCarry) {
+        // What is held: the open unit; with none, the last 3 bytes (a start code may straddle the cut). A sequence end, and
+        // the end of the stream (ef_end_streams: the last unit counts as complete), hold nothing. The held unit is dropped,
+        // and the stream flagged, when it exceeds max_carry.
+        uint8_t fl = C.flags[s];
+        uint64_t hold = 0;
+        uint32_t hcode = EF_NO_PICTURE;
+        if (stop || C.end[s]) { c_pic = n_pic; c_slice = n_slice; c_seq = n_seq; c_fp = fp_rs; fl = 0; }
+        else if (open) { hold = len - unit; hcode = open == 2 ? unit_code : EF_NO_PICTURE; }
+        else hold = min(len, (uint64_t)3);
+        if (hold > C.max_carry) { hold = 0; hcode = EF_NO_PICTURE; fl |= 1; }
+        n_pic = c_pic; n_slice = c_slice; n_seq = c_seq; fp_rs = c_fp;
+        if (lane == 0) {
+            C.held[s] = (uint32_t)hold;
+            C.held_code[s] = hcode;
+            C.flags[s] = fl;
+            if (fl & 1) atomicOr(&D.info[3], 4u);
+        }
+    }
+
     // fix-up: slice counts per picture = difference of consecutive first_slice
     const uint32_t np = min(n_pic, (uint32_t)D.max_pictures);
     const uint32_t ns = min(n_slice, (uint32_t)D.max_slices);
@@ -201,6 +242,13 @@ ef_scan_kernel(EfDev* __restrict__ Dp)
         atomicAdd(&D.info[2], ns);
         if (n_pic > (uint32_t)D.max_pictures || n_slice > (uint32_t)D.max_slices || n_seq > (uint32_t)D.max_seq) atomicOr(&D.info[3], 1u);
     }
+}
+
+cudaError_t ef_launch_scan(EfDev* Dp, const EfCarryArgs* carry, int n_streams, cudaStream_t st)
+{
+    if (carry) ef_scan_kernel<true><<<(n_streams * 32 + 127) / 128, 128, 0, st>>>(Dp, *carry);
+    else ef_scan_kernel<false><<<(n_streams * 32 + 127) / 128, 128, 0, st>>>(Dp, EfCarryArgs{});
+    return cudaGetLastError();
 }
 
 // exclusive prefix of slices-per-stream, one CTA of 1024 threads per picture index (grid = max_pictures); the
@@ -380,6 +428,70 @@ ef_ts_offsets_kernel(const uint64_t* __restrict__ stream_total, int n_streams, u
     if (threadIdx.x < 256) es[carry + threadIdx.x] = 0;
 }
 
+// ---- TS submits cut anywhere (ef_carry_enable) ------------------------------------------------------------------------
+// Each stream's region of a carrying submit is the bytes it held after the previous ef_index followed by its new payload:
+// ef_carry_lead_kernel adds the held bytes to the stream totals before ef_ts_offsets_kernel, ef_carry_copy_kernel moves them
+// from the front ES buffer to the head of the region and gives ef_ts_copy_kernel the payload offsets behind them.
+__global__ void ef_carry_lead_kernel(const uint32_t* __restrict__ held, int n_streams, uint64_t* __restrict__ stream_total, uint32_t* __restrict__ held_in)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_streams) return;
+    const uint32_t h = held[s];
+    held_in[s] = h;
+    stream_total[s] += h;
+}
+
+// one warp per stream: 16-byte stores aligned on the destination, the source words funnel-shifted into place
+__global__ void __launch_bounds__(128)
+ef_carry_copy_kernel(const uint8_t* __restrict__ src_es, const uint64_t* __restrict__ src_off, const uint32_t* __restrict__ held,
+                     const uint64_t* __restrict__ es_off, uint8_t* __restrict__ es, uint64_t* __restrict__ pay_off, int n_streams)
+{
+    const int lane = threadIdx.x & 31;
+    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (s >= n_streams) return;
+    const uint32_t h = held[s];
+    if (lane == 0) pay_off[s] = es_off[s] + h;
+    if (!h) return;
+    const uint8_t* src = src_es + src_off[s + 1] - h;
+    uint8_t* dst = es + es_off[s];
+    const uint32_t lead = min((uint32_t)((16 - ((uintptr_t)dst & 15)) & 15), h);
+    const uint32_t body = (h - lead) & ~15u;
+    for (uint32_t i = lane; i < lead; i += 32) dst[i] = src[i];
+    const uint8_t* s1 = src + lead;
+    const uint32_t sh = (uint32_t)((uintptr_t)s1 & 3) * 8;
+    const uint32_t* sw = (const uint32_t*)(s1 - ((uintptr_t)s1 & 3));
+    uint4* d16 = (uint4*)(dst + lead);
+    for (uint32_t k = lane; k < body / 16; k += 32) {
+        const uint32_t* w = sw + 4 * k;
+        const uint32_t a0 = w[0], a1 = w[1], a2 = w[2], a3 = w[3], a4 = sh ? w[4] : 0u;
+        d16[k] = make_uint4(__funnelshift_r(a0, a1, sh), __funnelshift_r(a1, a2, sh), __funnelshift_r(a2, a3, sh), __funnelshift_r(a3, a4, sh));
+    }
+    for (uint32_t i = lead + body + lane; i < h; i += 32) dst[i] = src[i];
+}
+
+// ef_restart_streams op 1 on a carrying context, one warp per stream of [first, first + count): the stream holds nothing and its
+// flag clears; a submit already queued (q_es != nullptr) loses the held bytes copied into it (filled with 0xFF, which holds no
+// start code whatever follows) and the PTS falls back to the last valid one before them. The filled bytes stay at the head of
+// the queued region, so its held length (q_held_in) stays too: the resolve pass places the queued submit's PES starts behind
+// them, and no picture latch can fall inside them.
+__global__ void __launch_bounds__(128)
+ef_carry_restart_kernel(const uint8_t* __restrict__ ops, int first, int count, EfCarryArgs C, int64_t* __restrict__ pts_carry,
+                        uint8_t* __restrict__ q_es, const uint64_t* __restrict__ q_off, const uint32_t* __restrict__ q_held_in)
+{
+    const int lane = threadIdx.x & 31;
+    const int k = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (k >= count || ops[k] != 1) return;
+    const int s = first + k;
+    if (q_es) {
+        const uint32_t h = q_held_in[s];
+        for (uint32_t i = lane; i < h; i += 32) q_es[q_off[s] + i] = 0xFF;
+    }
+    __syncwarp();
+    if (lane) return;
+    C.held[s] = 0; C.held_code[s] = EF_NO_PICTURE; C.flags[s] = 0;
+    if (pts_carry) pts_carry[s] = C.pts_pre[s];
+}
+
 // ---- presentation timestamps of the pictures of TS submits (ef_pts_enable) ------------------------------------------
 // The reference latches _pts in demux() when a video PES start carries a valid PTS (player.cpp:399-419; parse_pts()'s prefix
 // check, player.cpp:299-306) and hands it to the picture whose header is parsed next: picture() -> flush_picture() sets
@@ -443,9 +555,15 @@ ef_pts_packet_kernel(const uint8_t* __restrict__ ts, const uint64_t* __restrict_
 // stream's list, else the carried PTS. pic_pts[s][p] (-1 past the stream's pictures); carry[s] becomes the submit's last valid
 // PTS and last[s] the PTS of its most recent picture (get_pts(), player.cpp:653-656). Indexing the same submit again rolls
 // both as if the input followed itself.
+// kCarry: the list's offsets count from the end of the held bytes at the head of the region (held_in), and a picture whose
+// latch lies inside them is the picture the previous submit held: without a later entry it takes the pts resolved for it then
+// (C.pts_hold). Afterwards C.pts_hold becomes the pts of the picture this submit holds, by the same rule over the bytes so far,
+// and C.pts_pre the last valid PTS before the held bytes (what op 1 of ef_restart_streams keeps when it drops them).
+template <bool kCarry>
 __global__ void __launch_bounds__(128)
 ef_pts_resolve_kernel(const EfDev* __restrict__ Dp, const uint2* __restrict__ span, const uint32_t* __restrict__ list_off,
-                      const int64_t* __restrict__ list_pts, int64_t* __restrict__ carry, int64_t* __restrict__ last, int64_t* __restrict__ pic_pts)
+                      const int64_t* __restrict__ list_pts, int64_t* __restrict__ carry, int64_t* __restrict__ last, int64_t* __restrict__ pic_pts,
+                      EfCarryArgs C)
 {
     const EfDev& D = *Dp;
     const int lane = threadIdx.x & 31;
@@ -459,18 +577,24 @@ ef_pts_resolve_kernel(const EfDev* __restrict__ Dp, const uint2* __restrict__ sp
     const EfPic* pics = D.pics + (size_t)s * D.max_pictures;
     int64_t* out = pic_pts + (size_t)s * D.max_pictures;
     int64_t newest = last[s];
+    uint32_t hin = 0;
+    int64_t hold_in = -1;
+    if constexpr (kCarry) { hin = C.held_in[s]; hold_in = C.pts_hold[s]; }
+    // the pts of a picture whose code byte + 2 is `latch` (region offsets)
+    auto resolve = [&](uint64_t latch) -> int64_t {
+        uint32_t a = 0, b = sp.y;                                      // first entry with offset > latch
+        while (a < b) {
+            const uint32_t m = (a + b) >> 1;
+            if constexpr (kCarry) { if (lo[m] + (uint64_t)hin <= latch) a = m + 1; else b = m; }
+            else { if (lo[m] <= latch) a = m + 1; else b = m; }
+        }
+        if constexpr (kCarry) return a ? lp[a - 1] : latch < hin ? hold_in : carried;
+        else return a ? lp[a - 1] : carried;
+    };
     for (uint32_t p0 = 0; p0 < (uint32_t)D.max_pictures; p0 += 32) {
         const uint32_t p = p0 + lane;
         int64_t v = -1;
-        if (p < np) {
-            const uint64_t latch = (uint64_t)pics[p].code_off + 2;
-            uint32_t a = 0, b = sp.y;                                  // first entry with offset > latch
-            while (a < b) {
-                const uint32_t m = (a + b) >> 1;
-                if (lo[m] <= latch) a = m + 1; else b = m;
-            }
-            v = a ? lp[a - 1] : carried;
-        }
+        if (p < np) v = resolve((uint64_t)pics[p].code_off + 2);
         if (p < (uint32_t)D.max_pictures) out[p] = v;
         const int64_t at_last = __shfl_sync(0xFFFFFFFFu, v, (np - 1) & 31);
         if (np && (np - 1) / 32 == p0 / 32) newest = at_last;
@@ -478,5 +602,26 @@ ef_pts_resolve_kernel(const EfDev* __restrict__ Dp, const uint2* __restrict__ sp
     if (lane == 0) {
         carry[s] = sp.y ? lp[sp.y - 1] : carried;
         last[s] = newest;
+        if constexpr (kCarry) {
+            const uint32_t code = C.held_code[s];
+            if (code != EF_NO_PICTURE) C.pts_hold[s] = resolve((uint64_t)code + 2);
+            const uint64_t tail = D.es_off[s + 1] - D.es_off[s] - C.held[s];
+            uint32_t a = 0, b = sp.y;                                  // first entry at or after the held bytes
+            while (a < b) {
+                const uint32_t m = (a + b) >> 1;
+                if (lo[m] + (uint64_t)hin < tail) a = m + 1; else b = m;
+            }
+            if (a) C.pts_pre[s] = lp[a - 1];
+            else if (tail >= hin) C.pts_pre[s] = carried;              // else the held bytes began in an earlier submit: keep
+        }
     }
+}
+
+cudaError_t ef_launch_pts_resolve(const EfDev* Dp, const uint2* span, const uint32_t* list_off, const int64_t* list_pts, int64_t* carry,
+                                  int64_t* last, int64_t* pic_pts, const EfCarryArgs* C, int n_streams, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)((n_streams * 32 + 127) / 128);
+    if (C) ef_pts_resolve_kernel<true><<<grid, 128, 0, st>>>(Dp, span, list_off, list_pts, carry, last, pic_pts, *C);
+    else ef_pts_resolve_kernel<false><<<grid, 128, 0, st>>>(Dp, span, list_off, list_pts, carry, last, pic_pts, EfCarryArgs{});
+    return cudaGetLastError();
 }

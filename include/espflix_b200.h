@@ -52,6 +52,9 @@
  *   ef_present_*_async / ef_present_wait  the same, enqueued without waiting for the device
  *   ef_restart_streams           MpegDecoder::reset() + video_reset() (player.cpp:439, video.cpp:1070) or video_pause(0)
  *                                 (video.cpp:1060) for chosen streams of the batch
+ *   ef_carry_enable / ef_end_streams / ef_carry_info  the decoder pulling bytes on demand across the producer's Buffers
+ *                                 (FILL_BITS -> more(), player.cpp:348-352, 459-493; espflix.cpp:723-737): TS submits cut at any
+ *                                 packet boundary, and the len <= 0 Buffer that ends a stream (player.cpp:456, 469-473)
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -100,7 +103,8 @@ int ef_reset(ef_ctx* ctx);      /* zero frame stores, picture counters and seque
 /* Submit one batch. es/ts = all streams back to back; off[n_streams+1] = byte offsets of each
  * stream in it. The *_host forms copy from (pinned or pageable) host memory; *_device forms take
  * device pointers (inputs already resident in HBM). `stream` is a cudaStream_t (0 = default).
- * Each submit must hold whole pictures (cut at picture/sequence start codes). A submit is queued on an
+ * Each submit must hold whole pictures (cut at picture/sequence start codes), unless ef_carry_enable lets TS submits be cut at
+ * any packet boundary. A submit is queued on an
  * internal upload stream into the back one of two device buffers and returns at once when the input is
  * pinned (or device) memory, so batch k+1 can be submitted while batch k is still being decoded; the
  * next ef_index() orders the compute stream after the upload. */
@@ -389,6 +393,44 @@ int ef_present_overlay(ef_ctx* ctx, int first, int count, const uint8_t* bitmaps
  *                     picture indices of the current submit are unpresented, or on an audio context while the current TS
  *                     submit's audio has not been through ef_decode_audio. */
 int ef_restart_streams(ef_ctx* ctx, int first, int count, const uint8_t* ops);
+
+/* ---- TS submits cut at any packet boundary: each stream holds its unfinished picture on the device --------------------------
+ * Access unit: an optional sequence header, an optional GOP header, a picture header and its slices. A unit is complete once all
+ * four bytes of a later sequence (B3), GOP (B8), picture (00) or sequence-end (B7) start code are present in the bytes received
+ * so far (the marker dispatch, player.cpp:1318).
+ * ef_carry_enable  from the next submit on, TS submits may be cut at any 188-byte packet boundary, per stream. Each stream's part
+ *                  of a submit is the bytes it held after the previous one followed by the submit's new video ES; its pictures
+ *                  are the complete units in that part, and everything from the first byte of the first incomplete unit to the
+ *                  end is held for the next submit (a sequence header cut inside its matrices, a start code split across the
+ *                  cut, a picture whose last slice has arrived but no start code after it). With no unit open, the last 3
+ *                  bytes are held (they may begin a start code); after a sequence-end code nothing is. Held pictures count in
+ *                  no n_pictures, max_pictures, ef_index_info, ef_stream_info or base_pictures until the submit that completes
+ *                  them. Concatenated over the submits, decoded pictures, ef_picture_pts values (the rule above is over the
+ *                  whole ES already; a held picture's latch may fall in the next submit), paced fields with their info rows
+ *                  and audio equal what the uncut program gives.
+ *                  Capacity: both ES buffers and the coefficient lists sized from es_capacity (12 bytes per ES byte) grow by
+ *                  n_streams x max_carry, so the es_capacity check of a submit still suffices. A stream whose held bytes would
+ *                  exceed max_carry (which must exceed its largest picture) drops them: its flag (ef_carry_info) stays set and
+ *                  ef_index_info returns EF_ENOMEM with info bit 2 until op 1, the end of the stream or ef_reset; its output is
+ *                  unspecified meanwhile, every other stream's is exact.
+ *                  Interactions: ef_restart_streams op 1 drops the held bytes and the PES starts in them (also from a submit
+ *                  already queued); op 2 keeps them. ef_reset drops every stream's and keeps carry enabled. ef_index without a
+ *                  fresh submit, and ES submits, return EF_ESTATE. get_pts() (last_pts) refers to the complete pictures.
+ *                  Launches per TS submit: ef_ts_len_kernel (with packets), ef_ts_scan_kernel, ef_carry_lead_kernel,
+ *                  ef_ts_offsets_kernel, ef_carry_copy_kernel, ef_ts_copy_kernel (with packets). The held bytes are copied on
+ *                  the device after the previous ef_index; the host does not wait.
+ *                  Errors: EF_ESTATE with a submit pending or on a second call; EF_EINVAL for max_carry < 4.
+ * ef_end_streams   the input of streams [first, first + count) with ends[i] != 0 ends with the most recent (pending) submit, as
+ *                  the reference's len <= 0 Buffer ends it (player.cpp:456, 469-473): at its ef_index the stream's last unit
+ *                  counts as complete, as if SEQUENCE_END followed; held bytes that hold no picture are dropped, and afterwards
+ *                  the stream holds nothing (the next submit may start a new program). Calls for one submit accumulate.
+ *                  EF_ESTATE if no submit is pending or carry is off; EF_EINVAL for a bad stream range.
+ * ef_carry_info    synchronous: held_bytes[i] = bytes stream first + i holds after the current submit, flags[i] bit 0 = its held
+ *                  bytes exceeded max_carry. Either pointer may be NULL. EF_ESTATE before ef_carry_enable; EF_EINVAL for a bad
+ *                  stream range. */
+int ef_carry_enable(ef_ctx* ctx, uint32_t max_carry);
+int ef_end_streams(ef_ctx* ctx, int first, int count, const uint8_t* ends);
+int ef_carry_info(ef_ctx* ctx, int first, int count, uint32_t* held_bytes, uint8_t* flags);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
