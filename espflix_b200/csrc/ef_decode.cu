@@ -211,7 +211,9 @@ __device__ __forceinline__ uint32_t pin4(uint32_t pred, int r0, int r1, int r2, 
 {
     // PIN(b + (s >> 8)) for four pixels (add_block, player.cpp:1189; _pin clamps to [0,248], Q1), with the residuals r
     // still scaled by 256. Two pixels per DPX instruction: PRMT cuts (r >> 8) out of bytes 1-2 of two residuals as a pair
-    // of int16 (|r >> 8| < 30,500 for any coefficients within +-2048: the 64 basis amplitudes sum to 14.85), another PRMT
+    // of int16 (|r >> 8| <= 14,314 for any coefficients within +-2048: the prescaled basis amplitudes of the worst sample
+    // sum to 14,313.7 and rounding adds less than 0.6; an intra DC adds at most 16,384 after the column pass clamps it,
+    // and a prediction at most 255, so no lane leaves int16), another PRMT
     // spreads two prediction bytes to halfwords, VIADDMNMX.S16x2.RELU computes max(min(pred + res, 248), 0) on both.
     const uint32_t s01 = __viaddmin_s16x2_relu(__byte_perm(pred, 0, 0x4140), __byte_perm((uint32_t)r0, (uint32_t)r1, 0x6521), 0x00F800F8u);
     const uint32_t s23 = __viaddmin_s16x2_relu(__byte_perm(pred, 0, 0x4342), __byte_perm((uint32_t)r2, (uint32_t)r3, 0x6521), 0x00F800F8u);
@@ -769,7 +771,10 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
             int v[8];
 #pragma unroll
             for (int rr = 0; rr < 8; rr++) v[rr] = db[rr * 8];
-            if (intra_r && ccol == 0) v[0] = (int)((uint32_t)dc_col << 8);       // b[0] <<= 8, player.cpp:1065
+            // b[0] <<= 8, player.cpp:1065. The DC predictor is unbounded; every output sample is dc + an AC term of at
+            // most 14,059, so a DC clamped to +-16384 clamps to the same pixel and keeps pin4's int16 lanes from wrapping
+            // (the Q7 copy below reads the unclamped dc_row)
+            if (intra_r && ccol == 0) v[0] = (int)((uint32_t)max(-16384, min(dc_col, 16384)) << 8);
             idct8<false>(v);
 #pragma unroll
             for (int rr = 0; rr < 8; rr++) db[rr * 8] = v[rr];
