@@ -88,6 +88,8 @@ _SIGNATURES = {
     "ef_present_idle_async": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_wait": (_I, [_VP, ctypes.POINTER(_I)]),
     "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
+    "ef_present_font": (_I, [_VP, _VP, _VP, _I]),
+    "ef_present_clock": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
     "ef_restart_streams": (_I, [_VP, _I, _I, _VP]),
     "ef_carry_enable": (_I, [_VP, ctypes.c_uint32]),
     "ef_end_streams": (_I, [_VP, _I, _I, _VP]),
@@ -444,6 +446,26 @@ class Context:
                 for a, dt, shape in ((bm, np.uint8, (count, 1280)), (blend, np.int32, (count,)), (progress, np.int32, (count,)), (set, np.uint8, (count,)))]
         ptrs = [None if a is None or a.size == 0 else a.ctypes.data for a in keep]
         self._check(self.lib.ef_present_overlay(self._h, first, count, *ptrs))
+
+    def present_font(self, atlas, rights):
+        """ef_present_font: the glyph atlas of the overlay's time text. atlas: [16, 1024] uint8 (the reference's _font8), rights:
+        int16 glyph right edges (_font8_rights)."""
+        a = np.ascontiguousarray(atlas, dtype=np.uint8).reshape(-1)
+        r = np.ascontiguousarray(rights, dtype=np.int16).reshape(-1)
+        if a.size != 16 * 1024:
+            raise ValueError("the atlas is 16 x 1024 bytes")
+        self._check(self.lib.ef_present_font(self._h, a.ctypes.data, r.ctypes.data, r.size))
+
+    def present_clock(self, idx_hdrs, speed, flags, first=0, count=None):
+        """ef_present_clock: update_progress() on streams [first, first + count) from the next present call on. idx_hdrs: [count, 104]
+        uint8 video.idx headers (or one for all), speed: -1 / 0 / 1 per stream or one for all, flags: bit 0 on, bit 1 paused, bit 2
+        zero _last_seconds."""
+        count = self.n_streams - first if count is None else count
+        h = np.ascontiguousarray(np.broadcast_to(np.asarray(idx_hdrs, dtype=np.uint8).reshape(-1, 104), (count, 104)))
+        sp = np.ascontiguousarray(np.broadcast_to(np.asarray(speed, dtype=np.int8), (count,)))
+        fl = np.ascontiguousarray(np.broadcast_to(np.asarray(flags, dtype=np.uint8), (count,)))
+        ptrs = [a.ctypes.data if a.size else None for a in (h, sp, fl)]
+        self._check(self.lib.ef_present_clock(self._h, first, count, *ptrs))
 
     # -- per-stream restart ----------------------------------------------------------------------
     def restart_streams(self, ops, first=0):

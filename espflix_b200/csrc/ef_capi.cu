@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/espflix_b200.h"
+#include "../host/ef_indexer.h"
 #include "ef_common.cuh"
 #include <stdlib.h>
 
@@ -69,6 +70,11 @@ cudaError_t ef_launch_pace_fill(EfPaceState* st, const EfPaceState* next, const 
 __global__ void ef_pace_size_kernel(const EfPaceOut* out, int n_streams, uint64_t cap, uint64_t* first, EfPaceOut* info, uint64_t* total, int* chain,
                                     uint32_t* rec);
 __global__ void ef_overlay_stage_kernel(EfOverlayState* ovl, uint8_t* slots, const EfOverlayCmd* cmd, const uint8_t* bitmaps, int first);
+__global__ void ef_clock_kernel(EfClockState* clk, const EfOverlayState* ovl, EfOverlayState* ovl_clk, uint8_t* bm, const int64_t* pic_pts,
+                                const uint32_t* n_pics, const int64_t* pts_last, int pic, int max_pictures, const uint8_t* font, const int16_t* rights);
+cudaError_t ef_launch_clock_commit(EfClockState* clk, const EfOverlayState* ovl_clk, const uint8_t* bm, uint8_t* slots, int n_streams, const int* chain,
+                                   cudaStream_t stream);
+static_assert(sizeof(idx_hdr) == 104, "video.idx header: the reference's idx_hdr");
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
 
 namespace {
@@ -283,6 +289,13 @@ struct ef_ctx {
     EfOverlayCmd* d_ovl_cmd = nullptr;            // [n_streams]
     EfFieldOverlay* d_fovl = nullptr;             // one per emitted field, beside d_desc
     uint64_t fovl_cap = 0;
+    // clock of paced presentation: the glyph atlas (ef_present_font) and, from the first ef_present_clock, every stream's clock; until
+    // then the present calls run the kernels they ran before
+    uint8_t* d_font = nullptr;                    // [16][1024] _font8
+    int16_t* d_font_rights = nullptr;             // _font8_rights
+    EfClockState* d_clk = nullptr;                // [n_streams]
+    EfOverlayState* d_ovl_clk = nullptr;          // [n_streams] the overlay state with the clock's changes staged: ef_pace_kernel's input
+    uint8_t* d_clk_bm = nullptr;                  // [n_streams][1280] the bitmap a call rendered, until its commit
     uint8_t* d_restart_ops = nullptr;             // [n_streams] the ops of one ef_restart_streams call, allocated by its first call
     // ef_present_*_async, allocated by the first call: the chain of calls since the last ef_present_wait (or the last call that
     // resolved it) and its verdict. d_pace_chain = { a call did not fit, calls that took effect }, copied to h_pace_chain at the end
@@ -1847,9 +1860,15 @@ static int present_schedule(ef_ctx* c, int pic, const uint8_t* modes, const uint
     if (pic < 0) memcpy(pinned, idle_n, (size_t)n * 4);
     const bool arg = pic < 0 || modes;
     if (arg) CK(cudaMemcpyAsync(c->d_pace_arg, pinned, pic < 0 ? (size_t)n * 4 : (size_t)n, cudaMemcpyHostToDevice, st));
+    if (c->d_clk) {                                        // update_progress() at the call's start, staged after the caller's changes
+        ef_clock_kernel<<<n, 128, 0, st>>>(c->d_clk, c->d_ovl, c->d_ovl_clk, c->d_clk_bm, c->d_pic_pts, c->h.n_pics, c->d_pts_last, pic, c->cfg.max_pictures,
+                                           c->d_font, c->d_font_rights);
+        CK(cudaGetLastError());
+        c->launches++;
+    }
     ef_pace_kernel<<<(n + 127) / 128, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_out, c->d_pic_pts, c->h.n_pics, c->h.base_pics,
                                                    pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, (const uint32_t*)c->d_pace_arg, pic,
-                                                   c->cfg.max_pictures, n, c->pace_ntsc, c->d_ovl, c->d_ovl_next);
+                                                   c->cfg.max_pictures, n, c->pace_ntsc, c->d_clk ? c->d_ovl_clk : c->d_ovl, c->d_ovl_next);
     CK(cudaGetLastError());
     c->launches++;
     return EF_OK;
@@ -1900,6 +1919,10 @@ static int present_render(ef_ctx* c, uint16_t* dst, uint64_t slots, bool gated, 
     CK(ef_launch_pace_fill(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc, c->d_ovl, c->d_ovl_next, fovl, c->cfg.n_streams,
                            gated ? c->d_pace_chain : nullptr, st));
     c->launches++;
+    if (c->d_clk) {
+        CK(ef_launch_clock_commit(c->d_clk, c->d_ovl_clk, c->d_clk_bm, c->d_ovl_slots, c->cfg.n_streams, gated ? c->d_pace_chain : nullptr, st));
+        c->launches++;
+    }
     CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, slots, dst, st, &c->launches, fovl, c->d_ovl_slots, gated ? c->d_pace_total : nullptr));
     return EF_OK;
 }
@@ -2050,6 +2073,21 @@ int ef_present_wait(ef_ctx* c, int* n_presented)
 }
 
 // ---- overlay of paced presentation: _video_composite, _video_composite_blend, _video_composite_progress per stream (video.cpp:839-887) ----
+// the overlay state, allocated by the first ef_present_overlay or ef_present_clock
+static int overlay_alloc(ef_ctx* c)
+{
+    if (c->d_ovl) return EF_OK;
+    const int n = c->cfg.n_streams;
+    int rc;
+#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
+    A(c->d_ovl, (size_t)n); A(c->d_ovl_next, (size_t)n); A(c->d_ovl_cmd, (size_t)n);
+    A(c->d_ovl_slots, (size_t)n * 2 * EF_OVERLAY_BYTES); A(c->d_ovl_in, (size_t)n * EF_OVERLAY_BYTES);
+#undef A
+    CK(cudaMemset(c->d_ovl, 0, (size_t)n * sizeof(EfOverlayState)));   // blend 0: nothing drawn
+    CK(cudaMemset(c->d_ovl_slots, 0, (size_t)n * 2 * EF_OVERLAY_BYTES));
+    return EF_OK;
+}
+
 int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, const int32_t* blend, const int32_t* progress, const uint8_t* set)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
@@ -2067,15 +2105,8 @@ int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, 
         if ((m & 2u) && blend[i] < -1) return fail(EF_EINVAL, "blend %d of stream %d is below -1", blend[i], first + i);
         cmd[i] = { (m & 2u) ? blend[i] : 0, (m & 4u) ? progress[i] : 0, m, 0u };
     }
-    int rc;
-#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
-    if (!c->d_ovl) {
-        A(c->d_ovl, (size_t)n); A(c->d_ovl_next, (size_t)n); A(c->d_ovl_cmd, (size_t)n);
-        A(c->d_ovl_slots, (size_t)n * 2 * EF_OVERLAY_BYTES); A(c->d_ovl_in, (size_t)n * EF_OVERLAY_BYTES);
-        CK(cudaMemset(c->d_ovl, 0, (size_t)n * sizeof(EfOverlayState)));   // blend 0: nothing drawn
-        CK(cudaMemset(c->d_ovl_slots, 0, (size_t)n * 2 * EF_OVERLAY_BYTES));
-    }
-#undef A
+    int rc = overlay_alloc(c);
+    if (rc != EF_OK) return rc;
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(c->d_ovl_cmd, cmd.data(), cmd.size() * sizeof(EfOverlayCmd), cudaMemcpyHostToDevice));
@@ -2084,6 +2115,73 @@ int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, 
     CK(cudaGetLastError());
     c->launches++;
     CK(cudaDeviceSynchronize());
+    return EF_OK;
+}
+
+// ---- clock of paced presentation: ESPFlix::update_progress() (espflix.cpp:862-874) per stream ----
+int ef_present_font(ef_ctx* c, const uint8_t* atlas, const int16_t* rights, int n_rights)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !atlas || !rights) return fail(EF_EINVAL, "null argument");
+    if (n_rights < ':' - 0x18 + 1 || n_rights > EF_FONT_W) return fail(EF_EINVAL, "n_rights %d does not cover glyphs 0x18..':' (%d)", n_rights, ':' - 0x18 + 1);
+    for (int i = 0; i < n_rights; i++)
+        if (rights[i] > EF_FONT_W || rights[i] <= (i ? rights[i - 1] : 0))
+            return fail(EF_EINVAL, "rights[%d] = %d: the glyph edges must increase from above 0 up to %d", i, rights[i], EF_FONT_W);
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    int rc;
+    if (!c->d_font) {
+        if ((rc = dev_alloc(c, &c->d_font, (size_t)16 * EF_FONT_W)) != EF_OK) return rc;
+        if ((rc = dev_alloc(c, &c->d_font_rights, (size_t)EF_FONT_W)) != EF_OK) return rc;
+    }
+    CK(cudaDeviceSynchronize());                          // a present call may still draw with the old atlas
+    CK(cudaMemcpy(c->d_font, atlas, (size_t)16 * EF_FONT_W, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_font_rights, rights, (size_t)n_rights * 2, cudaMemcpyHostToDevice));
+    return EF_OK;
+}
+
+int ef_present_clock(ef_ctx* c, int first, int count, const uint8_t* idx_hdrs, const int8_t* speed, const uint8_t* flags)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->paced) return fail(EF_ESTATE, "ef_present_clock before ef_present_enable");
+    if (!c->d_font) return fail(EF_ESTATE, "ef_present_clock before ef_present_font");
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    if (count && (!idx_hdrs || !speed || !flags)) return fail(EF_EINVAL, "null argument");
+    std::vector<idx_hdr> hdr((size_t)count);
+    if (count) memcpy(hdr.data(), idx_hdrs, (size_t)count * sizeof(idx_hdr));
+    for (int i = 0; i < count; i++) {
+        if (speed[i] < -1 || speed[i] > 1) return fail(EF_EINVAL, "speed %d of stream %d is not -1..1", speed[i], first + i);
+        if (!(flags[i] & 1u)) continue;
+        const idx_hdr& h = hdr[(size_t)i];
+        if (h.video.last_pts == 0) return fail(EF_EINVAL, "stream %d: video.last_pts is 0 (the progress divides by it)", first + i);
+        if (speed[i] == 1 && h.fwd.last_pts == h.fwd.first_pts) return fail(EF_EINVAL, "stream %d: the fwd record spans no pts", first + i);
+        if (speed[i] == -1 && h.rev.last_pts == h.rev.first_pts) return fail(EF_EINVAL, "stream %d: the rwd record spans no pts", first + i);
+    }
+    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    int rc = overlay_alloc(c);
+    if (rc != EF_OK) return rc;
+    if (!c->d_clk) {
+#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
+        A(c->d_clk, (size_t)n); A(c->d_ovl_clk, (size_t)n); A(c->d_clk_bm, (size_t)n * EF_OVERLAY_BYTES);
+#undef A
+        CK(cudaMemset(c->d_clk, 0, (size_t)n * sizeof(EfClockState)));    // every clock off, _last_seconds 0
+    }
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());
+    std::vector<EfClockState> st((size_t)count);
+    CK(cudaMemcpy(st.data(), c->d_clk + first, (size_t)count * sizeof(EfClockState), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < count; i++) {
+        EfClockState& k = st[(size_t)i];
+        const idx_hdr& h = hdr[(size_t)i];
+        k.v_first = h.video.first_pts; k.v_last = h.video.last_pts;
+        k.f_first = h.fwd.first_pts; k.f_last = h.fwd.last_pts;
+        k.r_first = h.rev.first_pts; k.r_last = h.rev.last_pts;
+        k.speed = speed[i];
+        k.flags = flags[i] & 3u;
+        if (flags[i] & 4u) k.last_seconds = 0;
+    }
+    CK(cudaMemcpy(c->d_clk + first, st.data(), (size_t)count * sizeof(EfClockState), cudaMemcpyHostToDevice));
     return EF_OK;
 }
 

@@ -238,6 +238,24 @@ struct __align__(16) EfFieldOverlay {    // the overlay one paced K2 field is dr
     int32_t blend, progress;
     uint32_t slot, pad;
 };
+// The clock of paced presentation (ef_present_clock): ESPFlix::update_progress() (espflix.cpp:862-874) per stream, run at the start
+// of every present call. It maps the stream's pts to the title's main timeline with the title's video.idx header (idx_hdr::pts2pts,
+// espflix.cpp:589-604), redraws show_time()'s text into the overlay bitmap when the whole second changed and sets the progress; both
+// are staged as ef_present_overlay stages them. seconds / draw are scratch of the call being made, committed (last_seconds and the
+// bitmap slot) only once the call takes effect.
+#define EF_FONT_W 1024           // _font8 atlas: 16 rows of 1024 columns
+struct __align__(16) EfClockState {
+    int64_t v_first, v_last;     // idx_hdr: video.first_pts, video.last_pts
+    int64_t f_first, f_last;     // fwd.first_pts, fwd.last_pts
+    int64_t r_first, r_last;     // rwd.first_pts, rwd.last_pts
+    int32_t speed;               // _speed: 0 the title, 1 the fast-forward stream, -1 the rewind stream
+    uint32_t flags;              // bit 0 on (_nav != -1), bit 1 paused (_state == PAUSED: the pause icon)
+    int32_t last_seconds;        // _last_seconds
+    int32_t seconds;             // scratch: the seconds the call shows
+    uint32_t draw;               // scratch: the call rendered a new bitmap
+    uint32_t pad[3];
+};
+
 static inline __host__ __device__ int ef_overlay_blend(int32_t b, uint32_t blend_fc, uint32_t fc)
 {
     const uint32_t d = fc - blend_fc;    // fields since the latch, modulo 2^32

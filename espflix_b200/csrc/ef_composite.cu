@@ -550,6 +550,140 @@ __global__ void ef_overlay_stage_kernel(EfOverlayState* __restrict__ ovl, uint8_
     }
 }
 
+// ---- the clock of paced presentation (ef_present_clock): update_progress() (espflix.cpp:862-874) at the start of a present call ----
+namespace {
+// sprintf's "%d" (two = false) or "%02d" (two = true) of v at b + n; returns the new length
+__device__ int clock_put_int(char* b, int n, int v, bool two)
+{
+    uint32_t u = v < 0 ? 0u - (uint32_t)v : (uint32_t)v;
+    char d[10];
+    int k = 0;
+    do { d[k++] = (char)('0' + u % 10u); u /= 10u; } while (u);
+    if (two && v >= 0 && k < 2) d[k++] = '0';                              // a sign counts towards the width
+    if (v < 0) b[n++] = '-';
+    while (k) b[n++] = d[--k];
+    return n;
+}
+}  // namespace
+
+// One CTA per stream. Every stream gets ovl_clk[s] = its committed overlay state; a stream whose clock is on also stages there the
+// progress and, when the whole second changed, the bitmap that show_time() draws, rendered into its scratch bm[s]. ef_pace_kernel
+// takes ovl_clk as the staged state; nothing committed changes here (ef_clock_commit_kernel does that once the call takes effect).
+// The text: show_time()'s format (espflix.cpp:163-174) drawn from x = 0 into the erased 80 x 16 bitmap, glyph c - 0x18 being columns
+// [rights[c - 0x19], rights[c - 0x18]) of the atlas; rows are contiguous, so column x >= 80 lands at x - 80 of the next row and
+// what passes row 15 is dropped. Each byte folds the pixels that land on it in the order the reference writes them (glyph, then row,
+// then column) through p32() with _color 240 (espflix.cpp:87-96).
+__global__ void __launch_bounds__(128)
+ef_clock_kernel(EfClockState* __restrict__ clk, const EfOverlayState* __restrict__ ovl, EfOverlayState* __restrict__ ovl_clk, uint8_t* __restrict__ bm,
+                const int64_t* __restrict__ pic_pts, const uint32_t* __restrict__ n_pics, const int64_t* __restrict__ pts_last, int pic, int max_pictures,
+                const uint8_t* __restrict__ font, const int16_t* __restrict__ rights)
+{
+    __shared__ char text[24];
+    __shared__ int x0[25];                                                 // text column where each glyph starts; x0[len] = the width
+    __shared__ int16_t col[EF_OVERLAY_BYTES];                              // text column X < 1280 -> atlas column, -1 past the text
+    __shared__ uint8_t glyph[EF_OVERLAY_BYTES];                            // and the glyph it belongs to
+    __shared__ int s_len, s_draw;
+    const int s = blockIdx.x;
+    if (threadIdx.x == 0) {
+        EfClockState k = clk[s];
+        EfOverlayState v = ovl[s];
+        int draw = 0;
+        if (k.flags & 1u) {
+            const int64_t pts = pic >= 0 && (uint32_t)pic < n_pics[s] ? pic_pts[(size_t)s * max_pictures + pic] : pts_last[s];
+            int64_t main = pts;                                            // idx_hdr::pts2pts
+            if (k.speed == 1) main = k.v_first + (pts - k.f_first) * (k.v_last - k.v_first) / (k.f_last - k.f_first);
+            else if (k.speed == -1) main = k.v_last - (pts - k.r_first) * (k.v_last - k.v_first) / (k.r_last - k.r_first);
+            const int seconds = (int)(main / 90000);
+            draw = seconds != k.last_seconds;
+            v.p_progress = (int)(main * 240 / k.v_last);                   // VIDEO_COMPOSITE_PROGRESS_WIDTH
+            v.pending |= draw ? 5u : 4u;
+            if (draw) {
+                const int m = seconds / 60, h = m / 60;
+                const char icon = k.speed == 0 ? ((k.flags & 2u) ? 0x19 : 0x1A) : (k.speed == 1 ? 0x1B : 0x1C);   // PAUSE PLAY FFWD RWND
+                int n = 0;
+                text[n++] = icon;
+                text[n++] = ' ';
+                if (h) {
+                    n = clock_put_int(text, n, h, false);
+                    text[n++] = ':';
+                } else {
+                    text[n++] = ' '; text[n++] = ' ';
+                }
+                n = clock_put_int(text, n, m % 60, true);
+                text[n++] = ':';
+                n = clock_put_int(text, n, seconds % 60, true);
+                int x = 0;
+                for (int i = 0; i < n; i++) {
+                    x0[i] = x;
+                    const int g = text[i] - 0x18;
+                    x += rights[g] - rights[g - 1];
+                }
+                x0[n] = x;
+                s_len = n;
+            }
+            clk[s].seconds = seconds;
+        }
+        clk[s].draw = (uint32_t)draw;
+        ovl_clk[s] = v;
+        s_draw = draw;
+    }
+    __syncthreads();
+    if (!s_draw) return;
+    const int len = s_len;
+    for (int X = (int)threadIdx.x; X < EF_OVERLAY_BYTES; X += blockDim.x) {
+        int i = 0;
+        while (i < len && x0[i + 1] <= X) i++;
+        col[X] = i < len ? (int16_t)(rights[text[i] - 0x18 - 1] + X - x0[i]) : (int16_t)-1;
+        glyph[X] = (uint8_t)i;
+    }
+    __syncthreads();
+    uint8_t* out = bm + (size_t)s * EF_OVERLAY_BYTES;
+    for (int L = (int)threadIdx.x; L < EF_OVERLAY_BYTES; L += blockDim.x) {
+        const int y = L / 80, x = L % 80;
+        int ks[16], n = 0;                                                 // pixel (row y - k, column x + 80 k) lands on byte L
+        for (int k = 0; k <= y && x + 80 * k < EF_OVERLAY_BYTES && col[x + 80 * k] >= 0; k++) ks[n++] = k;
+        uint32_t v = 0;
+        for (int a = 0; a < n;) {                                          // glyph by glyph; inside a glyph, row by row
+            int b = a;
+            while (b + 1 < n && glyph[x + 80 * ks[b + 1]] == glyph[x + 80 * ks[a]]) b++;
+            for (int j = b; j >= a; j--) {
+                const int k = ks[j];
+                const uint32_t p = font[(y - k) * EF_FONT_W + col[x + 80 * k]];
+                if (p) v = (240u * p + (255u - p) * v) >> 8;
+            }
+            a = b + 1;
+        }
+        out[L] = (uint8_t)v;
+    }
+}
+
+// Once the call takes effect (after ef_pace_fill_kernel, before the paced K2): the rendered bitmap goes to the slot that was not
+// latched when the call began (ovl_clk[s].slot ^ 1, where ef_present_overlay stages), and last_seconds advances. kGated
+// (ef_present_*_async): nothing once chain[0] says a call of the chain did not fit.
+template <bool kGated>
+__global__ void __launch_bounds__(96) ef_clock_commit_kernel(EfClockState* __restrict__ clk, const EfOverlayState* __restrict__ ovl_clk,
+                                                             const uint8_t* __restrict__ bm, uint8_t* __restrict__ slots, const int* __restrict__ chain)
+{
+    if (kGated && *chain) return;
+    const int s = blockIdx.x;
+    const uint32_t flags = clk[s].flags, draw = clk[s].draw;
+    if (!(flags & 1u)) return;
+    if (draw) {
+        uint4* d = (uint4*)(slots + ((size_t)s * 2 + (ovl_clk[s].slot ^ 1u)) * EF_OVERLAY_BYTES);
+        const uint4* src = (const uint4*)(bm + (size_t)s * EF_OVERLAY_BYTES);
+        for (int k = (int)threadIdx.x; k < EF_OVERLAY_BYTES / 16; k += blockDim.x) d[k] = src[k];
+    }
+    if (threadIdx.x == 0) clk[s].last_seconds = clk[s].seconds;
+}
+
+cudaError_t ef_launch_clock_commit(EfClockState* clk, const EfOverlayState* ovl_clk, const uint8_t* bm, uint8_t* slots, int n_streams, const int* chain,
+                                   cudaStream_t stream)
+{
+    if (chain) ef_clock_commit_kernel<true><<<n_streams, 96, 0, stream>>>(clk, ovl_clk, bm, slots, chain);
+    else ef_clock_commit_kernel<false><<<n_streams, 96, 0, stream>>>(clk, ovl_clk, bm, slots, nullptr);
+    return cudaGetLastError();
+}
+
 // the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y). fovl != NULL: the overlay variant, with
 // the per-field overlay fovl and the bitmap slots `bitmaps`. total != NULL: the gated variant, n_fields is the capacity of dst and
 // only the slots below *total are drawn

@@ -50,6 +50,9 @@
  *   ef_present_enable / _picture / _idle  push_video(frame, front, pts, mode) video.cpp:1023-1057 against the frame flip
  *                                 of video_isr video.cpp:1122-1198: every stream's paced composite fields, in HBM
  *   ef_present_*_async / ef_present_wait  the same, enqueued without waiting for the device
+ *   ef_present_overlay            composite() video.cpp:839-887 of every paced field: the overlay bitmap, blend and progress
+ *   ef_present_font / _clock      ESPFlix::update_progress() espflix.cpp:862-874 with show_time() espflix.cpp:163-174: every
+ *                                 stream's time text and progress drawn into its paced overlay on the device
  *   ef_restart_streams           MpegDecoder::reset() + video_reset() (player.cpp:439, video.cpp:1070) or video_pause(0)
  *                                 (video.cpp:1060) for chosen streams of the batch
  *   ef_carry_enable / ef_end_streams / ef_carry_info  the decoder pulling bytes on demand across the producer's Buffers
@@ -377,6 +380,31 @@ int ef_present_wait(ef_ctx* ctx, int* n_presented);
  *                     (the reference's fade arithmetic wraps there). */
 int ef_present_overlay(ef_ctx* ctx, int first, int count, const uint8_t* bitmaps, const int32_t* blend, const int32_t* progress,
                        const uint8_t* set);
+
+/* ef_present_font     the glyph atlas of the overlay's time text, in the layout of the reference's _font8 / _font8_rights
+ *                     (font.h): atlas = 16 rows x 1024 columns of 8-bit coverage, glyph i (character i + 0x18) = columns
+ *                     [rights[i - 1], rights[i]) (from 0 for i = 0). Copied to the device; the library embeds no font.
+ *                     EF_EINVAL unless the rights increase from above 0 up to at most 1024 and n_rights covers 0x18..':' (35).
+ * ef_present_clock    ESPFlix::update_progress() (espflix.cpp:862-874) for streams [first, first + count): idx_hdrs = count x the
+ *                     104-byte video.idx header of the stream's title (idx_hdr, host/ef_indexer.h: what merge_index writes and nav()
+ *                     reads), speed[i] = _speed (0 the title, 1 the fast-forward stream, -1 the rewind stream), flags[i] bit 0 = the
+ *                     clock is on (off is _nav == -1, the default), bit 1 = paused (the pause icon at speed 0), bit 2 = _last_seconds
+ *                     = 0 (what play_pause() and the pause do, espflix.cpp:819, 935). From then on every ef_present_picture /
+ *                     ef_present_idle (and _async) call that is not a sizing call runs, at its start and on every stream whose clock
+ *                     is on: main = pts2pts(get_pts(), speed) (espflix.cpp:597-604; get_pts() = the pts of the picture the call
+ *                     pushes, else the stream's last_pts of ef_picture_pts), seconds = (int)(main / 90000); when seconds !=
+ *                     _last_seconds, show_time(seconds, icon) redraws the bitmap (espflix.cpp:163-174; icon PAUSE / PLAY at speed 0,
+ *                     FFWD, RWND) and _last_seconds = seconds; always progress = (int)(main * 240 / video.last_pts). Bitmap and
+ *                     progress are staged as ef_present_overlay stages them, after what it staged before the call (the last write
+ *                     wins per attribute) and latch by the same rule; the blend stays the caller's. A sizing call, EF_ENOMEM and an
+ *                     async call that does not take effect change no clock state and no bitmap slot. Outside the domain, not
+ *                     checked: products that overflow int64, |main / 90000| >= 2^31 and text over 15 characters. Synchronous, host
+ *                     memory. EF_ESTATE before ef_present_enable or ef_present_font; EF_EINVAL for a bad stream range, a speed
+ *                     outside -1..1, or a stream turned on with video.last_pts 0 or speed +-1 on a trick record whose last_pts
+ *                     equals its first_pts (the reference divides by zero there). ef_reset and ef_restart_streams keep the clocks.
+ *                     A context adds two launches per present call once a clock has been set (one for a sizing call). */
+int ef_present_font(ef_ctx* ctx, const uint8_t* atlas, const int16_t* rights, int n_rights);
+int ef_present_clock(ef_ctx* ctx, int first, int count, const uint8_t* idx_hdrs, const int8_t* speed, const uint8_t* flags);
 
 /* ---- per-stream restart: what the reference's player does on play / skip / fast_forward / rewind / load_poster / play_pause --
  * ef_restart_streams  ops[i] for stream first + i: 0 = nothing; 1 = MpegDecoder::reset() with its video_reset() (player.cpp:439-453,
