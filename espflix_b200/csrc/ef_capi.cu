@@ -17,7 +17,6 @@ int ef_build_tables(EfTables* t);
 void ef_build_color_tab(uint32_t* tab768, int ntsc);
 void ef_build_pal_burst(int16_t* b0, int16_t* b1, int width);
 cudaError_t ef_index_upload_constants();
-const unsigned char* ef_default_intra_ptr();
 cudaError_t ef_launch_scan(EfDev* Dp, const EfCarryArgs* carry, int n_streams, cudaStream_t st);
 cudaError_t ef_launch_pts_resolve(const EfDev* Dp, const uint2* span, const uint32_t* list_off, const int64_t* list_pts, int64_t* carry,
                                   int64_t* last, int64_t* pic_pts, const EfCarryArgs* C, int n_streams, cudaStream_t st);
@@ -96,6 +95,22 @@ int fail(int code, const char* fmt, ...)
         if (e_ != cudaSuccess) return fail(EF_ECUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
 
+// the counterpart of CK for calls that return an EF_* code (and have set the message already)
+#define TRY(call)                                                                                  \
+    do {                                                                                           \
+        const int rc_ = (call);                                                                    \
+        if (rc_ != EF_OK) return rc_;                                                              \
+    } while (0)
+
+int usable_device(int device)
+{
+    int ndev = 0;
+    const cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || device < 0 || ndev <= device)
+        return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", device, cudaGetErrorString(e));
+    return EF_OK;
+}
+
 // Every entry point runs on its context's device whatever the caller's current device is, and leaves the
 // caller's current device as it found it (several contexts on several GPUs may share a host thread).
 struct DeviceScope {
@@ -147,14 +162,13 @@ __global__ void ef_import_frame_kernel(uint8_t* __restrict__ frame, const uint8_
     *(uint32_t*)(frame + dst) = *(const uint32_t*)(src + b);
 }
 
-__global__ void ef_reset_seq_kernel(EfDev* Dp, const uint8_t* default_intra)
+__global__ void ef_reset_seq_kernel(EfDev* Dp)
 {
     EfDev& D = *Dp;
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= D.n_streams) return;
     EfSeq* q = D.seq + (size_t)s * (D.max_seq + 1);
     for (int n = 0; n < 128; n++) q->qz[n] = D.tables->qz[n];
-    (void)default_intra;
     q->mb_width = 22; q->mb_height = 12; q->valid = 1; q->custom = 0; q->fp_rs = 0;
     D.n_pics[s] = 0; D.base_pics[s] = 0; D.n_seq[s] = 0;
 }
@@ -180,13 +194,36 @@ __global__ void ef_restart_kernel(const uint8_t* __restrict__ ops, int first, in
 
 }  // namespace
 
+// Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
+// use a scratch of their own, a context keeps one.
+struct AudioScratch {
+    enum { PLAN, SB_LAST, SLOT, POFF, VROWS, PCM, PDM, INFO, VERDICT, N };
+    void* p[N] = {};
+    size_t cap[N] = {};
+    ~AudioScratch() { for (void* q : p) if (q) cudaFree(q); }
+    cudaError_t get(int k, size_t bytes, void** out)
+    {
+        if (cap[k] < bytes) {
+            if (p[k]) cudaFree(p[k]);
+            p[k] = nullptr; cap[k] = 0;
+            const cudaError_t e = cudaMalloc(&p[k], bytes);
+            if (e != cudaSuccess) return e;
+            cap[k] = bytes;
+        }
+        *out = p[k];
+        return cudaSuccess;
+    }
+    bool fits(int k, size_t bytes) const { return cap[k] >= bytes; }
+};
+
 struct ef_ctx {
     ef_config cfg;
     int sm_count = 0;
     EfDev h;                   // host copy of the device context
     EfDev* d = nullptr;           // = dd[active]
-    std::vector<void*> allocs;
-    std::vector<void*> allocs_host;               // pinned
+    // everything the context owns, released by ef_destroy: device memory (dev_alloc), pinned host memory (host_alloc), events (event)
+    std::vector<void*> allocs, pinned;
+    std::vector<cudaEvent_t> events;
     // Two elementary-stream buffers: a submit uploads into the back one on an internal stream while
     // the kernels of the previous submit still read the front one; ef_index flips them.
     uint8_t* d_es2[2] = { nullptr, nullptr };
@@ -209,9 +246,7 @@ struct ef_ctx {
     uint16_t* d_pkt_stream = nullptr;
     uint64_t* d_stream_total = nullptr;
     uint64_t* d_ts_off = nullptr;
-    uint8_t* d_stage = nullptr;      // read-back staging (I420 / strips)
-    size_t stage_bytes = 0;
-    uint8_t* d_default_intra = nullptr;
+    uint8_t* d_stage = nullptr;      // read-back staging (I420 / strips), one frame
     uint32_t* d_color_tab = nullptr;
     int16_t* d_pal_burst = nullptr;
     uint8_t* d_overlay = nullptr;     // _video_composite bitmap, 16 x 80
@@ -242,7 +277,7 @@ struct ef_ctx {
     uint64_t* d_blob_off = nullptr;
     uint8_t* d_ended = nullptr;
     uint8_t* h_ended = nullptr;                   // pinned
-    struct AudioScratch* aud_scratch = nullptr;
+    AudioScratch aud_scratch;
     // ef_decode_audio_async: whether a call is outstanding, whether it took the current submit's audio, and its verdict
     // (pinned, written by the call's stream). ev_aud_done follows every audio call; ev_ended_free the upload of h_ended.
     bool aud_async = false, aud_async_new = false;
@@ -328,28 +363,6 @@ struct ef_ctx {
     cudaEvent_t ev_scanned = nullptr;             // the last ef_index has written d_held (and resolved the held picture's pts)
 };
 
-// Device buffers of the audio decode whose size follows the frames of one call, grown on demand. The stateless calls
-// use a scratch of their own, a context keeps one.
-struct AudioScratch {
-    enum { PLAN, SB_LAST, SLOT, POFF, VROWS, PCM, PDM, INFO, VERDICT, N };
-    void* p[N] = {};
-    size_t cap[N] = {};
-    ~AudioScratch() { for (void* q : p) if (q) cudaFree(q); }
-    cudaError_t get(int k, size_t bytes, void** out)
-    {
-        if (cap[k] < bytes) {
-            if (p[k]) cudaFree(p[k]);
-            p[k] = nullptr; cap[k] = 0;
-            const cudaError_t e = cudaMalloc(&p[k], bytes);
-            if (e != cudaSuccess) return e;
-            cap[k] = bytes;
-        }
-        *out = p[k];
-        return cudaSuccess;
-    }
-    bool fits(int k, size_t bytes) const { return cap[k] >= bytes; }
-};
-
 namespace {
 
 template <typename T>
@@ -360,6 +373,30 @@ int dev_alloc(ef_ctx* c, T** p, size_t n)
     if (e != cudaSuccess) return fail(EF_ECUDA, "cudaMalloc(%zu bytes): %s", n * sizeof(T), cudaGetErrorString(e));
     c->allocs.push_back(v);
     *p = (T*)v;
+    return EF_OK;
+}
+
+template <typename T>
+int host_alloc(ef_ctx* c, T** p, size_t n)             // pinned
+{
+    CK(cudaHostAlloc((void**)p, n * sizeof(T), cudaHostAllocDefault));
+    c->pinned.push_back(*p);
+    return EF_OK;
+}
+
+int event(ef_ctx* c, cudaEvent_t* e, bool timing = false)
+{
+    CK(timing ? cudaEventCreate(e) : cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    c->events.push_back(*e);
+    return EF_OK;
+}
+
+// streams [first, first + count) of the context; args_ok: the per-stream arguments are there (when count > 0)
+int stream_range(const ef_ctx* c, int first, int count, bool args_ok = true)
+{
+    const int n = c->cfg.n_streams;
+    if (first < 0 || count < 0 || first > n || count > n - first || (count && !args_ok))
+        return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
     return EF_OK;
 }
 
@@ -400,28 +437,26 @@ int carry_clear(ef_ctx* c)
     return EF_OK;
 }
 
-// replace a device allocation of old_n elements by one of new_n, keeping its contents
+// Replace the device allocation *p of old_n elements (or none) by one of new_n, zero-filled after the old contents when keep.
+// The old one is freed (cudaFree waits for the whole device); whatever else may still use it, the caller has waited for.
 template <typename T>
-int dev_grow(ef_ctx* c, T** p, size_t old_n, size_t new_n)
+int dev_grow(ef_ctx* c, T** p, size_t old_n, size_t new_n, bool keep)
 {
     T* q = nullptr;
-    int rc = dev_alloc(c, &q, new_n);
-    if (rc != EF_OK) return rc;
-    CK(cudaMemset(q, 0, new_n * sizeof(T)));
-    CK(cudaMemcpy(q, *p, old_n * sizeof(T), cudaMemcpyDeviceToDevice));
-    for (size_t i = 0; i < c->allocs.size(); i++)
+    TRY(dev_alloc(c, &q, new_n));
+    if (keep) {
+        CK(cudaMemset(q, 0, new_n * sizeof(T)));
+        CK(cudaMemcpy(q, *p, old_n * sizeof(T), cudaMemcpyDeviceToDevice));
+    }
+    for (size_t i = 0; *p && i < c->allocs.size(); i++)
         if (c->allocs[i] == (void*)*p) { cudaFree(*p); c->allocs.erase(c->allocs.begin() + (long)i); break; }
     *p = q;
     return EF_OK;
 }
 
-int ensure_stage(ef_ctx* c, size_t bytes)
+int ensure_stage(ef_ctx* c)
 {
-    if (c->stage_bytes >= bytes) return EF_OK;
-    void* v = nullptr;
-    CK(cudaMalloc(&v, bytes));
-    c->allocs.push_back(v);
-    c->d_stage = (uint8_t*)v; c->stage_bytes = bytes;
+    if (!c->d_stage) TRY(dev_alloc(c, &c->d_stage, EF_FRAME));
     return EF_OK;
 }
 
@@ -461,10 +496,7 @@ int ef_create(ef_ctx** out, const ef_config* cfg)
         cfg->max_slices_per_picture < 1 || cfg->max_slices_per_picture > 176 || cfg->es_capacity < 16)
         return fail(EF_EINVAL, "bad config (n_streams=%d max_pictures=%d max_slices_per_picture=%d es_capacity=%zu)",
                     cfg->n_streams, cfg->max_pictures, cfg->max_slices_per_picture, cfg->es_capacity);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || cfg->device < 0 || ndev <= cfg->device)
-        return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", cfg->device, cudaGetErrorString(e));
+    TRY(usable_device(cfg->device));
     DeviceScope scope_(cfg->device);
     ef_ctx* c = new ef_ctx();
     c->cfg = *cfg;
@@ -488,52 +520,44 @@ int ef_create(ef_ctx** out, const ef_config* cfg)
     h.n_streams = n; h.max_pictures = cfg->max_pictures;
     h.max_slices = cfg->max_pictures * cfg->max_slices_per_picture;
     h.max_seq = cfg->max_pictures;
-    int rc;
-#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
     for (int b = 0; b < 2; b++) {
-        A(c->d_es2[b], cfg->es_capacity + 1024);
-        A(c->d_es_off2[b], (size_t)n + 1);
-        A(c->dd[b], 1);
-        CK(cudaHostAlloc((void**)&c->h_off[b], ((size_t)n + 1) * 8, cudaHostAllocDefault));
-        CK(cudaEventCreateWithFlags(&c->ev_up_done[b], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&c->ev_buf_free[b], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&c->ev_down_done[b], cudaEventDisableTiming));
+        TRY(dev_alloc(c, &c->d_es2[b], cfg->es_capacity + 1024));
+        TRY(dev_alloc(c, &c->d_es_off2[b], (size_t)n + 1));
+        TRY(dev_alloc(c, &c->dd[b], 1));
+        TRY(host_alloc(c, &c->h_off[b], (size_t)n + 1));
+        TRY(event(c, &c->ev_up_done[b])); TRY(event(c, &c->ev_buf_free[b])); TRY(event(c, &c->ev_down_done[b]));
     }
-    CK(cudaEventCreateWithFlags(&c->ev_user, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_export, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_frames_read, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_indexed, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_aud_done, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_ended_free, cudaEventDisableTiming));
+    TRY(event(c, &c->ev_user)); TRY(event(c, &c->ev_export)); TRY(event(c, &c->ev_frames_read));
+    TRY(event(c, &c->ev_indexed)); TRY(event(c, &c->ev_aud_done)); TRY(event(c, &c->ev_ended_free));
     CK(cudaStreamCreateWithFlags(&c->up_stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&c->down_stream, cudaStreamNonBlocking));
-    A(h.frames, (size_t)n * 2 * EF_FRAME + 1024);
-    A(h.seq, (size_t)n * (h.max_seq + 1));
-    A(h.pics, (size_t)n * h.max_pictures);
-    A(h.slice_off, (size_t)n * h.max_slices);
-    A(h.slice_code, (size_t)n * h.max_slices);
-    A(h.n_pics, n); A(h.base_pics, n); A(h.n_seq, n);
-    A(h.pic_pref, (size_t)n * h.max_pictures);
-    A(h.pic_total, h.max_pictures); A(h.pic_base, h.max_pictures); A(h.cursor, h.max_pictures);
+    TRY(dev_alloc(c, &h.frames, (size_t)n * 2 * EF_FRAME + 1024));
+    TRY(dev_alloc(c, &h.seq, (size_t)n * (h.max_seq + 1)));
+    TRY(dev_alloc(c, &h.pics, (size_t)n * h.max_pictures));
+    TRY(dev_alloc(c, &h.slice_off, (size_t)n * h.max_slices));
+    TRY(dev_alloc(c, &h.slice_code, (size_t)n * h.max_slices));
+    TRY(dev_alloc(c, &h.n_pics, n)); TRY(dev_alloc(c, &h.base_pics, n)); TRY(dev_alloc(c, &h.n_seq, n));
+    TRY(dev_alloc(c, &h.pic_pref, (size_t)n * h.max_pictures));
+    TRY(dev_alloc(c, &h.pic_total, h.max_pictures)); TRY(dev_alloc(c, &h.pic_base, h.max_pictures)); TRY(dev_alloc(c, &h.cursor, h.max_pictures));
     h.work_capacity = (size_t)n * h.max_slices;
-    A(h.work, h.work_capacity);
-    A(h.info, 8);
-    EfTables* dt; A(dt, 1);
+    TRY(dev_alloc(c, &h.work, h.work_capacity));
+    TRY(dev_alloc(c, &h.info, 8));
+    EfTables* dt;
+    TRY(dev_alloc(c, &dt, 1));
     {   // macroblock records: as many picture indices per K1a launch as fit in 2 GiB
         const size_t per_pic = (size_t)n * EF_MBW_MAX * EF_MBH_MAX * (sizeof(EfMbRec) + 4);
         size_t k = ((size_t)2 << 30) / per_pic;
         if (const char* e = getenv("EF_REC_PICS")) { const long v = atol(e); if (v >= 1) k = (size_t)v; }   // tuning / test knob
         h.rec_pics = (int)(k < 1 ? 1 : k > (size_t)h.max_pictures ? (size_t)h.max_pictures : k);
         const size_t slots = (size_t)h.rec_pics * n * EF_MBW_MAX * EF_MBH_MAX;
-        A(h.mb_info, slots); A(h.mb_rec, slots);
-        A(h.parse_cursor, (size_t)h.rec_pics + 4);      // [0] K1a, [1..] one per K1b launch
+        TRY(dev_alloc(c, &h.mb_info, slots)); TRY(dev_alloc(c, &h.mb_rec, slots));
+        TRY(dev_alloc(c, &h.parse_cursor, (size_t)h.rec_pics + 4));      // [0] K1a, [1..] one per K1b launch
         h.recon_cursor = h.parse_cursor + 1;
-        A(h.coef, 3 * (cfg->es_capacity + 1024) + 1024);
+        TRY(dev_alloc(c, &h.coef, 3 * (cfg->es_capacity + 1024) + 1024));
     }
-    A(c->d_color_tab, 768); A(c->d_pal_burst, 128); A(c->d_default_intra, 64); A(c->d_overlay, 1280);
+    TRY(dev_alloc(c, &c->d_color_tab, 768)); TRY(dev_alloc(c, &c->d_pal_burst, 128)); TRY(dev_alloc(c, &c->d_overlay, 1280));
     c->present.bitmap = c->d_overlay;
-    if (cfg->fields) { h.field_stride = EF_PAL_FIELD_SAMPLES; A(h.fields, (size_t)n * h.field_stride); }
-#undef A
+    if (cfg->fields) { h.field_stride = EF_PAL_FIELD_SAMPLES; TRY(dev_alloc(c, &h.fields, (size_t)n * h.field_stride)); }
     h.es = c->d_es2[0]; h.es_off = c->d_es_off2[0]; h.tables = dt;
     c->d = c->dd[0];
     h.color_tab = c->d_color_tab; h.pal_burst = c->d_pal_burst;
@@ -542,17 +566,14 @@ int ef_create(ef_ctx** out, const ef_config* cfg)
     const int bad = ef_build_tables(&t);
     if (bad) return fail(EF_EINVAL, "internal: VLC table %d does not fit its lookup shape", bad);
     CK(cudaMemcpy(dt, &t, sizeof(t), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(c->d_default_intra, ef_default_intra_ptr(), 64, cudaMemcpyHostToDevice));
     for (int b = 0; b < 2; b++) {
         CK(cudaMemset(c->d_es2[b], 0, cfg->es_capacity + 1024));
         CK(cudaMemset(c->d_es_off2[b], 0, ((size_t)n + 1) * 8));
     }
     CK(cudaMemset(c->d_overlay, 0, 1280));
-    { int rcp = push_dev(c); if (rcp != EF_OK) return rcp; }
-    rc = ef_reset(c);
-    if (rc != EF_OK) return rc;
-    rc = ef_video_init(c, 1);
-    if (rc != EF_OK) return rc;
+    TRY(push_dev(c));
+    TRY(ef_reset(c));
+    TRY(ef_video_init(c, 1));
     guard.c = nullptr;
     *out = c;
     return EF_OK;
@@ -564,28 +585,8 @@ void ef_destroy(ef_ctx* c)
     if (!c) return;
     cudaDeviceSynchronize();
     for (void* p : c->allocs) cudaFree(p);
-    for (void* p : c->allocs_host) cudaFreeHost(p);
-    if (c->d_desc) cudaFree(c->d_desc);
-    if (c->d_fovl) cudaFree(c->d_fovl);
-    delete c->aud_scratch;
-    if (c->h_ended) cudaFreeHost(c->h_ended);
-    for (int b = 0; b < 2; b++) {
-        if (c->h_off[b]) cudaFreeHost(c->h_off[b]);
-        if (c->ev_up_done[b]) cudaEventDestroy(c->ev_up_done[b]);
-        if (c->ev_buf_free[b]) cudaEventDestroy(c->ev_buf_free[b]);
-        if (c->ev_down_done[b]) cudaEventDestroy(c->ev_down_done[b]);
-    }
-    for (int i = 0; i < 5; i++) if (c->ev_prof[i]) cudaEventDestroy(c->ev_prof[i]);
-    if (c->ev_user) cudaEventDestroy(c->ev_user);
-    if (c->ev_export) cudaEventDestroy(c->ev_export);
-    if (c->ev_frames_read) cudaEventDestroy(c->ev_frames_read);
-    if (c->ev_indexed) cudaEventDestroy(c->ev_indexed);
-    if (c->ev_aud_done) cudaEventDestroy(c->ev_aud_done);
-    if (c->ev_ended_free) cudaEventDestroy(c->ev_ended_free);
-    if (c->ev_pace_done) cudaEventDestroy(c->ev_pace_done);
-    if (c->ev_scanned) cudaEventDestroy(c->ev_scanned);
-    for (cudaEvent_t e : c->ev_pace_ring) if (e) cudaEventDestroy(e);
-    if (c->h_aud_verdict) cudaFreeHost(c->h_aud_verdict);
+    for (void* p : c->pinned) cudaFreeHost(p);
+    for (cudaEvent_t e : c->events) cudaEventDestroy(e);
     if (c->up_stream) cudaStreamDestroy(c->up_stream);
     if (c->down_stream) cudaStreamDestroy(c->down_stream);
     delete c;
@@ -633,11 +634,11 @@ int ef_reset(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    { int rcw = wait_frames_read(c); if (rcw != EF_OK) return rcw; }
-    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    TRY(wait_frames_read(c));
+    TRY(audio_resolve(c));
+    TRY(pace_resolve(c));
     CK(cudaMemset(c->h.frames, 0, (size_t)c->cfg.n_streams * 2 * EF_FRAME + 1024));     // Frame::init zero-fills (player.cpp:25)
-    ef_reset_seq_kernel<<<(c->cfg.n_streams + 127) / 128, 128>>>(c->d, c->d_default_intra);
+    ef_reset_seq_kernel<<<(c->cfg.n_streams + 127) / 128, 128>>>(c->d);
     CK(cudaGetLastError());
     c->launches++;
     CK(cudaMemset(c->h.info, 0, 32));
@@ -657,8 +658,7 @@ int ef_reset(ef_ctx* c)
         CK(cudaMemset2D((uint8_t*)c->d_pace + offsetof(EfPaceState, fc_origin), sizeof(EfPaceState), 0, 4, (size_t)c->cfg.n_streams));
     if (c->carry) {                                       // every stream's held bytes are dropped; carry stays enabled
         CK(cudaDeviceSynchronize());
-        int rcc = carry_clear(c);
-        if (rcc != EF_OK) return rcc;
+        TRY(carry_clear(c));
     }
     CK(cudaDeviceSynchronize());
     c->indexed = false; c->submitted = false; c->pending = -1;
@@ -673,25 +673,23 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     const int n = c->cfg.n_streams;
-    if (first < 0 || count < 0 || first > n || count > n - first || (count && !ops))
-        return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    TRY(stream_range(c, first, count, ops));
     bool any_reset = false;
     for (int i = 0; i < count; i++) {
         if (ops[i] > 2) return fail(EF_EINVAL, "op %d of stream %d is not 0..2", ops[i], first + i);
         any_reset |= ops[i] == 1;
     }
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    TRY(pace_resolve(c));
     if (c->paced && c->pace_indexed) {                    // the schedule of the current submit must be complete
-        int rc = pace_pictures(c);
-        if (rc != EF_OK) return rc;
+        TRY(pace_pictures(c));
         if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_restart_streams while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
     }
-    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+    TRY(audio_resolve(c));
     if (c->audio && c->aud_unconsumed) return fail(EF_ESTATE, "ef_restart_streams before ef_decode_audio consumed the current submit's audio");
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     const bool audio = c->audio && any_reset;
-    if (!c->d_restart_ops) { int rc = dev_alloc(c, &c->d_restart_ops, (size_t)n); if (rc != EF_OK) return rc; }
+    if (!c->d_restart_ops) TRY(dev_alloc(c, &c->d_restart_ops, (size_t)n));
     CK(cudaMemcpy(c->d_restart_ops, ops, (size_t)count, cudaMemcpyHostToDevice));
     if (audio) CK(cudaMemset(c->d_ended, 0, (size_t)n));
     ef_restart_kernel<<<(count + 127) / 128, 128>>>(c->d_restart_ops, first, count, c->paced ? c->d_pace : nullptr, c->pts ? c->d_pts_last : nullptr,
@@ -753,19 +751,20 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
     } else {
         const uint64_t n_packets = total / 188;
         if (!c->d_ts) {
-            int rc;
-            if ((rc = dev_alloc(c, &c->d_ts, c->cfg.es_capacity + 64)) != EF_OK) return rc;
-            if ((rc = dev_alloc(c, &c->d_pkt_len, c->cfg.es_capacity / 188 + 1)) != EF_OK) return rc;
-            if ((rc = dev_alloc(c, &c->d_pkt_off, c->cfg.es_capacity / 188 + 1)) != EF_OK) return rc;
-            if ((rc = dev_alloc(c, &c->d_pkt_stream, c->cfg.es_capacity / 188 + 1)) != EF_OK) return rc;
-            if ((rc = dev_alloc(c, &c->d_stream_total, (size_t)n + 1)) != EF_OK) return rc;
-            if ((rc = dev_alloc(c, &c->d_ts_off, (size_t)n + 1)) != EF_OK) return rc;
+            TRY(dev_alloc(c, &c->d_ts, c->cfg.es_capacity + 64));
+            TRY(dev_alloc(c, &c->d_pkt_len, c->cfg.es_capacity / 188 + 1));
+            TRY(dev_alloc(c, &c->d_pkt_off, c->cfg.es_capacity / 188 + 1));
+            TRY(dev_alloc(c, &c->d_pkt_stream, c->cfg.es_capacity / 188 + 1));
+            TRY(dev_alloc(c, &c->d_stream_total, (size_t)n + 1));
+            TRY(dev_alloc(c, &c->d_ts_off, (size_t)n + 1));
         }
         CK(cudaMemcpyAsync(c->d_ts, src, total, kind, up));
         CK(cudaMemcpyAsync(c->d_ts_off, hoff, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, up));
-        if (c->carry) {
-            // every stream's region: its held bytes (known once the last ef_index has run), then the new payload
-            const int a = c->active;
+        // packet lengths, every stream's payload bytes and packet positions, the ES offsets, the payload copy; on a carrying
+        // context every stream's region starts with its held bytes (known once the last ef_index has run), then the new payload
+        const bool carry = c->carry;
+        const int a = c->active;
+        if (carry || n_packets) {
             if (n_packets) {
                 ef_ts_len_kernel<<<(unsigned)((n_packets + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_len);
                 CK(cudaGetLastError());
@@ -773,32 +772,32 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
             }
             ef_ts_scan_kernel<<<n, 256, 0, up>>>(c->d_pkt_len, c->d_ts_off, c->d_pkt_off, c->d_pkt_stream, c->d_stream_total);
             CK(cudaGetLastError());
-            CK(cudaStreamWaitEvent(up, c->ev_scanned, 0));
-            ef_carry_lead_kernel<<<(n + 255) / 256, 256, 0, up>>>(c->d_held, n, c->d_stream_total, c->d_held_in2[b]);
-            CK(cudaGetLastError());
-            ef_ts_offsets_kernel<<<1, 1024, 0, up>>>(c->d_stream_total, n, d_es_off, d_es);
-            CK(cudaGetLastError());
-            ef_carry_copy_kernel<<<(n * 32 + 127) / 128, 128, 0, up>>>(c->d_es2[a], c->d_es_off2[a], c->d_held, d_es_off, d_es, c->d_pay_off, n);
-            CK(cudaGetLastError());
-            c->launches += 4;
-            if (n_packets) {
-                ef_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_off, c->d_pkt_stream, c->d_pay_off, d_es);
+            c->launches++;
+            if (carry) {
+                CK(cudaStreamWaitEvent(up, c->ev_scanned, 0));
+                ef_carry_lead_kernel<<<(n + 255) / 256, 256, 0, up>>>(c->d_held, n, c->d_stream_total, c->d_held_in2[b]);
                 CK(cudaGetLastError());
                 c->launches++;
             }
-            CK(cudaMemsetAsync(c->d_end2[b], 0, (size_t)n, up));
-            c->h_end2[b].assign((size_t)n, 0);
-        } else if (n_packets) {
-            ef_ts_len_kernel<<<(unsigned)((n_packets + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_len);
-            CK(cudaGetLastError());
-            ef_ts_scan_kernel<<<n, 256, 0, up>>>(c->d_pkt_len, c->d_ts_off, c->d_pkt_off, c->d_pkt_stream, c->d_stream_total);
-            CK(cudaGetLastError());
             ef_ts_offsets_kernel<<<1, 1024, 0, up>>>(c->d_stream_total, n, d_es_off, d_es);
             CK(cudaGetLastError());
-            ef_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_off, c->d_pkt_stream, d_es_off, d_es);
-            CK(cudaGetLastError());
-            c->launches += 4;
+            c->launches++;
+            if (carry) {
+                ef_carry_copy_kernel<<<(n * 32 + 127) / 128, 128, 0, up>>>(c->d_es2[a], c->d_es_off2[a], c->d_held, d_es_off, d_es, c->d_pay_off, n);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
+            if (n_packets) {
+                ef_ts_copy_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, up>>>(c->d_ts, n_packets, c->d_pkt_off, c->d_pkt_stream,
+                                                                                            carry ? c->d_pay_off : d_es_off, d_es);
+                CK(cudaGetLastError());
+                c->launches++;
+            }
         } else CK(cudaMemsetAsync(d_es_off, 0, ((size_t)n + 1) * 8, up));
+        if (carry) {
+            CK(cudaMemsetAsync(c->d_end2[b], 0, (size_t)n, up));
+            c->h_end2[b].assign((size_t)n, 0);
+        }
     }
     if (c->pts) {                                         // the video PES starts of this submit, into its ES buffer's list
         if (ts) {
@@ -853,14 +852,13 @@ int ef_index(ef_ctx* c, void* stream)
     if (c->carry && c->pending < 0) return fail(EF_ESTATE, "ef_index without a fresh submit on a carrying context (its held bytes have moved on)");
     cudaStream_t st = (cudaStream_t)stream;
     const int n = c->cfg.n_streams;
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    TRY(pace_resolve(c));
     if (c->paced && c->pace_indexed) {                    // the schedule needs every picture of the current submit
-        int rc = pace_pictures(c);
-        if (rc != EF_OK) return rc;
+        TRY(pace_pictures(c));
         if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_index while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
     }
     if (c->pending >= 0) {                       // a fresh submit: wait for its upload, make it the front buffer
-        { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+        TRY(audio_resolve(c));
         if (c->audio && c->aud_unconsumed)       // the audio of a TS submit is delivered exactly once
             return fail(EF_ESTATE, "ef_index of a new submit before ef_decode_audio consumed the current submit's audio");
         CK(cudaStreamWaitEvent(st, c->ev_up_done[c->pending], 0));
@@ -930,25 +928,22 @@ int ef_carry_enable(ef_ctx* c, uint32_t max_carry)
     if (c->carry) return fail(EF_ESTATE, "carry is already enabled");
     if (c->pending >= 0) return fail(EF_ESTATE, "ef_carry_enable with a submit pending: enable it before the next submit");
     if (max_carry < 4) return fail(EF_EINVAL, "max_carry %u must be at least 4 bytes", max_carry);
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
-    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+    TRY(pace_resolve(c));
+    TRY(audio_resolve(c));
     const size_t n = (size_t)c->cfg.n_streams, extra = n * max_carry;
     const size_t es_old = c->cfg.es_capacity + 1024, es_new = es_old + extra;
     CK(cudaDeviceSynchronize());
-    int rc;
     // both ES buffers and everything sized from them (the coefficient lists of K1a, 3 entries per ES byte) grow by n x max_carry;
     // the front buffer keeps the current submit, which may still be decoded
-    for (int b = 0; b < 2; b++) if ((rc = dev_grow(c, &c->d_es2[b], es_old, es_new)) != EF_OK) return rc;
-    if ((rc = dev_grow(c, &c->h.coef, 3 * es_old + 1024, 3 * es_new + 1024)) != EF_OK) return rc;
-#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
-    A(c->d_held, n); A(c->d_held_code, n); A(c->d_carry_flags, n); A(c->d_pay_off, n + 1);
-    A(c->d_pts_hold, n); A(c->d_pts_pre, n);
-    for (int b = 0; b < 2; b++) { A(c->d_held_in2[b], n); A(c->d_end2[b], n); }
-#undef A
+    for (int b = 0; b < 2; b++) TRY(dev_grow(c, &c->d_es2[b], es_old, es_new, true));
+    TRY(dev_grow(c, &c->h.coef, 3 * es_old + 1024, 3 * es_new + 1024, true));
+    TRY(dev_alloc(c, &c->d_held, n)); TRY(dev_alloc(c, &c->d_held_code, n)); TRY(dev_alloc(c, &c->d_carry_flags, n));
+    TRY(dev_alloc(c, &c->d_pay_off, n + 1)); TRY(dev_alloc(c, &c->d_pts_hold, n)); TRY(dev_alloc(c, &c->d_pts_pre, n));
+    for (int b = 0; b < 2; b++) { TRY(dev_alloc(c, &c->d_held_in2[b], n)); TRY(dev_alloc(c, &c->d_end2[b], n)); }
     c->max_carry = max_carry;
-    if ((rc = carry_clear(c)) != EF_OK) return rc;
-    if ((rc = push_dev(c)) != EF_OK) return rc;
-    if (!c->ev_scanned) CK(cudaEventCreateWithFlags(&c->ev_scanned, cudaEventDisableTiming));
+    TRY(carry_clear(c));
+    TRY(push_dev(c));
+    if (!c->ev_scanned) TRY(event(c, &c->ev_scanned));
     CK(cudaEventRecord(c->ev_scanned, 0));
     CK(cudaDeviceSynchronize());
     c->carry = true;
@@ -959,9 +954,7 @@ int ef_end_streams(ef_ctx* c, int first, int count, const uint8_t* ends)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    const int n = c->cfg.n_streams;
-    if (first < 0 || count < 0 || first > n || count > n - first || (count && !ends))
-        return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    TRY(stream_range(c, first, count, ends));
     if (!c->carry) return fail(EF_ESTATE, "ef_end_streams before ef_carry_enable");
     if (c->pending < 0) return fail(EF_ESTATE, "ef_end_streams with no submit pending");
     if (!count) return EF_OK;
@@ -978,8 +971,7 @@ int ef_carry_info(ef_ctx* c, int first, int count, uint32_t* held_bytes, uint8_t
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    const int n = c->cfg.n_streams;
-    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    TRY(stream_range(c, first, count));
     if (!c->carry) return fail(EF_ESTATE, "ef_carry_info before ef_carry_enable");
     CK(cudaDeviceSynchronize());
     if (held_bytes && count) CK(cudaMemcpy(held_bytes, c->d_held + first, (size_t)count * 4, cudaMemcpyDeviceToHost));
@@ -1005,10 +997,8 @@ static int ensure_stage2(ef_ctx* c, int k, size_t bytes)
 {
     if (c->stage2_bytes[k] >= bytes) return EF_OK;
     CK(cudaEventSynchronize(c->ev_down_done[k]));
-    void* v = nullptr;
-    CK(cudaMalloc(&v, bytes));
-    c->allocs.push_back(v);
-    c->d_stage2[k] = (uint8_t*)v; c->stage2_bytes[k] = bytes;
+    TRY(dev_grow(c, &c->d_stage2[k], c->stage2_bytes[k], bytes, false));
+    c->stage2_bytes[k] = bytes;
     return EF_OK;
 }
 
@@ -1047,14 +1037,13 @@ static int decode_recon(ef_ctx* c, int i, cudaStream_t st)
 static int decode_range(ef_ctx* c, int p0, int k, cudaStream_t st, uint8_t* host_dst = nullptr, int layout = 0)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
-    int rc = decode_parse(c, p0, k, st);
-    if (rc != EF_OK) return rc;
+    TRY(decode_parse(c, p0, k, st));
     const size_t batch_bytes = (size_t)c->cfg.n_streams * EF_FRAME;
     for (int i = 0; i < k; i++) {
-        if ((rc = decode_recon(c, i, st)) != EF_OK) return rc;
+        TRY(decode_recon(c, i, st));
         if (host_dst) {
             const int b = c->stage_idx ^= 1;
-            if ((rc = ensure_stage2(c, b, batch_bytes)) != EF_OK) return rc;
+            TRY(ensure_stage2(c, b, batch_bytes));
             CK(cudaStreamWaitEvent(st, c->ev_down_done[b], 0));            // the previous copy out of this staging buffer has finished
             const uint64_t threads = (uint64_t)c->cfg.n_streams * (EF_FRAME / 8);
             ef_export_frames_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(c->h.frames, c->h.base_pics, c->h.n_pics, 0, c->cfg.n_streams, -2 - (p0 + i), layout, c->d_stage2[b]);
@@ -1080,50 +1069,68 @@ int ef_decode_picture(ef_ctx* c, int pic, void* stream)
     return decode_range(c, pic, 1, (cudaStream_t)stream);
 }
 
-int ef_decode_all(ef_ctx* c, int n_pictures, void* stream)
+// ef_decode_all(_to_host): picture indices [0, n_pictures), rec_pics of them per K1a launch
+static int decode_all(ef_ctx* c, const char* what, int n_pictures, void* stream, uint8_t* host_dst = nullptr, int layout = 0)
 {
-    if (!c) return fail(EF_EINVAL, "null context");
-    if (!c->indexed) return fail(EF_ESTATE, "ef_decode_all before ef_index");
-    if (c->paced) return fail(EF_ESTATE, "ef_decode_all on a presenting context: ef_present_picture decodes");
+    if (!c->indexed) return fail(EF_ESTATE, "%s before ef_index", what);
+    if (c->paced) return fail(EF_ESTATE, "%s on a presenting context: ef_present_picture decodes", what);
     if (n_pictures < 0 || n_pictures > c->cfg.max_pictures) return fail(EF_EINVAL, "n_pictures %d out of range", n_pictures);
     for (int p = 0; p < n_pictures; p += c->h.rec_pics) {
         const int k = n_pictures - p < c->h.rec_pics ? n_pictures - p : c->h.rec_pics;
-        int rc = decode_range(c, p, k, (cudaStream_t)stream);
-        if (rc != EF_OK) return rc;
+        TRY(decode_range(c, p, k, (cudaStream_t)stream, host_dst, layout));
     }
     return EF_OK;
+}
+
+int ef_decode_all(ef_ctx* c, int n_pictures, void* stream)
+{
+    if (!c) return fail(EF_EINVAL, "null context");
+    return decode_all(c, "ef_decode_all", n_pictures, stream);
 }
 
 int ef_decode_all_to_host(ef_ctx* c, int n_pictures, uint8_t* dst, int layout, void* stream)
 {
     if (!c || !dst) return fail(EF_EINVAL, "null argument");
     if (layout != 0 && layout != 1) return fail(EF_EINVAL, "layout must be 0 (I420) or 1 (strips)");
-    if (!c->indexed) return fail(EF_ESTATE, "ef_decode_all_to_host before ef_index");
-    if (c->paced) return fail(EF_ESTATE, "ef_decode_all_to_host on a presenting context: ef_present_picture decodes");
-    if (n_pictures < 0 || n_pictures > c->cfg.max_pictures) return fail(EF_EINVAL, "n_pictures %d out of range", n_pictures);
-    for (int p = 0; p < n_pictures; p += c->h.rec_pics) {
-        const int k = n_pictures - p < c->h.rec_pics ? n_pictures - p : c->h.rec_pics;
-        int rc = decode_range(c, p, k, (cudaStream_t)stream, dst, layout);
-        if (rc != EF_OK) return rc;
-    }
-    return EF_OK;
+    return decode_all(c, "ef_decode_all_to_host", n_pictures, stream, dst, layout);
 }
 
-int ef_read_frame(ef_ctx* c, int stream_index, int fb, uint8_t* dst)
+// one frame store to the host (ef_read_frame(_i420)) or from it (ef_write_frame(_i420)) in `layout`: 0 = I420, 1 = strips
+static int read_frame(ef_ctx* c, int stream_index, int fb, uint8_t* dst, int layout)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !dst) return fail(EF_EINVAL, "null argument");
     CK(cudaDeviceSynchronize());
-    int f; int rc = resolve_fb(c, stream_index, fb, &f);
-    if (rc != EF_OK) return rc;
-    rc = ensure_stage(c, EF_FRAME);
-    if (rc != EF_OK) return rc;
-    ef_export_frames_kernel<<<(EF_FRAME / 8 + 255) / 256, 256>>>(c->h.frames, c->h.base_pics, c->h.n_pics, stream_index, 1, f, 1, c->d_stage);
+    int f;
+    TRY(resolve_fb(c, stream_index, fb, &f));
+    TRY(ensure_stage(c));
+    ef_export_frames_kernel<<<(EF_FRAME / 8 + 255) / 256, 256>>>(c->h.frames, c->h.base_pics, c->h.n_pics, stream_index, 1, f, layout, c->d_stage);
     CK(cudaGetLastError());
     c->launches++;
     CK(cudaMemcpy(dst, c->d_stage, EF_FRAME, cudaMemcpyDeviceToHost));
     return EF_OK;
 }
+
+static int write_frame(ef_ctx* c, int stream_index, int fb, const uint8_t* src, int layout)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !src) return fail(EF_EINVAL, "null argument");
+    int f;
+    TRY(resolve_fb(c, stream_index, fb, &f));
+    TRY(ensure_stage(c));
+    TRY(wait_frames_read(c));
+    CK(cudaMemcpy(c->d_stage, src, EF_FRAME, cudaMemcpyHostToDevice));
+    ef_import_frame_kernel<<<(EF_FRAME / 4 + 255) / 256, 256>>>(c->h.frames + ef_frame_offset(stream_index, f), c->d_stage, layout);
+    CK(cudaGetLastError());
+    c->launches++;
+    CK(cudaDeviceSynchronize());
+    return EF_OK;
+}
+
+int ef_read_frame(ef_ctx* c, int stream_index, int fb, uint8_t* dst) { return read_frame(c, stream_index, fb, dst, 1); }
+int ef_read_frame_i420(ef_ctx* c, int stream_index, int fb, uint8_t* dst) { return read_frame(c, stream_index, fb, dst, 0); }
+int ef_write_frame(ef_ctx* c, int stream_index, int fb, const uint8_t* src) { return write_frame(c, stream_index, fb, src, 1); }
+int ef_write_frame_i420(ef_ctx* c, int stream_index, int fb, const uint8_t* src) { return write_frame(c, stream_index, fb, src, 0); }
 
 int ef_read_latest_i420_async(ef_ctx* c, int first, int count, uint8_t* dst, void* stream)
 {
@@ -1132,12 +1139,12 @@ int ef_read_latest_i420_async(ef_ctx* c, int first, int count, uint8_t* dst, voi
     if (first < 0 || count < 1 || first + count > c->cfg.n_streams) return fail(EF_EINVAL, "stream range out of bounds");
     const int k = c->stage_idx ^= 1;
     const size_t bytes = (size_t)count * EF_FRAME;
-    { int rc = ensure_stage2(c, k, bytes); if (rc != EF_OK) return rc; }
+    TRY(ensure_stage2(c, k, bytes));
     cudaStream_t st = (cudaStream_t)stream;
     // The tiled -> I420 export runs on the read-back stream, behind everything queued on the caller's stream so far and
     // behind the previous copy out of this staging buffer: it overlaps the index / parse kernels of the next submit. The
     // next reconstruction launch (the first thing that writes a frame store again) waits for ev_frames_read.
-    if (!c->d_fb_snap[k]) { int rc = dev_alloc(c, &c->d_fb_snap[k], (size_t)c->cfg.n_streams); if (rc != EF_OK) return rc; }
+    if (!c->d_fb_snap[k]) TRY(dev_alloc(c, &c->d_fb_snap[k], (size_t)c->cfg.n_streams));
     CK(cudaStreamWaitEvent(st, c->ev_down_done[k], 0));        // the previous read-back through this staging buffer (and its snapshot) has finished
     ef_latest_fb_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(c->h.base_pics, c->h.n_pics, first, count, c->d_fb_snap[k]);
     CK(cudaGetLastError());
@@ -1166,59 +1173,8 @@ int ef_sync(ef_ctx* c, void* stream)
 
 int ef_read_latest_i420(ef_ctx* c, int first, int count, uint8_t* dst, void* stream)
 {
-    int rc = ef_read_latest_i420_async(c, first, count, dst, stream);
-    if (rc != EF_OK) return rc;
+    TRY(ef_read_latest_i420_async(c, first, count, dst, stream));
     CK(cudaStreamSynchronize(c->down_stream));
-    return EF_OK;
-}
-
-int ef_read_frame_i420(ef_ctx* c, int stream_index, int fb, uint8_t* dst)
-{
-    DeviceScope scope_(c ? c->cfg.device : -1);
-    if (!c || !dst) return fail(EF_EINVAL, "null argument");
-    CK(cudaDeviceSynchronize());
-    int f; int rc = resolve_fb(c, stream_index, fb, &f);
-    if (rc != EF_OK) return rc;
-    rc = ensure_stage(c, EF_FRAME);
-    if (rc != EF_OK) return rc;
-    ef_export_frames_kernel<<<(EF_FRAME / 8 + 255) / 256, 256>>>(c->h.frames, c->h.base_pics, c->h.n_pics, stream_index, 1, f, 0, c->d_stage);
-    CK(cudaGetLastError());
-    c->launches++;
-    CK(cudaMemcpy(dst, c->d_stage, EF_FRAME, cudaMemcpyDeviceToHost));
-    return EF_OK;
-}
-
-int ef_write_frame_i420(ef_ctx* c, int stream_index, int fb, const uint8_t* src)
-{
-    DeviceScope scope_(c ? c->cfg.device : -1);
-    if (!c || !src) return fail(EF_EINVAL, "null argument");
-    int f; int rc = resolve_fb(c, stream_index, fb, &f);
-    if (rc != EF_OK) return rc;
-    rc = ensure_stage(c, EF_FRAME);
-    if (rc != EF_OK) return rc;
-    if ((rc = wait_frames_read(c)) != EF_OK) return rc;
-    CK(cudaMemcpy(c->d_stage, src, EF_FRAME, cudaMemcpyHostToDevice));
-    ef_import_frame_kernel<<<(EF_FRAME / 4 + 255) / 256, 256>>>(c->h.frames + ef_frame_offset(stream_index, f), c->d_stage, 0);
-    CK(cudaGetLastError());
-    c->launches++;
-    CK(cudaDeviceSynchronize());
-    return EF_OK;
-}
-
-int ef_write_frame(ef_ctx* c, int stream_index, int fb, const uint8_t* src)
-{
-    DeviceScope scope_(c ? c->cfg.device : -1);
-    if (!c || !src) return fail(EF_EINVAL, "null argument");
-    int f; int rc = resolve_fb(c, stream_index, fb, &f);
-    if (rc != EF_OK) return rc;
-    rc = ensure_stage(c, EF_FRAME);
-    if (rc != EF_OK) return rc;
-    if ((rc = wait_frames_read(c)) != EF_OK) return rc;
-    CK(cudaMemcpy(c->d_stage, src, EF_FRAME, cudaMemcpyHostToDevice));
-    ef_import_frame_kernel<<<(EF_FRAME / 4 + 255) / 256, 256>>>(c->h.frames + ef_frame_offset(stream_index, f), c->d_stage, 1);
-    CK(cudaGetLastError());
-    c->launches++;
-    CK(cudaDeviceSynchronize());
     return EF_OK;
 }
 
@@ -1234,7 +1190,7 @@ int ef_video_init(ef_ctx* c, int ntsc)
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     if (c->paced && (ntsc ? 1 : 0) != c->pace_ntsc) return fail(EF_ESTATE, "the standard of a presenting context is fixed by ef_present_enable");
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
+    TRY(pace_resolve(c));
     EfGeometry g;
     memset(&g, 0, sizeof(g));
     g.ntsc = ntsc ? 1 : 0;
@@ -1255,7 +1211,7 @@ int ef_video_init(ef_ctx* c, int ntsc)
     CK(cudaMemcpy(c->d_color_tab, tab, sizeof(tab), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(c->d_pal_burst, burst, sizeof(burst), cudaMemcpyHostToDevice));
     c->h.geo = g;
-    { int rcp = push_dev(c); if (rcp != EF_OK) return rcp; }
+    TRY(push_dev(c));
     c->video = true;
     return EF_OK;
 }
@@ -1326,12 +1282,11 @@ int ef_blit(ef_ctx* c, int stream_index, int fb, uint16_t* dst, int line, int x,
     if (!c || !dst) return fail(EF_EINVAL, "null argument");
     const int w8 = (width + 7) & ~7;          // the reference loop advances 8 pixels per iteration (video.cpp:709): the whole last group is written
     if (line < 0 || line >= EF_H || x < 0 || width < 0 || (x & ~3) + w8 > EF_W) return fail(EF_EINVAL, "blit span out of range (the width is rounded up to a multiple of 8 pixels)");
-    int f; int rc = resolve_fb(c, stream_index, fb, &f);
-    if (rc != EF_OK) return rc;
+    int f;
+    TRY(resolve_fb(c, stream_index, fb, &f));
     if (!w8) return EF_OK;
     CK(cudaDeviceSynchronize());              // like ef_read_frame: a decode may still be running on a non-blocking user stream
-    rc = ensure_stage(c, EF_FRAME);
-    if (rc != EF_OK) return rc;
+    TRY(ensure_stage(c));
     CK(ef_launch_blit(c->d, stream_index, f, line, x, w8, frame_counter, (uint16_t*)c->d_stage, 0));
     c->launches++;
     // blit() itself offsets PAL output by 80 samples (video.cpp:698)
@@ -1354,7 +1309,7 @@ int ef_set_profiling(ef_ctx* c, int on)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    if (on && !c->ev_prof[0]) for (int i = 0; i < 5; i++) CK(cudaEventCreate(&c->ev_prof[i]));
+    if (on && !c->ev_prof[0]) for (int i = 0; i < 5; i++) TRY(event(c, &c->ev_prof[i], true));
     c->profiling = on != 0;
     c->prof_index = c->prof_decode = false;
     return EF_OK;
@@ -1396,9 +1351,7 @@ int ef_tsidx_scan(int device, const uint8_t* ts, const uint64_t* off, int n_file
                   ef_tsidx_info* info, int64_t* seq_pts, uint32_t* seq_pos)
 {
     if (!ts || !off || !info || !seq_pts || !seq_pos || n_files < 1) return fail(EF_EINVAL, "null argument");
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev <= device) return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", device, cudaGetErrorString(e));
+    TRY(usable_device(device));
     DeviceScope scope_(device);
     for (int f = 0; f <= n_files; f++) if (off[f] % 188 || (f && off[f] < off[f - 1])) return fail(EF_EINVAL, "offsets must be non-decreasing multiples of 188");
     const uint64_t total = off[n_files] - off[0], n_packets = total / 188;
@@ -1437,9 +1390,7 @@ int ef_tsidx_samples(int device, const int64_t* seq_pts, const uint32_t* seq_pos
     *n_samples = n;
     if (!n) return EF_OK;
     if (!samples || cap < n) return fail(EF_ENOMEM, "%u samples needed, capacity %u", n, cap);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev <= device) return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", device, cudaGetErrorString(e));
+    TRY(usable_device(device));
     DeviceScope scope_(device);
     DevBuf d_pts, d_pos, d_out;
     CK(d_pts.alloc((size_t)n_seq * 8)); CK(d_pos.alloc((size_t)n_seq * 4)); CK(d_out.alloc((size_t)n * 4));
@@ -1452,14 +1403,6 @@ int ef_tsidx_samples(int device, const int64_t* seq_pts, const uint32_t* seq_pos
 }
 
 // ---- audio (SURVEY.md 8f-3): SBC decode + PDM ---------------------------------------------------------------------
-static int audio_device(int device)
-{
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || device < 0 || ndev <= device) return fail(EF_ECUDA, "no usable CUDA device %d (%s); this library has no CPU path", device, cudaGetErrorString(e));
-    return EF_OK;
-}
-
 static int audio_constants(int device)
 {
     static bool constants = false;                       // per process; every device gets its copy on first use
@@ -1542,10 +1485,9 @@ template <typename After>
 static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAudioState* st, const uint8_t* ended, int n, AudioScratch& w,
                              ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm, cudaStream_t cs, uint64_t* launches, After after)
 {
-    int rc;
-    if ((rc = audio_scratch(w, n, 0)) != EF_OK) return rc;
+    TRY(audio_scratch(w, n, 0));
     ef_audio_info* d_info = (ef_audio_info*)w.p[AudioScratch::INFO];
-    if ((rc = audio_plan(blob, blob_off, st, ended, n, w, pcm ? pcm_cap : ~0ull, d_info, cs, launches)) != EF_OK) return rc;
+    TRY(audio_plan(blob, blob_off, st, ended, n, w, pcm ? pcm_cap : ~0ull, d_info, cs, launches));
     CK(cudaMemcpyAsync(info, d_info, (size_t)n * sizeof(ef_audio_info), cudaMemcpyDeviceToHost, cs));
     CK(cudaStreamSynchronize(cs));
     const uint64_t n_pcm = info[n - 1].pcm_offset + (uint64_t)info[n - 1].n_frames * 128;
@@ -1553,11 +1495,11 @@ static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAu
     if (n_pcm > pcm_cap) return fail(EF_ENOMEM, "%llu PCM samples, capacity %llu", (unsigned long long)n_pcm, (unsigned long long)pcm_cap);
     int16_t* d_pcm = nullptr;
     uint16_t* d_pdm = nullptr;
-    if ((rc = audio_scratch(w, n, n_pcm)) != EF_OK) return rc;
+    TRY(audio_scratch(w, n, n_pcm));
     CK(w.get(AudioScratch::PCM, n_pcm * 2, (void**)&d_pcm));
     if (pdm) CK(w.get(AudioScratch::PDM, n_pcm * 4, (void**)&d_pdm));
-    if ((rc = audio_run(blob, blob_off, st, ended, n, w, n_pcm, d_pcm, pdm ? d_pdm : nullptr, false, cs, launches)) != EF_OK) return rc;
-    if ((rc = after()) != EF_OK) return rc;
+    TRY(audio_run(blob, blob_off, st, ended, n, w, n_pcm, d_pcm, pdm ? d_pdm : nullptr, false, cs, launches));
+    TRY(after());
     if (n_pcm) {
         CK(cudaMemcpyAsync(pcm, d_pcm, n_pcm * 2, cudaMemcpyDeviceToHost, cs));
         if (pdm) CK(cudaMemcpyAsync(pdm, d_pdm, n_pcm * 4, cudaMemcpyDeviceToHost, cs));
@@ -1570,8 +1512,7 @@ static int audio_decode_blob(const uint8_t* blob, const uint64_t* blob_off, EfAu
 int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_files, uint8_t* es, uint64_t es_cap, uint64_t* es_off)
 {
     if (!ts || !off || !es_off || n_files < 1) return fail(EF_EINVAL, "null argument");
-    int rc = audio_device(device);
-    if (rc != EF_OK) return rc;
+    TRY(usable_device(device));
     DeviceScope scope_(device);
     for (int f = 0; f <= n_files; f++) if (off[f] % 188 || (f && off[f] < off[f - 1])) return fail(EF_EINVAL, "offsets must be non-decreasing multiples of 188");
     const uint64_t total = off[n_files] - off[0], n_packets = total / 188;
@@ -1612,11 +1553,10 @@ int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_
 int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_streams, ef_audio_info* info, int16_t* pcm, uint64_t pcm_cap, uint16_t* pdm)
 {
     if (!sbc || !off || !info || n_streams < 1) return fail(EF_EINVAL, "null argument");
-    int rc = audio_device(device);
-    if (rc != EF_OK) return rc;
+    TRY(usable_device(device));
     DeviceScope scope_(device);
     for (int s = 0; s < n_streams; s++) if (off[s] > off[s + 1]) return fail(EF_EINVAL, "stream offsets must be non-decreasing");
-    if ((rc = audio_constants(device)) != EF_OK) return rc;
+    TRY(audio_constants(device));
     const uint64_t total = off[n_streams] - off[0];
     std::vector<uint64_t> roff((size_t)n_streams + 1);
     for (int s = 0; s <= n_streams; s++) roff[s] = off[s] - off[0];
@@ -1637,25 +1577,23 @@ int ef_audio_enable(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    { int rca = audio_resolve(c); if (rca != EF_OK) return rca; }
+    TRY(audio_resolve(c));
     if (c->audio) return EF_OK;
-    int rc = audio_constants(c->cfg.device);
-    if (rc != EF_OK) return rc;
+    TRY(audio_constants(c->cfg.device));
     const int n = c->cfg.n_streams;
     const size_t cap = c->cfg.es_capacity, packets = cap / 188 + 1;
-#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
-    A(c->d_aud_state, (size_t)n);
+    TRY(dev_alloc(c, &c->d_aud_state, (size_t)n));
     for (int b = 0; b < 2; b++) {
-        A(c->d_aud2[b], cap + 1024);                      // a submit's audio is never longer than its transport stream
-        A(c->d_aud_off2[b], (size_t)n + 1);
-        A(c->d_gate2[b], (size_t)n); A(c->d_lead2[b], (size_t)n); A(c->d_skip2[b], (size_t)n);
+        TRY(dev_alloc(c, &c->d_aud2[b], cap + 1024));     // a submit's audio is never longer than its transport stream
+        TRY(dev_alloc(c, &c->d_aud_off2[b], (size_t)n + 1));
+        TRY(dev_alloc(c, &c->d_gate2[b], (size_t)n)); TRY(dev_alloc(c, &c->d_lead2[b], (size_t)n)); TRY(dev_alloc(c, &c->d_skip2[b], (size_t)n));
     }
-    A(c->d_aud_start, packets); A(c->d_aud_kind, packets); A(c->d_aud_pos, packets); A(c->d_aud_len, (size_t)n + 1);
-    A(c->d_blob, cap + (size_t)n * EF_AUDIO_CARRY + 1024); A(c->d_blob_len, (size_t)n + 1); A(c->d_blob_off, (size_t)n + 1);
-    A(c->d_ended, (size_t)n);
-#undef A
-    if (!c->h_ended) CK(cudaHostAlloc((void**)&c->h_ended, (size_t)n, cudaHostAllocDefault));
-    if (!c->aud_scratch) c->aud_scratch = new AudioScratch();
+    TRY(dev_alloc(c, &c->d_aud_start, packets)); TRY(dev_alloc(c, &c->d_aud_kind, packets)); TRY(dev_alloc(c, &c->d_aud_pos, packets));
+    TRY(dev_alloc(c, &c->d_aud_len, (size_t)n + 1));
+    TRY(dev_alloc(c, &c->d_blob, cap + (size_t)n * EF_AUDIO_CARRY + 1024));
+    TRY(dev_alloc(c, &c->d_blob_len, (size_t)n + 1)); TRY(dev_alloc(c, &c->d_blob_off, (size_t)n + 1));
+    TRY(dev_alloc(c, &c->d_ended, (size_t)n));
+    if (!c->h_ended) TRY(host_alloc(c, &c->h_ended, (size_t)n));
     CK(cudaMemset(c->d_aud_state, 0, (size_t)n * sizeof(EfAudioState)));
     for (int b = 0; b < 2; b++) {
         CK(cudaMemset(c->d_gate2[b], 0, (size_t)n)); CK(cudaMemset(c->d_skip2[b], 0, (size_t)n)); CK(cudaMemset(c->d_lead2[b], 0, (size_t)n * 4));
@@ -1707,15 +1645,14 @@ int ef_decode_audio(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info* info
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !info) return fail(EF_EINVAL, "null argument");
     if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio before ef_audio_enable");
-    int rc = audio_constants(c->cfg.device);
-    if (rc != EF_OK) return rc;
-    if ((rc = audio_resolve(c)) != EF_OK) return rc;
+    TRY(audio_constants(c->cfg.device));
+    TRY(audio_resolve(c));
     const int n = c->cfg.n_streams;
     cudaStream_t cs = (cudaStream_t)stream;
     bool any_end = false;
-    if ((rc = audio_assemble(c, end_of_stream, cs, &any_end)) != EF_OK) return rc;
-    rc = audio_decode_blob(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, *c->aud_scratch, info, pcm, pcm_cap, pdm, cs, &c->launches,
-                           [&] { return any_end ? audio_end(c, nullptr, cs) : EF_OK; });
+    TRY(audio_assemble(c, end_of_stream, cs, &any_end));
+    const int rc = audio_decode_blob(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, c->aud_scratch, info, pcm, pcm_cap, pdm, cs, &c->launches,
+                                     [&] { return any_end ? audio_end(c, nullptr, cs) : EF_OK; });
     CK(cudaEventRecord(c->ev_aud_done, cs));
     if (rc != EF_OK || !pcm) return rc;
     c->aud_unconsumed = false;
@@ -1736,23 +1673,22 @@ int ef_decode_audio_async(ef_ctx* c, const uint8_t* end_of_stream, ef_audio_info
     if (!c->audio) return fail(EF_ESTATE, "ef_decode_audio_async before ef_audio_enable");
     if (!is_device_ptr(info) || !is_device_ptr(pcm) || (pdm && !is_device_ptr(pdm)))
         return fail(EF_EINVAL, "ef_decode_audio_async takes device memory for info, pcm and pdm");
-    int rc = audio_constants(c->cfg.device);
-    if (rc != EF_OK) return rc;
+    TRY(audio_constants(c->cfg.device));
     // whether this call takes the current submit's audio depends on the outstanding call only when that one took it
-    if (c->aud_async && c->aud_async_new && (rc = audio_resolve(c)) != EF_OK) return rc;
+    if (c->aud_async && c->aud_async_new) TRY(audio_resolve(c));
     const int n = c->cfg.n_streams;
-    AudioScratch& w = *c->aud_scratch;
+    AudioScratch& w = c->aud_scratch;
     if (!w.fits(AudioScratch::VROWS, audio_vrow_bytes(n, pcm_cap)) || !w.fits(AudioScratch::VERDICT, sizeof(int))) {
         CK(cudaEventSynchronize(c->ev_aud_done));            // the scratch grows: no earlier call may still use it
-        if ((rc = audio_scratch(w, n, pcm_cap)) != EF_OK) return rc;
+        TRY(audio_scratch(w, n, pcm_cap));
     }
-    if (!c->h_aud_verdict) CK(cudaHostAlloc((void**)&c->h_aud_verdict, sizeof(int), cudaHostAllocDefault));
+    if (!c->h_aud_verdict) TRY(host_alloc(c, &c->h_aud_verdict, 1));
     cudaStream_t cs = (cudaStream_t)stream;
     bool any_end = false;
-    if ((rc = audio_assemble(c, end_of_stream, cs, &any_end)) != EF_OK) return rc;
-    if ((rc = audio_plan(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, info, cs, &c->launches)) != EF_OK) return rc;
-    if ((rc = audio_run(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, pcm, pdm, true, cs, &c->launches)) != EF_OK) return rc;
-    if (any_end && (rc = audio_end(c, (const int*)w.p[AudioScratch::VERDICT], cs)) != EF_OK) return rc;
+    TRY(audio_assemble(c, end_of_stream, cs, &any_end));
+    TRY(audio_plan(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, info, cs, &c->launches));
+    TRY(audio_run(c->d_blob, c->d_blob_off, c->d_aud_state, c->d_ended, n, w, pcm_cap, pcm, pdm, true, cs, &c->launches));
+    if (any_end) TRY(audio_end(c, (const int*)w.p[AudioScratch::VERDICT], cs));
     CK(cudaMemcpyAsync(c->h_aud_verdict, w.p[AudioScratch::VERDICT], sizeof(int), cudaMemcpyDeviceToHost, cs));
     CK(cudaEventRecord(c->ev_aud_done, cs));
     c->aud_async = true;
@@ -1764,8 +1700,7 @@ int ef_audio_wait(ef_ctx* c)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    int rc = audio_resolve(c);
-    if (rc != EF_OK) return rc;
+    TRY(audio_resolve(c));
     if (c->aud_async_rc == EF_ENOMEM) return fail(EF_ENOMEM, "the last ef_decode_audio_async exceeded its pcm_cap: nothing was decoded, no state changed");
     return c->aud_async_rc;
 }
@@ -1778,11 +1713,11 @@ int ef_pts_enable(ef_ctx* c)
     if (c->pts) return EF_OK;
     const int n = c->cfg.n_streams;
     const size_t packets = c->cfg.es_capacity / 188 + 1;
-    int rc;
-#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
-    for (int b = 0; b < 2; b++) { A(c->d_pts_off2[b], packets); A(c->d_pts_val2[b], packets); A(c->d_pts_span2[b], (size_t)n); }
-    A(c->d_pts_carry, (size_t)n); A(c->d_pts_last, (size_t)n); A(c->d_pic_pts, (size_t)n * c->cfg.max_pictures);
-#undef A
+    for (int b = 0; b < 2; b++) {
+        TRY(dev_alloc(c, &c->d_pts_off2[b], packets)); TRY(dev_alloc(c, &c->d_pts_val2[b], packets)); TRY(dev_alloc(c, &c->d_pts_span2[b], (size_t)n));
+    }
+    TRY(dev_alloc(c, &c->d_pts_carry, (size_t)n)); TRY(dev_alloc(c, &c->d_pts_last, (size_t)n));
+    TRY(dev_alloc(c, &c->d_pic_pts, (size_t)n * c->cfg.max_pictures));
     CK(cudaDeviceSynchronize());                          // a queued TS submit was demuxed without PES lists: it carries none
     for (int b = 0; b < 2; b++) CK(cudaMemset(c->d_pts_span2[b], 0, (size_t)n * sizeof(uint2)));
     CK(cudaMemset(c->d_pts_carry, 0xFF, (size_t)n * 8));
@@ -1818,19 +1753,12 @@ int ef_present_enable(ef_ctx* c, const uint32_t* frame_counter0)
     if (c->paced) return fail(EF_ESTATE, "ef_present_enable: already enabled");
     if (!c->pts || !c->video) return fail(EF_ESTATE, "ef_present_enable needs ef_pts_enable and ef_video_init first");
     const int n = c->cfg.n_streams;
-    int rc;
-#define A(ptr, count) if ((rc = dev_alloc(c, &(ptr), (count))) != EF_OK) return rc;
     if (!c->d_pace) {
-        A(c->d_pace, (size_t)n); A(c->d_pace_next, (size_t)n); A(c->d_pace_run, (size_t)n); A(c->d_pace_out, (size_t)n);
-        A(c->d_pace_first, (size_t)n); A(c->d_pace_arg, (size_t)n);
-        CK(cudaHostAlloc((void**)&c->h_pace_out, (size_t)n * sizeof(EfPaceOut), cudaHostAllocDefault));
-        CK(cudaHostAlloc((void**)&c->h_pace_first, (size_t)n * 8, cudaHostAllocDefault));
-        CK(cudaHostAlloc((void**)&c->h_pace_arg, (size_t)n * 4, cudaHostAllocDefault));
-        CK(cudaHostAlloc((void**)&c->h_pace_npics, 4, cudaHostAllocDefault));
-        c->allocs_host.push_back(c->h_pace_out); c->allocs_host.push_back(c->h_pace_first); c->allocs_host.push_back(c->h_pace_arg);
-        c->allocs_host.push_back(c->h_pace_npics);
+        TRY(dev_alloc(c, &c->d_pace, (size_t)n)); TRY(dev_alloc(c, &c->d_pace_next, (size_t)n)); TRY(dev_alloc(c, &c->d_pace_run, (size_t)n));
+        TRY(dev_alloc(c, &c->d_pace_out, (size_t)n)); TRY(dev_alloc(c, &c->d_pace_first, (size_t)n)); TRY(dev_alloc(c, &c->d_pace_arg, (size_t)n));
+        TRY(host_alloc(c, &c->h_pace_out, (size_t)n)); TRY(host_alloc(c, &c->h_pace_first, (size_t)n)); TRY(host_alloc(c, &c->h_pace_arg, (size_t)n));
+        TRY(host_alloc(c, &c->h_pace_npics, 1));
     }
-#undef A
     std::vector<EfPaceState> st((size_t)n);
     for (int s = 0; s < n; s++) {                         // line 0 of field frame_counter0[s], no frame presented, no origin
         memset(&st[s], 0, sizeof(EfPaceState));
@@ -1885,8 +1813,7 @@ static int present_parse(ef_ctx* c, int pic, cudaStream_t st)
 
 static int present_recon(ef_ctx* c, int pic, cudaStream_t st)
 {
-    int rc = decode_recon(c, pic - c->pace_p0, st);
-    if (rc != EF_OK) return rc;
+    TRY(decode_recon(c, pic - c->pace_p0, st));
     CK(cudaEventRecord(c->ev_buf_free[c->active], st));   // the front ES buffer is in use until here
     c->pace_next = pic + 1;
     return EF_OK;
@@ -1898,18 +1825,8 @@ static int present_room(ef_ctx* c, uint64_t fields, cudaStream_t st)
     if (!desc && !fovl) return EF_OK;
     CK(cudaStreamSynchronize(st));
     if (c->pace_async) CK(cudaEventSynchronize(c->ev_pace_done));   // the calls of the outstanding chain, on whatever stream
-    if (desc) {
-        if (c->d_desc) CK(cudaFree(c->d_desc));
-        c->d_desc = nullptr; c->desc_cap = 0;
-        CK(cudaMalloc(&c->d_desc, fields * sizeof(EfFieldDesc)));
-        c->desc_cap = fields;
-    }
-    if (fovl) {
-        if (c->d_fovl) CK(cudaFree(c->d_fovl));
-        c->d_fovl = nullptr; c->fovl_cap = 0;
-        CK(cudaMalloc(&c->d_fovl, fields * sizeof(EfFieldOverlay)));
-        c->fovl_cap = fields;
-    }
+    if (desc) { TRY(dev_grow(c, &c->d_desc, c->desc_cap, fields, false)); c->desc_cap = fields; }
+    if (fovl) { TRY(dev_grow(c, &c->d_fovl, c->fovl_cap, fields, false)); c->fovl_cap = fields; }
     return EF_OK;
 }
 
@@ -1940,9 +1857,8 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
 {
     const int n = c->cfg.n_streams;
     if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
-    int rc = present_check_modes(c, pic, modes);
-    if (rc != EF_OK) return rc;
-    if ((rc = present_schedule(c, pic, modes, idle_n, c->h_pace_arg, st)) != EF_OK) return rc;
+    TRY(present_check_modes(c, pic, modes));
+    TRY(present_schedule(c, pic, modes, idle_n, c->h_pace_arg, st));
     CK(cudaMemcpyAsync(c->h_pace_out, c->d_pace_out, (size_t)n * sizeof(EfPaceOut), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     uint64_t total = 0;
@@ -1954,12 +1870,12 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
     if (!dst) return EF_OK;                                // sizing call: nothing decoded, no state changed
     if (total > dst_fields) return fail(EF_ENOMEM, "%llu fields, capacity %llu", (unsigned long long)total, (unsigned long long)dst_fields);
     if (pic >= 0) {
-        if ((rc = present_parse(c, pic, st)) != EF_OK) return rc;
-        if ((rc = present_recon(c, pic, st)) != EF_OK) return rc;
+        TRY(present_parse(c, pic, st));
+        TRY(present_recon(c, pic, st));
     }
-    if ((rc = present_room(c, total, st)) != EF_OK) return rc;
+    TRY(present_room(c, total, st));
     CK(cudaMemcpyAsync(c->d_pace_first, c->h_pace_first, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    if ((rc = present_render(c, dst, total, false, st)) != EF_OK) return rc;
+    TRY(present_render(c, dst, total, false, st));
     CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
     return EF_OK;
 }
@@ -1973,19 +1889,14 @@ static int present_async(ef_ctx* c, int pic, const uint8_t* modes, const uint32_
     const int n = c->cfg.n_streams;
     if (!dst || !info || !is_device_ptr(dst) || !is_device_ptr(info)) return fail(EF_EINVAL, "the async present calls take device memory for dst and info");
     if ((uintptr_t)dst & 15) return fail(EF_EINVAL, "dst must be 16-byte aligned");
-    int rc = present_check_modes(c, pic, modes);
-    if (rc != EF_OK) return rc;
+    TRY(present_check_modes(c, pic, modes));
     if (!c->d_pace_chain) {
-        if ((rc = dev_alloc(c, &c->d_pace_chain, 2)) != EF_OK) return rc;
-        if ((rc = dev_alloc(c, &c->d_pace_total, 1)) != EF_OK) return rc;
-        CK(cudaHostAlloc((void**)&c->h_pace_chain, 2 * sizeof(int), cudaHostAllocDefault));
-        c->allocs_host.push_back(c->h_pace_chain);
-        CK(cudaHostAlloc((void**)&c->h_pace_ring, (size_t)ef_ctx::kPaceRing * n * 4, cudaHostAllocDefault));
-        c->allocs_host.push_back(c->h_pace_ring);
-        CK(cudaEventCreateWithFlags(&c->ev_pace_done, cudaEventDisableTiming));
-        for (cudaEvent_t& e : c->ev_pace_ring) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        TRY(dev_alloc(c, &c->d_pace_chain, 2)); TRY(dev_alloc(c, &c->d_pace_total, 1));
+        TRY(host_alloc(c, &c->h_pace_chain, 2)); TRY(host_alloc(c, &c->h_pace_ring, (size_t)ef_ctx::kPaceRing * n));
+        TRY(event(c, &c->ev_pace_done));
+        for (cudaEvent_t& e : c->ev_pace_ring) TRY(event(c, &e));
     }
-    if ((rc = present_room(c, dst_fields, st)) != EF_OK) return rc;
+    TRY(present_room(c, dst_fields, st));
     if (!c->pace_async) {                                  // a new chain
         CK(cudaMemsetAsync(c->d_pace_chain, 0, 2 * sizeof(int), st));
         c->chain_next.clear(); c->chain_pic.clear();
@@ -1995,17 +1906,17 @@ static int present_async(ef_ctx* c, int pic, const uint8_t* modes, const uint32_
     const int k = c->pace_ring_i;
     c->pace_ring_i = (k + 1) % ef_ctx::kPaceRing;
     CK(cudaEventSynchronize(c->ev_pace_ring[k]));
-    if ((rc = present_schedule(c, pic, modes, idle_n, c->h_pace_ring + (size_t)k * n, st)) != EF_OK) return rc;
+    TRY(present_schedule(c, pic, modes, idle_n, c->h_pace_ring + (size_t)k * n, st));
     CK(cudaEventRecord(c->ev_pace_ring[k], st));
     c->chain_next.push_back(c->pace_next);
     c->chain_pic.push_back(pic);
-    if (pic >= 0 && (rc = present_parse(c, pic, st)) != EF_OK) return rc;   // before the size kernel, which may zero its records
+    if (pic >= 0) TRY(present_parse(c, pic, st));       // before the size kernel, which may zero its records
     uint32_t* rec = pic >= 0 ? c->h.mb_info + (size_t)(pic - c->pace_p0) * n * EF_MBW_MAX * EF_MBH_MAX : nullptr;
     ef_pace_size_kernel<<<1, 1024, 0, st>>>(c->d_pace_out, n, dst_fields, c->d_pace_first, (EfPaceOut*)info, c->d_pace_total, c->d_pace_chain, rec);
     CK(cudaGetLastError());
     c->launches++;
-    if (pic >= 0 && (rc = present_recon(c, pic, st)) != EF_OK) return rc;
-    if ((rc = present_render(c, dst, dst_fields, true, st)) != EF_OK) return rc;
+    if (pic >= 0) TRY(present_recon(c, pic, st));
+    TRY(present_render(c, dst, dst_fields, true, st));
     CK(cudaMemcpyAsync(c->h_pace_chain, c->d_pace_chain, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(c->ev_pace_done, st));
     return EF_OK;
@@ -2016,8 +1927,7 @@ static int present_picture_check(ef_ctx* c, int pic, const char* what)
 {
     if (!c->paced) return fail(EF_ESTATE, "%s before ef_present_enable", what);
     if (!c->pace_indexed) return fail(EF_ESTATE, "%s before an ef_index that followed ef_present_enable", what);
-    int rc = pace_pictures(c);
-    if (rc != EF_OK) return rc;
+    TRY(pace_pictures(c));
     if (pic != c->pace_next || pic >= c->pace_npics)
         return fail(EF_ESTATE, "%s(%d): the next picture index is %d of %d", what, pic, c->pace_next, c->pace_npics);
     return EF_OK;
@@ -2027,9 +1937,8 @@ int ef_present_picture(ef_ctx* c, int pic, const uint8_t* modes, uint16_t* dst, 
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !info) return fail(EF_EINVAL, "null argument");
-    int rc = pace_resolve(c);
-    if (rc != EF_OK) return rc;
-    if ((rc = present_picture_check(c, pic, "ef_present_picture")) != EF_OK) return rc;
+    TRY(pace_resolve(c));
+    TRY(present_picture_check(c, pic, "ef_present_picture"));
     return present_common(c, pic, modes, nullptr, dst, dst_fields, info, (cudaStream_t)stream);
 }
 
@@ -2038,8 +1947,7 @@ int ef_present_idle(ef_ctx* c, const uint32_t* n_fields, uint16_t* dst, uint64_t
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !info || !n_fields) return fail(EF_EINVAL, "null argument");
     if (!c->paced) return fail(EF_ESTATE, "ef_present_idle before ef_present_enable");
-    int rc = pace_resolve(c);
-    if (rc != EF_OK) return rc;
+    TRY(pace_resolve(c));
     return present_common(c, -1, nullptr, n_fields, dst, dst_fields, info, (cudaStream_t)stream);
 }
 
@@ -2047,8 +1955,7 @@ int ef_present_picture_async(ef_ctx* c, int pic, const uint8_t* modes, uint16_t*
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    int rc = present_picture_check(c, pic, "ef_present_picture_async");
-    if (rc != EF_OK) return rc;
+    TRY(present_picture_check(c, pic, "ef_present_picture_async"));
     return present_async(c, pic, modes, nullptr, dst, dst_fields, info, (cudaStream_t)stream);
 }
 
@@ -2064,8 +1971,7 @@ int ef_present_wait(ef_ctx* c, int* n_presented)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
-    int rc = pace_resolve(c);
-    if (rc != EF_OK) return rc;
+    TRY(pace_resolve(c));
     if (n_presented) *n_presented = c->pace_async_n;
     if (c->pace_async_rc == EF_ENOMEM)
         return fail(EF_ENOMEM, "call %d of the last ef_present_*_async chain exceeded its dst_fields: it and the calls after it changed nothing", c->pace_async_n);
@@ -2078,11 +1984,8 @@ static int overlay_alloc(ef_ctx* c)
 {
     if (c->d_ovl) return EF_OK;
     const int n = c->cfg.n_streams;
-    int rc;
-#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
-    A(c->d_ovl, (size_t)n); A(c->d_ovl_next, (size_t)n); A(c->d_ovl_cmd, (size_t)n);
-    A(c->d_ovl_slots, (size_t)n * 2 * EF_OVERLAY_BYTES); A(c->d_ovl_in, (size_t)n * EF_OVERLAY_BYTES);
-#undef A
+    TRY(dev_alloc(c, &c->d_ovl, (size_t)n)); TRY(dev_alloc(c, &c->d_ovl_next, (size_t)n)); TRY(dev_alloc(c, &c->d_ovl_cmd, (size_t)n));
+    TRY(dev_alloc(c, &c->d_ovl_slots, (size_t)n * 2 * EF_OVERLAY_BYTES)); TRY(dev_alloc(c, &c->d_ovl_in, (size_t)n * EF_OVERLAY_BYTES));
     CK(cudaMemset(c->d_ovl, 0, (size_t)n * sizeof(EfOverlayState)));   // blend 0: nothing drawn
     CK(cudaMemset(c->d_ovl_slots, 0, (size_t)n * 2 * EF_OVERLAY_BYTES));
     return EF_OK;
@@ -2093,9 +1996,8 @@ int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, 
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c) return fail(EF_EINVAL, "null context");
     if (!c->paced) return fail(EF_ESTATE, "ef_present_overlay before ef_present_enable");
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
-    const int n = c->cfg.n_streams;
-    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    TRY(pace_resolve(c));
+    TRY(stream_range(c, first, count));
     std::vector<EfOverlayCmd> cmd((size_t)count);
     for (int i = 0; i < count; i++) {
         uint32_t m = set ? set[i] & 7u : 7u;
@@ -2105,8 +2007,7 @@ int ef_present_overlay(ef_ctx* c, int first, int count, const uint8_t* bitmaps, 
         if ((m & 2u) && blend[i] < -1) return fail(EF_EINVAL, "blend %d of stream %d is below -1", blend[i], first + i);
         cmd[i] = { (m & 2u) ? blend[i] : 0, (m & 4u) ? progress[i] : 0, m, 0u };
     }
-    int rc = overlay_alloc(c);
-    if (rc != EF_OK) return rc;
+    TRY(overlay_alloc(c));
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(c->d_ovl_cmd, cmd.data(), cmd.size() * sizeof(EfOverlayCmd), cudaMemcpyHostToDevice));
@@ -2127,12 +2028,8 @@ int ef_present_font(ef_ctx* c, const uint8_t* atlas, const int16_t* rights, int 
     for (int i = 0; i < n_rights; i++)
         if (rights[i] > EF_FONT_W || rights[i] <= (i ? rights[i - 1] : 0))
             return fail(EF_EINVAL, "rights[%d] = %d: the glyph edges must increase from above 0 up to %d", i, rights[i], EF_FONT_W);
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
-    int rc;
-    if (!c->d_font) {
-        if ((rc = dev_alloc(c, &c->d_font, (size_t)16 * EF_FONT_W)) != EF_OK) return rc;
-        if ((rc = dev_alloc(c, &c->d_font_rights, (size_t)EF_FONT_W)) != EF_OK) return rc;
-    }
+    TRY(pace_resolve(c));
+    if (!c->d_font) { TRY(dev_alloc(c, &c->d_font, (size_t)16 * EF_FONT_W)); TRY(dev_alloc(c, &c->d_font_rights, (size_t)EF_FONT_W)); }
     CK(cudaDeviceSynchronize());                          // a present call may still draw with the old atlas
     CK(cudaMemcpy(c->d_font, atlas, (size_t)16 * EF_FONT_W, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(c->d_font_rights, rights, (size_t)n_rights * 2, cudaMemcpyHostToDevice));
@@ -2146,7 +2043,7 @@ int ef_present_clock(ef_ctx* c, int first, int count, const uint8_t* idx_hdrs, c
     if (!c->paced) return fail(EF_ESTATE, "ef_present_clock before ef_present_enable");
     if (!c->d_font) return fail(EF_ESTATE, "ef_present_clock before ef_present_font");
     const int n = c->cfg.n_streams;
-    if (first < 0 || count < 0 || first > n || count > n - first) return fail(EF_EINVAL, "streams [%d, %d + %d) out of range", first, first, count);
+    TRY(stream_range(c, first, count));
     if (count && (!idx_hdrs || !speed || !flags)) return fail(EF_EINVAL, "null argument");
     std::vector<idx_hdr> hdr((size_t)count);
     if (count) memcpy(hdr.data(), idx_hdrs, (size_t)count * sizeof(idx_hdr));
@@ -2158,13 +2055,10 @@ int ef_present_clock(ef_ctx* c, int first, int count, const uint8_t* idx_hdrs, c
         if (speed[i] == 1 && h.fwd.last_pts == h.fwd.first_pts) return fail(EF_EINVAL, "stream %d: the fwd record spans no pts", first + i);
         if (speed[i] == -1 && h.rev.last_pts == h.rev.first_pts) return fail(EF_EINVAL, "stream %d: the rwd record spans no pts", first + i);
     }
-    { int rcp = pace_resolve(c); if (rcp != EF_OK) return rcp; }
-    int rc = overlay_alloc(c);
-    if (rc != EF_OK) return rc;
+    TRY(pace_resolve(c));
+    TRY(overlay_alloc(c));
     if (!c->d_clk) {
-#define A(ptr, cnt) if ((rc = dev_alloc(c, &(ptr), (cnt))) != EF_OK) return rc;
-        A(c->d_clk, (size_t)n); A(c->d_ovl_clk, (size_t)n); A(c->d_clk_bm, (size_t)n * EF_OVERLAY_BYTES);
-#undef A
+        TRY(dev_alloc(c, &c->d_clk, (size_t)n)); TRY(dev_alloc(c, &c->d_ovl_clk, (size_t)n)); TRY(dev_alloc(c, &c->d_clk_bm, (size_t)n * EF_OVERLAY_BYTES));
         CK(cudaMemset(c->d_clk, 0, (size_t)n * sizeof(EfClockState)));    // every clock off, _last_seconds 0
     }
     if (!count) return EF_OK;

@@ -32,8 +32,6 @@ bool place(uint16_t* tab, int max_lz, const char* code, uint16_t entry)
 
 }  // namespace
 
-const unsigned char* ef_default_intra_ptr() { return ef_default_intra_q; }
-
 // combined per-scan-position entry of the parser: quantiser byte | AAN prescale << 8 | raster index << 18
 uint32_t ef_qz_entry(unsigned q, int n) { return (q & 255u) | ((uint32_t)ef_aan_prescale[ef_zigzag[n]] << 8) | ((uint32_t)ef_zigzag[n] << 18); }
 

@@ -170,6 +170,26 @@ def test_pipelined_submits_and_async_readback(oracle):
     ctx.close()
 
 
+def test_growing_readback_frees_replaced_staging():
+    """Read-backs whose stream count grows call after call: each staging buffer that grows frees the one it replaces, so the
+    context holds two buffers of the largest count (2 x 52 MB here), not every earlier one (about 13 GB)."""
+    import torch
+    n = 512
+    es, _ = synth.generate(synth.SEED0, n_pictures=2, gop=2)
+    ctx = espflix_b200.Context(n_streams=n, max_pictures=2, es_capacity=n * len(es) + 4096, fields=False)
+    ctx.submit_es(*ctx.pack([es] * n))
+    ctx.index()
+    out = torch.empty(n * 101376, dtype=torch.uint8, pin_memory=True)
+    ctx.sync()
+    free0, _ = torch.cuda.mem_get_info()
+    for k in range(1, n + 1):
+        ctx.read_latest_i420_async(0, k, out.data_ptr())
+    ctx.sync()
+    free1, _ = torch.cuda.mem_get_info()
+    ctx.close()
+    assert free0 - free1 < 2 << 30, "%.1f GB of device memory held after the read-backs" % ((free0 - free1) / 2**30)
+
+
 @pytest.mark.parametrize("rec_pics", [None, "1", "5"])
 def test_decode_all_multi_picture_parse(oracle, monkeypatch, rec_pics):
     """ef_decode_all parses every slice of up to rec_pics picture indices in ONE K1a launch and rebuilds
