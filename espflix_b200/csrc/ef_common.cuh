@@ -46,10 +46,11 @@
 #define EF_K1A_UNROLL 3          // K1a: symbol steps per pass of the loop (one vote + branch per pass)
 #endif
 #ifndef EF_K1B_WARPS
-#define EF_K1B_WARPS 7       // K1b (reconstruct): warps per CTA, CTAs per SM
+#define EF_K1B_WARPS 2       // K1b (reconstruct): warps per CTA, CTAs per SM. 30 warps per SM at 64 registers in small CTAs: of 7 x 4, 8 x 4, 16 x 2,
+                             // 6 x 5, 5 x 6, 10 x 3, 4 x 7, 4 x 8, 3 x 10 and 2 x 15, measured fastest on the H100 (DESIGN.md 4)
 #endif
 #ifndef EF_K1B_CTAS
-#define EF_K1B_CTAS 4
+#define EF_K1B_CTAS 15
 #endif
 
 // ---- decode tables (built on the host by ef_tables.cpp from ISO 11172-2 Annex B) -------------

@@ -49,6 +49,17 @@ constexpr int kHdrBatch = EF_K1A_HDR_BATCH;        // waiting lanes that end a s
 constexpr int kReconWarps = EF_K1B_WARPS;       // per CTA
 constexpr int kReconCtasPerSm = EF_K1B_CTAS;
 
+// -DEF_K1B_PHASE_CLOCKS: a measurement build of K1b (tools/phase_k1b.py), never the product. Lane 0 of every warp adds up
+// the clock64() ticks it spends in each phase of an iteration and the kernel leaves the sums in g_k1b_phase. Without the
+// definition EF_PHASE() is empty and the kernel compiles to the same instructions as before.
+#ifdef EF_K1B_PHASE_CLOCKS
+enum { kPhHead, kPhExpand, kPhColumns, kPhWait, kPhRowIdct, kPhPredict, kPhStore, kPhases };
+__device__ unsigned long long g_k1b_phase[kPhases + 1];      // ticks per phase, then the number of warp iterations
+#define EF_PHASE(i) { const long long t_ = clock64(); ph[i] += t_ - ph_t; ph_t = t_; }
+#else
+#define EF_PHASE(i)
+#endif
+
 // macroblock info word (EfDev::mb_info): bit0 valid, 1 intra, 2-7 coded blocks, 8-13 n==1 mask,
 // 14-19 abort mask (bit b = block b), 20-24 mb_width of the stream, 25 destination frame store
 constexpr int kDenseStride = 72;                // words per block in the dense scratch: 64 + 8 pad -> the 4 luma blocks hit distinct banks
@@ -681,17 +692,24 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
 
     // Work distribution: the first two pairs of a warp are static, later ones come from a global cursor
     // (the warp schedulers do not share the issue slots evenly, so a static split leaves a long tail). The
-    // atomic is issued two iterations ahead of its use and the record one iteration ahead.
+    // atomic is issued two iterations ahead of its use and the record one iteration ahead. pair_fut keeps the
+    // atomic's raw result, and its address carries threadIdx.y (always 0: the block is one-dimensional): an atom.add
+    // (or atom.inc) on an address the assembler can prove warp-uniform is compiled into its warp-aggregated form even
+    // under `lane == 0`, and the shuffle of that form reads the result at once, so that every iteration waited a round
+    // trip to L2 for a cursor value it needs two iterations later.
     const uint32_t n_warps = gridDim.x * kReconWarps;
     uint32_t* cursor = D.recon_cursor + pic_rel;
     uint32_t pair = blockIdx.x * kReconWarps + warp, pair_next = pair + n_warps, pair_fut = 0;
     uint32_t pre = fetch(pair * 2 + half);
-    for (;; pair = pair_next, pair_next = __shfl_sync(0xFFFFFFFFu, pair_fut, 0)) {
+#ifdef EF_K1B_PHASE_CLOCKS
+    long long ph[kPhases] = {}, ph_t = clock64(), ph_n = 0;
+#endif
+    for (;; pair = pair_next, pair_next = 2 * n_warps + __shfl_sync(0xFFFFFFFFu, pair_fut, 0)) {
         if (pair * 2 >= n_slots) break;
         const uint32_t slot = pair * 2 + half;
         const uint32_t recw = pre;
         pre = fetch(pair_next * 2 + half);
-        if (lane == 0) pair_fut = 2 * n_warps + atomicAdd(cursor, 1u);
+        if (lane == 0) asm volatile("atom.global.add.u32 %0, [%1], 1;" : "=r"(pair_fut) : "l"(cursor + threadIdx.y));
         const uint32_t info = __shfl_sync(0xFFFFFFFFu, recw, hb + 12);
         const bool valid = info & 1u;
         if (!__any_sync(0xFFFFFFFFu, valid)) continue;
@@ -749,6 +767,7 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
             }
         }
 
+        EF_PHASE(kPhHead)
         // expand the coefficient list into the dense scratch (entries of aborted blocks are dropped)
         // entry = (block << 24 | raster position << 18) + value, |value| < 2^17: adding 2^17 undoes the borrow of a negative value
 #define EF_EXPAND(ent) { const uint32_t hi_ = (ent) + 0x20000u; const int eb = (hi_ >> 24) & 7; if (!((abm >> eb) & 1)) dense[eb * kDenseStride + ((hi_ >> 18) & 63)] = ((int)((ent) << 14)) >> 14; }
@@ -758,6 +777,7 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
         for (int j = hl + 48; j < entries; j += 16) { const uint32_t ent = __ldg(rl + j); EF_EXPAND(ent) }
 #undef EF_EXPAND
         __syncwarp();                                                           // dense[] complete
+        EF_PHASE(kPhExpand)
 
         // ---- column passes, in place: lane (block, column) owns the 8 words dense[block][0..7][column]
         unsigned pass_on = 0;
@@ -780,8 +800,10 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
             for (int rr = 0; rr < 8; rr++) db[rr * 8] = v[rr];
         }
         __syncwarp();
+        EF_PHASE(kPhColumns)
 
         if (do_mc && inside) { mbar_wait(sbar, bar_phase); bar_phase ^= 1; }
+        EF_PHASE(kPhWait)
 
         // ---- row passes: residual row, prediction, clamped add, store ---------------------------------
 #pragma unroll
@@ -807,6 +829,7 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
                     }
                 }
             }
+            EF_PHASE(kPhRowIdct)
             // prediction: the four cases of mocomp()
             uint32_t q0 = 0, q1 = 0;
             if (do_mc) {
@@ -823,6 +846,7 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
                     pred_finish(pw, kx, cx & 1, cy & 1, q0, q1);
                 }
             }
+            EF_PHASE(kPhPredict)
             // combine + store (copy_block / copy_block_dc / add_block / add_block_dc)
             const bool coded = (cbp >> oblk) & 1, aborted = (abm >> oblk) & 1, n1 = (n1m >> oblk) & 1;
             uint32_t o0 = q0, o1 = q1;
@@ -838,9 +862,19 @@ ef_recon_kernel(const __grid_constant__ EfDev D, int pic_rel)
             } else if (intra_r) store = false;                        // aborted intra block: destination untouched
             uint8_t* dst = cur + tile + (luma ? (p * 8 + prow) * 16 + phalf * 8 : 256 + cplane * 64 + crow * 8);
             if (store) *(uint2*)dst = make_uint2(o0, o1);
+            EF_PHASE(kPhStore)
         }
         __syncwarp();
+#ifdef EF_K1B_PHASE_CLOCKS
+        ph_n++;
+#endif
     }
+#ifdef EF_K1B_PHASE_CLOCKS
+    if (lane == 0) {
+        for (int i = 0; i < kPhases; i++) atomicAdd(&g_k1b_phase[i], (unsigned long long)ph[i]);
+        atomicAdd(&g_k1b_phase[kPhases], (unsigned long long)ph_n);
+    }
+#endif
 }
 
 // host-side launch helpers -----------------------------------------------------------------------
@@ -867,6 +901,18 @@ cudaError_t ef_decode_configure()
     if (n >= 1) g_parse_ctas = n;
     return cudaSuccess;
 }
+
+#ifdef EF_K1B_PHASE_CLOCKS
+// out[0..6] = ticks of lane 0 summed over all warps since the last call (head, expansion, column passes, barrier wait,
+// row IDCT, prediction, combine + store), out[7] = warp iterations; the sums are cleared
+extern "C" int ef_k1b_phase_clocks(unsigned long long* out)
+{
+    const unsigned long long zero[kPhases + 1] = {};
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (cudaMemcpyFromSymbol(out, g_k1b_phase, sizeof zero) != cudaSuccess) return -1;
+    return cudaMemcpyToSymbol(g_k1b_phase, zero, sizeof zero) == cudaSuccess ? 0 : -1;
+}
+#endif
 
 int ef_decode_resident_ctas(int which) { return which == 0 ? g_parse_ctas : g_recon_ctas; }
 
