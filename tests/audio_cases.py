@@ -53,3 +53,34 @@ def mux_audio_ts(es, pid=0x101, pes_bytes=1024, first_pts=90000, drop_pts_on=())
             first = False
         pes_index += 1
     return np.frombuffer(b"".join(pkts), dtype=np.uint8).copy()
+
+
+AUDIO_CASES = ["bp28", "snr_bp12_f0", "bp60_loud", "rejected_frames", "muted_pes", "pid102"]
+
+
+def synthetic_case(case):
+    """(elementary stream, transport stream) of a synthetic audio case"""
+    kw = {"bp28": dict(bitpool=28), "snr_bp12_f0": dict(bitpool=12, allocation=1, frequency=0), "bp60_loud": dict(bitpool=60, loud=True, frequency=3),
+          "rejected_frames": dict(bitpool=28, bad_frames=(3, 4, 17)), "muted_pes": dict(bitpool=28), "pid102": dict(bitpool=28, frequency=1)}[case]
+    es = sbc_stream(1000 + len(case), 40, **kw)
+    return es, mux_audio_ts(es, pid=0x102 if case == "pid102" else 0x101, drop_pts_on=(1,) if case == "muted_pes" else ())
+
+
+def synthetic_batch():
+    """51 streams: rejected frames, inconsistent scale factors, loud, empty, shorter than a frame, no sync byte"""
+    streams = []
+    for i in range(48):
+        streams.append(sbc_stream(5000 + i, 3 + i % 11, bitpool=[2, 7, 12, 28, 31, 60, 97, 120][i % 8], allocation=i & 1, frequency=i % 4,
+                                  consistent=i % 3 != 0, bad_frames=(2, 5) if i % 5 == 0 else (), loud=i % 7 == 0))
+    streams.append(np.zeros(0, dtype=np.uint8))                          # empty
+    streams.append(sbc_stream(1, 1)[:40].copy())                         # shorter than its frame
+    streams.append(np.full(200, 0x55, dtype=np.uint8))                   # no sync byte at all: rejected
+    return streams
+
+
+def overrun_stream(seed):
+    """a stream whose frames 1, 2, 6, 7, 9 and 23 ask for a larger bit pool than frame 0's and read into the next frame"""
+    es = sbc_stream(seed, 24, bitpool=28, consistent=False, bad_frames=(3, 4, 11))
+    for k in (1, 2, 6, 7, 9, 23):
+        es[k * 64 + 2] = 40                              # bit pool 40: 8 + 2 * 40 bytes read
+    return es

@@ -124,6 +124,37 @@ def schedule(pts, modes, ntsc, frame_counter0, tail_fields):
     return len(out), ff, fl, [h for _, _, h in out], per, out
 
 
+def irregular_cases():
+    """(pts, ntsc, frame_counter0, modes, tail_fields) of 24 schedules with jitter, repeated and decreasing PTS (late
+    frames, 'resetting v timing') and long gaps, both standards"""
+    rng = np.random.default_rng(2024)
+    for case in range(24):
+        ntsc = case % 2
+        n = int(rng.integers(2, 14))
+        step = rng.choice([3003, 3003, 3003, 1501, 6006, 0, -4000, 45045], size=n)
+        pts = (129003 + np.cumsum(step)).astype(np.int64)
+        pts = np.maximum(pts, 0)
+        fc0 = int(rng.integers(0, 4)) if case < 8 else int(rng.integers(1, 100000))
+        modes = np.where(rng.random(n) < 0.2, rng.integers(1, 4, size=n), 0).astype(np.int32)      # 1 at once, 2 / 3 poster scroll
+        tail = int(rng.integers(0, 20))
+        yield pts, ntsc, fc0, modes, tail
+
+
+def irregular_programs():
+    """the 24 irregular schedules as TS programs, one PES per picture carrying the pinned pts:
+    [(case, ts, pts, ntsc, frame_counter0, modes, tail_fields)]"""
+    from tests.overlay_cases import segment_ts
+    return [(case, segment_ts(200 + case, pts), [int(v) for v in pts], ntsc, fc0, [int(m) for m in modes], tail)
+            for case, (pts, ntsc, fc0, modes, tail) in enumerate(irregular_cases())]
+
+
+def synth_ts(seed, n):
+    """synthetic stream `seed` of n pictures as TS"""
+    from espflix_b200 import synth
+    es, off = synth.generate(synth.SEED0 + seed, n_pictures=n)
+    return synth.wrap_ts(es, off)
+
+
 def blank_field(field, ntsc):
     """a field with no frame presented (video.cpp:1140): active lines are blanking lines, which repeat with period 2"""
     lines, top, bottom, _ = geometry(ntsc)

@@ -1,19 +1,18 @@
 """Audio path on the CPU (SURVEY.md 8f-3): the oracle restatement (oracle/ef_oracle_audio.c) against the pins the
 unmodified reference produced on its own fixtures (tests/golden/audio_pins.json, tools/make_audio_golden.py) and on
 synthetic transport streams (tests/golden/ref_pins.json, tools/make_ref_pins.py), and the constant tables."""
-import hashlib
 import json
 import os
 
 import numpy as np
 import pytest
 
-from tests import audio_cases
+from tests.audio_cases import AUDIO_CASES, synthetic_case
+from tests.harness import sha
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, "tests", "golden")
 REF_PINS = json.load(open(os.path.join(G, "ref_pins.json")))["audio"]
-AUDIO_CASES = ["bp28", "snr_bp12_f0", "bp60_loud", "rejected_frames", "muted_pes", "pid102"]
 
 
 def _masked(pcm, ranges):
@@ -27,13 +26,13 @@ def _masked(pcm, ranges):
 def test_oracle_matches_reference_pins(oracle, name):
     pins = json.load(open(os.path.join(G, "audio_pins.json")))[name]
     es = oracle.demux_audio_ts(open(os.path.join(G, name + ".ts"), "rb").read())
-    assert es.size == pins["es_bytes"] and hashlib.sha256(es.tobytes()).hexdigest() == pins["es_sha256"]
+    assert es.size == pins["es_bytes"] and sha(es) == pins["es_sha256"]
     pcm = oracle.sbc_decode(es)
     assert pcm.size == pins["n_frames"] * 128 and [int(x) for x in pcm[:16]] == pins["pcm_head"]
-    assert hashlib.sha256(_masked(pcm, pins["undefined"]).tobytes()).hexdigest() == pins["pcm_sha256_masked"]
+    assert sha(_masked(pcm, pins["undefined"])) == pins["pcm_sha256_masked"]
     pdm = oracle.pdm(pcm)
     k = pins["pdm_defined_words"]
-    assert hashlib.sha256(pdm[:k].tobytes()).hexdigest() == pins["pdm_sha256_defined"]
+    assert sha(pdm[:k]) == pins["pdm_sha256_defined"]
 
 
 def test_sbc_tables_match_reference_arrays():
@@ -53,26 +52,14 @@ def test_sbc_tables_match_reference_arrays():
     assert table("ef_sbc_offset8[4][8]") == g["SBC_offset8"]
 
 
-def synthetic_case(case):
-    """(elementary stream, transport stream) of a synthetic audio case"""
-    kw = {"bp28": dict(bitpool=28), "snr_bp12_f0": dict(bitpool=12, allocation=1, frequency=0), "bp60_loud": dict(bitpool=60, loud=True, frequency=3),
-          "rejected_frames": dict(bitpool=28, bad_frames=(3, 4, 17)), "muted_pes": dict(bitpool=28), "pid102": dict(bitpool=28, frequency=1)}[case]
-    es = audio_cases.sbc_stream(1000 + len(case), 40, **kw)
-    return es, audio_cases.mux_audio_ts(es, pid=0x102 if case == "pid102" else 0x101, drop_pts_on=(1,) if case == "muted_pes" else ())
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
 @pytest.mark.parametrize("case", AUDIO_CASES)
 def test_oracle_matches_reference_on_synthetic_streams(oracle, case):
     es, ts = synthetic_case(case)
     ref = REF_PINS[case]
     got_es = oracle.demux_audio_ts(ts)
-    assert got_es.size == ref["es_bytes"] and _sha(got_es) == ref["es_sha256"]
+    assert got_es.size == ref["es_bytes"] and sha(got_es) == ref["es_sha256"]
     if case == "muted_pes":
         assert got_es.size == es.size - 1024              # the second PES (no PTS) is dropped whole; the third one opens the stream again
     pcm = oracle.sbc_decode(got_es)
-    assert ref["pcm_samples"] > 0 and pcm.size == ref["pcm_samples"] and _sha(pcm) == ref["pcm_sha256"]
-    assert _sha(oracle.pdm(pcm)) == ref["pdm_sha256"]
+    assert ref["pcm_samples"] > 0 and pcm.size == ref["pcm_samples"] and sha(pcm) == ref["pcm_sha256"]
+    assert sha(oracle.pdm(pcm)) == ref["pdm_sha256"]

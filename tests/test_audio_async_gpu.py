@@ -11,21 +11,12 @@ import torch
 import espflix_b200
 from espflix_b200 import capi
 from tests import audio_cases, restart_cases as rc
-from tests.test_audio_stream_gpu import _cut, _join, _overrun_stream, _packets, _synthetic_batch
-from tests.test_present_overlay_gpu import _call, _context
+from tests.carry_cases import cut, packets
+from tests.harness import audio_results, present_call, presenting_context, same_audio, submits
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 SENTINEL = 0x5A5A
-
-
-def _results(ctx, info, pcm, pdm):
-    out = []
-    for i in espflix_b200.Context.audio_info(info):
-        a, k = int(i["pcm_offset"]), int(i["n_frames"]) * 128
-        out.append({"frame_size": int(i["frame_size"]), "n_frames": int(i["n_frames"]),
-                    "pcm": pcm[a:a + k].view(torch.int16).cpu().numpy(), "pdm": pdm[2 * a:2 * (a + k)].view(torch.int16).cpu().numpy().view(np.uint16)})
-    return out
 
 
 def decode_async(ctx, end=None, stream=0):
@@ -39,15 +30,7 @@ def decode_async(ctx, end=None, stream=0):
         pdm = torch.empty(2 * need, dtype=torch.int16, device="cuda").view(torch.uint16)
         info = ctx.decode_audio_async(pcm, pdm, end=end, stream=stream)
         assert ctx.audio_wait() == capi.EF_OK
-    return _results(ctx, info, pcm, pdm)
-
-
-def _same(a, b, what):
-    assert len(a) == len(b)
-    for s, (x, y) in enumerate(zip(a, b)):
-        assert x["frame_size"] == y["frame_size"] and x["n_frames"] == y["n_frames"], "%s stream %d" % (what, s)
-        assert np.array_equal(x["pcm"].astype(np.int16), y["pcm"].astype(np.int16)), "%s stream %d: PCM" % (what, s)
-        assert np.array_equal(x["pdm"].astype(np.uint16), y["pdm"].astype(np.uint16)), "%s stream %d: PDM" % (what, s)
+    return audio_results(info, pcm, pdm)
 
 
 def _pair(chunks, ends=None, queue_ahead=False, ops=None, mode="async", **kw):
@@ -78,7 +61,7 @@ def _pair(chunks, ends=None, queue_ahead=False, ops=None, mode="async", **kw):
                 c.restart_streams(ops[k])
             if not queue_ahead and k + 1 < K:
                 c.submit_ts(*packed[k + 1])
-        _same(res[0], res[1], "submit %d" % k)
+        same_audio(res[0], res[1], "submit %d" % k)
         got.append(res[1])
     for c in ctxs:
         c.close()
@@ -89,13 +72,10 @@ def test_reference_fixtures_cut_at_video_pes_starts():
     ts = [open(os.path.join(G, n + ".ts"), "rb").read() for n in ("splash", "vmedia")]
     per_stream = []
     for i, t in enumerate(ts):
-        pk = _packets(t)
+        pk = packets(t)
         starts = [k for k, q in enumerate(pk) if ((int(q[1]) << 8 | int(q[2])) & 0x1FFF) == 0x100 and q[1] & 0x40]
-        per_stream.append(_cut(t, starts[7 + 3 * i::9 + 2 * i]))
-    K = max(len(c) for c in per_stream)
-    for c in per_stream:
-        c += [np.zeros(0, dtype=np.uint8)] * (K - len(c))
-    got = _pair([[per_stream[0][k], per_stream[1][k]] for k in range(K)], max_pictures=13, max_slices_per_picture=8, es_capacity=1 << 21)
+        per_stream.append(cut(t, starts[7 + 3 * i::9 + 2 * i]))
+    got = _pair(submits(per_stream), max_pictures=13, max_slices_per_picture=8, es_capacity=1 << 21)
     whole = espflix_b200.audio_decode(espflix_b200.audio_demux_ts(ts))
     for s in range(2):
         assert np.array_equal(np.concatenate([g[s]["pcm"] for g in got]), whole[s]["pcm"])
@@ -104,14 +84,14 @@ def test_reference_fixtures_cut_at_video_pes_starts():
 
 @pytest.mark.parametrize("mode", ["async", "alternate"])
 def test_cut_anywhere_batch_with_rejected_frames(mode):
-    streams = _synthetic_batch() + [_overrun_stream(31), _overrun_stream(32)]
+    streams = audio_cases.synthetic_batch() + [audio_cases.overrun_stream(31), audio_cases.overrun_stream(32)]
     K = 7
     ts = [audio_cases.mux_audio_ts(es, pid=0x101 if i % 2 else 0x102, pes_bytes=[61, 188, 333, 1024, 2000][i % 5]) for i, es in enumerate(streams)]
     chunks = []
     for i, t in enumerate(ts):
         r = np.random.RandomState(1900 + i)
-        chunks.append(_cut(t, sorted(r.randint(0, t.size // 188 + 1, size=K - 1).tolist())))
-    got = _pair([[chunks[s][k] for s in range(len(streams))] for k in range(K)], mode=mode)
+        chunks.append(cut(t, sorted(r.randint(0, t.size // 188 + 1, size=K - 1).tolist())))
+    got = _pair(submits(chunks), mode=mode)
     whole = espflix_b200.audio_decode(streams)
     for s in range(len(streams)):
         assert np.array_equal(np.concatenate([g[s]["pcm"] for g in got]).astype(np.int16), whole[s]["pcm"]), s
@@ -123,10 +103,10 @@ def test_streams_ending_at_different_submits(queue_ahead):
     b = audio_cases.sbc_stream(12, 25, bitpool=12, allocation=1, frequency=0)
     c = audio_cases.sbc_stream(13, 20, bitpool=60, loud=True)
     ta, tb, tc = (audio_cases.mux_audio_ts(x, pes_bytes=400) for x in (a, b, c))
-    tb_tail = _join(_packets(tb)[1:])
-    pa, pb, pc = (_cut(t, [t.size // 188 // 3, 2 * t.size // 188 // 3]) for t in (ta, tb_tail, tc))
+    tb_tail = b"".join(packets(tb)[1:])
+    pa, pb, pc = (cut(t, [len(t) // 188 // 3, 2 * len(t) // 188 // 3]) for t in (ta, tb_tail, tc))
     empty = np.zeros(0, dtype=np.uint8)
-    chunks = [[pa[0], pc[0], _join(_packets(tc)[:5])], [pa[1], empty, _join(_packets(tc)[5:])], [pa[2], pc[1], empty],
+    chunks = [[pa[0], pc[0], b"".join(packets(tc)[:5])], [pa[1], empty, b"".join(packets(tc)[5:])], [pa[2], pc[1], empty],
               [pb[0], empty, empty], [pb[1], pc[2], empty], [pb[2], empty, empty]]
     ends = [[0, 0, 0], [0, 0, 1], [1, 0, 0], [0, 0, 0], [0, 0, 0], [1, 1, 1]]
     _pair(chunks, ends, queue_ahead=queue_ahead)
@@ -169,14 +149,14 @@ def test_returns_before_the_decode_is_done():
     info = ctx.decode_audio_async(pcm, pdm, stream=side)
     assert not side.query()
     assert ctx.audio_wait() == capi.EF_OK
-    _same(want, _results(ctx, info, pcm, pdm), "behind a busy stream")
+    same_audio(want, audio_results(info, pcm, pdm), "behind a busy stream")
     ref.close()
     ctx.close()
 
 
 def test_overflow_changes_nothing_and_a_retry_fits():
     ts = _streams(3)
-    halves = [_cut(t, [t.size // 188 // 2]) for t in ts]
+    halves = [cut(t, [t.size // 188 // 2]) for t in ts]
     ref, ctx = _two_contexts(3, [h[0] for h in halves])
     for c in (ref, ctx):
         c.submit_ts(*c.pack([h[1] for h in halves]))    # queued: the failed call must not touch its demux gate either
@@ -194,10 +174,10 @@ def test_overflow_changes_nothing_and_a_retry_fits():
     with pytest.raises(espflix_b200.EspflixError) as e:
         ctx.index()
     assert e.value.code == capi.EF_ESTATE
-    _same(want, decode_async(ctx, end=end), "retry")
+    same_audio(want, decode_async(ctx, end=end), "retry")
     for c in (ref, ctx):                                 # the calls after it: the state really was untouched
         c.index()
-    _same(ref.decode_audio(end=True), decode_async(ctx, end=True), "after the retry")
+    same_audio(ref.decode_audio(end=True), decode_async(ctx, end=True), "after the retry")
     ref.close()
     ctx.close()
 
@@ -208,7 +188,7 @@ def test_runs_beside_paced_presentation():
     progs = [[rc.program(700 + 10 * s + k, 12, 300000 + 36036 * k, audio=dict(seed=90 + 7 * s + k, frames=60, cut=0)) for k in range(K)] for s in range(n)]
     runs = []
     for audio in (False, True):
-        ctx = _context(n, 1, [0, 3, 1000, 7], max_pictures=12)
+        ctx = presenting_context(n, 1, [0, 3, 1000, 7], max_pictures=12)
         ref = espflix_b200.Context(n_streams=n, max_pictures=12, es_capacity=n * 12 * 40000, fields=False)
         if audio:
             ctx.enable_audio()
@@ -226,10 +206,10 @@ def test_runs_beside_paced_presentation():
                 pdm = torch.empty(2 * need, dtype=torch.int16, device="cuda").view(torch.uint16)
                 info = ctx.decode_audio_async(pcm, pdm, stream=ast)
             for p in range(12):
-                fields.append(_call(ctx, lambda out: ctx.present_picture(p, out=out, stream=pst.cuda_stream)))
+                fields.append(present_call(ctx, lambda out: ctx.present_picture(p, out=out, stream=pst.cuda_stream)))
             if audio:
                 assert ctx.audio_wait() == capi.EF_OK
-                _same(want, _results(ctx, info, pcm, pdm), "submit %d" % k)
+                same_audio(want, audio_results(info, pcm, pdm), "submit %d" % k)
                 sound.append(want)
         runs.append(fields)
         ctx.close()
@@ -245,10 +225,9 @@ def test_batch_scale():
     assert scale_cases.period_is_coprime_to_tiles() and b.n > 1024
     first, second = [], []
     for k in range(b.n):
-        pk = _packets(b.ts(k))
-        c = b.cut(k)[0]
-        first.append(_join(pk[:c]))
-        second.append(_join(pk[c:]))
+        first_k, second_k = cut(b.ts(k), [b.cut(k)[0]])
+        first.append(first_k)
+        second.append(second_k)
     empty = [np.zeros(0, dtype=np.uint8)] * b.n
     cap = sum(len(b.ts(k)) for k in range(b.n)) + (1 << 20)
     got = _pair([first, second, empty], ends=[[0] * b.n, [k % 3 == 0 for k in range(b.n)], [1] * b.n], max_pictures=12, es_capacity=cap)

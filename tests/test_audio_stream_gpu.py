@@ -1,7 +1,6 @@
 """Audio through the decoder context (ef_audio_enable / ef_decode_audio): every stream's TS cut into submits at packet
 boundaries, the stream ended in its last submit. Concatenated over the calls, PCM and PDM must equal the whole-stream
 call (ef_audio_decode on ef_audio_demux_ts), the restatement and the reference's pins, element for element."""
-import hashlib
 import json
 import os
 
@@ -11,19 +10,12 @@ import pytest
 import espflix_b200
 from espflix_b200 import capi
 from tests import audio_cases
+from tests.carry_cases import cut, packets
+from tests.harness import sha, submits
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, "tests", "golden")
-
-
-def _packets(ts):
-    ts = np.frombuffer(bytes(ts), dtype=np.uint8)
-    return [ts[i:i + 188] for i in range(0, ts.size, 188)]
-
-
-def _join(pkts):
-    return np.concatenate(pkts) if len(pkts) else np.zeros(0, dtype=np.uint8)
 
 
 def _masked(pcm, ranges):
@@ -31,13 +23,6 @@ def _masked(pcm, ranges):
     for a, b in ranges:
         p[a:b] = 0
     return p
-
-
-def _cut(ts, cuts):
-    """TS -> list of chunks at the packet indices `cuts` (sorted, may repeat: empty chunks)"""
-    pk = _packets(ts)
-    edges = [0] + list(cuts) + [len(pk)]
-    return [_join(pk[a:b]) for a, b in zip(edges[:-1], edges[1:])]
 
 
 def _run(ctx, chunks, ends=None, queue_ahead=False):
@@ -94,7 +79,7 @@ def test_whole_program_across_submits(oracle):
     sizes = [[5, 12, 1, 9, 7, 12, 3], [11, 2, 12, 8, 6, 4, 10]]
     per_stream = []
     for i, t in enumerate(ts):
-        pk = _packets(t)
+        pk = packets(t)
         starts = [k for k, q in enumerate(pk) if ((int(q[1]) << 8 | int(q[2])) & 0x1FFF) == 0x100 and q[1] & 0x40]
         cuts, p, j = [], 0, 0
         while True:
@@ -103,18 +88,16 @@ def test_whole_program_across_submits(oracle):
             if p >= len(starts):
                 break
             cuts.append(starts[p])
-        per_stream.append(_cut(t, cuts))
-    K = max(len(c) for c in per_stream)
-    for c in per_stream:                                 # the shorter program ends early; empty chunks after it
-        c += [np.zeros(0, dtype=np.uint8)] * (K - len(c))
-    lens = [sum(1 for x in c if x.size) for c in per_stream]
-    ends = [[k == lens[s] - 1 for s in range(2)] for k in range(K)]
+        per_stream.append(cut(t, cuts))
+    lens = [sum(1 for x in c if len(x)) for c in per_stream]
+    chunks = submits(per_stream)                         # the shorter program ends early; empty chunks after it
+    ends = [[k == lens[s] - 1 for s in range(2)] for k in range(len(chunks))]
     ctx = espflix_b200.Context(n_streams=2, max_pictures=13, max_slices_per_picture=8, es_capacity=1 << 21)
     ctx.enable_audio()
     frames = [[], []]
     audio = [[], []]
-    for k in range(K):
-        ctx.submit_ts(*ctx.pack([per_stream[0][k], per_stream[1][k]]))
+    for k, chunk in enumerate(chunks):
+        ctx.submit_ts(*ctx.pack(chunk))
         ctx.index()
         counts = [ctx.stream_info(s)[0] for s in range(2)]
         for p in range(max(counts)):
@@ -129,38 +112,20 @@ def test_whole_program_across_submits(oracle):
     for s, n in enumerate(names):
         assert len(frames[s]) == dpins[n]["frames"]
         for k, f in enumerate(frames[s]):
-            assert hashlib.sha256(f.tobytes()).hexdigest() == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
+            assert sha(f) == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
         _check_equal(audio[s], whole[s], what=n)
         pcm, pdm = _cat(audio[s], "pcm").astype(np.int16), _cat(audio[s], "pdm").astype(np.uint16)
         assert max(c["frame_size"] for c in audio[s]) == apins[n]["frame_size"] and pcm.size == apins[n]["n_frames"] * 128
-        assert hashlib.sha256(_masked(pcm, apins[n]["undefined"]).tobytes()).hexdigest() == apins[n]["pcm_sha256_masked"]
-        assert hashlib.sha256(pdm[:apins[n]["pdm_defined_words"]].tobytes()).hexdigest() == apins[n]["pdm_sha256_defined"]
+        assert sha(_masked(pcm, apins[n]["undefined"])) == apins[n]["pcm_sha256_masked"]
+        assert sha(pdm[:apins[n]["pdm_defined_words"]]) == apins[n]["pdm_sha256_defined"]
     ctx.close()
-
-
-def _synthetic_batch():
-    streams = []
-    for i in range(48):
-        streams.append(audio_cases.sbc_stream(5000 + i, 3 + i % 11, bitpool=[2, 7, 12, 28, 31, 60, 97, 120][i % 8], allocation=i & 1, frequency=i % 4,
-                                              consistent=i % 3 != 0, bad_frames=(2, 5) if i % 5 == 0 else (), loud=i % 7 == 0))
-    streams.append(np.zeros(0, dtype=np.uint8))                          # empty
-    streams.append(audio_cases.sbc_stream(1, 1)[:40].copy())             # shorter than its frame
-    streams.append(np.full(200, 0x55, dtype=np.uint8))                   # no sync byte at all: rejected
-    return streams
-
-
-def _overrun_stream(seed):
-    es = audio_cases.sbc_stream(seed, 24, bitpool=28, consistent=False, bad_frames=(3, 4, 11))
-    for k in (1, 2, 6, 7, 9, 23):
-        es[k * 64 + 2] = 40                              # bit pool 40: 8 + 2 * 40 bytes read
-    return es
 
 
 def test_batch_cut_anywhere(oracle):
     """the 51 synthetic streams of test_batch_of_synthetic_streams (rejected frames, inconsistent scale factors, loud,
     empty, sub-frame, no sync) and two whose frames read into the next frame, muxed with
     varied PES sizes, each cut at its own seeded packet boundaries over 7 submits (empty and single-packet chunks)"""
-    streams = _synthetic_batch() + [_overrun_stream(31), _overrun_stream(32)]
+    streams = audio_cases.synthetic_batch() + [audio_cases.overrun_stream(31), audio_cases.overrun_stream(32)]
     n, K = len(streams), 7
     ts = [audio_cases.mux_audio_ts(es, pid=0x101 if i % 2 else 0x102, pes_bytes=[61, 188, 333, 1024, 2000][i % 5]) for i, es in enumerate(streams)]
     chunks = []
@@ -171,11 +136,11 @@ def test_batch_cut_anywhere(oracle):
         if i % 4 == 0 and n_pk > 2:                      # a single-packet chunk followed by an empty one
             a = int(r.randint(0, n_pk - 1))
             cuts = sorted(cuts[:K - 4] + [a, a + 1, a + 1])
-        chunks.append(_cut(t, cuts))
+        chunks.append(cut(t, cuts))
     assert all(len(c) == K for c in chunks)
     ctx = espflix_b200.Context(n_streams=n, max_pictures=2, es_capacity=1 << 22, fields=False)
     ctx.enable_audio()
-    out = _run(ctx, [[chunks[s][k] for s in range(n)] for k in range(K)])
+    out = _run(ctx, submits(chunks))
     whole = _whole(streams)
     for s in range(n):
         _check_equal(out[s], whole[s], oracle, streams[s], "stream %d" % s)
@@ -200,7 +165,7 @@ def test_cuts_placed_on_purpose(oracle):
     # one frame per submit. Frames whose header asks for a larger bit pool than frame 0's read 88 bytes where the frame
     # size is 64: their bit loader runs into the next frame, whose bytes come one submit later (the frame is held back),
     # the last one past the end of the stream. Rejected frames repeat an accepted frame decoded one or two submits earlier.
-    es = _overrun_stream(4242)
+    es = audio_cases.overrun_stream(4242)
     fs = 8 + 2 * 28
     pieces = [audio_cases.mux_audio_ts(es[a:a + fs]) for a in range(0, es.size, fs)]
 
@@ -218,9 +183,9 @@ def test_cuts_placed_on_purpose(oracle):
     # and cut right after a PES start with PTS: it stays open
     es = audio_cases.sbc_stream(77, 40)
     ts = audio_cases.mux_audio_ts(es, pes_bytes=512, drop_pts_on=(1, 3))
-    pk = _packets(ts)
+    pk = packets(ts)
     starts = [k for k, q in enumerate(pk) if q[1] & 0x40]
-    pieces = _cut(ts, [starts[1] + 1, starts[2] + 1, starts[3] + 1, starts[3] + 2])
+    pieces = cut(ts, [starts[1] + 1, starts[2] + 1, starts[3] + 1, starts[3] + 2])
     want_es = oracle.demux_audio_ts(ts)
     assert np.array_equal(espflix_b200.audio_demux_ts([ts])[0], want_es) and want_es.size == es.size - 1024
     _one(oracle, es, pieces, "gate cut", whole_es=want_es)
@@ -233,14 +198,14 @@ def test_streams_ending_at_different_submits(oracle):
     b = audio_cases.sbc_stream(12, 25, bitpool=12, allocation=1, frequency=0)
     c = audio_cases.sbc_stream(13, 20, bitpool=60, loud=True)
     ta, tb, tc = (audio_cases.mux_audio_ts(x, pes_bytes=400) for x in (a, b, c))
-    tb_tail = _join(_packets(tb)[1:])                    # program b without its first packet: starts with continuation packets
+    tb_tail = b"".join(packets(tb)[1:])                    # program b without its first packet: starts with continuation packets
     b_alone = oracle.demux_audio_ts(tb_tail)
     assert b_alone.size < b.size
-    pa, pb, pc = (_cut(t, [t.size // 188 // 3, 2 * t.size // 188 // 3]) for t in (ta, tb_tail, tc))
+    pa, pb, pc = (cut(t, [len(t) // 188 // 3, 2 * len(t) // 188 // 3]) for t in (ta, tb_tail, tc))
     empty = np.zeros(0, dtype=np.uint8)
     # stream 0: a over submits 0-2, ends at 2, then b (tail) over 3-5; stream 1: c over 0-5 ends at 5; stream 2: c ends at 1
-    chunks = [[pa[0], pc[0], _join(_packets(tc)[:5])],
-              [pa[1], empty, _join(_packets(tc)[5:])],
+    chunks = [[pa[0], pc[0], b"".join(packets(tc)[:5])],
+              [pa[1], empty, b"".join(packets(tc)[5:])],
               [pa[2], pc[1], empty],
               [pb[0], empty, empty],
               [pb[1], pc[2], empty],
@@ -271,7 +236,7 @@ def test_streams_ending_at_different_submits(oracle):
 def test_sizing_and_errors(oracle):
     es = [audio_cases.sbc_stream(21, 30), audio_cases.sbc_stream(22, 17, bitpool=60, consistent=False)]
     ts = [audio_cases.mux_audio_ts(e) for e in es]
-    halves = [_cut(t, [t.size // 188 // 2]) for t in ts]
+    halves = [cut(t, [t.size // 188 // 2]) for t in ts]
     ctx = espflix_b200.Context(n_streams=2, max_pictures=2, es_capacity=1 << 20, fields=False)
     with pytest.raises(espflix_b200.EspflixError) as e:
         ctx.decode_audio()

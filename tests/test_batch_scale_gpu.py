@@ -12,6 +12,7 @@ import pytest
 import espflix_b200
 from tests import present_cases as pc
 from tests import pts_cases, scale_cases
+from tests.harness import present_call, presenting_context
 from tests.scale_cases import D, N, PICTURES
 
 I420 = 101376
@@ -193,11 +194,6 @@ def test_audio_of_every_stream_across_submits(batch, oracle):
 
 
 # ---- paced presentation --------------------------------------------------------------------------------------------------
-def _rows(out, w, nl):
-    import torch
-    return out.view(torch.int16).view(-1, w * nl)
-
-
 def _equal_rows(F, a, b, tag, where):
     """on the device: rows a[i] of F equal rows b[i]; where(i) names a failing pair"""
     import torch
@@ -217,7 +213,6 @@ class _Paced:
         self.disp = [pc.Display(ntsc, batch.fc0(d)) for d in range(min(n, D))]
         self.rend = [pc.Renderer(oracle, ntsc) for _ in range(min(n, D))]
         self.frames = frames
-        self.w, self.nl = ctx.geometry()
 
     def _expect(self, per_d, flips):
         """expected info of every stream from the distinct streams' fields -> numpy arrays"""
@@ -229,11 +224,7 @@ class _Paced:
 
     def call(self, fn, per_d, flips, tag):
         import torch
-        info0 = fn(None)
-        total = int(info0["n_fields"].sum())
-        out = torch.empty(max(total, 1) * self.w * self.nl, dtype=torch.uint16, device="cuda")
-        info = fn(out)
-        assert (info == info0).all(), tag
+        info, fields = present_call(self.ctx, fn, device=True)
         nf, first, fc, idx = self._expect(per_d, flips)
         for name, got, want in (("n_fields", info["n_fields"], nf), ("first", info["first"], first)):
             bad = np.nonzero(got.astype(np.int64) != want)[0]
@@ -248,7 +239,7 @@ class _Paced:
             fl = np.array([f[1] for f in flips], dtype=np.int64)[idx]
             bad = np.nonzero((info["flip_field"].astype(np.int64) != ff) | (info["flip_line"].astype(np.int64) != fl))[0]
             assert bad.size == 0, "%s: flip of %s" % (tag, _where(bad[0]))
-        F = _rows(out, self.w, self.nl)
+        F = fields.view(torch.int16)
         nd = min(self.n, D)
         host = F[:int(first[nd - 1] + nf[nd - 1])].cpu().numpy().view(np.uint16)
         for d in range(nd):                                        # the distinct streams against the restatement
@@ -264,7 +255,7 @@ class _Paced:
             who += [(s, j) for j in range(nf[s])]
         if a:
             _equal_rows(F, a, b, tag, lambda i: "%s, field %d" % (_where(who[i][0]), who[i][1]))
-        del F, out
+        del F, fields
         torch.cuda.empty_cache()                                   # the next call's buffer has another size
         return info
 
@@ -290,10 +281,7 @@ def test_paced_fields_of_every_stream(batch, frames, packed, oracle, ntsc):
     stream's present info against the restatement, the distinct streams' fields against its rendering by the C
     restatement, every other stream's fields against its original's"""
     import torch
-    ctx = espflix_b200.Context(n_streams=N, max_pictures=PICTURES, max_slices_per_picture=12, es_capacity=int(packed[1][-1]) + 4096, fields=False)
-    ctx.enable_pts()
-    ctx.video_init(ntsc)
-    ctx.enable_present([batch.fc0(s) for s in range(N)])
+    ctx = presenting_context(N, ntsc, [batch.fc0(s) for s in range(N)], max_pictures=PICTURES, es_capacity=int(packed[1][-1]) + 4096)
     ctx.submit_ts(*packed)
     ctx.index()
     r = _Paced(ctx, ntsc, batch, frames, oracle, N)
@@ -313,10 +301,7 @@ def test_paced_k2_split_over_launches(batch, frames, oracle):
     total = n_streams * per_stream
     assert total >= 65535 + 8
     es_total = sum(len(batch.ts(s)) for s in range(n_streams))
-    ctx = espflix_b200.Context(n_streams=n_streams, max_pictures=PICTURES, max_slices_per_picture=12, es_capacity=es_total + 4096, fields=False)
-    ctx.enable_pts()
-    ctx.video_init(1)
-    ctx.enable_present([batch.fc0(s) for s in range(n_streams)])
+    ctx = presenting_context(n_streams, 1, [batch.fc0(s) for s in range(n_streams)], max_pictures=PICTURES, es_capacity=es_total + 4096)
     ctx.submit_ts(*ctx.pack([batch.ts(s) for s in range(n_streams)]))
     ctx.index()
     r = _Paced(ctx, 1, batch, frames, oracle, n_streams)
@@ -340,7 +325,7 @@ def test_paced_k2_split_over_launches(batch, frames, oracle):
         assert (info == info0).all()
         first = [int(x) for x in info["first"]]
         assert first == [per_stream * s for s in range(n_streams)]
-        F = _rows(out, w, nl)
+        F = out.view(torch.int16).view(-1, w * nl)
 
         def check_slot(g):
             s, j = g // per_stream, g % per_stream

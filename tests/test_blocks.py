@@ -2,7 +2,6 @@
 (pinned by tools/make_block_pins.py in tests/golden/block_pins.json), which cases leave the clamp table's domain, and
 the census that shows each case reaches every combination it targets."""
 import functools
-import hashlib
 import json
 import os
 
@@ -10,14 +9,11 @@ import numpy as np
 import pytest
 
 from tests import block_cases as bc
+from tests.harness import sha
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "block_pins.json")))
 PINNED = [n for n in bc.case_names() if n not in bc.UNPINNED]
-
-
-def sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 @functools.lru_cache(maxsize=None)

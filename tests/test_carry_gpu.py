@@ -1,7 +1,6 @@
 """TS submits cut at any packet boundary (ef_carry_enable / ef_end_streams / ef_carry_info) on the GPU: decoded pictures, pts,
 per-submit picture counts and held bytes, against the reference's pins, the whole-program decode of a non-carrying context and
 the restatement in tests/carry_cases.py."""
-import hashlib
 import json
 import os
 
@@ -10,21 +9,12 @@ import pytest
 
 import espflix_b200
 from espflix_b200 import capi
-from tests import carry_cases, pts_cases, restart_cases
-from tests.test_present_gpu import Run as PresentRun, _call, _irregular_programs
+from tests import carry_cases, present_cases as pc, pts_cases, restart_cases
+from tests.harness import Paced, presenting_context, sha, submits
 
 pytestmark = pytest.mark.gpu
 G = pts_cases.GOLDEN
 MAX_CARRY = 65536
-
-
-def _sha(a):
-    return hashlib.sha256(a.tobytes()).hexdigest()
-
-
-def _pad(per_stream):
-    K = max(len(c) for c in per_stream)
-    return [list(c) + [b""] * (K - len(c)) for c in per_stream]
 
 
 class Run:
@@ -47,7 +37,7 @@ def _index_and_read(ctx, run, n, decode=True, check_info=True):
             ctx.decode_picture(p)
             for s in range(n):
                 if p < counts[s]:
-                    run.frames[s].append(_sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
+                    run.frames[s].append(sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
     pic, _ = ctx.picture_pts()
     held, _ = ctx.carry_info()
     for s in range(n):
@@ -62,10 +52,9 @@ def _drive(ctx, per_stream, end_at=None, decode=True, run=None):
     n = len(per_stream)
     if end_at is None:
         end_at = [len(c) - 1 for c in per_stream]
-    per_stream = _pad(per_stream)
     run = run or Run(n)
-    for k in range(len(per_stream[0])):
-        ctx.submit_ts(*ctx.pack([per_stream[s][k] for s in range(n)]))
+    for k, chunk in enumerate(submits(per_stream)):
+        ctx.submit_ts(*ctx.pack(chunk))
         ends = np.array([1 if end_at[s] == k else 0 for s in range(n)], dtype=np.uint8)
         if ends.any():
             ctx.end_streams(ends)
@@ -100,7 +89,7 @@ def _whole(programs, max_pictures=100):
         ctx.decode_picture(p)
         for s in range(len(programs)):
             if p < counts[s]:
-                run.frames[s].append(_sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
+                run.frames[s].append(sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
     pic, _ = ctx.picture_pts()
     for s in range(len(programs)):
         run.pts[s] = [int(v) for v in pic[s, :counts[s]]]
@@ -165,11 +154,10 @@ def test_audio_beside_carry():
     per_stream = [carry_cases.cut(ts, carry_cases.seeded_cuts(ts, 500 + i, 9)) for i, ts in enumerate(progs)]
     ctx = _carrying(3)
     ctx.enable_audio()
-    per = _pad(per_stream)
     run = Run(3)
     pcm, pdm = [[] for _ in progs], [[] for _ in progs]
-    for k in range(len(per[0])):
-        ctx.submit_ts(*ctx.pack([per[s][k] for s in range(3)]))
+    for k, chunk in enumerate(submits(per_stream)):
+        ctx.submit_ts(*ctx.pack(chunk))
         last = [k == len(per_stream[s]) - 1 for s in range(3)]
         if any(last):
             ctx.end_streams(np.array(last, dtype=np.uint8))
@@ -297,9 +285,8 @@ def test_streams_end_at_different_submits_then_new_programs():
     ends = [[len(p) - 1, len(p) + len(q) - 1] for p, q in zip(parts, parts2)]
     ctx = _carrying(3)
     run = Run(3)
-    per = _pad(per)
-    for k in range(len(per[0])):
-        ctx.submit_ts(*ctx.pack([per[s][k] for s in range(3)]))
+    for k, chunk in enumerate(submits(per)):
+        ctx.submit_ts(*ctx.pack(chunk))
         e = np.array([1 if k in ends[s] else 0 for s in range(3)], dtype=np.uint8)
         if e.any():
             ctx.end_streams(e)
@@ -326,10 +313,9 @@ def test_capacity_flag_and_neighbours():
     assert max(_restated(big_parts).held_sizes) > max_carry
     ctx = _carrying(2, max_carry=max_carry)
     run = Run(2)
-    per = _pad([big_parts, small_parts])
     flagged = False
-    for k in range(len(per[0])):
-        ctx.submit_ts(*ctx.pack([per[0][k], per[1][k]]))
+    for k, chunk in enumerate(submits([big_parts, small_parts])):
+        ctx.submit_ts(*ctx.pack(chunk))
         if k == len(small_parts) - 1:
             ctx.end_streams(np.array([0, 1], dtype=np.uint8))
         try:
@@ -357,7 +343,7 @@ def _index_and_read_after_error(ctx, run):
         ctx.decode_picture(p)
         for s in range(2):
             if p < counts[s]:
-                run.frames[s].append(_sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
+                run.frames[s].append(sha(ctx.read_frame_i420(s, (ctx.stream_info(s)[1] + p + 1) & 1)))
     pic, _ = ctx.picture_pts()
     held, _ = ctx.carry_info()
     for s in range(2):
@@ -410,72 +396,22 @@ def test_errors_and_launch_counts():
 
 
 # -- paced presentation of carried submits -------------------------------------------------------------------------------------
-class _PacedRun(PresentRun):
-    """tests/test_present_gpu.py's driver, with ef_end_streams before each ef_index and the synchronous or asynchronous calls"""
-
-    def submit_carry(self, chunk, mode_of, ends, use_async):
-        import torch
-        ctx = self.ctx
-        ctx.submit_ts(*ctx.pack(chunk))
-        if ends is not None and any(ends):
-            ctx.end_streams(np.array(ends, dtype=np.uint8))
-        ctx.index()
-        npics = ctx.index_info()["max_pictures"]
-        counts = [ctx.stream_info(s)[0] for s in range(self.n)]
-        pic_pts, _ = ctx.picture_pts()
-        w, nl = ctx.geometry()
-        for p in range(npics):
-            modes = [mode_of(s, self.seen[s] + p) if p < counts[s] else 0 for s in range(self.n)]
-            want = [[] for _ in range(self.n)]
-            for s in range(self.n):
-                if p < counts[s]:
-                    g = self.seen[s] + p
-                    self.rend[s].decoded(g, self.frames[s][g])
-                    want[s], _, _ = self.disp[s].push(int(pic_pts[s, p]), modes[s])
-                    self.pts[s].append(int(pic_pts[s, p]))
-            if use_async:
-                total = int(ctx.present_picture(p, modes)["n_fields"].sum())        # synchronous sizing call
-                out = torch.empty(max(total, 1) * w * nl, dtype=torch.uint16, device="cuda")
-                info_t = ctx.present_picture_async(p, out, modes=modes)
-                assert ctx.present_wait() == (capi.EF_OK, 1)
-                info = ctx.present_info(info_t)
-                host = out[:total * w * nl].view(torch.int16).cpu().numpy().view(np.uint16).reshape(total, w * nl)
-            else:
-                info, host = _call(ctx, lambda o: ctx.present_picture(p, modes, o))
-            for s in range(self.n):
-                if p < counts[s]:
-                    self.flips[s].append((int(info[s]["flip_field"]), int(info[s]["flip_line"])))
-                    assert self.flips[s][-1] == (self.disp[s].F, self.disp[s].L - 1)
-                    assert int(info[s]["flags"]) == 0
-                else:
-                    assert int(info[s]["flip_line"]) == -1 and int(info[s]["n_fields"]) == 0
-            self._collect(info, host, want)
-        self.seen = [a + b for a, b in zip(self.seen, counts)]
-
-
 def _paced(progs, ntsc, cut_seed=None, use_async=False):
     """progs: [(ts, fc0, modes, tail fields)]; whole on a non-carrying context, or every program cut at its own seeded packets
     on a carrying one and ended with its last submit"""
     from tests.oracle_lib import Oracle
     o = Oracle()
-    n = len(progs)
     fc0 = [p[1] for p in progs]
-    ctx = espflix_b200.Context(n_streams=n, max_pictures=13, max_slices_per_picture=12, es_capacity=n * 13 * 40000, fields=False)
-    ctx.enable_pts()
-    if cut_seed is not None:
-        ctx.enable_carry(MAX_CARRY)
-    ctx.video_init(ntsc)
-    ctx.enable_present(fc0)
-    r = _PacedRun(ctx, ntsc, [o.decode_ts(p[0]) for p in progs], fc0, o)
+    ctx = presenting_context(len(progs), ntsc, fc0, carry=None if cut_seed is None else MAX_CARRY)
+    r = Paced(ctx, [pc.Display(ntsc, f) for f in fc0], [pc.Renderer(o, ntsc) for _ in progs], [o.decode_ts(p[0]) for p in progs])
     mode_of = lambda s, g: progs[s][2][g]                                        # noqa: E731
     if cut_seed is None:
-        r.submit_carry([p[0] for p in progs], mode_of, None, use_async)
+        r.submit([p[0] for p in progs], mode_of, None, use_async)
     else:
         per = [carry_cases.cut(p[0], carry_cases.seeded_cuts(p[0], cut_seed + s, 25)) for s, p in enumerate(progs)]
         last = [len(c) - 1 for c in per]
-        per = _pad(per)
-        for k in range(len(per[0])):
-            r.submit_carry([per[s][k] for s in range(n)], mode_of, [k == last[s] for s in range(n)], use_async)
+        for k, chunk in enumerate(submits(per)):
+            r.submit(chunk, mode_of, [k == last[s] for s in range(len(progs))], use_async)
     r.idle([p[3] + 1 for p in progs])
     ctx.close()
     return r
@@ -485,7 +421,7 @@ def _paced(progs, ntsc, cut_seed=None, use_async=False):
 def test_paced_presentation_of_carried_submits(ntsc):
     """the irregular schedules of tests/test_present_gpu.py (modes 1 to 3 included) cut anywhere, through the synchronous and
     the asynchronous present calls: fields, flips and pts equal the run on whole programs, and the restatement"""
-    progs = [(ts, fc0, modes, tail) for _, ts, _, n, fc0, modes, tail in _irregular_programs() if n == ntsc]
+    progs = [(ts, fc0, modes, tail) for _, ts, _, n, fc0, modes, tail in pc.irregular_programs() if n == ntsc]
     whole = _paced(progs, ntsc)
     for seed, use_async in ((20 + ntsc, False), (40 + ntsc, True)):
         r = _paced(progs, ntsc, cut_seed=seed, use_async=use_async)
@@ -510,16 +446,16 @@ def test_scale_batch_cut_anywhere():
     per = [carry_cases.cut(b.ts(k), carry_cases.seeded_cuts(b.ts(k), 7000 + k)) for k in range(N)]
     want = [_restated(c) for c in per]
     last = [len(c) - 1 for c in per]
-    per = _pad(per)
-    K = len(per[0])
-    cap = max(sum(len(per[s][k]) for s in range(N)) for k in range(K)) + 4096
+    chunks = submits(per)
+    K = len(chunks)
+    cap = max(sum(len(c) for c in chunk) for chunk in chunks) + 4096
     ctx = espflix_b200.Context(n_streams=N, max_pictures=P, max_slices_per_picture=12, es_capacity=cap, fields=False)
     ctx.enable_pts()
     ctx.enable_carry(MAX_CARRY)
     seen = np.zeros(N, dtype=np.int64)
     pts = [[] for _ in range(N)]
     for k in range(K):
-        ctx.submit_ts(*ctx.pack([per[s][k] for s in range(N)]))
+        ctx.submit_ts(*ctx.pack(chunks[k]))
         ends = np.array([1 if last[s] == k else 0 for s in range(N)], dtype=np.uint8)
         if ends.any():
             ctx.end_streams(ends)

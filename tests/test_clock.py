@@ -1,18 +1,14 @@
 """The overlay clock's restatement (tests/clock_cases.py) against what the unmodified reference's update_progress() and show_time()
 produced (tests/golden/clock_pins.json, tools/make_clock_golden.py), and its staging into the restated overlay display."""
-import hashlib
 
 import numpy as np
 
 from tests import clock_cases as cc
 from tests import overlay_cases as oc
+from tests.harness import sha
 
 PINS = cc.pins()
 ATLAS, RIGHTS = cc.font()
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint8).tobytes()).hexdigest()
 
 
 def test_font_fixture():
@@ -32,7 +28,7 @@ def test_show_time_pins():
     for p in PINS["show_time"]:
         text = cc.time_text(p["seconds"], p["icon"])
         assert cc.text_width(text, RIGHTS) == p["width"]
-        assert _sha(cc.render(text, ATLAS, RIGHTS)) == p["sha256"], text
+        assert sha(cc.render(text, ATLAS, RIGHTS)) == p["sha256"], text
     widths = {cc.text_width(cc.time_text(s, cc.PLAY), RIGHTS) for s in (3723, 36671)}
     assert widths == {68, 76}                                   # one- and two-digit hours fit in a row; three digits wrap
     assert any(p["width"] > 80 for p in PINS["show_time"])
@@ -61,8 +57,8 @@ def test_pins_reject_wrong_rules():
                     out[:, x + j] = np.where(col > 0, (cc.COLOR * col) >> 8, 0)
             x += right - left
         return out.reshape(-1)
-    assert any(_sha(clipped(cc.time_text(p["seconds"], p["icon"]), ATLAS, RIGHTS)) != p["sha256"] for p in PINS["show_time"])
-    assert all(_sha(clipped(cc.time_text(p["seconds"], p["icon"]), ATLAS, RIGHTS)) == p["sha256"] for p in PINS["show_time"] if p["width"] <= 80)
+    assert any(sha(clipped(cc.time_text(p["seconds"], p["icon"]), ATLAS, RIGHTS)) != p["sha256"] for p in PINS["show_time"])
+    assert all(sha(clipped(cc.time_text(p["seconds"], p["icon"]), ATLAS, RIGHTS)) == p["sha256"] for p in PINS["show_time"] if p["width"] <= 80)
 
     def zeroing(steps_):
         return cc.restate([(h, sp, pa, True, pts) for h, sp, pa, _, pts in steps_], ATLAS, RIGHTS)
@@ -91,5 +87,5 @@ def test_clock_staging_in_the_restated_display():
     assert len(ovs) == len(d.emitted)
     seconds = sorted({p // 90000 for p in pts})
     assert seconds == [1, 2, 3, 4] and sum(1 for bm, _ in shown if bm is not None) == len(seconds)
-    assert all(_sha(bm) == _sha(cc.render(cc.time_text(4, cc.PLAY), ATLAS, RIGHTS)) for _, _, bm in ovs[-3:])
+    assert all(sha(bm) == sha(cc.render(cc.time_text(4, cc.PLAY), ATLAS, RIGHTS)) for _, _, bm in ovs[-3:])
     assert ovs[-1][1] == shown[-1][1] == (pts[-1] * 240) // (129003 + 90000 * 30)

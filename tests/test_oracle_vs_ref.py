@@ -1,54 +1,17 @@
 """The oracle restatement against the UNMODIFIED reference on the synthetic coverage streams, plus assertions that
 those streams really exercise the paths the reference's fixtures lack. What the reference computed for the same
 inputs is pinned in tests/golden/ref_pins.json (SHA-256 of its outputs, tools/make_ref_pins.py)."""
-import hashlib
 import json
 import os
 
 import numpy as np
 import pytest
 
-from espflix_b200 import synth
-from tests.synth_cases import COVERAGE, make
+from tests.harness import sha
+from tests.synth_cases import COVERAGE, coverage_stream, make, presentation_cases, video_cases
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_pins.json")))
-
-
-def sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def coverage_stream(idx):
-    """(elementary stream, transport stream) of coverage case `idx`"""
-    es, off = make(idx, COVERAGE[idx][1])
-    return es, synth.wrap_ts(es, off)
-
-
-def video_cases():
-    """(key, call): composite fields and blits of random frames; `call` takes the oracle or the reference alike."""
-    rng = np.random.default_rng(7)
-    for ntsc in (1, 0):
-        for fc in (0, 1, 2):
-            fr = rng.integers(0, 249, 101376, dtype=np.uint8)
-            yield "field/%d/%d" % (ntsc, fc), lambda v, fr=fr, ntsc=ntsc, fc=fc: v.field(fr, ntsc, fc)
-        fr = rng.integers(0, 256, 101376, dtype=np.uint8)          # bytes above 248: dither carries cross bytes
-        yield "field/%d/1/carry" % ntsc, lambda v, fr=fr, ntsc=ntsc: v.field(fr, ntsc, 1)
-        for line, x, w in ((0, 0, 352), (191, 0, 352), (77, 16, 64), (100, 8, 344)):
-            yield "blit/%d/%d/%d/%d" % (ntsc, line, x, w), lambda v, fr=fr, ntsc=ntsc, line=line, x=x, w=w: v.blit(fr, ntsc, line, x, w, 1)
-
-
-PRESENTATION_CASES = [(0, 0, 0), (8, 0, 0), (-8, 0, 0), (176, 0, 0), (-344, 0, 0), (344, -1, 100), (0, 32, 0), (0, 5, 239), (0, 31, 17), (24, 1, 300)]
-
-
-def presentation_cases():
-    """(key, call): _hscroll two-frame scroll and the composite() overlay / progress bar / fade, both standards."""
-    rng = np.random.default_rng(11)
-    a, b = rng.integers(0, 249, 101376, dtype=np.uint8), rng.integers(0, 249, 101376, dtype=np.uint8)
-    bm = rng.integers(0, 256, 1280, dtype=np.uint8)
-    for ntsc in (1, 0):
-        for hs, blend, prog in PRESENTATION_CASES:
-            yield "%d/%d/%d/%d" % (ntsc, hs, blend, prog), lambda v, ntsc=ntsc, hs=hs, blend=blend, prog=prog: v.field_ex(a, b, ntsc, 1, hs, bm, blend, prog)
 
 
 @pytest.mark.parametrize("idx", range(len(COVERAGE)), ids=[c[0] for c in COVERAGE])

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from tests.oracle_lib import Oracle
+from tests.present_cases import irregular_cases
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "pacing_pins.json")))
@@ -22,22 +23,6 @@ def test_schedule_matches_reference_pins(name):
     fields, ff, fl, hs = Oracle().paced_schedule(pts, p["ntsc"], p["frame_counter0"], p["max_fields"], modes=p["modes"], tail_fields=p["tail_fields"], want_hscroll=True)
     assert fields == p["fields"] and ff.tolist() == p["flip_field"] and fl.tolist() == p["flip_line"]
     assert hs.tolist() == p["hscroll"]                    # the poster scroll (_animate / _easd) field by field
-
-
-def irregular_cases():
-    """(pts, ntsc, frame_counter0, modes, tail_fields) of 24 schedules with jitter, repeated and decreasing PTS (late
-    frames, 'resetting v timing') and long gaps, both standards"""
-    rng = np.random.default_rng(2024)
-    for case in range(24):
-        ntsc = case % 2
-        n = int(rng.integers(2, 14))
-        step = rng.choice([3003, 3003, 3003, 1501, 6006, 0, -4000, 45045], size=n)
-        pts = (129003 + np.cumsum(step)).astype(np.int64)
-        pts = np.maximum(pts, 0)
-        fc0 = int(rng.integers(0, 4)) if case < 8 else int(rng.integers(1, 100000))
-        modes = np.where(rng.random(n) < 0.2, rng.integers(1, 4, size=n), 0).astype(np.int32)      # 1 at once, 2 / 3 poster scroll
-        tail = int(rng.integers(0, 20))
-        yield pts, ntsc, fc0, modes, tail
 
 
 def test_schedule_matches_reference_on_irregular_pts():

@@ -11,7 +11,7 @@ import pytest
 from espflix_b200 import synth
 from tests import present_cases as pc
 from tests.oracle_lib import Oracle
-from tests.test_pacing import irregular_cases
+from tests.present_cases import irregular_cases
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "pacing_pins.json")))

@@ -4,6 +4,8 @@ call must be equal, on the pinned reference cases (whose field streams must stil
 whole and cut, with sync and async calls alternating, behind a busy stream, through a call that does not fit and its retry,
 around the calls that resolve a chain, beside the asynchronous audio decode, and at the benchmark's batch size."""
 import hashlib
+import json
+import os
 
 import numpy as np
 import pytest
@@ -11,10 +13,11 @@ import torch
 
 import espflix_b200
 from espflix_b200 import capi
-from tests import pts_cases, scale_cases
-from tests.test_present_gpu import PINS, _call, _context, _irregular_programs, _synth_ts
+from tests import carry_cases, present_cases as pc, pts_cases, scale_cases
+from tests.harness import audio_results, error_code, host_fields, present_call, presenting_context, same_audio, submits
 
 pytestmark = pytest.mark.gpu
+PINS = json.load(open(os.path.join(pts_cases.GOLDEN, "pacing_pins.json")))
 SENTINEL = 0x5A5A
 INFO_FIELDS = ("first", "n_fields", "frame_counter", "flip_field", "flip_line", "flags")
 
@@ -34,13 +37,13 @@ def build(ctx, submits, mode_of=None, idle_after=None):
         for p in range(npics):
             modes = np.array([mode_of(s, seen[s] + p) if mode_of and p < counts[s] else 0 for s in range(n)], dtype=np.uint8)
             steps.append(("pic", p, modes))
-            recs[len(steps) - 1] = _call(ctx, lambda o: ctx.present_picture(p, modes, o))
+            recs[len(steps) - 1] = present_call(ctx, lambda o: ctx.present_picture(p, modes, o))
         seen = [a + b for a, b in zip(seen, counts)]
         nf = idle_after(k) if idle_after else None
         if nf is not None:
             nf = np.ascontiguousarray(np.broadcast_to(nf, (n,)), dtype=np.uint32)
             steps.append(("idle", nf))
-            recs[len(steps) - 1] = _call(ctx, lambda o: ctx.present_idle(nf, o))
+            recs[len(steps) - 1] = present_call(ctx, lambda o: ctx.present_idle(nf, o))
     return steps, recs
 
 
@@ -64,9 +67,9 @@ def replay(ctx, steps, how=lambda i: "async", caps=None, stream=0, between=None)
             ctx.index()
         elif how(i) == "sync":
             if st[0] == "pic":
-                recs[i] = _call(ctx, lambda o: ctx.present_picture(st[1], st[2], o))
+                recs[i] = present_call(ctx, lambda o: ctx.present_picture(st[1], st[2], o))
             else:
-                recs[i] = _call(ctx, lambda o: ctx.present_idle(st[1], o))
+                recs[i] = present_call(ctx, lambda o: ctx.present_idle(st[1], o))
         else:
             out = torch.full((max(caps[i] * w * nl, 8),), SENTINEL, dtype=torch.int16, device="cuda").view(torch.uint16)
             if st[0] == "pic":
@@ -79,8 +82,7 @@ def replay(ctx, steps, how=lambda i: "async", caps=None, stream=0, between=None)
     for i, out, info in pend:
         inf = ctx.present_info(info)
         total = min(int(inf["n_fields"].sum()), out.numel() // (w * nl))     # a call that did not fit reports more
-        host = out[:total * w * nl].view(torch.int16).cpu().numpy().view(np.uint16).reshape(total, w * nl)
-        recs[i] = (inf, host)
+        recs[i] = (inf, host_fields(out[:total * w * nl].view(total, w * nl)))
     return recs, rc, k, bufs
 
 
@@ -104,14 +106,14 @@ def stream_hashes(recs, n):
 
 
 def _pair_contexts(n, ntsc, fc0, **kw):
-    return _context(n, ntsc, fc0=fc0, **kw), _context(n, ntsc, fc0=fc0, **kw)
+    return presenting_context(n, ntsc, fc0=fc0, **kw), presenting_context(n, ntsc, fc0=fc0, **kw)
 
 
 # ---- the pinned cases as one chain -------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("ntsc", [1, 0])
 def test_pinned_cases_as_one_chain(ntsc):
     names = [n for n in sorted(PINS) if PINS[n]["ntsc"] == ntsc]
-    ts = [_synth_ts(PINS[n]["seed"], PINS[n]["pictures"]) for n in names] + [_synth_ts(60 + ntsc, 7), _synth_ts(62 + ntsc, 12)]
+    ts = [pc.synth_ts(PINS[n]["seed"], PINS[n]["pictures"]) for n in names] + [pc.synth_ts(60 + ntsc, 7), pc.synth_ts(62 + ntsc, 12)]
     fc0 = [PINS[n]["frame_counter0"] for n in names] + [3, 100]
     modes = {i: PINS[n]["modes"] for i, n in enumerate(names)}
     ref, ctx = _pair_contexts(len(ts), ntsc, fc0)
@@ -123,7 +125,7 @@ def test_pinned_cases_as_one_chain(ntsc):
     tails = [((PINS[n]["flip_field"][-1] + 1 + PINS[n]["tail_fields"] - PINS[n]["frame_counter0"]) & 0xFFFFFFFF) - emitted[i] for i, n in enumerate(names)]
     nf = np.array(tails + [5, 0], dtype=np.uint32)
     steps.append(("idle", nf))
-    want[len(steps) - 1] = _call(ref, lambda o: ref.present_idle(nf, o))
+    want[len(steps) - 1] = present_call(ref, lambda o: ref.present_idle(nf, o))
     got, rc, k, _ = replay(ctx, steps, caps=totals(want))
     assert rc == capi.EF_OK and k == len(steps) - 1
     same(got, want, what="pinned")
@@ -139,7 +141,7 @@ def test_pinned_cases_as_one_chain(ntsc):
 # ---- irregular programs, whole and cut, sync and async alternating -----------------------------------------------------------
 @pytest.fixture(scope="module")
 def irregular():
-    return _irregular_programs()
+    return pc.irregular_programs()
 
 
 def _chunks(progs, cuts_seed):
@@ -150,11 +152,8 @@ def _chunks(progs, cuts_seed):
     per = []
     for p in progs:
         cand = pts_cases.cut_points(p[1])
-        cuts = sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []
-        pk = np.frombuffer(bytes(p[1]), dtype=np.uint8).reshape(-1, 188)
-        edges = [0] + cuts + [pk.shape[0]]
-        per.append([pk[a:b].reshape(-1) for a, b in zip(edges[:-1], edges[1:])] + [np.zeros(0, np.uint8)] * (K - 1 - len(cuts)))
-    return [[per[s][k] for s in range(len(progs))] for k in range(K)]
+        per.append(carry_cases.cut(p[1], sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []))
+    return submits(per, n=K)
 
 
 @pytest.mark.parametrize("ntsc", [1, 0])
@@ -166,12 +165,12 @@ def test_irregular_programs_mixed(irregular, ntsc, cuts_seed):
     rng = np.random.RandomState(5 + ntsc)
     idles = [rng.randint(0, 3, size=len(progs)) for _ in chunks[:-1]] + [np.array([p[6] + 1 for p in progs])]
     mode_of = lambda s, g: progs[s][5][g]                                           # noqa: E731
-    ref = _context(len(progs), ntsc, fc0=fc0)
+    ref = presenting_context(len(progs), ntsc, fc0=fc0)
     steps, want = build(ref, chunks, mode_of, lambda k: idles[k])
     ref.close()
     caps = totals(want)
     for how in (lambda i: "async", lambda i: "async" if (i // 2) % 2 == 0 else "sync", lambda i: "sync" if i % 3 == 0 else "async"):
-        ctx = _context(len(progs), ntsc, fc0=fc0)
+        ctx = presenting_context(len(progs), ntsc, fc0=fc0)
         got, rc, _, _ = replay(ctx, steps, how, caps)
         assert rc == capi.EF_OK
         same(got, want, what="irregular")
@@ -180,7 +179,7 @@ def test_irregular_programs_mixed(irregular, ntsc, cuts_seed):
 
 # ---- behind a busy stream --------------------------------------------------------------------------------------------------
 def test_call_behind_a_busy_stream_returns_before_it_runs():
-    ts = [_synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
+    ts = [pc.synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
     chunk = [np.frombuffer(bytes(t), dtype=np.uint8) for t in ts]
     ref, ctx = _pair_contexts(2, 1, [1, 2])
     steps, want = build(ref, [chunk])
@@ -214,7 +213,7 @@ def test_call_behind_a_busy_stream_returns_before_it_runs():
 @pytest.mark.parametrize("j", [3, 4])                  # rec_pics 3: picture 3 starts a K1a range, picture 4 is inside one
 def test_short_call_and_retry(j, monkeypatch):
     monkeypatch.setenv("EF_REC_PICS", "3")
-    ts = [_synth_ts(120 + i, n) for i, n in enumerate((7, 6, 7))]
+    ts = [pc.synth_ts(120 + i, n) for i, n in enumerate((7, 6, 7))]
     chunk = [np.frombuffer(bytes(t), dtype=np.uint8) for t in ts]
     ref, ctx = _pair_contexts(3, 0, [5, 6, 7], max_pictures=8)
     steps, want = build(ref, [chunk], lambda s, g: 3 if (s, g) == (1, 2) else 0, lambda k: [2, 3, 4])
@@ -250,8 +249,8 @@ def test_calls_that_resolve_a_chain():
     """overlay changes staged between async calls, ef_restart_streams, ef_index and ef_reset after a chain nobody waited for,
     and synchronous calls in the middle of one: the same fields and info as the all-synchronous run"""
     n = 3
-    subs = [[np.frombuffer(bytes(_synth_ts(140 + 3 * k + s, 4 + s)), dtype=np.uint8) for s in range(n)] for k in range(4)]
-    c0 = _context(n, 1, fc0=[0, 5, 9])
+    subs = [[np.frombuffer(bytes(pc.synth_ts(140 + 3 * k + s, 4 + s)), dtype=np.uint8) for s in range(n)] for k in range(4)]
+    c0 = presenting_context(n, 1, fc0=[0, 5, 9])
     steps, _ = build(c0, subs, idle_after=lambda k: [1, 0, 2])
     c0.close()
     starts = [i for i, st in enumerate(steps) if st[0] == "submit"]
@@ -266,12 +265,12 @@ def test_calls_that_resolve_a_chain():
             c.restart_streams([1, 2, 0])
         if i == starts[3]:
             c.reset()
-    ref = _context(n, 1, fc0=[0, 5, 9])
+    ref = presenting_context(n, 1, fc0=[0, 5, 9])
     want, rc, _, _ = replay(ref, steps, lambda i: "sync", between=hooks)
     ref.close()
     caps = totals(want)
     for how in (lambda i: "async", lambda i: "sync" if i in (starts[1] + 2, starts[2] + 1) else "async"):
-        ctx = _context(n, 1, fc0=[0, 5, 9])
+        ctx = presenting_context(n, 1, fc0=[0, 5, 9])
         got, rc, _, _ = replay(ctx, steps, how, caps, between=hooks)
         assert rc == capi.EF_OK
         same(got, want, what="resolving calls")
@@ -283,15 +282,14 @@ def test_beside_async_audio():
     """ef_decode_audio_async on one stream, a submit's presentation as one async chain on another: the fields equal a run
     without audio, the audio the synchronous decode"""
     from tests import restart_cases as rc
-    from tests.test_audio_async_gpu import _results, _same
     n, K = 4, 2
     progs = [[rc.program(700 + 10 * s + k, 12, 300000 + 36036 * k, audio=dict(seed=90 + 7 * s + k, frames=60, cut=0)) for k in range(K)] for s in range(n)]
     subs = [[np.frombuffer(p[k], dtype=np.uint8) for p in progs] for k in range(K)]
-    plain = _context(n, 1, fc0=[0, 3, 1000, 7], max_pictures=12)
+    plain = presenting_context(n, 1, fc0=[0, 3, 1000, 7], max_pictures=12)
     steps, want = build(plain, subs)
     plain.close()
     caps = totals(want)
-    ctx = _context(n, 1, fc0=[0, 3, 1000, 7], max_pictures=12)
+    ctx = presenting_context(n, 1, fc0=[0, 3, 1000, 7], max_pictures=12)
     ref = espflix_b200.Context(n_streams=n, max_pictures=12, es_capacity=n * 12 * 40000, fields=False)
     ctx.enable_audio()
     ref.enable_audio()
@@ -302,7 +300,7 @@ def test_beside_async_audio():
         if heard:                                       # the previous submit's audio, decoded beside its presentation
             want_a, info, pcm, pdm = heard.pop()
             assert c.audio_wait() == capi.EF_OK
-            _same(want_a, _results(c, info, pcm, pdm), "step %d" % i)
+            same_audio(want_a, audio_results(info, pcm, pdm), "step %d" % i)
 
     def audio(i, c):
         if steps[i][0] == "submit":
@@ -324,22 +322,16 @@ def test_beside_async_audio():
 
 
 # ---- API rules and launch counts ---------------------------------------------------------------------------------------------
-def _code(fn):
-    with pytest.raises(espflix_b200.EspflixError) as e:
-        fn()
-    return e.value.code
-
-
 def test_api_rules_and_launch_counts():
-    ts = [_synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
+    ts = [pc.synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
     blob, off = espflix_b200.Context.pack(ts)
     ctx = espflix_b200.Context(n_streams=2, max_pictures=5, fields=False)
     out = torch.zeros(4 * 1136 * 312, dtype=torch.uint16, device="cuda")
-    assert _code(lambda: ctx.present_idle_async([1, 1], out)) == capi.EF_ESTATE                   # before ef_present_enable
+    assert error_code(lambda: ctx.present_idle_async([1, 1], out)) == capi.EF_ESTATE                   # before ef_present_enable
     ctx.enable_pts()
     ctx.video_init(0)
     ctx.enable_present([10, 20])
-    assert _code(lambda: ctx.present_picture_async(0, out)) == capi.EF_ESTATE                    # no ef_index since enabling
+    assert error_code(lambda: ctx.present_picture_async(0, out)) == capi.EF_ESTATE                    # no ef_index since enabling
     ctx.submit_ts(blob, off)
     ctx.index()
     w, nl = ctx.geometry()
@@ -355,8 +347,8 @@ def test_api_rules_and_launch_counts():
     assert lib.ef_present_idle_async(h, None, out.data_ptr(), 3, info.data_ptr(), None) == capi.EF_EINVAL
     with pytest.raises(TypeError):
         ctx.present_idle_async(nf, out.cpu())
-    assert _code(lambda: ctx.present_picture_async(1, out)) == capi.EF_ESTATE                    # out of order
-    assert _code(lambda: ctx.present_picture_async(0, out, modes=[4, 0])) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_picture_async(1, out)) == capi.EF_ESTATE                    # out of order
+    assert error_code(lambda: ctx.present_picture_async(0, out, modes=[4, 0])) == capi.EF_EINVAL
     assert ctx.present_wait() == (capi.EF_OK, 0)                                                  # nothing enqueued
     cap = 65535 + 3                                                                               # two K2 launches per call
     big = torch.empty(cap * w * nl, dtype=torch.uint16, device="cuda")
@@ -380,7 +372,7 @@ def test_api_rules_and_launch_counts():
     ctx.present_picture_async(2, big[:need * w * nl])
     assert ctx.launch_count() - n0 == 1 + 1 + 1 + 1 + 1 + 1
     assert ctx.present_wait() == (capi.EF_OK, 1)
-    assert _code(lambda: ctx.submit_ts(blob, off) or ctx.index()) == capi.EF_ESTATE               # pictures 3, 4 unpresented
+    assert error_code(lambda: ctx.submit_ts(blob, off) or ctx.index()) == capi.EF_ESTATE               # pictures 3, 4 unpresented
     ctx.present_picture_async(3, big[:8 * w * nl])
     ctx.present_picture_async(4, big[:8 * w * nl])
     ctx.submit_ts(blob, off)

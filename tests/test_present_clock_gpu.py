@@ -8,24 +8,18 @@ import torch
 
 import espflix_b200
 from espflix_b200 import capi
-from tests import clock_cases as cc
+from tests import carry_cases, clock_cases as cc
 from tests import overlay_cases as oc
 from tests import pts_cases, scale_cases
-from tests.test_pacing import irregular_cases
+from tests.harness import error_code, overlay_arrays, present_call, presenting_context, submits
+from tests.present_cases import irregular_cases
 
 pytestmark = pytest.mark.gpu
 ATLAS, RIGHTS = cc.font()
 
 
-def _ctx(n, ntsc, fc0, font=True, max_pictures=13, es_capacity=None):
-    ctx = espflix_b200.Context(n_streams=n, max_pictures=max_pictures, max_slices_per_picture=12,
-                               es_capacity=es_capacity or n * max_pictures * 40000, fields=False)
-    ctx.enable_pts()
-    ctx.video_init(ntsc)
-    ctx.enable_present(fc0)
-    if font:
-        ctx.present_font(ATLAS, RIGHTS)
-    return ctx
+def _ctx(n, ntsc, fc0, font=True, **kw):
+    return presenting_context(n, ntsc, fc0, font=(ATLAS, RIGHTS) if font else None, **kw)
 
 
 def _header(rng, base):
@@ -97,7 +91,7 @@ class Pair:
             self.b.present_overlay(bm, None, pr, st)
 
     def _b_call(self, pic, arg):
-        return _call(self.b, pic, arg)
+        return present_call(self.b, _fn(self.b, pic, arg), device=True)
 
     def _same(self, info_a, out_a, info_b, out_b):
         assert (info_a == info_b).all(), "info rows differ (call %d)" % self.calls
@@ -172,16 +166,6 @@ def _fn(ctx, pic, arg):
     return lambda o: ctx.present_idle(arg, o)
 
 
-def _call(ctx, pic, arg):
-    """a sizing call, then the call into a buffer of exactly that size -> (info, fields [total, samples] on the device)"""
-    w, nl = ctx.geometry()
-    fn = _fn(ctx, pic, arg)
-    total = int(fn(None)["n_fields"].sum())
-    out = torch.empty(max(total, 1) * w * nl, dtype=torch.uint16, device="cuda")
-    info = fn(out)
-    return info, out[:total * w * nl].view(total, w * nl)
-
-
 def _programs(ntsc, seed):
     """the irregular schedules of one standard as TS programs, plus a header, speed and flags per stream"""
     rng = np.random.default_rng(seed)
@@ -199,13 +183,9 @@ def _chunks(progs, rng, cut):
     K = int(rng.integers(2, 4))
     per = []
     for p in progs:
-        t = p["ts"]
-        pk = np.frombuffer(bytes(t), dtype=np.uint8).reshape(-1, 188)
-        cand = pts_cases.cut_points(t)
-        cuts = sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []
-        edges = [0] + cuts + [pk.shape[0]]
-        per.append([pk[a:b].reshape(-1).tobytes() for a, b in zip(edges[:-1], edges[1:])] + [b""] * (K - 1 - len(cuts)))
-    return [[per[s][i] for s in range(len(progs))] for i in range(K)]
+        cand = pts_cases.cut_points(p["ts"])
+        per.append(carry_cases.cut(p["ts"], sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []))
+    return submits(per, n=K)
 
 
 def _run(ntsc, seed, cut, async_p):
@@ -288,15 +268,7 @@ def test_pinned_overlay_cases_with_host_changes(ntsc):
         segs = [c["segments"][si] if si < len(c["segments"]) else None for c in cases]
         pair.submit([oc.segment_ts(*sg) if sg else b"" for sg in segs])
         for p in range(max(pair.counts)):
-            bm, bl, pr, st = np.zeros((n, 1280), np.uint8), np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.uint8)
-            for s, c in enumerate(cases):
-                cmd = c["cmds"][k[s] + p] if p < pair.counts[s] else None
-                if cmd:
-                    for bit, key, arr in ((1, "bitmap", bm), (2, "blend", bl), (4, "progress", pr)):
-                        if cmd[key] is not None:
-                            arr[s] = oc.bitmap(cmd[key]) if key == "bitmap" else cmd[key]
-                            st[s] |= bit
-            pair.overlay(bm, bl, pr, st)
+            pair.overlay(*overlay_arrays([c["cmds"][k[s] + p] if p < pair.counts[s] else None for s, c in enumerate(cases)]))
             modes = np.array([c["modes"][k[s] + p] if p < pair.counts[s] else 0 for s, c in enumerate(cases)], np.uint8)
             pair.sync(p, modes)
         k = [a + b for a, b in zip(k, pair.counts)]
@@ -334,7 +306,7 @@ def test_batch_scale_clock_on_a_subset():
                 _, (info_a, out_a) = pair.chain([(pic, arg)])
             else:
                 info_a, out_a = pair.sync(pic, arg, sizing=False)
-            info_p, out_p = _call(plain, pic, arg)
+            info_p, out_p = present_call(plain, _fn(plain, pic, arg), device=True)
             assert (info_a == info_p).all()
             first = torch.as_tensor(info_p["first"].astype(np.int64), device="cuda")
             nf = torch.as_tensor(info_p["n_fields"].astype(np.int64), device="cuda")
@@ -386,39 +358,33 @@ def test_launch_counts():
         c.close()
 
 
-def _code(fn):
-    with pytest.raises(espflix_b200.EspflixError) as e:
-        fn()
-    return e.value.code
-
-
 def test_error_codes():
     ctx = espflix_b200.Context(n_streams=3, max_pictures=4, fields=False)
     h = np.frombuffer(cc.H_MAIN, dtype=np.uint8)
-    assert _code(lambda: ctx.present_clock(h, 0, 1)) == capi.EF_ESTATE                # before ef_present_enable
+    assert error_code(lambda: ctx.present_clock(h, 0, 1)) == capi.EF_ESTATE                # before ef_present_enable
     ctx.enable_pts()
     ctx.enable_present()
-    assert _code(lambda: ctx.present_clock(h, 0, 1)) == capi.EF_ESTATE                # before ef_present_font
-    assert _code(lambda: ctx.present_font(ATLAS, RIGHTS[:34])) == capi.EF_EINVAL      # does not reach ':'
+    assert error_code(lambda: ctx.present_clock(h, 0, 1)) == capi.EF_ESTATE                # before ef_present_font
+    assert error_code(lambda: ctx.present_font(ATLAS, RIGHTS[:34])) == capi.EF_EINVAL      # does not reach ':'
     bad = RIGHTS.copy()
     bad[5] = bad[4]
-    assert _code(lambda: ctx.present_font(ATLAS, bad)) == capi.EF_EINVAL              # not increasing
+    assert error_code(lambda: ctx.present_font(ATLAS, bad)) == capi.EF_EINVAL              # not increasing
     bad = RIGHTS.copy()
     bad[-1] = 1025
-    assert _code(lambda: ctx.present_font(ATLAS, bad)) == capi.EF_EINVAL              # past the atlas
+    assert error_code(lambda: ctx.present_font(ATLAS, bad)) == capi.EF_EINVAL              # past the atlas
     with pytest.raises(ValueError):
         ctx.present_font(ATLAS[:, :512], RIGHTS)
     ctx.present_font(ATLAS, RIGHTS)
-    assert _code(lambda: ctx.present_clock(h, 0, 1, first=-1, count=1)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_clock(h, 0, 1, first=2, count=2)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_clock(h, 2, 1)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_clock(h, -2, 0)) == capi.EF_EINVAL               # checked on streams that stay off too
+    assert error_code(lambda: ctx.present_clock(h, 0, 1, first=-1, count=1)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_clock(h, 0, 1, first=2, count=2)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_clock(h, 2, 1)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_clock(h, -2, 0)) == capi.EF_EINVAL               # checked on streams that stay off too
     zero_last = cc.header((5, 0), (0, 10), (0, 10))
     flat_fwd = cc.header((5, 100), (7, 7), (0, 10))
     flat_rwd = cc.header((5, 100), (0, 10), (-3, -3))
     for hdr, speed in ((zero_last, 0), (flat_fwd, 1), (flat_rwd, -1)):
         a = np.frombuffer(hdr, dtype=np.uint8)
-        assert _code(lambda: ctx.present_clock(a, speed, 1)) == capi.EF_EINVAL
+        assert error_code(lambda: ctx.present_clock(a, speed, 1)) == capi.EF_EINVAL
         ctx.present_clock(a, speed, 0)                                                # off: the header is not read
     ctx.present_clock(np.frombuffer(flat_fwd, dtype=np.uint8), -1, 1)                 # the flat record is not the one used
     ctx.present_clock(np.frombuffer(flat_rwd, dtype=np.uint8), 1, 1)

@@ -1,7 +1,6 @@
 """Paced presentation through the decoder context (ef_present_enable / ef_present_picture / ef_present_idle): every stream's
 composite fields, concatenated over the calls, must hash to the field stream the unmodified reference emitted
 (tests/golden/pacing_pins.json) and equal, field by field, K2's rendering of the restatement in tests/present_cases.py."""
-import hashlib
 import json
 import os
 
@@ -11,10 +10,9 @@ import torch
 
 import espflix_b200
 from espflix_b200 import capi, synth
-from tests import present_cases as pc
-from tests import pts_cases
+from tests import carry_cases, overlay_cases as oc, present_cases as pc, pts_cases
+from tests.harness import Paced, error_code, present_call, presenting_context, sha, submits
 from tests.oracle_lib import Oracle
-from tests.test_pacing import irregular_cases
 
 pytestmark = pytest.mark.gpu
 G = pts_cases.GOLDEN
@@ -22,96 +20,9 @@ PINS = json.load(open(os.path.join(G, "pacing_pins.json")))
 IRREGULAR = json.load(open(os.path.join(G, "ref_pins.json")))["pacing_irregular"]
 
 
-def _call(ctx, fn):
-    """sizing call, then the call into a buffer of exactly that size -> (info, fields on the host [total, samples])"""
-    w, nl = ctx.geometry()
-    info = fn(None)
-    total = int(info["n_fields"].sum())
-    out = torch.empty(max(total, 1) * w * nl, dtype=torch.uint16, device="cuda")
-    got = fn(out)
-    assert (got == info).all()                          # the sizing call reported what the call did
-    host = out[:total * w * nl].view(torch.int16).cpu().numpy().view(np.uint16).reshape(total, w * nl)
-    return got, host
-
-
-class Run:
-    """drives a presenting context over TS submits, and the restatement alongside it"""
-
-    def __init__(self, ctx, ntsc, frames, fc0, oracle):
-        n = len(frames)
-        self.ctx, self.frames, self.n = ctx, frames, n
-        self.disp = [pc.Display(ntsc, int(f)) for f in fc0]
-        self.rend = [pc.Renderer(oracle, ntsc) for _ in range(n)]
-        self.seen = [0] * n
-        self.dev = [[] for _ in range(n)]               # per-field SHA-256 of what the device emitted
-        self.want = [[] for _ in range(n)]              # ... and of the restatement's rendering
-        self.stream_hash = [hashlib.sha256() for _ in range(n)]
-        self.flips = [[] for _ in range(n)]
-        self.pts = [[] for _ in range(n)]
-        self.fc = [int(f) for f in fc0]
-
-    def _collect(self, info, host, want_fields):
-        for s in range(self.n):
-            a, k = int(info[s]["first"]), int(info[s]["n_fields"])
-            assert k == len(want_fields[s]), (s, k, len(want_fields[s]))
-            if k:
-                assert int(info[s]["frame_counter"]) == self.fc[s] & pc.M32    # consecutive frame counters over all calls
-            self.fc[s] += k
-            for j in range(k):
-                f = host[a + j]
-                self.stream_hash[s].update(f.tobytes())
-                self.dev[s].append(hashlib.sha256(f.tobytes()).hexdigest())
-                self.want[s].append(hashlib.sha256(self.rend[s].field(want_fields[s][j]).tobytes()).hexdigest())
-
-    def submit(self, chunk, mode_of=None):
-        ctx = self.ctx
-        ctx.submit_ts(*ctx.pack(chunk))
-        ctx.index()
-        npics = ctx.index_info()["max_pictures"]
-        counts = [ctx.stream_info(s)[0] for s in range(self.n)]
-        pic_pts, _ = ctx.picture_pts()
-        for p in range(npics):
-            modes = [mode_of(s, self.seen[s] + p) if mode_of and p < counts[s] else 0 for s in range(self.n)]
-            want = [[] for _ in range(self.n)]
-            for s in range(self.n):
-                if p < counts[s]:
-                    g = self.seen[s] + p
-                    self.rend[s].decoded(g, self.frames[s][g])
-                    want[s], ff, fl = self.disp[s].push(int(pic_pts[s, p]), modes[s])
-                    self.pts[s].append(int(pic_pts[s, p]))
-            info, host = _call(ctx, lambda o: ctx.present_picture(p, modes, o))
-            for s in range(self.n):
-                if p < counts[s]:
-                    self.flips[s].append((int(info[s]["flip_field"]), int(info[s]["flip_line"])))
-                    assert self.flips[s][-1] == (self.disp[s].F, self.disp[s].L - 1)
-                else:
-                    assert int(info[s]["flip_line"]) == -1 and int(info[s]["n_fields"]) == 0
-            self._collect(info, host, want)
-        self.seen = [a + b for a, b in zip(self.seen, counts)]
-
-    def idle(self, n_fields):
-        n_fields = [int(x) for x in np.broadcast_to(n_fields, (self.n,))]
-        want = [self.disp[s].idle(n_fields[s]) for s in range(self.n)]
-        info, host = _call(self.ctx, lambda o: self.ctx.present_idle(n_fields, o))
-        self._collect(info, host, want)
-
-    def check(self):
-        for s in range(self.n):
-            assert self.dev[s] == self.want[s], "stream %d: first differing field %d" % (
-                s, next(i for i, (a, b) in enumerate(zip(self.dev[s], self.want[s])) if a != b) if len(self.dev[s]) == len(self.want[s]) else -1)
-
-
-def _context(n, ntsc, max_pictures=13, fc0=None):
-    ctx = espflix_b200.Context(n_streams=n, max_pictures=max_pictures, max_slices_per_picture=12, es_capacity=n * max_pictures * 40000, fields=False)
-    ctx.enable_pts()
-    ctx.video_init(ntsc)
-    ctx.enable_present(fc0)
-    return ctx
-
-
-def _synth_ts(seed, n):
-    es, off = synth.generate(synth.SEED0 + seed, n_pictures=n)
-    return synth.wrap_ts(es, off)
+def _driver(ctx, ntsc, frames, fc0, oracle):
+    """the paced driver over present_cases' displays and renderers"""
+    return Paced(ctx, [pc.Display(ntsc, int(f)) for f in fc0], [pc.Renderer(oracle, ntsc) for _ in frames], frames)
 
 
 @pytest.mark.parametrize("ntsc", [1, 0])
@@ -120,11 +31,11 @@ def test_pinned_streams_hash_to_the_reference(ntsc):
     field stream of each pinned case as the reference emitted it"""
     o = Oracle()
     names = [n for n in sorted(PINS) if PINS[n]["ntsc"] == ntsc]
-    ts = [_synth_ts(PINS[n]["seed"], PINS[n]["pictures"]) for n in names] + [_synth_ts(60 + ntsc, 7), _synth_ts(62 + ntsc, 12)]
+    ts = [pc.synth_ts(PINS[n]["seed"], PINS[n]["pictures"]) for n in names] + [pc.synth_ts(60 + ntsc, 7), pc.synth_ts(62 + ntsc, 12)]
     fc0 = [PINS[n]["frame_counter0"] for n in names] + [3, 100]
     frames = [o.decode_ts(t) for t in ts]
-    ctx = _context(len(ts), ntsc, fc0=fc0)
-    r = Run(ctx, ntsc, frames, fc0, o)
+    ctx = presenting_context(len(ts), ntsc, fc0=fc0)
+    r = _driver(ctx, ntsc, frames, fc0, o)
     modes = {i: PINS[n]["modes"] for i, n in enumerate(names)}
     r.submit([np.frombuffer(bytes(t), dtype=np.uint8) for t in ts], lambda s, g: modes[s][g] if s in modes else (2 if g == 4 else 0))
     tails = [((PINS[n]["flip_field"][-1] + 1 + PINS[n]["tail_fields"] - PINS[n]["frame_counter0"]) & pc.M32) - len(r.dev[i]) for i, n in enumerate(names)]
@@ -139,32 +50,18 @@ def test_pinned_streams_hash_to_the_reference(ntsc):
     ctx.close()
 
 
-def _one_pes_per_picture(seed, pts):
-    """a synthetic stream as TS with one video PES per picture, starting at its start code and carrying pts[k]"""
-    es = bytes(synth.generate(synth.SEED0 + seed, n_pictures=len(pts), gop=6)[0])
-    codes = pts_cases.picture_codes(es)
-    assert len(codes) == len(pts)
-    return pts_cases.wrap(es, [0] + [c - 3 for c in codes[1:]], ["pts"] * len(pts), [int(v) for v in pts], seed=seed + 1000)
-
-
-def _irregular_programs():
-    """the 24 irregular schedules as TS programs: one PES per picture carrying the pinned pts"""
-    return [(case, _one_pes_per_picture(200 + case, pts), [int(v) for v in pts], ntsc, fc0, [int(m) for m in modes], tail)
-            for case, (pts, ntsc, fc0, modes, tail) in enumerate(irregular_cases())]
-
-
 @pytest.fixture(scope="module")
 def irregular():
     o = Oracle()
-    return [(c, ts, pts, ntsc, fc0, modes, tail, o.decode_ts(ts)) for c, ts, pts, ntsc, fc0, modes, tail in _irregular_programs()]
+    return [(c, ts, pts, ntsc, fc0, modes, tail, o.decode_ts(ts)) for c, ts, pts, ntsc, fc0, modes, tail in pc.irregular_programs()]
 
 
 def _run_irregular(progs, ntsc, cuts_seed=None, idle_between=False):
     progs = [p for p in progs if p[3] == ntsc]
     o = Oracle()
     fc0 = [p[4] for p in progs]
-    ctx = _context(len(progs), ntsc, fc0=fc0)
-    r = Run(ctx, ntsc, [p[7] for p in progs], fc0, o)
+    ctx = presenting_context(len(progs), ntsc, fc0=fc0)
+    r = _driver(ctx, ntsc, [p[7] for p in progs], fc0, o)
     mode_of = lambda s, g: progs[s][5][g]                                         # noqa: E731
     if cuts_seed is None:
         chunks = [[np.frombuffer(bytes(p[1]), dtype=np.uint8) for p in progs]]
@@ -174,11 +71,8 @@ def _run_irregular(progs, ntsc, cuts_seed=None, idle_between=False):
         per = []
         for p in progs:
             cand = pts_cases.cut_points(p[1])
-            cuts = sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []
-            pk = np.frombuffer(bytes(p[1]), dtype=np.uint8).reshape(-1, 188)
-            edges = [0] + cuts + [pk.shape[0]]
-            per.append([pk[a:b].reshape(-1) for a, b in zip(edges[:-1], edges[1:])] + [np.zeros(0, np.uint8)] * (K - 1 - len(cuts)))
-        chunks = [[per[s][k] for s in range(len(progs))] for k in range(K)]
+            per.append(carry_cases.cut(p[1], sorted(rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []))
+        chunks = submits(per, n=K)
     rng = np.random.RandomState(99)
     for k, c in enumerate(chunks):
         r.submit(c, mode_of)
@@ -222,8 +116,8 @@ def test_fixtures_step_by_step():
     ts = [open(os.path.join(G, n + ".ts"), "rb").read() for n in names]
     frames = [o.decode_ts(t) for t in ts]
     for ntsc in (1, 0):
-        ctx = _context(2, ntsc, max_pictures=100, fc0=[1, 2])
-        r = Run(ctx, ntsc, frames, [1, 2], o)
+        ctx = presenting_context(2, ntsc, max_pictures=100, fc0=[1, 2])
+        r = _driver(ctx, ntsc, frames, [1, 2], o)
         got = [[], []]
         orig = r.ctx.present_picture
 
@@ -240,57 +134,51 @@ def test_fixtures_step_by_step():
         for s, n in enumerate(names):
             assert len(got[s]) == dpins[n]["frames"]
             for k, f in enumerate(got[s]):
-                assert hashlib.sha256(f.tobytes()).hexdigest() == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
+                assert sha(f) == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
         r.check()
         ctx.close()
 
 
-def _code(fn):
-    with pytest.raises(espflix_b200.EspflixError) as e:
-        fn()
-    return e.value.code
-
-
 def test_api_rules_and_launch_counts():
     o = Oracle()
-    ts = [_synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
+    ts = [pc.synth_ts(70 + i, n) for i, n in enumerate((5, 3))]
     frames = [o.decode_ts(t) for t in ts]
     blob, off = espflix_b200.Context.pack(ts)
 
     ctx = espflix_b200.Context(n_streams=2, max_pictures=5, fields=False)
-    assert _code(lambda: ctx.enable_present()) == capi.EF_ESTATE                  # needs PTS first
+    assert error_code(lambda: ctx.enable_present()) == capi.EF_ESTATE                  # needs PTS first
     ctx.enable_pts()
     ctx.video_init(0)
     ctx.enable_present([10, 20])
-    assert _code(lambda: ctx.enable_present()) == capi.EF_ESTATE
-    assert _code(lambda: ctx.video_init(1)) == capi.EF_ESTATE                      # the standard is fixed
+    assert error_code(lambda: ctx.enable_present()) == capi.EF_ESTATE
+    assert error_code(lambda: ctx.video_init(1)) == capi.EF_ESTATE                      # the standard is fixed
     ctx.video_init(0)
-    assert _code(lambda: ctx.present_picture(0)) == capi.EF_ESTATE                # no ef_index since enabling
+    assert error_code(lambda: ctx.present_picture(0)) == capi.EF_ESTATE                # no ef_index since enabling
     ctx.submit_ts(blob, off)
     ctx.index()
-    assert _code(lambda: ctx.decode_picture(0)) == capi.EF_ESTATE
-    assert _code(lambda: ctx.decode_all(5)) == capi.EF_ESTATE
+    assert error_code(lambda: ctx.decode_picture(0)) == capi.EF_ESTATE
+    assert error_code(lambda: ctx.decode_all(5)) == capi.EF_ESTATE
     out_host = np.zeros((5, 2, 101376), dtype=np.uint8)
-    assert _code(lambda: ctx.decode_all_to_host(5, out_host)) == capi.EF_ESTATE
-    assert _code(lambda: ctx.present_picture(1)) == capi.EF_ESTATE                # out of order
-    assert _code(lambda: ctx.present_picture(0, [4, 0])) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.decode_all_to_host(5, out_host)) == capi.EF_ESTATE
+    assert error_code(lambda: ctx.present_picture(1)) == capi.EF_ESTATE                # out of order
+    assert error_code(lambda: ctx.present_picture(0, [4, 0])) == capi.EF_EINVAL
     w, nl = ctx.geometry()
     # a sizing call changes nothing; too small a buffer is EF_ENOMEM and changes nothing either
     n0 = ctx.launch_count()
     i1 = ctx.present_picture(0)
     i2 = ctx.present_picture(0)
     assert (i1 == i2).all() and ctx.launch_count() == n0 + 2
-    assert _code(lambda: ctx.present_picture(1)) == capi.EF_ESTATE                # sizing did not advance it
-    r = Run(ctx, 0, frames, [10, 20], o)
+    assert error_code(lambda: ctx.present_picture(1)) == capi.EF_ESTATE                # sizing did not advance it
+    r = _driver(ctx, 0, frames, [10, 20], o)
     fields = [[], []]
     for p in range(5):
         info = ctx.present_picture(p)
         total = int(info["n_fields"].sum())
         if total:
             small = torch.empty(total * w * nl - 8, dtype=torch.uint16, device="cuda")   # room for total - 1 fields
-            assert _code(lambda: ctx.present_picture(p, None, small)) == capi.EF_ENOMEM
+            assert error_code(lambda: ctx.present_picture(p, None, small)) == capi.EF_ENOMEM
         if p == 2:
-            assert _code(lambda: ctx.submit_ts(blob, off) or ctx.index()) == capi.EF_ESTATE   # pictures 3, 4 unpresented
+            assert error_code(lambda: ctx.submit_ts(blob, off) or ctx.index()) == capi.EF_ESTATE   # pictures 3, 4 unpresented
         n0 = ctx.launch_count()
         want = []
         for s in range(2):
@@ -299,11 +187,11 @@ def test_api_rules_and_launch_counts():
                 want.append(r.disp[s].push(129003 + 3003 * p)[0])
             else:
                 want.append([])
-        got, host = _call(ctx, lambda o_: ctx.present_picture(p, None, o_))
+        got, host = present_call(ctx, lambda o_: ctx.present_picture(p, None, o_))
         # sizing (1) + schedule (1) + K1a at picture 0 + K1b (1) + descriptors (1) + one K2 per 65,535 fields
         assert ctx.launch_count() - n0 == 1 + 1 + (p == 0) + 1 + 1 + (1 if total else 0)
-        r._collect(got, host, want)
-    assert _code(lambda: ctx.present_picture(5)) == capi.EF_ESTATE
+        r.collect(got, host, want)
+    assert error_code(lambda: ctx.present_picture(5)) == capi.EF_ESTATE
     r.idle(2)
     r.check()
     # ef_reset mid-run is video_reset(): new origin, position / store / scroll kept; the frame stores are zero-filled
@@ -312,7 +200,7 @@ def test_api_rules_and_launch_counts():
         r.disp[s].reset()
         r.rend[s].reset()
     r.seen = [0, 0]
-    late = [_one_pes_per_picture(80 + i, [9000000 + 3003 * k for k in range(3)]) for i in range(2)]
+    late = [oc.segment_ts(80 + i, [9000000 + 3003 * k for k in range(3)]) for i in range(2)]
     r.frames = [o.decode_ts(t) for t in late]
     r.submit([np.frombuffer(t, dtype=np.uint8) for t in late])
     r.idle(1)
@@ -320,11 +208,11 @@ def test_api_rules_and_launch_counts():
     ctx.close()
 
     # a picture without pts (an ES submit carries no PES) is not pushed: flag 1
-    ctx = _context(1, 1, max_pictures=4)
+    ctx = presenting_context(1, 1, max_pictures=4)
     es, _ = synth.generate(synth.SEED0 + 90, n_pictures=2)
     ctx.submit_es(*ctx.pack([es]))
     ctx.index()
-    info, _ = _call(ctx, lambda o_: ctx.present_picture(0, None, o_))
+    info, _ = present_call(ctx, lambda o_: ctx.present_picture(0, None, o_))
     assert int(info[0]["flags"]) == 1 and int(info[0]["flip_line"]) == -1 and int(info[0]["n_fields"]) == 0
     ctx.close()
 

@@ -1,7 +1,6 @@
 """The overlay of paced presentation through the decoder context (ef_present_overlay): every stream's fields, concatenated over
 the calls, must hash to the field stream the unmodified reference emitted (tests/golden/overlay_pins.json) and equal, field by
 field, the C checker's rendering of the restatement in tests/overlay_cases.py."""
-import hashlib
 import json
 import os
 
@@ -11,85 +10,32 @@ import torch
 
 import espflix_b200
 from espflix_b200 import capi
-from tests import overlay_cases as oc
+from tests import carry_cases, overlay_cases as oc
 from tests import present_cases as pc
 from tests import pts_cases, scale_cases
+from tests.harness import Paced, error_code, host_fields, present_call, presenting_context, stage_overlay, submits
 from tests.oracle_lib import Oracle
-from tests.test_pacing import irregular_cases
 
 pytestmark = pytest.mark.gpu
 PINS = json.load(open(os.path.join(pts_cases.GOLDEN, "overlay_pins.json")))
 CASES = oc.cases()
 
 
-def _context(n, ntsc, fc0, max_pictures=13):
-    ctx = espflix_b200.Context(n_streams=n, max_pictures=max_pictures, max_slices_per_picture=12, es_capacity=n * max_pictures * 40000, fields=False)
-    ctx.enable_pts()
-    ctx.video_init(ntsc)
-    ctx.enable_present(fc0)
-    return ctx
-
-
-def _call(ctx, fn):
-    """sizing call, then the call into a buffer of exactly that size -> (info, fields on the host [total, samples])"""
-    w, nl = ctx.geometry()
-    info = fn(None)
-    total = int(info["n_fields"].sum())
-    out = torch.empty(max(total, 1) * w * nl, dtype=torch.uint16, device="cuda")
-    got = fn(out)
-    assert (got == info).all()
-    return got, out[:total * w * nl].view(torch.int16).cpu().numpy().view(np.uint16).reshape(total, w * nl)
-
-
-def _stage(ctx, disps, cmds):
-    """one ef_present_overlay call for every stream (cmd None: set 0), and the same changes in the restatement"""
-    n = len(cmds)
-    bm, bl, pr, st = np.zeros((n, 1280), np.uint8), np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.uint8)
-    for s, c in enumerate(cmds):
-        if not c:
-            continue
-        if c["bitmap"] is not None:
-            bm[s], st[s] = oc.bitmap(c["bitmap"]), st[s] | 1
-        if c["blend"] is not None:
-            bl[s], st[s] = c["blend"], st[s] | 2
-        if c["progress"] is not None:
-            pr[s], st[s] = c["progress"], st[s] | 4
-        oc.stage(disps[s], c)
-    ctx.present_overlay(bm, bl, pr, st)
-
-
-class Drive:
-    """drives an overlay context over cases (tests/overlay_cases.py's dicts, one per stream) and the restatement alongside it.
-    cut_seed: every segment goes in as 2-4 TS submits with idle runs (and overlay changes) between them."""
+class Drive(Paced):
+    """the paced driver over an overlay context, cases (tests/overlay_cases.py's dicts, one per stream) and the overlay
+    restatement: every segment after the first follows ef_reset, overlay changes are staged before the pushes and idle runs
+    of the tail. cut_seed: every segment goes in as 2-4 TS submits with idle runs (and overlay changes) between them."""
 
     def __init__(self, ctx, cases, oracle, cut_seed=None):
-        self.ctx, self.cases, self.o = ctx, cases, oracle
-        n, ntsc = len(cases), cases[0]["ntsc"]
-        self.disp = [oc.OverlayDisplay(ntsc, c["fc0"]) for c in cases]
-        self.rend = [oc.OverlayRenderer(oracle, ntsc) for _ in cases]
-        self.dev = [[] for _ in range(n)]
-        self.want = [[] for _ in range(n)]
-        self.whole = [hashlib.sha256() for _ in range(n)]
-        self.k = [0] * n
-        self.last = [None] * n
+        ntsc = cases[0]["ntsc"]
+        super().__init__(ctx, [oc.OverlayDisplay(ntsc, c["fc0"]) for c in cases], [oc.OverlayRenderer(oracle, ntsc) for _ in cases], None)
+        self.cases, self.o = cases, oracle
         self.rng = np.random.default_rng(cut_seed)
         self.cut = cut_seed is not None
 
-    def _collect(self, info, host, want):
-        for s in range(len(self.cases)):
-            a, k = int(info[s]["first"]), int(info[s]["n_fields"])
-            assert k == len(want[s]), (s, k, len(want[s]))
-            ovs = self.disp[s].overlays()[len(self.disp[s].emitted) - k:]
-            for j in range(k):
-                f = host[a + j].tobytes()
-                self.whole[s].update(f)
-                self.dev[s].append(hashlib.sha256(f).hexdigest())
-                self.want[s].append(hashlib.sha256(self.rend[s].field(want[s][j], ovs[j]).tobytes()).hexdigest())
-
-    def _idle(self, nf, cmds):
-        _stage(self.ctx, self.disp, cmds)
-        want = [self.disp[s].idle(int(nf[s])) for s in range(len(self.cases))]
-        self._collect(*_call(self.ctx, lambda o: self.ctx.present_idle(nf, o)), want)
+    def render(self, s, fields):
+        ovs = self.disp[s].overlays()[len(self.disp[s].emitted) - len(fields):]
+        return [self.rend[s].field(f, ov) for f, ov in zip(fields, ovs)]
 
     def _random_cmd(self):
         r = self.rng
@@ -102,63 +48,46 @@ class Drive:
         n = len(self.cases)
         for si in range(max(len(c["segments"]) for c in self.cases)):
             segs = [c["segments"][si] if si < len(c["segments"]) else None for c in self.cases]
+            base = [len(x) for x in self.pts]                # pushes before this segment
             pre = [False] * n
             if si:                                          # the first push's changes are staged before the reset: they survive it
                 pre = [sg is not None for sg in segs]
-                _stage(self.ctx, self.disp, [self.cases[s]["cmds"][self.k[s]] if pre[s] else None for s in range(n)])
+                stage_overlay(self.ctx, self.disp, [self.cases[s]["cmds"][base[s]] if pre[s] else None for s in range(n)])
                 self.ctx.reset()
                 for s in range(n):
                     self.disp[s].reset()
                     self.rend[s].reset()
             ts = [oc.segment_ts(*sg) if sg else b"" for sg in segs]
-            frames = [self.o.decode_ts(t) if sg else [] for t, sg in zip(ts, segs)]
+            self.frames = [self.o.decode_ts(t) if sg else [] for t, sg in zip(ts, segs)]
+            self.seen = [0] * n
             chunks = [ts]
             if self.cut:
                 K = int(self.rng.integers(2, 5))
                 per = []
                 for t in ts:
-                    pk = np.frombuffer(bytes(t), dtype=np.uint8).reshape(-1, 188)
                     cand = pts_cases.cut_points(t) if len(t) else []
-                    cuts = sorted(self.rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []
-                    edges = [0] + cuts + [pk.shape[0]]
-                    per.append([pk[a:b].reshape(-1).tobytes() for a, b in zip(edges[:-1], edges[1:])] + [b""] * (K - 1 - len(cuts)))
-                chunks = [[per[s][i] for s in range(n)] for i in range(K)]
-            seen = [0] * n
+                    per.append(carry_cases.cut(t, sorted(self.rng.choice(cand, size=K - 1, replace=True).tolist()) if cand else []))
+                chunks = submits(per, n=K)
+
+            def stage_pushes(p, pushes):
+                stage_overlay(self.ctx, self.disp, [self.cases[s]["cmds"][len(self.pts[s])] if pushes[s] and not pre[s] else None for s in range(n)])
+                pre[:] = [a and not b for a, b in zip(pre, pushes)]
             for ci, chunk in enumerate(chunks):
-                self.ctx.submit_ts(*self.ctx.pack(chunk))
-                self.ctx.index()
-                counts = [self.ctx.stream_info(s)[0] for s in range(n)]
-                pic_pts, _ = self.ctx.picture_pts()
-                for p in range(max(counts)):
-                    has = [p < counts[s] for s in range(n)]
-                    _stage(self.ctx, self.disp, [self.cases[s]["cmds"][self.k[s]] if has[s] and not pre[s] else None for s in range(n)])
-                    pre = [a and not b for a, b in zip(pre, has)]
-                    modes = [self.cases[s]["modes"][self.k[s]] if has[s] else 0 for s in range(n)]
-                    want = [[] for _ in range(n)]
-                    for s in range(n):
-                        if has[s]:
-                            j = seen[s] + p
-                            assert int(pic_pts[s, p]) == segs[s][1][j]
-                            self.rend[s].decoded(j, frames[s][j])
-                            want[s], self.last[s], _ = self.disp[s].push(int(pic_pts[s, p]), modes[s])
-                            self.k[s] += 1
-                    self._collect(*_call(self.ctx, lambda o: self.ctx.present_picture(p, modes, o)), want)
-                seen = [a + b for a, b in zip(seen, counts)]
+                self.submit(chunk, lambda s, g: self.cases[s]["modes"][base[s] + g], before_call=stage_pushes)
                 if self.cut and ci + 1 < len(chunks):
-                    self._idle(self.rng.integers(0, 3, size=n).astype(np.uint32), [self._random_cmd() for _ in range(n)])
-        total = [(self.last[s] + 1 + c["tail_fields"] - c["fc0"]) & pc.M32 for s, c in enumerate(self.cases)]
+                    nf = self.rng.integers(0, 3, size=n).astype(np.uint32)
+                    cmds = [self._random_cmd() for _ in range(n)]
+                    self.idle(nf, lambda: stage_overlay(self.ctx, self.disp, cmds))
+            for s in range(n):
+                assert self.pts[s][base[s]:] == (list(segs[s][1]) if segs[s] else []), s
+        last = [f[-1][0] for f in self.flips]
+        total = [(last[s] + 1 + c["tail_fields"] - c["fc0"]) & pc.M32 for s, c in enumerate(self.cases)]
         while any(len(d.emitted) < t for d, t in zip(self.disp, total)):
             need = [len(d.emitted) < t for d, t in zip(self.disp, total)]
-            cmds = [self.cases[s]["tail_cmds"].get((d.F + (0 if d.L == 0 else 1) - self.last[s] - 1) & pc.M32) if need[s] else None
+            cmds = [self.cases[s]["tail_cmds"].get((d.F + (0 if d.L == 0 else 1) - last[s] - 1) & pc.M32) if need[s] else None
                     for s, d in enumerate(self.disp)]
-            self._idle(np.array(need, dtype=np.uint32), cmds)
+            self.idle(np.array(need, dtype=np.uint32), lambda: stage_overlay(self.ctx, self.disp, cmds))
         return self
-
-    def check(self):
-        for s in range(len(self.cases)):
-            assert len(self.dev[s]) == len(self.want[s])
-            bad = [i for i, (a, b) in enumerate(zip(self.dev[s], self.want[s])) if a != b]
-            assert not bad, "stream %d: fields %s differ from the restatement" % (s, bad[:8])
 
 
 def _filler(ntsc, seed, overlay):
@@ -179,11 +108,11 @@ def test_pinned_cases_among_filler_streams(ntsc):
     names = [n for n in sorted(CASES) if CASES[n]["ntsc"] == ntsc]
     for group in ([n for n in names if len(CASES[n]["segments"]) == 1], [n for n in names if len(CASES[n]["segments"]) > 1]):
         cases = [CASES[n] for n in group] + [_filler(ntsc, 1, True), _filler(ntsc, 2, False)]
-        ctx = _context(len(cases), ntsc, [c["fc0"] for c in cases])
+        ctx = presenting_context(len(cases), ntsc, [c["fc0"] for c in cases])
         d = Drive(ctx, cases, o).run()
         for i, n in enumerate(group):
             assert len(d.dev[i]) == PINS[n]["fields"], n
-            assert d.whole[i].hexdigest() == PINS[n]["stream_sha256"], n
+            assert d.stream_hash[i].hexdigest() == PINS[n]["stream_sha256"], n
         d.check()
         ctx.close()
 
@@ -191,7 +120,7 @@ def test_pinned_cases_among_filler_streams(ntsc):
 def _irregular_cases(ntsc, seed):
     rng = np.random.default_rng(seed)
     out = []
-    for case, (pts, nt, fc0, modes, tail) in enumerate(irregular_cases()):
+    for case, (pts, nt, fc0, modes, tail) in enumerate(pc.irregular_cases()):
         if nt != ntsc:
             continue
         cmd = lambda: (oc._cmd(int(rng.integers(1, 999)) if rng.random() < 0.5 else None, int(rng.integers(-1, 50)) if rng.random() < 0.6 else None,  # noqa: E731
@@ -208,11 +137,11 @@ def test_irregular_schedules_with_overlay_commands(ntsc):
     o = Oracle()
     cases = _irregular_cases(ntsc, 40 + ntsc)
     fc0 = [c["fc0"] for c in cases]
-    ctx = _context(len(cases), ntsc, fc0)
+    ctx = presenting_context(len(cases), ntsc, fc0)
     Drive(ctx, cases, o).run().check()
     ctx.close()
     for seed in (3, 4):
-        ctx = _context(len(cases), ntsc, fc0)
+        ctx = presenting_context(len(cases), ntsc, fc0)
         Drive(ctx, cases, o, cut_seed=seed + 10 * ntsc).run().check()
         ctx.close()
 
@@ -241,10 +170,7 @@ def test_batch_scale_overlay_on_every_stream(oracle):
     for ntsc in (1, 0):
         ctxs = []
         for _ in range(2):
-            c = espflix_b200.Context(n_streams=N, max_pictures=PICTURES, max_slices_per_picture=12, es_capacity=int(off[-1]) + 4096, fields=False)
-            c.enable_pts()
-            c.video_init(ntsc)
-            c.enable_present([b.fc0(s) for s in range(N)])
+            c = presenting_context(N, ntsc, [b.fc0(s) for s in range(N)], max_pictures=PICTURES, es_capacity=int(off[-1]) + 4096)
             c.submit_ts(blob, off)
             c.index()
             ctxs.append(c)
@@ -299,7 +225,7 @@ def test_batch_scale_overlay_on_every_stream(oracle):
 
         for p in range(PICTURES):
             cmds = [_batch_cmd(s, p) for s in range(N)]
-            _stage(ovl, disp, cmds)
+            stage_overlay(ovl, disp, cmds)
             modes = [b.modes(s)[p] for s in range(N)]
             want = []
             for s in range(N):
@@ -340,11 +266,11 @@ def _fields(ctx, cases, sizing=True, stage=None, enomem=False):
                 assert e.value.code == capi.EF_ENOMEM
         n0 = ctx.launch_count()
         if sizing:
-            info, host = _call(ctx, fn)
+            info, host = present_call(ctx, fn)
         else:
             out = torch.empty(64 * w * nl, dtype=torch.uint16, device="cuda")
             info = fn(out)
-            host = out[:int(info["n_fields"].sum()) * w * nl].view(torch.int16).cpu().numpy().view(np.uint16).reshape(-1, w * nl)
+            host = host_fields(out[:int(info["n_fields"].sum()) * w * nl].view(-1, w * nl))
         launches.append(ctx.launch_count() - n0 - (1 if sizing else 0))
         got.append(host.copy())
     return got, launches
@@ -359,15 +285,15 @@ def test_never_staging_and_staging_change_only_what_they_should():
     for ntsc in (1, 0):
         cases = _two_streams(ntsc)
         fc0 = [c["fc0"] for c in cases]
-        plain, lp = _fields(_context(2, ntsc, fc0), cases)
-        off, lo = _fields(_context(2, ntsc, fc0), cases, stage=lambda c, p: c.present_overlay(oc.bitmap(p), 0, p, None))   # blend 0: nothing drawn
-        on, ln = _fields(_context(2, ntsc, fc0), cases, stage=_stager)
+        plain, lp = _fields(presenting_context(2, ntsc, fc0), cases)
+        off, lo = _fields(presenting_context(2, ntsc, fc0), cases, stage=lambda c, p: c.present_overlay(oc.bitmap(p), 0, p, None))   # blend 0: nothing drawn
+        on, ln = _fields(presenting_context(2, ntsc, fc0), cases, stage=_stager)
         assert lp == lo == ln
         assert all(np.array_equal(a, b) for a, b in zip(plain, off))
         assert any(not np.array_equal(a, b) for a, b in zip(plain, on))
         # the same fields without sizing calls, and with an EF_ENOMEM call before every real one
-        bare, _ = _fields(_context(2, ntsc, fc0), cases, sizing=False, stage=_stager)
-        nomem, _ = _fields(_context(2, ntsc, fc0), cases, stage=_stager, enomem=True)
+        bare, _ = _fields(presenting_context(2, ntsc, fc0), cases, sizing=False, stage=_stager)
+        nomem, _ = _fields(presenting_context(2, ntsc, fc0), cases, stage=_stager, enomem=True)
         assert all(np.array_equal(a, b) and np.array_equal(a, c) for a, b, c in zip(on, bare, nomem))
 
 
@@ -379,27 +305,21 @@ def test_reset_keeps_latched_and_staged_overlays():
             c["cmds"] = [oc._cmd(3, 50, 77), None, None, None, oc._cmd(4, -1, 200)]
         cases = [dict(c, segments=c["segments"] + [(80 + i, [900000 + 3003 * k for k in range(3)])], modes=[0] * 8,
                       cmds=c["cmds"] + [oc._cmd(5, 9, None), None, None]) for i, c in enumerate(cases)]
-        ctx = _context(2, ntsc, [c["fc0"] for c in cases])
+        ctx = presenting_context(2, ntsc, [c["fc0"] for c in cases])
         d = Drive(ctx, cases, o).run()
         d.check()
         ctx.close()
 
 
-def _code(fn):
-    with pytest.raises(espflix_b200.EspflixError) as e:
-        fn()
-    return e.value.code
-
-
 def test_error_codes():
     ctx = espflix_b200.Context(n_streams=3, max_pictures=4, fields=False)
-    assert _code(lambda: ctx.present_overlay(None, 5, 0)) == capi.EF_ESTATE          # before ef_present_enable
+    assert error_code(lambda: ctx.present_overlay(None, 5, 0)) == capi.EF_ESTATE          # before ef_present_enable
     ctx.enable_pts()
     ctx.enable_present()
-    assert _code(lambda: ctx.present_overlay(None, 5, 0, first=-1, count=1)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_overlay(None, 5, 0, first=2, count=2)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_overlay(None, -2, 0)) == capi.EF_EINVAL
-    assert _code(lambda: ctx.present_overlay(None, [0, -1, -3], 0, first=0, count=3)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_overlay(None, 5, 0, first=-1, count=1)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_overlay(None, 5, 0, first=2, count=2)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_overlay(None, -2, 0)) == capi.EF_EINVAL
+    assert error_code(lambda: ctx.present_overlay(None, [0, -1, -3], 0, first=0, count=3)) == capi.EF_EINVAL
     ctx.present_overlay(None, [0, -1, -3], 0, set=[2, 2, 4])                        # the blend of stream 2 is not set
     ctx.present_overlay(np.zeros((1, 1280), np.uint8), -1, (1 << 31) - 1, first=2, count=1)
     ctx.present_overlay(None, None, None, first=3, count=0)

@@ -1,7 +1,6 @@
 """Presentation timestamps through the decoder context (ef_pts_enable / ef_picture_pts): the pts of every picture of every
 TS submit, concatenated over the submits, must equal the pts the unmodified reference pushes with it (tests/golden/
 pts_pins.json) and, outside the reference's domain, the restatement in tests/pts_cases.py."""
-import hashlib
 import json
 import os
 
@@ -11,6 +10,8 @@ import pytest
 import espflix_b200
 from espflix_b200 import capi
 from tests import audio_cases, pts_cases
+from tests.carry_cases import cut, packets
+from tests.harness import sha, submits
 
 pytestmark = pytest.mark.gpu
 G = pts_cases.GOLDEN
@@ -24,17 +25,6 @@ def pins():
 @pytest.fixture(scope="module")
 def cases():
     return pts_cases.cases()
-
-
-def _packets(ts):
-    ts = np.frombuffer(bytes(ts), dtype=np.uint8)
-    return [ts[i:i + 188] for i in range(0, ts.size, 188)]
-
-
-def _cut(ts, cuts):
-    pk = _packets(ts)
-    edges = [0] + list(cuts) + [len(pk)]
-    return [np.concatenate(pk[a:b]) if b > a else np.zeros(0, dtype=np.uint8) for a, b in zip(edges[:-1], edges[1:])]
 
 
 def _expected(ts, name, pins):
@@ -85,7 +75,7 @@ def test_fixtures_whole_and_cut_at_pes_starts(pins):
     sizes = [[5, 12, 1, 9, 7, 12, 3], [11, 2, 12, 8, 6, 4, 10]]
     per_stream = []
     for i, t in enumerate(ts):
-        pk = _packets(t)
+        pk = packets(t)
         starts = [k for k, q in enumerate(pk) if ((int(q[1]) << 8 | int(q[2])) & 0x1FFF) == 0x100 and q[1] & 0x40]
         cuts, p, j = [], 0, 0
         while True:
@@ -94,10 +84,7 @@ def test_fixtures_whole_and_cut_at_pes_starts(pins):
             if p >= len(starts):
                 break
             cuts.append(starts[p])
-        per_stream.append(_cut(t, cuts))
-    K = max(len(c) for c in per_stream)
-    for c in per_stream:
-        c += [np.zeros(0, dtype=np.uint8)] * (K - len(c))
+        per_stream.append(cut(t, cuts))
     frames = [[], []]
 
     def decode(ctx, counts):
@@ -109,13 +96,13 @@ def test_fixtures_whole_and_cut_at_pes_starts(pins):
 
     ctx = espflix_b200.Context(n_streams=2, max_pictures=13, max_slices_per_picture=12, es_capacity=1 << 21)
     ctx.enable_pts()
-    pts, last = _run(ctx, [[per_stream[0][k], per_stream[1][k]] for k in range(K)], decode=decode)
+    pts, last = _run(ctx, submits(per_stream), decode=decode)
     for s, n in enumerate(names):
         assert pts[s] == pins[n]["pts"], n
         assert last[s][-1] == pins[n]["pts"][-1]
         assert len(frames[s]) == dpins[n]["frames"]
         for k, f in enumerate(frames[s]):
-            assert hashlib.sha256(f.tobytes()).hexdigest() == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
+            assert sha(f) == dpins[n]["frame_sha256"][k], "%s picture %d" % (n, k)
     ctx.close()
 
 
@@ -126,8 +113,8 @@ def _cut_cases(cases, K, seed):
         cand = pts_cases.cut_points(ts)
         r = np.random.RandomState(seed + i)
         cuts = sorted(r.choice(cand, size=K - 1, replace=True).tolist()) if cand else [len(ts) // 188] * (K - 1)
-        chunks.append(_cut(ts, cuts))
-    return [[chunks[s][k] for s in range(len(cases))] for k in range(K)]
+        chunks.append(cut(ts, cuts))
+    return submits(chunks)
 
 
 @pytest.mark.parametrize("queue_ahead", [False, True])
@@ -162,7 +149,7 @@ def test_es_submits_reindex_reset_and_audio(pins, cases):
     byname = dict(cases)
     ts = byname["synth20_shift"]
     cuts = pts_cases.cut_points(ts)
-    a, b, c = _cut(ts, [cuts[len(cuts) // 3], cuts[2 * len(cuts) // 3]])
+    a, b, c = cut(ts, [cuts[len(cuts) // 3], cuts[2 * len(cuts) // 3]])
     want = pins["synth20_shift"]["pts"]
     ctx = espflix_b200.Context(n_streams=1, max_pictures=24, max_slices_per_picture=12, es_capacity=1 << 20, fields=False)
     ctx.enable_pts()
@@ -210,9 +197,9 @@ def test_es_submits_reindex_reset_and_audio(pins, cases):
     progs = [byname["synth12_shift"], byname["synth9_shift"]]
     chunks = []
     for i in range(2):
-        video = np.concatenate([q for q in _packets(progs[i]) if ((int(q[1]) << 8 | int(q[2])) & 0x1FFF) == 0x100])   # without the filler audio PES
+        video = b"".join(q for q in packets(progs[i]) if ((int(q[1]) << 8 | int(q[2])) & 0x1FFF) == 0x100)   # without the filler audio PES
         vc = pts_cases.cut_points(video)
-        v = _cut(video, [vc[len(vc) // 2]])
+        v = [np.frombuffer(x, dtype=np.uint8) for x in cut(video, [vc[len(vc) // 2]])]
         au = audio_cases.mux_audio_ts(es[i], pid=0x102)
         h = au.size // 188 // 2
         chunks.append([np.concatenate([v[0], au[:h * 188]]), np.concatenate([v[1], au[h * 188:]])])

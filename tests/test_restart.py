@@ -1,21 +1,16 @@
 """The per-stream restart restated (tests/restart_cases.py) against what the unmodified reference produced on the same programs
 (tests/golden/restart_pins.json, tools/make_restart_golden.py), and the tempting wrong rules that the pins reject: the carried
 PTS reset to -1, the audio state zeroed as for end_of_stream, and frame stores zero-filled as ef_reset does."""
-import hashlib
 import json
 import os
 
-import numpy as np
 import pytest
 
 from tests import overlay_cases as oc, restart_cases as rc
+from tests.harness import sha
 from tests.oracle_lib import Oracle
 
 PINS = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "restart_pins.json")))
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 @pytest.fixture(scope="module")
@@ -43,8 +38,8 @@ def test_decoder_restatement_matches_pins(name, oracle):
     assert [len(p) for p in want["pic_pts"]] == pin["pictures"]
     pcms, pdm = rc.audio_restate(oracle, progs)
     assert [p.size for p in pcms] == pin["pcm_samples"]
-    assert [_sha(p) for p in pcms] == pin["pcm_sha256"]
-    assert _sha(pdm) == pin["pdm_sha256"]
+    assert [sha(p) for p in pcms] == pin["pcm_sha256"]
+    assert sha(pdm) == pin["pdm_sha256"]
 
 
 @pytest.mark.parametrize("name", sorted(rc.paced_cases()))
@@ -65,7 +60,7 @@ def test_pins_reject_zeroed_audio_state(oracle):
     changed = 0
     for n, progs in rc.decoder_cases().items():
         pcms, pdm = rc.audio_restate(oracle, progs, zero_state=True)
-        changed += [_sha(p) for p in pcms] != PINS["decoder"][n]["pcm_sha256"] or _sha(pdm) != PINS["decoder"][n]["pdm_sha256"]
+        changed += [sha(p) for p in pcms] != PINS["decoder"][n]["pcm_sha256"] or sha(pdm) != PINS["decoder"][n]["pdm_sha256"]
     assert changed == len(rc.decoder_cases())
 
 

@@ -12,17 +12,13 @@ import pytest
 import espflix_b200
 from espflix_b200 import capi
 from tests import overlay_cases as oc, restart_cases as rc
-from tests.test_present_overlay_gpu import _call, _context, _stage
+from tests.harness import present_call, presenting_context, sha, stage_overlay
 
 pytestmark = pytest.mark.gpu
 PINS = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "restart_pins.json")))
 DEC = rc.decoder_cases()
 NAMES = sorted(DEC)
 FILLERS = 3
-
-
-def _sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def _filler_programs(i, k):
@@ -84,8 +80,8 @@ def test_mixed_batch_decoder(queued, plain):
             pic = got[s]["pic"][p][:npics]
             assert pic == want["pic_pts"][p], (name, p, pic, want["pic_pts"][p])
             assert got[s]["last"][p] == pin["get_pts"][p], (name, p)
-            assert got[s]["pcm"][p].size == pin["pcm_samples"][p] and _sha(got[s]["pcm"][p]) == pin["pcm_sha256"][p], (name, p)
-        assert _sha(np.concatenate(got[s]["pdm"][:P])) == pin["pdm_sha256"], name
+            assert got[s]["pcm"][p].size == pin["pcm_samples"][p] and sha(got[s]["pcm"][p]) == pin["pcm_sha256"][p], (name, p)
+        assert sha(np.concatenate(got[s]["pdm"][:P])) == pin["pdm_sha256"], name
         # the reference's pushes: every program's pictures but its last, all of the last program's
         pushes = [v for p in range(P) for v in (want["pic_pts"][p] if p == P - 1 else want["pic_pts"][p][:-1])]
         assert pushes == pin["pushes"]
@@ -106,7 +102,7 @@ def _paced_run(case, restart):
     around it. restart: ef_restart_streams(op) on the case's stream alone (first = CASE_AT) before every later segment.
     -> (per stream SHA-256 of its field stream, the case's flip fields, the case's fields)"""
     n = 4
-    ctx = _context(n, case["ntsc"], case["fc0"])
+    ctx = presenting_context(n, case["ntsc"], case["fc0"])
     disps = [oc.OverlayDisplay(case["ntsc"], case["fc0"]) for _ in range(n)]
     whole = [hashlib.sha256() for _ in range(n)]
     flips, emitted, k, base = [], [0] * n, 0, 0
@@ -121,7 +117,7 @@ def _paced_run(case, restart):
         if si and case.get("idle_before") and case["idle_before"][si]:
             nf = np.zeros(n, np.uint32)
             nf[CASE_AT] = case["idle_before"][si]
-            take(*_call(ctx, lambda o: ctx.present_idle(nf, o)))
+            take(*present_call(ctx, lambda o: ctx.present_idle(nf, o)))
         if si and restart:
             ctx.restart_streams([case["op"]], first=CASE_AT)
         ts = [oc.segment_ts(600 + 10 * s + si, [200000 + 50000 * s + 3003 * (base + j) for j in range(len(pts))]) for s in range(n)]
@@ -132,10 +128,10 @@ def _paced_run(case, restart):
         for j in range(len(pts)):
             cmds = [None] * n
             cmds[CASE_AT] = case["cmds"][k] if restart else None
-            _stage(ctx, disps, cmds)
+            stage_overlay(ctx, disps, cmds)
             modes = np.zeros(n, np.uint8)
             modes[CASE_AT] = case["modes"][k] if restart else 0
-            info, host = _call(ctx, lambda o: ctx.present_picture(j, modes=modes, out=o))
+            info, host = present_call(ctx, lambda o: ctx.present_picture(j, modes=modes, out=o))
             take(info, host)
             flips.append(int(info[CASE_AT]["flip_field"]))
             k += 1
@@ -156,7 +152,7 @@ def test_paced_mixed_batch_with_overlay(name, oracle_frames):
         ctx, whole, flips, emitted, take = _paced_run(case, restart)
         nf = np.full(4, 5, np.uint32)
         nf[CASE_AT] = want_fields - emitted[CASE_AT] if restart else 5
-        take(*_call(ctx, lambda o: ctx.present_idle(nf, o)))
+        take(*present_call(ctx, lambda o: ctx.present_idle(nf, o)))
         ctx.close()
         runs.append(([h.hexdigest() for h in whole], flips))
     (got, flips), (plain, _) = runs
@@ -203,15 +199,15 @@ def test_errors_and_launches():
     ctx.restart_streams([2, 0])                                 # no op 1: no demux-gate kernel
     assert ctx.launch_count() - before == 1
     ctx.close()
-    ctx = _context(2, 1, 0)
+    ctx = presenting_context(2, 1, 0)
     ctx.submit_ts(*ctx.pack([ts, ts]))
     ctx.index()
-    _call(ctx, lambda o: ctx.present_picture(0, out=o))
+    present_call(ctx, lambda o: ctx.present_picture(0, out=o))
     with pytest.raises(capi.EspflixError) as e:                 # pictures 1.. of the current submit are unpresented
         ctx.restart_streams([1, 1])
     assert e.value.code == capi.EF_ESTATE
     for p in range(1, 4):
-        _call(ctx, lambda o: ctx.present_picture(p, out=o))
+        present_call(ctx, lambda o: ctx.present_picture(p, out=o))
     ctx.restart_streams([1, 1])
     ctx.close()
 

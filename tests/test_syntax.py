@@ -2,7 +2,6 @@
 (pinned as SHA-256 by tools/make_syntax_pins.py in tests/golden/syntax_pins.json), and proof that those streams reach the
 syntax the motion-search generator never writes."""
 import functools
-import hashlib
 import json
 import os
 from collections import Counter
@@ -11,6 +10,7 @@ import numpy as np
 import pytest
 
 from tests import syntax_cases as sc
+from tests.harness import sha
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "syntax_pins.json")))
@@ -45,10 +45,6 @@ FEATURES = [
     "mb_width_lt22", "mb_height_lt12", "slice_rows_past_picture", "sequence_header_mid_stream",
     "extra_information_slice", "picture_type_3", "picture_type_4",
 ] + ["f_code_%d" % f for f in range(1, 8)] + ["vector_wrap_f_code_%d" % f for f in range(1, 7)]
-
-
-def sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 @functools.lru_cache(maxsize=None)

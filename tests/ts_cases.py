@@ -1,7 +1,12 @@
 """tests/ts_cases.py — small synthetic transport streams for the trick-mode index tests: PES starts with and
 without a sequence header, PTS present / absent / malformed, adaptation fields, audio and PSI packets in
 between, non-monotonic PTS (so the nearest-entry search has ties and far entries)."""
+import os
+
 import numpy as np
+
+G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+FUZZ_SEEDS = range(40, 52)
 
 
 def _pts_bytes(pts, prefix=0x20):
@@ -55,3 +60,20 @@ def make_ts(seed, n_pes=120, monotonic=True, ref_domain=True):
         step = int(rng.integers(1500, 9000))
         pts = pts + step if monotonic or rng.random() < 0.88 else max(0, pts - int(rng.integers(0, 30000)))
     return b"".join(out)
+
+
+def fuzzed_stream(seed):
+    return make_ts(seed, n_pes=90, monotonic=seed % 3 != 0)
+
+
+def fuzzed_image_files():
+    return [make_ts(s, monotonic=s != 61) for s in (60, 61, 62)]
+
+
+def files_of(key):
+    """the files of a pinned video.idx image, keyed 'fixture:<names>' or 'fuzz:<seeds>:<monotonic>'"""
+    kind, rest = key.split(":", 1)
+    if kind == "fixture":
+        return [open(os.path.join(G, n + ".ts"), "rb").read() for n in rest.split(",")]
+    seeds, mono = rest.split(":")
+    return [make_ts(int(s), monotonic=bool(int(mono))) for s in seeds.split(",")]

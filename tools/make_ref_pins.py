@@ -2,9 +2,8 @@
 """tools/make_ref_pins.py — tests/golden/ref_pins.json: what the UNMODIFIED reference (oracle/_ref, built by
 `make -C oracle ref REF=<checkout of the reference>`) computes on the synthetic inputs of the tests that compare the
 C restatement with it: decoded coverage streams, composite fields / blits / presentation extras, SBC audio, irregular
-PTS pacing and the trick-mode index of fuzzed streams. Inputs come from the tests' own case generators, so the pins
+PTS pacing and the trick-mode index of fuzzed streams. Inputs come from the case modules the tests draw on, so the pins
 and the tests cannot drift apart; outputs are stored as SHA-256 (and short lists where they are small)."""
-import hashlib
 import json
 import os
 import subprocess
@@ -17,15 +16,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = os.path.join(ROOT, "tests", "golden", "ref_pins.json")
 SECTIONS = ("decode", "video", "presentation", "audio", "pacing_irregular", "index_fuzzed")
 sys.path.insert(0, ROOT)
-if not os.path.exists(PINS):                  # the test modules read their section at import
-    json.dump({k: {} for k in SECTIONS}, open(PINS, "w"))
-from tests import oracle_lib  # noqa: E402
-from tests import test_audio, test_oracle_vs_ref, test_pacing, test_tsindex  # noqa: E402
-from tests.synth_cases import COVERAGE  # noqa: E402
-
-
-def sha(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+from tests import audio_cases, oracle_lib, present_cases, synth_cases, ts_cases  # noqa: E402
+from tests.harness import sha  # noqa: E402
 
 
 def ref_audio(ts):
@@ -46,35 +38,35 @@ def main():
     assert oracle_lib.have_ref() and oracle_lib.have_ref_index(), "build oracle/_ref first: make -C oracle ref REF=<checkout of the reference>"
     pins = {"decode": {}, "video": {}, "presentation": {}, "audio": {}, "pacing_irregular": [], "index_fuzzed": {"tables": {}}}
 
-    for idx, (name, kw) in enumerate(COVERAGE):
-        _, ts = test_oracle_vs_ref.coverage_stream(idx)
+    for idx, (name, kw) in enumerate(synth_cases.COVERAGE):
+        _, ts = synth_cases.coverage_stream(idx)
         info, frames = oracle_lib.ref_decode_ts(ts)
         assert frames.shape[0] == info["frames"]
         pins["decode"][name] = {"frames": int(info["frames"]), "sha256": sha(frames)}
 
     rv = oracle_lib.RefVideo()
-    for key, call in test_oracle_vs_ref.video_cases():
+    for key, call in synth_cases.video_cases():
         pins["video"][key] = sha(call(rv))
-    for key, call in test_oracle_vs_ref.presentation_cases():
+    for key, call in synth_cases.presentation_cases():
         pins["presentation"][key] = sha(call(rv))
 
-    for case in test_audio.AUDIO_CASES:
-        _, ts = test_audio.synthetic_case(case)
+    for case in audio_cases.AUDIO_CASES:
+        _, ts = audio_cases.synthetic_case(case)
         es, pcm, pdm = ref_audio(ts)
         pins["audio"][case] = {"es_bytes": int(es.size), "es_sha256": sha(es), "pcm_samples": int(pcm.size), "pcm_sha256": sha(pcm), "pdm_sha256": sha(pdm)}
 
-    for pts, ntsc, fc0, modes, tail in test_pacing.irregular_cases():
+    for pts, ntsc, fc0, modes, tail in present_cases.irregular_cases():
         frames = np.zeros((len(pts), 101376), dtype=np.uint8)             # content is irrelevant to the schedule
         f, ff, fl, _, hs = rv.paced(frames, pts, ntsc, fc0, 400, want_fields=False, modes=modes, tail_fields=tail, want_hscroll=True)
         pins["pacing_irregular"].append({"fields": int(f), "flip_field": [int(x) for x in ff], "flip_line": [int(x) for x in fl], "hscroll": [int(x) for x in hs]})
 
     ri = oracle_lib.RefIndexer()
-    for seed in test_tsindex.FUZZ_SEEDS:
-        t = ri.make_index(test_tsindex.fuzzed_stream(seed))
+    for seed in ts_cases.FUZZ_SEEDS:
+        t = ri.make_index(ts_cases.fuzzed_stream(seed))
         pins["index_fuzzed"]["tables"][str(seed)] = {"first_pts": int(t["first_pts"]), "last_pts": int(t["last_pts"]), "entries": int(t["seq_pts"].size),
                                                      "seq_pts_sha256": sha(t["seq_pts"]), "seq_pos_sha256": sha(t["seq_pos"])}
-    img = ri.build_idx(test_tsindex.fuzzed_image_files())
-    pins["index_fuzzed"]["image"] = {"bytes": len(img), "sha256": hashlib.sha256(img).hexdigest()}
+    img = ri.build_idx(ts_cases.fuzzed_image_files())
+    pins["index_fuzzed"]["image"] = {"bytes": len(img), "sha256": sha(img)}
 
     assert tuple(pins) == SECTIONS
     with open(PINS, "w") as f:
