@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 FRAME_BYTES = 101376
 I420_BYTES = 101376
 EF_OK, EF_EINVAL, EF_ECUDA, EF_ENOMEM, EF_ESTATE = 0, -1, -2, -3, -4
+EF_FIELD_U16, EF_FIELD_DAC8 = 0, 1          # ef_present_format: the uint16 DMA line buffer, or the bytes the video DAC plays
 
 
 class EspflixError(RuntimeError):
@@ -87,6 +88,7 @@ _SIGNATURES = {
     "ef_present_picture_async": (_I, [_VP, _I, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_idle_async": (_I, [_VP, _VP, _VP, ctypes.c_uint64, _VP, _VP]),
     "ef_present_wait": (_I, [_VP, ctypes.POINTER(_I)]),
+    "ef_present_format": (_I, [_VP, _I]),
     "ef_present_overlay": (_I, [_VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ef_present_font": (_I, [_VP, _VP, _VP, _I]),
     "ef_present_clock": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
@@ -133,6 +135,7 @@ class Context:
         cfg = _Config(device, n_streams, max_pictures, max_slices_per_picture, es_capacity, 1 if fields else 0)
         self._h = _VP()
         self.n_streams, self.max_pictures = n_streams, max_pictures
+        self.field_format = EF_FIELD_U16
         self._check(self.lib.ef_create(ctypes.byref(self._h), ctypes.byref(cfg)))
 
     def _check(self, rc):
@@ -373,12 +376,29 @@ class Context:
         fc = None if frame_counter0 is None else np.ascontiguousarray(np.broadcast_to(frame_counter0, (self.n_streams,)), dtype=np.uint32)
         self._check(self.lib.ef_present_enable(self._h, _ptr(fc)))
 
+    def present_format(self, fmt):
+        """ef_present_format, before enable_present(): EF_FIELD_U16 (the default) has the present calls write the reference's
+        uint16 DMA line buffer, EF_FIELD_DAC8 the bytes the video DAC plays (byte t of a line = sample t ^ 1's high byte). A DAC8
+        context takes contiguous CUDA torch.uint8 tensors for `out`."""
+        self._check(self.lib.ef_present_format(self._h, int(fmt)))
+        self.field_format = int(fmt)
+
+    def _dac8_out(self, out):
+        """on a DAC8 context, out must be a contiguous CUDA uint8 tensor (TypeError otherwise) -> True"""
+        if self.field_format != EF_FIELD_DAC8:
+            return False
+        import torch
+        if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()):
+            raise TypeError("out must be a contiguous CUDA torch.uint8 tensor on an EF_FIELD_DAC8 context")
+        return True
+
     def _present(self, call, out, stream):
         info = np.zeros(self.n_streams, dtype=PRESENT_INFO)
         if out is None:
             dst, cap = None, 0
         else:
-            assert out.is_cuda and str(out.dtype) == "torch.uint16" and out.is_contiguous()
+            if not self._dac8_out(out):
+                assert out.is_cuda and str(out.dtype) == "torch.uint16" and out.is_contiguous()
             w, n = self.geometry()
             dst, cap = out.data_ptr(), out.numel() // (w * n)       # whole fields only
         self._check(call(dst, cap, info.ctypes.data, stream))
@@ -386,7 +406,7 @@ class Context:
 
     def present_picture(self, pic, modes=None, out=None, stream=0):
         """ef_present_picture: decode picture index `pic` and push it on every stream that has it. out: CUDA uint16 tensor of
-        whole fields (None: sizing call). Returns info (PRESENT_INFO per stream)."""
+        whole fields, uint8 on a DAC8 context (None: sizing call). Returns info (PRESENT_INFO per stream)."""
         md = None if modes is None else np.ascontiguousarray(np.broadcast_to(modes, (self.n_streams,)), dtype=np.uint8)
         return self._present(lambda d, c, i, st: self.lib.ef_present_picture(self._h, pic, _ptr(md), d, c, i, st), out, stream)
 
@@ -399,7 +419,8 @@ class Context:
         import torch
         if info is None:
             info = torch.zeros((self.n_streams, 8), dtype=torch.int32, device=out.device)
-        for t, dt, what in ((out, torch.uint16, "out"), (info, torch.int32, "info")):
+        checks = ((info, torch.int32, "info"),) if self._dac8_out(out) else ((out, torch.uint16, "out"), (info, torch.int32, "info"))
+        for t, dt, what in checks:
             if not (t.is_cuda and t.dtype == dt and t.is_contiguous()):
                 raise TypeError("%s must be a contiguous CUDA %s tensor" % (what, dt))
         assert info.numel() == 8 * self.n_streams
@@ -408,7 +429,7 @@ class Context:
         return info
 
     def present_picture_async(self, pic, out, info=None, modes=None, stream=0):
-        """ef_present_picture_async: present_picture() into the CUDA uint16 tensor `out`, returning once the work is enqueued on
+        """ef_present_picture_async: present_picture() into the CUDA uint16 (DAC8: uint8) tensor `out`, returning once the work is enqueued on
         `stream` (a torch.cuda.Stream or a raw handle). info: None or an int32 tensor [n_streams, 8] that receives the
         ef_present_info rows (see present_info()). Returns info. present_wait() says how far the chain of async calls got."""
         md = None if modes is None else np.ascontiguousarray(np.broadcast_to(modes, (self.n_streams,)), dtype=np.uint8)

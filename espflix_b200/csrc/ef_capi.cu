@@ -59,8 +59,8 @@ cudaError_t ef_launch_parse(const EfDev& dev, int pic0, int n_pics, int sm_count
 cudaError_t ef_launch_recon(const EfDev& dev, int pic_rel, int sm_count, size_t n_slots, cudaStream_t stream);
 cudaError_t ef_launch_composite(const EfDev* dev, int n_streams, const EfGeometry& g, int fb, int frame_counter, const EfPresent& pr, cudaStream_t stream);
 cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line, int x, int width, int frame_counter, uint16_t* dst, cudaStream_t stream);
-cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total);
+cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint8_t* dst, bool dac8,
+                                      cudaStream_t stream, uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total);
 __global__ void ef_pace_kernel(const EfPaceState* st, EfPaceState* next, EfPaceRun* run, EfPaceOut* out, const int64_t* pic_pts, const uint32_t* n_pics,
                                const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc,
                                const EfOverlayState* ovl, EfOverlayState* ovl_next);
@@ -298,6 +298,7 @@ struct ef_ctx {
     bool paced = false;
     bool pace_indexed = false;                    // an ef_index followed ef_present_enable: its pictures are to be presented
     int pace_ntsc = 1;                            // the standard, fixed at ef_present_enable
+    int pace_format = EF_FIELD_U16;               // what the present calls write (ef_present_format), fixed at ef_present_enable
     int pace_next = 0;                            // the picture index ef_present_picture takes next
     int pace_npics = -1;                          // picture indices of the current submit (-1: not read yet)
     int pace_p0 = 0;                              // first picture index of the current K1a range
@@ -1773,6 +1774,15 @@ int ef_present_enable(ef_ctx* c, const uint32_t* frame_counter0)
     return EF_OK;
 }
 
+int ef_present_format(ef_ctx* c, int format)
+{
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (format != EF_FIELD_U16 && format != EF_FIELD_DAC8) return fail(EF_EINVAL, "unknown field format %d", format);
+    if (c->paced) return fail(EF_ESTATE, "ef_present_format after ef_present_enable");
+    c->pace_format = format;
+    return EF_OK;
+}
+
 // The halves of a presentation call that the synchronous and the asynchronous calls share, all on `st`:
 //   present_schedule  the call's modes / idle field counts (through the pinned buffer `pinned`) and the schedule, one thread per
 //                     stream, into scratch
@@ -1830,7 +1840,7 @@ static int present_room(ef_ctx* c, uint64_t fields, cudaStream_t st)
     return EF_OK;
 }
 
-static int present_render(ef_ctx* c, uint16_t* dst, uint64_t slots, bool gated, cudaStream_t st)
+static int present_render(ef_ctx* c, uint8_t* dst, uint64_t slots, bool gated, cudaStream_t st)
 {
     EfFieldOverlay* fovl = c->d_ovl ? c->d_fovl : nullptr;
     CK(ef_launch_pace_fill(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_first, c->d_desc, c->d_ovl, c->d_ovl_next, fovl, c->cfg.n_streams,
@@ -1840,7 +1850,8 @@ static int present_render(ef_ctx* c, uint16_t* dst, uint64_t slots, bool gated, 
         CK(ef_launch_clock_commit(c->d_clk, c->d_ovl_clk, c->d_clk_bm, c->d_ovl_slots, c->cfg.n_streams, gated ? c->d_pace_chain : nullptr, st));
         c->launches++;
     }
-    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, slots, dst, st, &c->launches, fovl, c->d_ovl_slots, gated ? c->d_pace_total : nullptr));
+    CK(ef_launch_composite_paced(c->d, c->h.geo, c->d_desc, slots, dst, c->pace_format == EF_FIELD_DAC8, st, &c->launches, fovl, c->d_ovl_slots,
+                                 gated ? c->d_pace_total : nullptr));
     return EF_OK;
 }
 
@@ -1875,7 +1886,7 @@ static int present_common(ef_ctx* c, int pic, const uint8_t* modes, const uint32
     }
     TRY(present_room(c, total, st));
     CK(cudaMemcpyAsync(c->d_pace_first, c->h_pace_first, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    TRY(present_render(c, dst, total, false, st));
+    TRY(present_render(c, (uint8_t*)dst, total, false, st));
     CK(cudaStreamSynchronize(st));                         // the pinned offsets and the scratch are free for the next call
     return EF_OK;
 }
@@ -1916,7 +1927,7 @@ static int present_async(ef_ctx* c, int pic, const uint8_t* modes, const uint32_
     CK(cudaGetLastError());
     c->launches++;
     if (pic >= 0) TRY(present_recon(c, pic, st));
-    TRY(present_render(c, dst, dst_fields, true, st));
+    TRY(present_render(c, (uint8_t*)dst, dst_fields, true, st));
     CK(cudaMemcpyAsync(c->h_pace_chain, c->d_pace_chain, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(c->ev_pace_done, st));
     return EF_OK;

@@ -10,6 +10,9 @@
 // Pure streaming, HBM bound: each thread produces 8 samples (one 16-byte store) from 4 luma pixels
 // and 2+2 chroma bytes; the packed 4x8-bit expressions of blit() are reproduced verbatim because
 // the low byte of every sample carries deterministic carry "junk" that parity depends on.
+// Paced presentation can also emit what the DAC plays instead of the line buffer: one byte per sample (EF_FIELD_DAC8, dac_word).
+#include <type_traits>
+
 #include "ef_common.cuh"
 
 namespace {
@@ -111,6 +114,15 @@ __device__ __forceinline__ uint4 blit_quad(uint32_t y4, uint32_t dither, uint32_
                       ((p1 << 16) | (p0 >> 8)) + cb, (((p1 << 8) & 0xFF000000u) | (p0 >> 16)) + (cb << 8));
 }
 
+// EF_FIELD_DAC8: what the video DAC plays. The I2S unit sends the two 16-bit halves of each word in swapped order (burst_pal()
+// writes line[i ^ 1] = b[i], video.cpp:640-644; blit() stores each pixel before the sample interpolated ahead of it,
+// video.cpp:727-733), so buffer sample t ^ 1 plays at time t, and only its high byte drives the 8-bit DAC. Two words holding
+// samples 0..3 give the bytes played as samples 1, 0, 3, 2: one byte permute per pair of words.
+__device__ __forceinline__ uint32_t dac_word(uint32_t w0, uint32_t w1) { return __byte_perm(w0, w1, 0x5713); }
+__device__ __forceinline__ uint2 dac_chunk(uint4 c) { return make_uint2(dac_word(c.x, c.y), dac_word(c.z, c.w)); }   // 8 samples -> 8 bytes
+
+template <bool kDac8> using K2Out = std::conditional_t<kDac8, uint8_t, uint16_t>;   // one output sample
+
 // ---- K2 v6: a CTA synthesises a BAND of 16 consecutive lines of one stream in shared memory and hands the finished
 // rows to the TMA engine (cp.async.bulk.global.shared::cta): the field leaves the SM as bulk stores instead of 16-byte
 // STG, which took the output off the L1/TEX pipe - the v4 kernel was bound there (86 % busy at 42 % DRAM throughput,
@@ -155,22 +167,31 @@ __device__ __forceinline__ int blank_class(const EfPresent& pr, int line)
 // bitmap slots, two per stream.
 // kGated (paced only, ef_present_*_async): the grid follows the caller's capacity, not the call's fields; a CTA whose output slot
 // slot0 + y is at or past *total (ef_pace_size_kernel: the call's fields, 0 when its chain failed) exits at once.
-template <bool kNtsc, bool kPaced, bool kOverlay = false, bool kGated = false>
+// kDac8 (paced only, ef_present_format EF_FIELD_DAC8): rows are built as DAC bytes in playback order (dac_word), and the field is
+// one byte per sample. An active line's own row then spans X0..X1: PAL's blit span [280, 984) is 8 mod 16 at both ends and bulk
+// copies move 16-byte aligned runs, so PAL rows also carry the black margin bytes 272..279 and 984..991 and a line is cut at
+// [0, 272) | [272, 992) | [992, 1136).
+template <bool kNtsc, bool kPaced, bool kOverlay = false, bool kGated = false, bool kDac8 = false>
 __global__ void __launch_bounds__(kK2Threads)
 ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter, const EfPresent pr, const EfFieldDesc* __restrict__ desc,
-                    uint16_t* __restrict__ dst, const EfFieldOverlay* __restrict__ fovl = nullptr, const uint64_t* __restrict__ total = nullptr,
+                    K2Out<kDac8>* __restrict__ dst, const EfFieldOverlay* __restrict__ fovl = nullptr, const uint64_t* __restrict__ total = nullptr,
                     uint64_t slot0 = 0)
 {
     static_assert(kPaced || !kOverlay, "the per-field overlay is a paced variant");
     static_assert(kPaced || !kGated, "the gate is on the paced variant");
+    static_assert(kPaced || !kDac8, "the DAC byte format is a paced variant");
     if constexpr (kGated) {
         if (slot0 + blockIdx.y >= *total) return;
     }
     using G = Geo<kNtsc>;
-    constexpr int CPL = G::W / 8;                                          // 16-byte chunks per line
-    constexpr int LB = G::W * 2, LS = LB + 16;                             // bytes per line in the field / in shared memory
+    constexpr int OB = kDac8 ? 1 : 2;                                      // bytes per output sample
+    constexpr int CPL = G::W / 8;                                          // 8-sample chunks per line
+    constexpr int LB = G::W * OB, LS = LB + 16;                            // bytes per line in the field / in shared memory
     constexpr int BLIT_C = G::BLIT / 8, BLIT_N = 2 * EF_W / 8;             // the blit span in chunks: [BLIT_C, BLIT_C + 88)
     constexpr int MARGIN_N = CPL - BLIT_N;                                 // chunks of a line outside it
+    constexpr int X0 = (G::BLIT * OB) % 16 ? G::BLIT - 8 : G::BLIT;        // the samples a line takes from its own row: [X0, X1)
+    constexpr int X1 = (G::BLIT * OB) % 16 ? G::BLIT + 2 * EF_W + 8 : G::BLIT + 2 * EF_W;
+    static_assert(X0 * OB % 16 == 0 && X1 * OB % 16 == 0 && LB % 16 == 0, "bulk copies move 16-byte aligned runs");
     __shared__ __align__(128) uint8_t sm[16 * LS];
     __shared__ int s_src[16], s_distinct[16], s_n;
     const EfDev& D = *Dp;
@@ -178,7 +199,7 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
     const int line0 = (int)blockIdx.x * 16;
     int stream = (int)blockIdx.y;
     EfPresent p = pr;
-    uint16_t* out0;
+    K2Out<kDac8>* out0;
     if constexpr (kPaced) {
         const EfFieldDesc f = desc[blockIdx.y];
         stream = (int)f.stream; fb_sel = f.fb; frame_counter = (int)f.frame_counter; p.hscroll = f.hscroll;
@@ -214,7 +235,8 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
         const int n = s_n;
         for (int i = (int)threadIdx.x; i < n * CPL; i += kK2Threads) {
             const int l = s_distinct[i / CPL], c = i % CPL;
-            *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
+            if constexpr (kDac8) *(uint2*)(sm + l * LS + c * 8) = dac_chunk(blank_chunk<kNtsc>(D, p, line0 + l, c * 8));
+            else *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> async proxy
         __syncthreads();
@@ -230,7 +252,14 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
     for (int i = (int)threadIdx.x; i < 2 * MARGIN_N; i += kK2Threads) {
         const int l = i / MARGIN_N, k = i % MARGIN_N;
         const int c = k >= BLIT_C ? k + BLIT_N : k;
-        *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
+        if constexpr (kDac8) *(uint2*)(sm + l * LS + c * 8) = dac_chunk(blank_chunk<kNtsc>(D, p, line0 + l, c * 8));
+        else *(uint4*)(sm + l * LS + c * 16) = blank_chunk<kNtsc>(D, p, line0 + l, c * 8);
+    }
+    if constexpr (X0 != G::BLIT) {                                         // the margin chunks of rows 2..15 that their lines copy
+        for (int i = (int)threadIdx.x; i < 2 * 14; i += kK2Threads) {
+            const int l = 2 + (i >> 1), c = (i & 1) ? BLIT_C + BLIT_N : BLIT_C - 1;
+            *(uint2*)(sm + l * LS + c * 8) = dac_chunk(blank_chunk<kNtsc>(D, p, line0 + l, c * 8));
+        }
     }
     {
         const int lane = (int)threadIdx.x & 31, warp = (int)threadIdx.x >> 5;
@@ -278,20 +307,29 @@ ef_composite_kernel(const EfDev* __restrict__ Dp, int fb_sel, int frame_counter,
             uint32_t lum = cstart[t] ? 0u : ((((lumw[t] + dither) & 0xFCFCFCFCu) >> 2) >> 24);   // carry = last pixel of the previous group
             const uint4 o0 = blit_quad(y8[t].x, dither, chroma_word(tab, u, v, vt), chroma_word(tab, u >> 8, v >> 8, vt), lum);
             const uint4 o1 = blit_quad(y8[t].y, dither, chroma_word(tab, u >> 16, v >> 16, vt), chroma_word(tab, u >> 24, v >> 24, vt), lum);
-            uint8_t* o = sm + row * LS + (G::BLIT + gd * 16) * 2;
-            *(uint4*)o = o0;
-            *(uint4*)(o + 16) = o1;
+            uint8_t* o = sm + row * LS + (G::BLIT + gd * 16) * OB;
+            if constexpr (kDac8) {                                         // 16 samples -> 16 bytes
+                const uint4 b = make_uint4(dac_word(o0.x, o0.y), dac_word(o0.z, o0.w), dac_word(o1.x, o1.y), dac_word(o1.z, o1.w));
+                if constexpr (G::BLIT % 16 == 0) *(uint4*)o = b;
+                else {                                                     // PAL: 8 mod 16
+                    *(uint2*)o = make_uint2(b.x, b.y);
+                    *(uint2*)(o + 8) = make_uint2(b.z, b.w);
+                }
+            } else {
+                *(uint4*)o = o0;
+                *(uint4*)(o + 16) = o1;
+            }
         }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     if (threadIdx.x < 16) {
         const int l = (int)threadIdx.x;
-        uint16_t* out = out0 + (size_t)l * G::W;
+        K2Out<kDac8>* out = out0 + (size_t)l * G::W;
         const uint8_t* tmpl = sm + (l & 1) * LS;
-        bulk_store(out, tmpl, G::BLIT * 2);
-        bulk_store(out + G::BLIT, sm + l * LS + G::BLIT * 2, 2 * EF_W * 2);
-        bulk_store(out + G::BLIT + 2 * EF_W, tmpl + (G::BLIT + 2 * EF_W) * 2, (G::W - G::BLIT - 2 * EF_W) * 2);
+        bulk_store(out, tmpl, X0 * OB);
+        bulk_store(out + X0, sm + l * LS + X0 * OB, (X1 - X0) * OB);
+        bulk_store(out + X1, tmpl + X1 * OB, (G::W - X1) * OB);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
     }
@@ -684,28 +722,34 @@ cudaError_t ef_launch_clock_commit(EfClockState* clk, const EfOverlayState* ovl_
     return cudaGetLastError();
 }
 
+// one launch of the paced K2 in the standard and output format of the instantiation; the overlay and gated variants as
+// ef_launch_composite_paced picks them
+template <bool kNtsc, bool kDac8>
+static void launch_paced(dim3 grid, cudaStream_t stream, const EfDev* dev, const EfFieldDesc* desc, uint8_t* dst, const EfFieldOverlay* fovl,
+                         const uint8_t* bitmaps, const uint64_t* total, uint64_t f0)
+{
+    K2Out<kDac8>* d = (K2Out<kDac8>*)dst;
+    const EfPresent pr = { 0, 0, 0, bitmaps };
+    if (total && fovl) ef_composite_kernel<kNtsc, true, true, true, kDac8><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc, d, fovl, total, f0);
+    else if (total) ef_composite_kernel<kNtsc, true, false, true, kDac8><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc, d, nullptr, total, f0);
+    else if (fovl) ef_composite_kernel<kNtsc, true, true, false, kDac8><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc, d, fovl);
+    else ef_composite_kernel<kNtsc, true, false, false, kDac8><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc, d);
+}
+
 // the paced K2: fields [0, n_fields) of desc into dst, at most 65,535 per launch (grid y). fovl != NULL: the overlay variant, with
 // the per-field overlay fovl and the bitmap slots `bitmaps`. total != NULL: the gated variant, n_fields is the capacity of dst and
-// only the slots below *total are drawn
-cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint16_t* dst, cudaStream_t stream,
-                                      uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total)
+// only the slots below *total are drawn. dac8: EF_FIELD_DAC8 fields (line_count x line_width bytes), else uint16 samples.
+cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint8_t* dst, bool dac8,
+                                      cudaStream_t stream, uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total)
 {
-    const size_t per = (size_t)g.line_count * g.line_width;
+    const size_t per = (size_t)g.line_count * g.line_width * (dac8 ? 1 : 2);   // bytes per field
     for (uint64_t f0 = 0; f0 < n_fields; f0 += 65535) {
         const dim3 grid((unsigned)(g.line_count + 15) / 16, (unsigned)(n_fields - f0 < 65535 ? n_fields - f0 : 65535));
-        if (total) {
-            const EfPresent pr = { 0, 0, 0, bitmaps };
-            const EfFieldOverlay* fo = fovl ? fovl + f0 : nullptr;
-            if (fovl && g.ntsc) ef_composite_kernel<true, true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
-            else if (fovl) ef_composite_kernel<false, true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
-            else if (g.ntsc) ef_composite_kernel<true, true, false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
-            else ef_composite_kernel<false, true, false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fo, total, f0);
-        } else if (fovl) {
-            const EfPresent pr = { 0, 0, 0, bitmaps };
-            if (g.ntsc) ef_composite_kernel<true, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);
-            else ef_composite_kernel<false, true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, pr, desc + f0, dst + f0 * per, fovl + f0);
-        } else if (g.ntsc) ef_composite_kernel<true, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
-        else ef_composite_kernel<false, true><<<grid, kK2Threads, 0, stream>>>(dev, 0, 0, EfPresent{}, desc + f0, dst + f0 * per);
+        const EfFieldOverlay* fo = fovl ? fovl + f0 : nullptr;
+        if (g.ntsc && dac8) launch_paced<true, true>(grid, stream, dev, desc + f0, dst + f0 * per, fo, bitmaps, total, f0);
+        else if (g.ntsc) launch_paced<true, false>(grid, stream, dev, desc + f0, dst + f0 * per, fo, bitmaps, total, f0);
+        else if (dac8) launch_paced<false, true>(grid, stream, dev, desc + f0, dst + f0 * per, fo, bitmaps, total, f0);
+        else launch_paced<false, false>(grid, stream, dev, desc + f0, dst + f0 * per, fo, bitmaps, total, f0);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         ++*launches;

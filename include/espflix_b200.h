@@ -50,6 +50,7 @@
  *   ef_present_enable / _picture / _idle  push_video(frame, front, pts, mode) video.cpp:1023-1057 against the frame flip
  *                                 of video_isr video.cpp:1122-1198: every stream's paced composite fields, in HBM
  *   ef_present_*_async / ef_present_wait  the same, enqueued without waiting for the device
+ *   ef_present_format             the paced fields as the DMA line buffer (uint16) or as the bytes the video DAC plays
  *   ef_present_overlay            composite() video.cpp:839-887 of every paced field: the overlay bitmap, blend and progress
  *   ef_present_font / _clock      ESPFlix::update_progress() espflix.cpp:862-874 with show_time() espflix.cpp:163-174: every
  *                                 stream's time text and progress drawn into its paced overlay on the device
@@ -302,7 +303,8 @@ int ef_picture_pts(ef_ctx* ctx, int first, int count, int n_pictures, int64_t* p
  * line below vsync_start that is not an active line of a presented frame, once F >= _next_frame_time. animate() runs at the
  * flip and at every field end (video.cpp:1076-1088). A push emits the fields whose line active_bottom - 1 it draws, each as
  * K2 draws it from the current store (picture k - 1), the other store (picture k), the hscroll of its active lines, its F and
- * the stream's overlay (ef_present_overlay; none until it is called). Fields are line_count x line_width uint16 samples.
+ * the stream's overlay (ef_present_overlay; none until it is called). Fields are line_count x line_width uint16 samples
+ * (ef_present_format EF_FIELD_DAC8: bytes).
  * ef_present_enable   needs ef_pts_enable and ef_video_init first (else EF_ESTATE) and fixes the standard: a later
  *                     ef_video_init that changes it returns EF_ESTATE. Each display starts at line 0 of field
  *                     frame_counter0[s] (NULL: 0) with no frame presented. Presentation starts with the next ef_index. From
@@ -363,6 +365,21 @@ int ef_present_picture_async(ef_ctx* ctx, int pic, const uint8_t* modes, uint16_
 int ef_present_idle_async(ef_ctx* ctx, const uint32_t* n_fields, uint16_t* dst, uint64_t dst_fields, ef_present_info* info,
                           void* stream);
 int ef_present_wait(ef_ctx* ctx, int* n_presented);
+
+/* ef_present_format   what the four present calls write to dst, chosen before ef_present_enable (after it: EF_ESTATE; an unknown
+ *                     format: EF_EINVAL; ef_reset keeps it). EF_FIELD_U16, the default, is the reference's DMA line buffer: uint16
+ *                     samples whose high byte drives the 8-bit DAC (levels IRE(x) << 8, video.cpp:520) and whose low byte is
+ *                     blit()'s junk. The I2S unit plays the two 16-bit halves of each word in swapped order, which the reference's
+ *                     buffers are written for (burst_pal(), video.cpp:640-644; blit(), video.cpp:727-733), so buffer sample t ^ 1
+ *                     plays at time t. EF_FIELD_DAC8 is what the DAC plays: byte t of line l is u16[l][t ^ 1] >> 8, where u16 is the
+ *                     same field in EF_FIELD_U16; a field is line_count x line_width bytes (NTSC 238,944, PAL 354,432), half the
+ *                     bytes to write and to move. dst stays a uint16_t* in the prototypes: on a DAC8 context pass a byte buffer
+ *                     cast to it. dst_fields, info[] and the 16-byte alignment of dst, the capacity checks, sizing calls, EF_ENOMEM,
+ *                     the async gate and retries, the schedule, overlay and clock are the same in both formats. ef_composite_field,
+ *                     ef_read_field, ef_video_isr and ef_blit stay uint16: they stand for the line buffer itself. */
+#define EF_FIELD_U16   0   /* default: the reference's uint16 DMA buffer, as today */
+#define EF_FIELD_DAC8  1   /* what the video DAC plays: one byte per sample, in playback order */
+int ef_present_format(ef_ctx* ctx, int format);
 
 /* ef_present_overlay  composite() of every paced field (video.cpp:839-887, 1181-1194): the 80 x 16 bitmap and the progress bar
  *                     on the 16 lines from active_bottom + 2, faded by the blend. Stages changes for streams [first, first +
