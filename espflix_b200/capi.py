@@ -97,7 +97,16 @@ _SIGNATURES = {
     "ef_end_streams": (_I, [_VP, _I, _I, _VP]),
     "ef_carry_info": (_I, [_VP, _I, _I, _VP, _VP]),
     "ef_tsidx_samples": (_I, [_I, _VP, _VP, _I, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, _VP, ctypes.c_uint32, _VP]),
+    "ef_library_add": (_I, [_VP, _VP, ctypes.c_uint64, _VP, _VP, ctypes.POINTER(_I)]),
+    "ef_library_command": (_I, [_VP, _I, _I, _I, _I, ctypes.c_int64]),
+    "ef_library_submit": (_I, [_VP, ctypes.c_uint32, _VP, _VP]),
+    "ef_library_info": (_I, [_VP, _I, _I, _VP]),
 }
+
+# ef_library_command's commands and ef_library_info's stream states (include/espflix_b200.h)
+LIB_PLAY_AT, LIB_PLAY, LIB_SKIP, LIB_FAST_FORWARD, LIB_REWIND, LIB_PAUSE, LIB_RESUME, LIB_STOP = range(8)
+LIB_IDLE, LIB_PLAYING, LIB_PAUSED, LIB_STOPPED, LIB_ENDED = range(5)
+LIBRARY_STATUS = np.dtype([("title", "<i4"), ("speed", "<i4"), ("state", "<i4"), ("file", "<i4"), ("cursor", "<u8"), ("pos", "<i8")])
 
 
 def load_library():
@@ -515,6 +524,37 @@ class Context:
         flags = np.zeros(max(count, 1), dtype=np.uint8)
         self._check(self.lib.ef_carry_info(self._h, first, count, held.ctypes.data, flags.ctypes.data))
         return held[:count], flags[:count]
+
+    # -- titles held in device memory ---------------------------------------------------------------
+    def library_add(self, idx, main, fwd=None, rwd=None):
+        """ef_library_add: copy one title to device memory -> its number. idx: the video.idx image; main / fwd / rwd: its
+        transport streams (video.ts, video_fwd.ts, video_rwd.ts; the trick files may be None)"""
+        keep = [None if f is None or len(f) == 0 else np.frombuffer(bytes(f), dtype=np.uint8) for f in (rwd, main, fwd)]
+        ptrs = (ctypes.c_void_p * 3)(*[None if a is None else a.ctypes.data for a in keep])
+        sizes = (ctypes.c_uint64 * 3)(*[0 if a is None else a.size for a in keep])
+        im = np.frombuffer(bytes(idx), dtype=np.uint8)
+        t = _I()
+        self._check(self.lib.ef_library_add(self._h, im.ctypes.data if im.size else None, im.size, ptrs, sizes, ctypes.byref(t)))
+        return t.value
+
+    def library_command(self, cmd, first=0, count=1, title=0, arg=0):
+        """ef_library_command: cmd (LIB_PLAY_AT ... LIB_STOP) on streams [first, first + count); title and arg (main pts for
+        PLAY_AT, seconds for SKIP) as the header describes"""
+        self._check(self.lib.ef_library_command(self._h, first, count, int(cmd), int(title), int(arg)))
+
+    def library_submit(self, packets=0, per_stream=None, stream=0):
+        """ef_library_submit: a TS submit of every PLAYING stream's next min(budget, packets left) packets; per_stream: one
+        budget per stream (else `packets` for all)"""
+        ps = None if per_stream is None else np.ascontiguousarray(np.broadcast_to(per_stream, (self.n_streams,)), dtype=np.uint32)
+        st = getattr(stream, "cuda_stream", stream)
+        self._check(self.lib.ef_library_submit(self._h, int(packets), _ptr(ps), st))
+
+    def library_info(self, first=0, count=None):
+        """ef_library_info -> LIBRARY_STATUS rows (title, speed, state, file, cursor, pos) of streams [first, first + count)"""
+        count = self.n_streams - first if count is None else count
+        out = np.zeros(max(count, 1), dtype=LIBRARY_STATUS)
+        self._check(self.lib.ef_library_info(self._h, first, count, out.ctypes.data))
+        return out[:count]
 
     def launch_count(self):
         return int(self.lib.ef_launch_count(self._h))

@@ -73,7 +73,13 @@ __global__ void ef_clock_kernel(EfClockState* clk, const EfOverlayState* ovl, Ef
                                 const uint32_t* n_pics, const int64_t* pts_last, int pic, int max_pictures, const uint8_t* font, const int16_t* rights);
 cudaError_t ef_launch_clock_commit(EfClockState* clk, const EfOverlayState* ovl_clk, const uint8_t* bm, uint8_t* slots, int n_streams, const int* chain,
                                    cudaStream_t stream);
+cudaError_t ef_launch_library_resolve(EfLibStream* ls, const EfLibTitle* titles, const int64_t* pts_last, int first, int count, int cmd, int title,
+                                      int64_t arg);
+cudaError_t ef_launch_library_gather(EfLibStream* ls, const EfLibTitle* titles, const uint32_t* budget, uint32_t packets, int n_streams,
+                                     const uint8_t** src, uint64_t* off, uint8_t* end, uint8_t* dst, uint64_t max_bytes, cudaStream_t st,
+                                     uint64_t* launches);
 static_assert(sizeof(idx_hdr) == 104, "video.idx header: the reference's idx_hdr");
+static_assert(sizeof(EfLibStream) == sizeof(ef_library_status), "EfLibStream mirrors ef_library_status");
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
 
 namespace {
@@ -362,6 +368,18 @@ struct ef_ctx {
     int64_t* d_pts_hold = nullptr;                // [n_streams] EfCarryArgs::pts_hold
     int64_t* d_pts_pre = nullptr;                 // [n_streams] EfCarryArgs::pts_pre
     cudaEvent_t ev_scanned = nullptr;             // the last ef_index has written d_held (and resolved the held picture's pts)
+    // the title library (ef_library_*): allocated by the first ef_library_add; until then nothing of it exists
+    std::vector<EfLibTitle> lib_titles;           // host copies of the titles' records
+    EfLibTitle* d_lib_titles = nullptr;           // [lib_cap]
+    size_t lib_cap = 0;
+    EfLibStream* d_lib = nullptr;                 // [n_streams] every stream's title, speed, state, file, cursor and pos
+    uint8_t* d_lib_stage = nullptr;               // [es_capacity + 64] the gathered TS of a library submit
+    const uint8_t** d_lib_src = nullptr;          // [n_streams] where each stream's run starts
+    uint64_t* d_lib_off = nullptr;                // [n_streams + 1] each stream's run in the staging buffer
+    uint8_t* d_lib_end = nullptr;                 // [n_streams] the streams the submit ends
+    uint32_t* d_lib_budget = nullptr;             // [n_streams] per-stream packet budgets of a submit
+    cudaEvent_t ev_lib_staged = nullptr;          // the upload has copied the staging buffer
+    bool lib_submit = false;                      // the pending submit is a library submit (its ends are the library's)
 };
 
 namespace {
@@ -667,26 +685,26 @@ int ef_reset(ef_ctx* c)
     return EF_OK;
 }
 
-// Per-stream restart between the current submit and the next one (queued or not). Synchronous: everything already
-// queued on the device (a resolve pass, a queued submit's demux) has finished before the state changes.
-int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
+// When a restart may fall between the current submit and the next one: every picture index of the current submit presented, and
+// its audio consumed (EF_ESTATE otherwise). `what` names the caller in the message.
+static int restart_ready(ef_ctx* c, const char* what)
 {
-    DeviceScope scope_(c ? c->cfg.device : -1);
-    if (!c) return fail(EF_EINVAL, "null context");
-    const int n = c->cfg.n_streams;
-    TRY(stream_range(c, first, count, ops));
-    bool any_reset = false;
-    for (int i = 0; i < count; i++) {
-        if (ops[i] > 2) return fail(EF_EINVAL, "op %d of stream %d is not 0..2", ops[i], first + i);
-        any_reset |= ops[i] == 1;
-    }
     TRY(pace_resolve(c));
     if (c->paced && c->pace_indexed) {                    // the schedule of the current submit must be complete
         TRY(pace_pictures(c));
-        if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "ef_restart_streams while pictures %d..%d of the current submit are not presented", c->pace_next, c->pace_npics - 1);
+        if (c->pace_next < c->pace_npics) return fail(EF_ESTATE, "%s while pictures %d..%d of the current submit are not presented", what, c->pace_next, c->pace_npics - 1);
     }
     TRY(audio_resolve(c));
-    if (c->audio && c->aud_unconsumed) return fail(EF_ESTATE, "ef_restart_streams before ef_decode_audio consumed the current submit's audio");
+    if (c->audio && c->aud_unconsumed) return fail(EF_ESTATE, "%s before ef_decode_audio consumed the current submit's audio", what);
+    return EF_OK;
+}
+
+// The restart itself (ops checked, restart_ready passed): ef_restart_streams and ef_library_command
+static int restart_apply(ef_ctx* c, int first, int count, const uint8_t* ops)
+{
+    const int n = c->cfg.n_streams;
+    bool any_reset = false;
+    for (int i = 0; i < count; i++) any_reset |= ops[i] == 1;
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     const bool audio = c->audio && any_reset;
@@ -713,6 +731,19 @@ int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
     }
     CK(cudaDeviceSynchronize());
     return EF_OK;
+}
+
+// Per-stream restart between the current submit and the next one (queued or not). Synchronous: everything already
+// queued on the device (a resolve pass, a queued submit's demux) has finished before the state changes.
+int ef_restart_streams(ef_ctx* c, int first, int count, const uint8_t* ops)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    TRY(stream_range(c, first, count, ops));
+    for (int i = 0; i < count; i++)
+        if (ops[i] > 2) return fail(EF_EINVAL, "op %d of stream %d is not 0..2", ops[i], first + i);
+    TRY(restart_ready(c, "ef_restart_streams"));
+    return restart_apply(c, first, count, ops);
 }
 
 // Uploads go to the BACK elementary-stream buffer on the context's own upload stream, so that a
@@ -837,6 +868,7 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
     c->es_bytes = total;                        // for TS input an upper bound; the exact ES size is on the device
     c->pending = b;
     c->submitted = true; c->indexed = false;
+    c->lib_submit = false;
     return EF_OK;
 }
 
@@ -958,6 +990,7 @@ int ef_end_streams(ef_ctx* c, int first, int count, const uint8_t* ends)
     TRY(stream_range(c, first, count, ends));
     if (!c->carry) return fail(EF_ESTATE, "ef_end_streams before ef_carry_enable");
     if (c->pending < 0) return fail(EF_ESTATE, "ef_end_streams with no submit pending");
+    if (c->lib_submit) return fail(EF_ESTATE, "ef_end_streams on an ef_library_submit: the library ends its streams itself");
     if (!count) return EF_OK;
     const int p = c->pending;
     std::vector<uint8_t>& h = c->h_end2[p];
@@ -2087,6 +2120,150 @@ int ef_present_clock(ef_ctx* c, int first, int count, const uint8_t* idx_hdrs, c
         if (flags[i] & 4u) k.last_seconds = 0;
     }
     CK(cudaMemcpy(c->d_clk + first, st.data(), (size_t)count * sizeof(EfClockState), cudaMemcpyHostToDevice));
+    return EF_OK;
+}
+
+// ---- titles held in device memory: the reference's Streamer (espflix.cpp:723-747) and ESPFlix's navigation (espflix.cpp:787-859) --
+int ef_library_add(ef_ctx* c, const uint8_t* idx, uint64_t idx_bytes, const uint8_t* const* ts, const uint64_t* bytes, int* title)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !idx || !ts || !bytes || !title) return fail(EF_EINVAL, "null argument");
+    if (idx_bytes < sizeof(idx_hdr) || idx_bytes >> 32) return fail(EF_EINVAL, "video.idx of %llu bytes: a header of 104 bytes and below 4 GiB", (unsigned long long)idx_bytes);
+    idx_hdr h;
+    memcpy(&h, idx, sizeof(h));
+    if (h.sig != 0x00584449u || h.len != 3) return fail(EF_EINVAL, "video.idx: signature %08x and %u records, not 'IDX' and 3", h.sig, h.len);
+    if (!ts[1] || !bytes[1]) return fail(EF_EINVAL, "the title needs its main file (video.ts)");
+    for (int f = 0; f < 3; f++) {
+        if (!ts[f] != !bytes[f]) return fail(EF_EINVAL, "file %d: a pointer and a size, or neither", f);
+        if (bytes[f] % 188 || bytes[f] >> 32) return fail(EF_EINVAL, "file %d of %llu bytes: whole 188-byte packets below 4 GiB", f, (unsigned long long)bytes[f]);
+    }
+    const uint64_t samples = (uint64_t)h.video.sample_count + h.fwd.sample_count + h.rev.sample_count;
+    if (sizeof(idx_hdr) + 4 * samples > idx_bytes) return fail(EF_EINVAL, "video.idx: %llu samples run past its %llu bytes", (unsigned long long)samples, (unsigned long long)idx_bytes);
+    if (!h.video.bin_size || !h.video.sample_count) return fail(EF_EINVAL, "video.idx: the video record has bin_size %u and %u samples", h.video.bin_size, h.video.sample_count);
+    const idx_rec* trick[2] = { &h.rev, &h.fwd };
+    for (int k = 0; k < 2; k++) {
+        const idx_rec& r = *trick[k];
+        if (ts[2 * k] && (!r.trick_speed || !r.bin_size || !r.sample_count || r.last_pts == r.first_pts))
+            return fail(EF_EINVAL, "video.idx: the %s record (trick_speed %u, bin_size %u, %u samples, pts %lld..%lld) cannot be played", k ? "fwd" : "rwd",
+                        r.trick_speed, r.bin_size, r.sample_count, (long long)r.first_pts, (long long)r.last_pts);
+    }
+    const int n = c->cfg.n_streams;
+    if (!c->d_lib) {                                      // the first title: every stream's state, the staging buffer of the submits
+        TRY(dev_alloc(c, &c->d_lib, (size_t)n));
+        TRY(dev_alloc(c, &c->d_lib_stage, c->cfg.es_capacity + 64));
+        TRY(dev_alloc(c, &c->d_lib_src, (size_t)n)); TRY(dev_alloc(c, &c->d_lib_off, (size_t)n + 1));
+        TRY(dev_alloc(c, &c->d_lib_end, (size_t)n)); TRY(dev_alloc(c, &c->d_lib_budget, (size_t)n));
+        TRY(event(c, &c->ev_lib_staged));
+        CK(cudaEventRecord(c->ev_lib_staged, 0));
+        std::vector<EfLibStream> idle((size_t)n, EfLibStream{ -1, 0, EF_LIB_IDLE, 1, 0, 0 });
+        CK(cudaMemcpy(c->d_lib, idle.data(), (size_t)n * sizeof(EfLibStream), cudaMemcpyHostToDevice));
+    }
+    if (c->lib_titles.size() == c->lib_cap) {
+        const size_t cap = c->lib_cap ? 2 * c->lib_cap : 16;
+        CK(cudaDeviceSynchronize());                      // a command or a submit may still read the title table
+        TRY(dev_grow(c, &c->d_lib_titles, c->lib_cap, cap, c->lib_cap > 0));
+        c->lib_cap = cap;
+    }
+    EfLibTitle t;
+    memset(&t, 0, sizeof(t));
+    uint8_t* p = nullptr;
+    TRY(dev_alloc(c, &p, idx_bytes));
+    CK(cudaMemcpy(p, idx, idx_bytes, cudaMemcpyHostToDevice));
+    t.idx = p; t.idx_bytes = (uint32_t)idx_bytes;
+    for (int f = 0; f < 3; f++) {
+        if (!bytes[f]) continue;
+        TRY(dev_alloc(c, &p, bytes[f]));
+        CK(cudaMemcpy(p, ts[f], bytes[f], cudaMemcpyHostToDevice));
+        t.ts[f] = p; t.bytes[f] = (uint32_t)bytes[f];
+    }
+    t.v_first = h.video.first_pts; t.v_last = h.video.last_pts; t.f_first = h.fwd.first_pts; t.f_last = h.fwd.last_pts;
+    t.r_first = h.rev.first_pts; t.r_last = h.rev.last_pts;
+    t.v_bin = h.video.bin_size; t.f_bin = h.fwd.bin_size; t.r_bin = h.rev.bin_size;
+    t.f_trick = h.fwd.trick_speed; t.r_trick = h.rev.trick_speed;
+    t.v_n = h.video.sample_count; t.f_n = h.fwd.sample_count; t.r_n = h.rev.sample_count;
+    CK(cudaMemcpy(c->d_lib_titles + c->lib_titles.size(), &t, sizeof(t), cudaMemcpyHostToDevice));
+    *title = (int)c->lib_titles.size();
+    c->lib_titles.push_back(t);
+    return EF_OK;
+}
+
+// The state that commands and submits need: a title loaded, PTS (get_pts()) and carry (submits cut at any packet) enabled
+static int library_ready(ef_ctx* c, const char* what)
+{
+    if (!c->d_lib) return fail(EF_ESTATE, "%s before the first ef_library_add", what);
+    if (!c->pts || !c->carry) return fail(EF_ESTATE, "%s needs ef_pts_enable and ef_carry_enable", what);
+    return EF_OK;
+}
+
+int ef_library_command(ef_ctx* c, int first, int count, int cmd, int title, int64_t arg)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    TRY(library_ready(c, "ef_library_command"));
+    TRY(stream_range(c, first, count));
+    if (cmd < EF_LIB_PLAY_AT || cmd > EF_LIB_STOP) return fail(EF_EINVAL, "unknown command %d", cmd);
+    if (cmd == EF_LIB_PLAY_AT && (title < 0 || (size_t)title >= c->lib_titles.size())) return fail(EF_EINVAL, "unknown title %d", title);
+    if (cmd == EF_LIB_SKIP && (arg < INT32_MIN || arg > INT32_MAX)) return fail(EF_EINVAL, "skip of %lld seconds is not an int", (long long)arg);
+    TRY(restart_ready(c, "ef_library_command"));
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());                          // a library submit may still move the cursors
+    std::vector<EfLibStream> st((size_t)count);
+    CK(cudaMemcpy(st.data(), c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < count; i++) {
+        const EfLibStream& v = st[(size_t)i];
+        if (cmd == EF_LIB_PLAY_AT) continue;
+        if (v.state == EF_LIB_IDLE) return fail(EF_EINVAL, "stream %d has never played: start it with EF_LIB_PLAY_AT", first + i);
+        if (cmd == EF_LIB_RESUME && v.state != EF_LIB_PAUSED) return fail(EF_EINVAL, "EF_LIB_RESUME on stream %d, which is not paused", first + i);
+        const EfLibTitle& t = c->lib_titles[(size_t)v.title];
+        if ((cmd == EF_LIB_FAST_FORWARD && !t.ts[2]) || (cmd == EF_LIB_REWIND && !t.ts[0]))
+            return fail(EF_EINVAL, "stream %d: title %d has no %s file", first + i, v.title, cmd == EF_LIB_REWIND ? "rewind" : "fast-forward");
+    }
+    CK(ef_launch_library_resolve(c->d_lib, c->d_lib_titles, c->d_pts_last, first, count, cmd, title, arg));
+    c->launches++;
+    const uint8_t op = cmd <= EF_LIB_REWIND ? 1 : cmd == EF_LIB_RESUME ? 2 : 0;   // play(): reset + video_reset; video_pause(0)
+    if (op) {
+        const std::vector<uint8_t> ops((size_t)count, op);
+        return restart_apply(c, first, count, ops.data());
+    }
+    CK(cudaDeviceSynchronize());
+    return EF_OK;
+}
+
+int ef_library_submit(ef_ctx* c, uint32_t packets, const uint32_t* per_stream, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    TRY(library_ready(c, "ef_library_submit"));
+    if (c->pending >= 0) return fail(EF_ESTATE, "ef_library_submit with a submit pending: ef_index it first");
+    const int n = c->cfg.n_streams;
+    uint64_t bound = 0;                                   // packets the submit can hold at most, known without reading the device
+    if (per_stream) for (int i = 0; i < n; i++) bound += per_stream[i];
+    else bound = (uint64_t)n * packets;
+    if (bound * 188 > c->cfg.es_capacity)
+        return fail(EF_ENOMEM, "a library submit of up to %llu packets exceeds es_capacity %zu", (unsigned long long)bound, c->cfg.es_capacity);
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(cudaStreamWaitEvent(st, c->ev_lib_staged, 0));   // the upload of the previous library submit has copied the staging buffer
+    if (per_stream) CK(cudaMemcpyAsync(c->d_lib_budget, per_stream, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    CK(ef_launch_library_gather(c->d_lib, c->d_lib_titles, per_stream ? c->d_lib_budget : nullptr, packets, n, c->d_lib_src, c->d_lib_off,
+                                c->d_lib_end, c->d_lib_stage, bound * 188, st, &c->launches));
+    TRY(submit_common(c, c->d_lib_stage, c->d_lib_off, false, true, st));
+    const int b = c->pending;                             // the streams whose file ends with this submit, as ef_end_streams marks them
+    CK(cudaMemcpyAsync(c->d_end2[b], c->d_lib_end, (size_t)n, cudaMemcpyDeviceToDevice, c->up_stream));
+    CK(cudaEventRecord(c->ev_up_done[b], c->up_stream));
+    CK(cudaEventRecord(c->ev_lib_staged, c->up_stream));
+    c->lib_submit = true;
+    return EF_OK;
+}
+
+int ef_library_info(ef_ctx* c, int first, int count, ef_library_status* status)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->d_lib) return fail(EF_ESTATE, "ef_library_info before the first ef_library_add");
+    TRY(stream_range(c, first, count, status));
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(status, c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
     return EF_OK;
 }
 

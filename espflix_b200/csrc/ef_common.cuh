@@ -257,6 +257,43 @@ struct __align__(16) EfClockState {
     uint32_t pad[3];
 };
 
+// idx_hdr::pts2pts (espflix.cpp:589-604): a pts of the stream played at `speed` (0 the title, 1 the fast-forward stream, -1 the
+// rewind stream) on the title's main timeline, from the video.idx records (first, last) of the main stream (v), fwd (f) and rwd (r).
+// int64 throughout, truncating division; a trick record whose last_pts equals its first_pts divides by zero (callers refuse it).
+static inline __host__ __device__ int64_t ef_pts2pts(int64_t pts, int speed, int64_t v_first, int64_t v_last, int64_t f_first, int64_t f_last,
+                                                     int64_t r_first, int64_t r_last)
+{
+    if (speed == 1) return v_first + (pts - f_first) * (v_last - v_first) / (f_last - f_first);
+    if (speed == -1) return v_last - (pts - r_first) * (v_last - v_first) / (r_last - r_first);
+    return pts;
+}
+
+// The title library (ef_library_*, ef_library.cu): titles held in device memory and every stream's place in one of them.
+// A title is its video.idx image and its three transport streams in the reference's _vid_names order (espflix.cpp:641):
+// 0 video_rwd.ts, 1 video.ts, 2 video_fwd.ts; a missing trick file has ts NULL and bytes 0. Stream states and commands: EF_LIB_* of
+// include/espflix_b200.h.
+struct __align__(16) EfLibTitle {
+    const uint8_t* idx;          // the video.idx image: idx_hdr (104 bytes), then the main, fwd and rwd sample arrays (uint32)
+    const uint8_t* ts[3];
+    uint32_t bytes[3];           // file sizes, multiples of 188 below 4 GiB
+    uint32_t idx_bytes;
+    int64_t v_first, v_last, f_first, f_last, r_first, r_last;   // the header's records
+    uint32_t v_bin, f_bin, r_bin, f_trick, r_trick, v_n, f_n, r_n;
+};
+struct __align__(16) EfLibStream {   // layout of ef_library_status (include/espflix_b200.h)
+    int32_t title;               // -1 before the first PLAY_AT
+    int32_t speed;               // _speed: -1, 0, 1
+    int32_t state;               // EF_LIB_IDLE ... EF_LIB_ENDED
+    int32_t file;                // speed + 1: the file the cursor is in
+    uint64_t cursor;             // byte offset of the next packet in that file
+    int64_t pos;                 // _info[_nav].pos: the main pts the next PLAY, SKIP, FAST_FORWARD or REWIND starts from
+};
+
+static inline __host__ __device__ int64_t ef_lib_pts2pts(const EfLibTitle& t, int64_t pts, int speed)
+{
+    return ef_pts2pts(pts, speed, t.v_first, t.v_last, t.f_first, t.f_last, t.r_first, t.r_last);
+}
+
 static inline __host__ __device__ int ef_overlay_blend(int32_t b, uint32_t blend_fc, uint32_t fc)
 {
     const uint32_t d = fc - blend_fc;    // fields since the latch, modulo 2^32

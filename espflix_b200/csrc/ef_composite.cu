@@ -628,9 +628,7 @@ ef_clock_kernel(EfClockState* __restrict__ clk, const EfOverlayState* __restrict
         int draw = 0;
         if (k.flags & 1u) {
             const int64_t pts = pic >= 0 && (uint32_t)pic < n_pics[s] ? pic_pts[(size_t)s * max_pictures + pic] : pts_last[s];
-            int64_t main = pts;                                            // idx_hdr::pts2pts
-            if (k.speed == 1) main = k.v_first + (pts - k.f_first) * (k.v_last - k.v_first) / (k.f_last - k.f_first);
-            else if (k.speed == -1) main = k.v_last - (pts - k.r_first) * (k.v_last - k.v_first) / (k.r_last - k.r_first);
+            const int64_t main = ef_pts2pts(pts, k.speed, k.v_first, k.v_last, k.f_first, k.f_last, k.r_first, k.r_last);
             const int seconds = (int)(main / 90000);
             draw = seconds != k.last_seconds;
             v.p_progress = (int)(main * 240 / k.v_last);                   // VIDEO_COMPOSITE_PROGRESS_WIDTH

@@ -59,6 +59,9 @@
  *   ef_carry_enable / ef_end_streams / ef_carry_info  the decoder pulling bytes on demand across the producer's Buffers
  *                                 (FILL_BITS -> more(), player.cpp:348-352, 459-493; espflix.cpp:723-737): TS submits cut at any
  *                                 packet boundary, and the len <= 0 Buffer that ends a stream (player.cpp:456, 469-473)
+ *   ef_library_add / _command / _submit / _info  Streamer::get() + read() of a title (espflix.cpp:723-747) and ESPFlix's play, skip,
+ *                                 fast_forward, rewind, play_pause, get_index and save_pos (espflix.cpp:787-859): titles in HBM, every
+ *                                 stream's seek resolved from video.idx and its bytes gathered on the device
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -476,6 +479,67 @@ int ef_restart_streams(ef_ctx* ctx, int first, int count, const uint8_t* ops);
 int ef_carry_enable(ef_ctx* ctx, uint32_t max_carry);
 int ef_end_streams(ef_ctx* ctx, int first, int count, const uint8_t* ends);
 int ef_carry_info(ef_ctx* ctx, int first, int count, uint32_t* held_bytes, uint8_t* flags);
+
+/* ---- titles held in device memory: the reference's Streamer and ESPFlix's play / skip / fast_forward / rewind / pause ------------
+ * The reference reads a title through Streamer::get(url, offset) and 8-packet Buffers (espflix.cpp:723-747, 787-798) and seeks with
+ * the uint32 packet number that video.idx holds at idx_hdr::pts2offset(pts, speed) (get_index, espflix.cpp:607-629, 823-829). Here
+ * the titles live in HBM: a viewer's action is a few bytes from the host, and no TS byte crosses the host link again.
+ * ef_library_add      copies one title to device memory: its video.idx image (idx_hdr, host/ef_indexer.h, then the main, fwd and rwd
+ *                     sample arrays) and its three transport streams in _vid_names order (espflix.cpp:641): ts[0] video_rwd.ts,
+ *                     ts[1] video.ts, ts[2] video_fwd.ts; the trick files may be NULL / 0. *title = its number (0, 1, ...). Titles stay
+ *                     until ef_destroy. The first call allocates every stream's state and a staging buffer of es_capacity bytes.
+ *                     EF_EINVAL: a bad sig or len != 3; samples past the end of the image; a video record with bin_size or
+ *                     sample_count 0; a present trick file whose record has trick_speed, bin_size or sample_count 0 or last_pts ==
+ *                     first_pts (the reference divides by zero there); no main file; a file size that is not a multiple of 188 or is
+ *                     >= 4 GiB, or an image >= 4 GiB (the offset arithmetic is uint32).
+ * ef_library_command  cmd for every stream of [first, first + count): the ESPFlix methods (espflix.cpp:800-859), with the restart op
+ *                     each one implies run as ef_restart_streams runs it (same EF_ESTATE cases):
+ *                       EF_LIB_PLAY_AT (title, arg = main pts)  nav(title) with pos = arg, then play_pause() from NAV        op 1
+ *                       EF_LIB_PLAY                             play(nav, 0, get_index(0, pos) * 188)                          op 1
+ *                       EF_LIB_SKIP (arg = seconds, an int)     skip(s): pos += s * 90000 (an int product), kept unclamped      op 1
+ *                       EF_LIB_FAST_FORWARD / EF_LIB_REWIND     fast_forward() / rewind(): play at speed +-1 from pos          op 1
+ *                       EF_LIB_PAUSE                            pause: a PLAYING stream becomes PAUSED and gets no more bytes  op 0
+ *                       EF_LIB_RESUME                           video_pause(0): a PAUSED stream plays on from its cursor        op 2
+ *                       EF_LIB_STOP                             menu: the stream gets no more bytes (STOPPED)                   op 0
+ *                     Every command but PLAY_AT and RESUME first saves, on a PLAYING stream, pos = pts2pts(get_pts(), speed)
+ *                     (save_pos, espflix.cpp:843-852), get_pts() being ef_picture_pts's last_pts after the current submit; PAUSED,
+ *                     STOPPED and ENDED streams keep the pos they have. The offset arithmetic and the sample read run on the device,
+ *                     one thread per stream; the host never reads a pts. A sample that names a packet at or past the end of its file
+ *                     puts the cursor there (the reference's uint32 product would wrap only for such samples). Synchronous, host
+ *                     memory. EF_ESTATE before the first ef_library_add or without ef_pts_enable and ef_carry_enable. EF_EINVAL: a bad
+ *                     stream range or command; PLAY_AT of an unknown title; any other command on a stream that never played;
+ *                     FAST_FORWARD / REWIND on a title without that file; RESUME on a stream that is not PAUSED; SKIP outside int.
+ * ef_library_submit   a TS submit made on the device (as ef_submit_ts_device): every PLAYING stream gets min(per_stream[s], or
+ *                     packets when per_stream is NULL, the packets left in its file) packets from its cursor, every other stream
+ *                     none. A stream whose cursor reaches the end of its file ends with this submit (as ef_end_streams ends it) and
+ *                     becomes ENDED with pos = pts2pts(0, speed), what save_pos(0) leaves at DONE (espflix.cpp:906-911): 0 at speed 0.
+ *                     ef_index follows as usual. per_stream is host memory. EF_ESTATE before the first ef_library_add, without
+ *                     ef_pts_enable and ef_carry_enable, or with a submit pending; EF_ENOMEM, nothing changed, when the budgets'
+ *                     packets x 188 exceed es_capacity (a bound the host checks, so nothing is read back but the upload's offsets).
+ *                     ef_end_streams on a library submit returns EF_ESTATE. Launches: a count kernel, a gather kernel (its grid
+ *                     follows the bound) and the TS upload sequence of ef_carry_enable. ef_reset keeps titles, states and cursors
+ *                     (video_reset() leaves the Streamer alone); a library submit it drops is not given again.
+ * ef_library_info     synchronous: status[i] = stream first + i's title (-1 before PLAY_AT), speed, state, file (speed + 1), byte
+ *                     cursor in that file and pos (what save_pos(..., true) writes to NVS). EF_ESTATE before the first
+ *                     ef_library_add; EF_EINVAL for a bad stream range. */
+#define EF_LIB_PLAY_AT      0
+#define EF_LIB_PLAY         1
+#define EF_LIB_SKIP         2
+#define EF_LIB_FAST_FORWARD 3
+#define EF_LIB_REWIND       4
+#define EF_LIB_PAUSE        5
+#define EF_LIB_RESUME       6
+#define EF_LIB_STOP         7
+#define EF_LIB_IDLE    0         /* stream states: never played */
+#define EF_LIB_PLAYING 1
+#define EF_LIB_PAUSED  2
+#define EF_LIB_STOPPED 3
+#define EF_LIB_ENDED   4         /* its cursor reached the end of its file */
+typedef struct { int32_t title, speed, state, file; uint64_t cursor; int64_t pos; } ef_library_status;
+int ef_library_add(ef_ctx* ctx, const uint8_t* idx, uint64_t idx_bytes, const uint8_t* const* ts, const uint64_t* bytes, int* title);
+int ef_library_command(ef_ctx* ctx, int first, int count, int cmd, int title, int64_t arg);
+int ef_library_submit(ef_ctx* ctx, uint32_t packets, const uint32_t* per_stream, void* stream);
+int ef_library_info(ef_ctx* ctx, int first, int count, ef_library_status* status);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
