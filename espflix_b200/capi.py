@@ -101,6 +101,10 @@ _SIGNATURES = {
     "ef_library_command": (_I, [_VP, _I, _I, _I, _I, ctypes.c_int64]),
     "ef_library_submit": (_I, [_VP, ctypes.c_uint32, _VP, _VP]),
     "ef_library_info": (_I, [_VP, _I, _I, _VP]),
+    "ef_trick_build": (_I, [_I, _VP, _VP, _I, _I, _VP, ctypes.c_uint64, _VP, _VP, ctypes.c_uint64, _VP]),
+    "ef_trick_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 4),
+    "ef_library_add_trick": (_I, [_VP, _I, _I]),
+    "ef_library_read": (_I, [_VP, _I, _I, _VP, ctypes.c_uint64, _U64P]),
 }
 
 # ef_library_command's commands and ef_library_info's stream states (include/espflix_b200.h)
@@ -537,6 +541,22 @@ class Context:
         self._check(self.lib.ef_library_add(self._h, im.ctypes.data if im.size else None, im.size, ptrs, sizes, ctypes.byref(t)))
         return t.value
 
+    def library_add_trick(self, title, qscale=None):
+        """ef_library_add_trick: build the fast-forward and rewind files of a title added with its main only, attach them and
+        rewrite the fwd and rwd records and samples of its video.idx (qscale None: TRICK_QSCALE)"""
+        self._check(self.lib.ef_library_add_trick(self._h, int(title), TRICK_QSCALE if qscale is None else int(qscale)))
+
+    def library_read(self, title, what):
+        """ef_library_read: a title's video.idx image (what -1) or its rwd / main / fwd file (0 / 1 / 2) as bytes (b"" when absent)"""
+        n = ctypes.c_uint64()
+        rc = self.lib.ef_library_read(self._h, int(title), int(what), None, 0, ctypes.byref(n))
+        if rc != EF_ENOMEM:
+            self._check(rc)
+            return b""
+        out = np.zeros(n.value, dtype=np.uint8)
+        self._check(self.lib.ef_library_read(self._h, int(title), int(what), out.ctypes.data, out.size, ctypes.byref(n)))
+        return out.tobytes()
+
     def library_command(self, cmd, first=0, count=1, title=0, arg=0):
         """ef_library_command: cmd (LIB_PLAY_AT ... LIB_STOP) on streams [first, first + count); title and arg (main pts for
         PLAY_AT, seconds for SKIP) as the header describes"""
@@ -614,6 +634,36 @@ def tsidx_samples(seq_pts, seq_pos, first_pts, last_pts, bin_size=IDX_BIN, devic
     _check_rc(lib, lib.ef_tsidx_samples(device, seq_pts.ctypes.data, seq_pos.ctypes.data, len(seq_pts), first_pts, last_pts, bin_size,
                                         out.ctypes.data, cap, ctypes.byref(n)))
     return out[:n.value].copy()
+
+
+TRICK_QSCALE = 8                 # ef_trick_build's default quantiser scale (tests/trick_cases.DEFAULT_QSCALE)
+
+
+def trick_build(mains, qscale=TRICK_QSCALE, device=0):
+    """ef_trick_build: video_fwd.ts and video_rwd.ts of every main (bytes-like transport streams) -> [(fwd bytes, rwd bytes), ...]"""
+    lib = load_library()
+    blob, off = Context.pack(mains)
+    n = len(mains)
+    fo, ro = np.zeros(n + 1, dtype=np.uint64), np.zeros(n + 1, dtype=np.uint64)
+    cap = int(off[-1]) + 188 * 1024          # intra pictures at 1/15 of the rate: the main's size is a generous first guess
+    for _ in range(2):
+        fwd, rwd = np.zeros(cap, dtype=np.uint8), np.zeros(cap, dtype=np.uint8)
+        rc = lib.ef_trick_build(device, blob.ctypes.data, off.ctypes.data, n, int(qscale), fwd.ctypes.data, fwd.size, fo.ctypes.data,
+                                rwd.ctypes.data, rwd.size, ro.ctypes.data)
+        need = max(int(fo[-1]), int(ro[-1]))
+        if rc != EF_ENOMEM or need <= cap:
+            break
+        cap = need
+    _check_rc(lib, rc)
+    return [(fwd[int(fo[i]):int(fo[i + 1])].tobytes(), rwd[int(ro[i]):int(ro[i + 1])].tobytes()) for i in range(n)]
+
+
+def trick_stage_ms():
+    """(decode, gather, encode, mux) device milliseconds of the last trick_build on this thread"""
+    lib = load_library()
+    v = [ctypes.c_float() for _ in range(4)]
+    _check_rc(lib, lib.ef_trick_stage_ms(*[ctypes.byref(x) for x in v]))
+    return tuple(x.value for x in v)
 
 
 def idct_tc_run(coefs, L, repeats=5, device=0):

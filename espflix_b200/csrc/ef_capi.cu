@@ -35,6 +35,12 @@ __global__ void ef_pts_packet_kernel(const uint8_t* ts, const uint64_t* ts_off, 
 size_t ef_recon_smem_bytes();
 cudaError_t ef_decode_configure();
 int ef_decode_resident_ctas(int which);
+cudaError_t ef_trick_upload_tables();
+cudaError_t ef_trick_launch_gather(const uint8_t* frames, const uint32_t* streams, const uint32_t* slots, int count, int fb, uint8_t* dst, cudaStream_t st);
+cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st);
+cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int n_pics,
+                                     uint8_t* es, cudaStream_t st);
+cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st);
 __global__ void ef_tsidx_packet_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, int64_t* pkt_pts, uint8_t* pkt_kind);
 __global__ void ef_tsidx_compact_kernel(const uint64_t* pkt_off, const int64_t* pkt_pts, const uint8_t* pkt_kind, int64_t* seq_pts, uint32_t* seq_pos, int64_t* info);
 __global__ void ef_tsidx_sample_kernel(const int64_t* seq_pts, const uint32_t* seq_pos, int n, int64_t first_pts, uint32_t bin_size, uint32_t n_samples, uint32_t* samples);
@@ -1068,13 +1074,16 @@ static int decode_recon(ef_ctx* c, int i, cudaStream_t st)
 // K1a over picture indices [p0, p0 + k), then K1b once per picture index. host_dst != nullptr: every picture index
 // is exported (I420) straight after its K1b launch and copied to host_dst[p][stream] on the read-back stream while
 // the next picture index is being rebuilt - what push_video() sees, picture by picture (video.h:49).
-static int decode_range(ef_ctx* c, int p0, int k, cudaStream_t st, uint8_t* host_dst = nullptr, int layout = 0)
+// after (optional) runs after the K1b launch of every picture index (ef_trick_build gathers the frames it encodes).
+static int decode_range(ef_ctx* c, int p0, int k, cudaStream_t st, uint8_t* host_dst = nullptr, int layout = 0,
+                        int (*after)(void*, int, cudaStream_t) = nullptr, void* after_arg = nullptr)
 {
     DeviceScope scope_(c ? c->cfg.device : -1);
     TRY(decode_parse(c, p0, k, st));
     const size_t batch_bytes = (size_t)c->cfg.n_streams * EF_FRAME;
     for (int i = 0; i < k; i++) {
         TRY(decode_recon(c, i, st));
+        if (after) TRY(after(after_arg, p0 + i, st));
         if (host_dst) {
             const int b = c->stage_idx ^= 1;
             TRY(ensure_stage2(c, b, batch_bytes));
@@ -2264,6 +2273,476 @@ int ef_library_info(ef_ctx* c, int first, int count, ef_library_status* status)
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(status, c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
+    return EF_OK;
+}
+
+}  // extern "C"
+
+// ---- trick streams: video_fwd.ts and video_rwd.ts of many mains (csrc/ef_trick.cu; the rule is tests/trick_cases.py) --------------
+namespace {
+
+constexpr int kTrickSpeed = 15;                  // merge_index's trick_speed
+constexpr int kTrickChunkStreams = 256;          // segments decoded in one batch (about 2.2 MB of device memory each)
+constexpr uint64_t kTrickChunkBytes = 64u << 20; // TS bytes of one batch (a longer segment is a batch of its own)
+constexpr int kTrickEncodeBatch = 256;           // pictures per encode launch (26 MB of frames, 90 MB of slice regions)
+
+struct GrowBuf {                                 // device buffer that keeps its contents when it grows
+    uint8_t* p = nullptr;
+    size_t cap = 0;
+    ~GrowBuf() { if (p) cudaFree(p); }
+    cudaError_t reserve(size_t n, size_t keep = 0)
+    {
+        if (n <= cap) return cudaSuccess;
+        uint8_t* q = nullptr;
+        cudaError_t e = cudaMalloc(&q, n);
+        if (e != cudaSuccess) return e;
+        if (keep) { e = cudaMemcpy(q, p, keep, cudaMemcpyDeviceToDevice); if (e != cudaSuccess) { cudaFree(q); return e; } }
+        if (p) cudaFree(p);
+        p = q; cap = n;
+        return cudaSuccess;
+    }
+};
+
+// The video ES of the first packets from packet `pkt` on (PID 0x100 payloads, as demux() reads them, player.cpp:381-432), at most
+// `cap` bytes; *pts_ok = packet `pkt` starts a video PES whose PTS parse_pts() accepts (player.cpp:299-306).
+void trick_video_es(const uint8_t* ts, uint64_t pkt, uint64_t end, size_t cap, std::vector<uint8_t>& es, bool* pts_ok)
+{
+    es.clear();
+    *pts_ok = false;
+    for (uint64_t k = pkt; k < end && es.size() < cap; k++) {
+        const uint8_t* d = ts + k * 188;
+        if (d[0] != 0x47 || (((d[1] << 8) | d[2]) & 0x1FFF) != 0x100 || !(d[3] & 0x10)) continue;
+        int o = (d[3] & 0x20) ? 5 + d[4] : 4;
+        if ((d[1] & 0x40) && o + 14 <= 188) {
+            const int flags = (d[o + 6] << 8) | d[o + 7];
+            if (k == pkt) *pts_ok = (flags & 0x80) && (d[o + 9] & 0xF0) == ((flags >> 2) & 0x30);
+            o += 9 + d[o + 8];
+        }
+        if (o < 188) es.insert(es.end(), d + o, d + 188);
+    }
+}
+
+// picture_coding_type of the first picture in es (0: none found)
+int trick_first_picture_type(const std::vector<uint8_t>& es)
+{
+    for (size_t i = 0; i + 5 < es.size(); i++)
+        if (es[i] == 0 && es[i + 1] == 0 && es[i + 2] == 1 && es[i + 3] == 0) return (es[i + 5] >> 3) & 7;
+    return 0;
+}
+
+void trick_bits(std::vector<uint8_t>& out, uint32_t& acc, int& n, uint32_t v, int bits)
+{
+    for (int i = bits - 1; i >= 0; i--) {
+        acc = (acc << 1) | ((v >> i) & 1);
+        if (++n == 8) { out.push_back((uint8_t)acc); acc = 0; n = 0; }
+    }
+}
+
+// sequence header (352 x 192, the main's aspect and picture-rate codes, bit_rate 0x3FFFF, vbv 20, default matrices), closed GOP
+// header, I picture header: tests/trick_cases.header_bytes()
+std::vector<uint8_t> trick_header(int aspect, int rate)
+{
+    std::vector<uint8_t> h = { 0, 0, 1, 0xB3 };
+    uint32_t acc = 0; int n = 0;
+    trick_bits(h, acc, n, 352, 12); trick_bits(h, acc, n, 192, 12); trick_bits(h, acc, n, aspect, 4); trick_bits(h, acc, n, rate, 4);
+    trick_bits(h, acc, n, 0x3FFFF, 18); trick_bits(h, acc, n, 1, 1); trick_bits(h, acc, n, 20, 10); trick_bits(h, acc, n, 0, 3);
+    h.insert(h.end(), { 0, 0, 1, 0xB8 });
+    trick_bits(h, acc, n, 1u << 12, 25); trick_bits(h, acc, n, 1, 1); trick_bits(h, acc, n, 0, 6);
+    h.insert(h.end(), { 0, 0, 1, 0x00 });
+    trick_bits(h, acc, n, 0, 10); trick_bits(h, acc, n, 1, 3); trick_bits(h, acc, n, 0xFFFF, 16); trick_bits(h, acc, n, 0, 3);
+    return h;
+}
+
+struct TrickSeg { int file; uint64_t pkt0, pkt1; };
+
+struct TrickTimer {                              // CUDA event pairs per phase, read once the build has finished
+    std::vector<std::pair<int, std::pair<cudaEvent_t, cudaEvent_t>>> spans;
+    cudaEvent_t open_ev = nullptr;
+    ~TrickTimer() { for (auto& s : spans) { cudaEventDestroy(s.second.first); cudaEventDestroy(s.second.second); } if (open_ev) cudaEventDestroy(open_ev); }
+    cudaError_t begin(cudaStream_t st)
+    {
+        cudaError_t e = cudaEventCreate(&open_ev);
+        return e != cudaSuccess ? e : cudaEventRecord(open_ev, st);
+    }
+    cudaError_t end(int phase, cudaStream_t st)
+    {
+        cudaEvent_t b;
+        cudaError_t e = cudaEventCreate(&b);
+        if (e != cudaSuccess) return e;
+        spans.push_back({ phase, { open_ev, b } });
+        open_ev = nullptr;
+        return cudaEventRecord(b, st);
+    }
+};
+thread_local float g_trick_ms[4] = { 0, 0, 0, 0 };
+
+// the state of one decode batch, for the K1b hook: after picture index p, gather the frames of the selected pictures with that index
+struct TrickGather {
+    ef_ctx* c;
+    const std::vector<uint32_t>* first;          // [p]: first entry of picture index p in the lists
+    const uint32_t* d_streams;
+    const uint32_t* d_slots;
+    uint8_t* d_in;
+    TrickTimer* timer;
+};
+
+int trick_gather(void* arg, int p, cudaStream_t st)
+{
+    TrickGather& g = *(TrickGather*)arg;
+    const std::vector<uint32_t>& f = *g.first;
+    const int count = (int)(f[p + 1] - f[p]);
+    if (!count) return EF_OK;
+    CK(g.timer->end(0, st));
+    CK(g.timer->begin(st));
+    CK(ef_trick_launch_gather(g.c->h.frames, g.d_streams + f[p], g.d_slots + f[p], count, (p + 1) & 1, g.d_in, st));
+    g.c->launches++;
+    CK(g.timer->end(1, st));
+    CK(g.timer->begin(st));
+    return EF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_files, int qscale, uint8_t* fwd, uint64_t fwd_cap, uint64_t* fwd_off,
+                   uint8_t* rwd, uint64_t rwd_cap, uint64_t* rwd_off)
+{
+    if (!off || n_files < 1 || !fwd_off || !rwd_off) return fail(EF_EINVAL, "null argument");
+    if (qscale < 1 || qscale > 31) return fail(EF_EINVAL, "qscale %d outside 1..31", qscale);
+    for (int f = 0; f <= n_files; f++)
+        if (off[f] % 188 || (f && off[f] < off[f - 1])) return fail(EF_EINVAL, "offsets must be non-decreasing multiples of 188");
+    if (off[n_files] > off[0] && !ts) return fail(EF_EINVAL, "null argument");
+    TRY(usable_device(device));
+    DeviceScope scope_(device);
+    const uint8_t* base = ts + off[0];
+    std::vector<uint64_t> poff((size_t)n_files + 1);
+    for (int f = 0; f <= n_files; f++) poff[f] = (off[f] - off[0]) / 188;
+    const uint64_t n_packets = poff[n_files];
+
+    // sequence headers: make_index()'s table (ef_tsidx_scan); cut before each one that starts a PES with a PTS and an I picture
+    std::vector<ef_tsidx_info> info((size_t)n_files);
+    std::vector<int64_t> spts(n_packets + 1);
+    std::vector<uint32_t> spos(n_packets + 1);
+    std::vector<uint64_t> soff(poff.begin(), poff.end());
+    for (auto& o : soff) o *= 188;
+    for (int f = 0; f < n_files; f++) if (poff[f + 1] == poff[f]) return fail(EF_EINVAL, "main %d is empty: it has no sequence header", f);
+    TRY(ef_tsidx_scan(device, base, soff.data(), n_files, 7500, info.data(), spts.data(), spos.data()));
+    std::vector<TrickSeg> segs;
+    std::vector<std::vector<uint8_t>> headers((size_t)n_files);
+    std::vector<uint8_t> es;
+    for (int f = 0; f < n_files; f++) {
+        if (!info[f].n_seq) return fail(EF_EINVAL, "main %d has no sequence header", f);
+        bool ok;
+        trick_video_es(base, poff[f] + spos[poff[f]], poff[f + 1], 16, es, &ok);
+        int i = 0;
+        while (i + 8 <= (int)es.size() && !(es[i] == 0 && es[i + 1] == 0 && es[i + 2] == 1 && es[i + 3] == 0xB3)) i++;
+        if (i + 8 > (int)es.size()) return fail(EF_EINVAL, "main %d: its first sequence header is cut short", f);
+        headers[f] = trick_header(es[i + 7] >> 4, es[i + 7] & 15);
+        segs.push_back({ f, poff[f], poff[f + 1] });
+        for (uint32_t k = 1; k < info[f].n_seq; k++) {
+            const uint64_t p = poff[f] + spos[poff[f] + k];
+            if (p <= segs.back().pkt0) continue;
+            trick_video_es(base, p, poff[f + 1], 4096, es, &ok);
+            if (!ok || trick_first_picture_type(es) != 1) continue;    // joins the segment before it
+            segs.back().pkt1 = p;
+            segs.push_back({ f, p, poff[f + 1] });
+        }
+    }
+
+    // batches of segments
+    std::vector<size_t> chunk = { 0 };
+    for (size_t s = 0; s < segs.size(); s++) {
+        const size_t c0 = chunk.back();
+        if (s > c0 && (s - c0 >= (size_t)kTrickChunkStreams || (segs[s].pkt1 - segs[c0].pkt0) * 188 > kTrickChunkBytes)) chunk.push_back(s);
+    }
+    chunk.push_back(segs.size());
+    int max_streams = 1;
+    uint64_t max_bytes = 188, max_pusi = 1;
+    for (size_t c = 0; c + 1 < chunk.size(); c++) {
+        max_streams = std::max(max_streams, (int)(chunk[c + 1] - chunk[c]));
+        max_bytes = std::max(max_bytes, (segs[chunk[c + 1] - 1].pkt1 - segs[chunk[c]].pkt0) * 188);
+    }
+    for (const TrickSeg& s : segs) {                 // a first guess of the pictures per segment: its video PES starts
+        uint64_t n = 1;
+        for (uint64_t k = s.pkt0; k < s.pkt1; k++) {
+            const uint8_t* d = base + k * 188;
+            n += (d[1] & 0x40) && (((d[1] << 8) | d[2]) & 0x1FFF) == 0x100;
+        }
+        max_pusi = std::max(max_pusi, n);
+    }
+
+    CK(ef_trick_upload_tables());
+    cudaStream_t st = 0;
+    TrickTimer timer;
+    GrowBuf d_ts, d_off, d_list, d_in, d_slots, d_len, d_es, d_dst, d_hdr;
+    CK(d_ts.reserve(n_packets * 188 + 16));
+    CK(cudaMemcpy(d_ts.p, base, n_packets * 188, cudaMemcpyHostToDevice));
+    CK(d_off.reserve(((size_t)max_streams + 1) * 8));
+    int max_pictures = (int)std::min<uint64_t>(max_pusi, 4096);
+    ef_ctx* ctx = nullptr;
+    struct CtxGuard { ef_ctx** c; ~CtxGuard() { if (*c) ef_destroy(*c); } } ctx_guard{ &ctx };
+
+    // every encoded picture: its file, its main pts, where its bytes are in d_es
+    struct Enc { int file; int64_t main_pts; uint64_t es_off; uint32_t es_len; };
+    std::vector<Enc> enc;
+    std::vector<std::vector<uint32_t>> fwd_of((size_t)n_files);   // encoded picture ids of every file's fwd pictures, in order
+    std::vector<uint64_t> seen((size_t)n_files, 0);                 // main pictures of every file so far
+    std::vector<int64_t> p0((size_t)n_files, -1);
+    uint64_t es_total = 0;
+    size_t pending = 0;                                             // gathered, not yet encoded: enc[enc.size() - pending ..)
+    size_t in_cap = 0;
+
+    auto encode_pending = [&]() -> int {
+        if (!pending) return EF_OK;
+        const int n = (int)pending;
+        const size_t e0 = enc.size() - pending;
+        CK(d_slots.reserve((size_t)n * EF_MBH_MAX * kTrickSliceBytes));
+        CK(d_len.reserve((size_t)n * EF_MBH_MAX * 4));
+        CK(timer.begin(st));
+        CK(ef_trick_launch_encode(d_in.p, n, qscale, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
+        std::vector<uint32_t> len((size_t)n * EF_MBH_MAX);
+        CK(cudaMemcpyAsync(len.data(), d_len.p, len.size() * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        std::vector<uint64_t> dst((size_t)n);
+        std::vector<uint8_t> hdr((size_t)n * kTrickHeaderBytes);
+        const uint64_t es0 = es_total;
+        for (int p = 0; p < n; p++) {
+            uint32_t bytes = kTrickHeaderBytes;
+            for (int s = 0; s < EF_MBH_MAX; s++) bytes += len[(size_t)p * EF_MBH_MAX + s];
+            Enc& e = enc[e0 + p];
+            e.es_off = dst[p] = es_total; e.es_len = bytes;
+            es_total += bytes;
+            memcpy(&hdr[(size_t)p * kTrickHeaderBytes], headers[e.file].data(), kTrickHeaderBytes);
+        }
+        if (es_total + 16 > d_es.cap) CK(d_es.reserve(std::max<size_t>(es_total + 16, d_es.cap * 2), es0));   // grows geometrically
+        CK(d_dst.reserve(dst.size() * 8)); CK(d_hdr.reserve(hdr.size()));
+        CK(cudaMemcpyAsync(d_dst.p, dst.data(), dst.size() * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_hdr.p, hdr.data(), hdr.size(), cudaMemcpyHostToDevice, st));
+        CK(ef_trick_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, n, d_es.p, st));
+        CK(timer.end(2, st));
+        CK(cudaStreamSynchronize(st));                    // the host buffers above go out of scope
+        pending = 0;
+        return EF_OK;
+    };
+
+    for (size_t c = 0; c + 1 < chunk.size(); c++) {
+        const size_t s0 = chunk[c], ns = chunk[c + 1] - s0;
+        std::vector<uint32_t> npics(ns);
+        std::vector<int64_t> pts;
+        for (;;) {                                        // (re)create the decode context until a batch's pictures fit it
+            if (!ctx) {
+                ef_config cfg = { device, max_streams, max_pictures, 16, (size_t)max_bytes, 0 };
+                TRY(ef_create(&ctx, &cfg));
+                TRY(ef_pts_enable(ctx));
+            } else TRY(ef_reset(ctx));
+            std::vector<uint64_t> so((size_t)max_streams + 1);
+            for (int s = 0; s <= max_streams; s++) so[s] = ((s < (int)ns ? segs[s0 + s].pkt0 : segs[s0 + ns - 1].pkt1) - segs[s0].pkt0) * 188;
+            CK(cudaMemcpy(d_off.p, so.data(), so.size() * 8, cudaMemcpyHostToDevice));
+            CK(timer.begin(st));
+            TRY(ef_submit_ts_device(ctx, d_ts.p + segs[s0].pkt0 * 188, (const uint64_t*)d_off.p, st));
+            TRY(ef_index(ctx, st));
+            const int rc = ef_index_info(ctx, nullptr, nullptr, nullptr, nullptr);
+            CK(timer.end(0, st));
+            if (rc == EF_ENOMEM && max_pictures < 4096) {
+                max_pictures = std::min(4096, max_pictures * 2);
+                ef_destroy(ctx); ctx = nullptr;
+                continue;
+            }
+            if (rc == EF_ENOMEM)                          // EF_ENOMEM stays the output-capacity answer
+                return fail(EF_EINVAL, "a main holds more than 4,096 pictures between two sequence headers that start a segment, or "
+                                       "pictures of more than 16 slices: outside what ef_trick_build decodes");
+            TRY(rc);
+            break;
+        }
+        CK(cudaMemcpy(npics.data(), ctx->h.n_pics, ns * 4, cudaMemcpyDeviceToHost));
+        pts.resize((size_t)max_streams * max_pictures);
+        CK(cudaMemcpy(pts.data(), ctx->d_pic_pts, pts.size() * 8, cudaMemcpyDeviceToHost));
+        // the selected pictures of the batch, listed by picture index
+        int maxp = 0;
+        for (size_t s = 0; s < ns; s++) maxp = std::max(maxp, (int)npics[s]);
+        std::vector<std::vector<std::pair<uint32_t, uint32_t>>> by_p((size_t)maxp);    // (stream, index in the batch's selection)
+        std::vector<Enc> sel;
+        for (size_t s = 0; s < ns; s++) {
+            const int f = segs[s0 + s].file;
+            for (uint32_t p = 0; p < npics[s]; p++, seen[f]++) {
+                const int64_t v = pts[s * max_pictures + p];
+                if (seen[f] == 0) p0[f] = v;
+                if (seen[f] % kTrickSpeed) continue;
+                by_p[p].push_back({ (uint32_t)s, (uint32_t)sel.size() });
+                sel.push_back({ f, v, 0, 0 });
+            }
+        }
+        if (pending + sel.size() > in_cap) {             // room for the batch's frames: encode what is waiting, grow if still short
+            TRY(encode_pending());
+            if (sel.size() > in_cap) { in_cap = std::max(sel.size(), (size_t)kTrickEncodeBatch); CK(d_in.reserve(in_cap * EF_FRAME)); }
+        }
+        for (auto& v : by_p) for (auto& e : v) e.second += (uint32_t)pending;
+        for (const Enc& e : sel) { fwd_of[e.file].push_back((uint32_t)enc.size()); enc.push_back(e); }
+        std::vector<uint32_t> first((size_t)maxp + 1, 0), lst_s, lst_slot;
+        for (int p = 0; p < maxp; p++) {
+            first[p + 1] = first[p] + (uint32_t)by_p[p].size();
+            for (auto& e : by_p[p]) { lst_s.push_back(e.first); lst_slot.push_back(e.second); }
+        }
+        CK(d_list.reserve(std::max<size_t>(lst_s.size(), 1) * 8));
+        if (!lst_s.empty()) {
+            CK(cudaMemcpy(d_list.p, lst_s.data(), lst_s.size() * 4, cudaMemcpyHostToDevice));
+            CK(cudaMemcpy(d_list.p + lst_s.size() * 4, lst_slot.data(), lst_slot.size() * 4, cudaMemcpyHostToDevice));
+        }
+        TrickGather g = { ctx, &first, (const uint32_t*)d_list.p, (const uint32_t*)(d_list.p + lst_s.size() * 4), d_in.p, &timer };
+        CK(timer.begin(st));
+        for (int p = 0; p < maxp && !sel.empty(); p += ctx->h.rec_pics)
+            TRY(decode_range(ctx, p, std::min(ctx->h.rec_pics, maxp - p), st, nullptr, 0, trick_gather, &g));
+        CK(timer.end(0, st));
+        pending += sel.size();
+        if (pending >= (size_t)kTrickEncodeBatch) TRY(encode_pending());
+        else CK(cudaStreamSynchronize(st));
+    }
+    TRY(encode_pending());
+
+    // the plan of both outputs: every file's fwd pictures, then every file's rwd pictures
+    std::vector<EfTrickPic> plan;
+    uint64_t pk = 0;
+    for (int dir = 0; dir < 2; dir++) {
+        uint64_t* o = dir ? rwd_off : fwd_off;
+        o[0] = 0;
+        for (int f = 0; f < n_files; f++) {
+            const std::vector<uint32_t>& ids = fwd_of[f];
+            const size_t n = ids.size();
+            std::vector<int64_t> fp(n);
+            for (size_t k = 0; k < n; k++) fp[k] = p0[f] + (enc[ids[k]].main_pts - p0[f]) / kTrickSpeed;
+            uint32_t cc = 0;
+            for (size_t k = 0; k < n; k++) {
+                const size_t src = dir ? n - 1 - k : k;
+                const Enc& e = enc[ids[src]];
+                const int64_t t = dir ? fp[0] + (fp[n - 1] - fp[n - 1 - k]) : fp[k];
+                plan.push_back({ e.es_off, pk, t, e.es_len, cc });
+                const uint32_t pkts = (14 + e.es_len + 183) / 184;
+                pk += pkts; cc += pkts;
+            }
+            o[f + 1] = o[f] + (uint64_t)cc * 188;
+        }
+    }
+    const uint64_t fwd_need = fwd_off[n_files], rwd_need = rwd_off[n_files];
+    if (fwd_cap < fwd_need || rwd_cap < rwd_need || (fwd_need && !fwd) || (rwd_need && !rwd))
+        return fail(EF_ENOMEM, "the trick files need %llu (fwd) and %llu (rwd) bytes", (unsigned long long)fwd_need, (unsigned long long)rwd_need);
+    GrowBuf d_plan, d_out;
+    CK(d_plan.reserve(std::max<size_t>(plan.size(), 1) * sizeof(EfTrickPic)));
+    CK(d_out.reserve(pk * 188 + 16));
+    CK(cudaMemcpy(d_plan.p, plan.data(), plan.size() * sizeof(EfTrickPic), cudaMemcpyHostToDevice));
+    CK(timer.begin(st));
+    CK(ef_trick_launch_mux(d_es.p, (const EfTrickPic*)d_plan.p, (int)plan.size(), pk, d_out.p, st));
+    CK(timer.end(3, st));
+    if (fwd_need) CK(cudaMemcpy(fwd, d_out.p, fwd_need, cudaMemcpyDeviceToHost));
+    if (rwd_need) CK(cudaMemcpy(rwd, d_out.p + fwd_need, rwd_need, cudaMemcpyDeviceToHost));
+    CK(cudaDeviceSynchronize());
+    for (float& m : g_trick_ms) m = 0;
+    for (auto& s : timer.spans) {
+        float ms = 0;
+        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
+        g_trick_ms[s.first] += ms;
+    }
+    return EF_OK;
+}
+
+// ef_library_add_trick: ef_trick_build on a title's main, then merge_index()'s fwd and rwd records and samples for the built files
+int ef_library_add_trick(ef_ctx* c, int title, int qscale)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->d_lib) return fail(EF_ESTATE, "ef_library_add_trick before the first ef_library_add");
+    if (title < 0 || title >= (int)c->lib_titles.size()) return fail(EF_EINVAL, "no title %d", title);
+    if (qscale < 1 || qscale > 31) return fail(EF_EINVAL, "qscale %d outside 1..31", qscale);
+    EfLibTitle t = c->lib_titles[title];
+    if (t.ts[0] || t.ts[2]) return fail(EF_ESTATE, "title %d already has a trick file", title);
+    CK(cudaDeviceSynchronize());
+    // the plan reads the main's packets on the host (make_index()'s table, the segment cuts): one copy of the main back
+    std::vector<uint8_t> main(t.bytes[1]), img(t.idx_bytes);
+    CK(cudaMemcpy(main.data(), t.ts[1], main.size(), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(img.data(), t.idx, img.size(), cudaMemcpyDeviceToHost));
+    const uint64_t moff[2] = { 0, main.size() };
+    uint64_t fo[2], ro[2], cap = main.size() + 188 * 1024;
+    std::vector<uint8_t> fwd, rwd;
+    for (int attempt = 0;; attempt++) {
+        fwd.resize(cap); rwd.resize(cap);
+        const int rc = ef_trick_build(c->cfg.device, main.data(), moff, 1, qscale, fwd.data(), cap, fo, rwd.data(), cap, ro);
+        if (rc == EF_ENOMEM && attempt == 0 && std::max(fo[1], ro[1]) > cap) { cap = std::max(fo[1], ro[1]); continue; }
+        TRY(rc);
+        break;
+    }
+    fwd.resize(fo[1]); rwd.resize(ro[1]);
+    // merge_index() (indexer.cpp:230) for the two built files: records of bin IDX_BIN and trick speed 15, pts2seq()'s samples
+    const uint32_t bin = 90000 / 12;
+    std::vector<uint8_t> both(fwd);
+    both.insert(both.end(), rwd.begin(), rwd.end());
+    const uint64_t off2[3] = { 0, fwd.size(), both.size() };
+    const size_t np = both.size() / 188 + 1;
+    std::vector<int64_t> spts(np);
+    std::vector<uint32_t> spos(np);
+    ef_tsidx_info info[2];
+    TRY(ef_tsidx_scan(c->cfg.device, both.data(), off2, 2, bin, info, spts.data(), spos.data()));
+    idx_hdr h;
+    memcpy(&h, img.data(), sizeof(h));
+    std::vector<uint32_t> smp[2];
+    idx_rec* rec[2] = { &h.fwd, &h.rev };
+    for (int k = 0; k < 2; k++) {
+        const size_t p0 = off2[k] / 188;
+        smp[k].resize(std::max<uint32_t>(info[k].n_samples, 1));
+        uint32_t n = 0;
+        TRY(ef_tsidx_samples(c->cfg.device, spts.data() + p0, spos.data() + p0, (int)info[k].n_seq, info[k].first_pts, info[k].last_pts, bin,
+                             smp[k].data(), (uint32_t)smp[k].size(), &n));
+        smp[k].resize(n);
+        *rec[k] = idx_rec{ info[k].first_pts, info[k].last_pts, bin, 15, n };
+        if (!n || info[k].last_pts == info[k].first_pts)
+            return fail(EF_EINVAL, "title %d: its %s file has one picture (pts %lld): the reference divides by zero playing it", title,
+                        k ? "rwd" : "fwd", (long long)info[k].first_pts);
+    }
+    std::vector<uint8_t> out(sizeof(idx_hdr) + 4 * ((size_t)h.video.sample_count + smp[0].size() + smp[1].size()));
+    memcpy(out.data(), img.data(), sizeof(idx_hdr));                          // the padding bytes stay as added
+    for (int k = 0; k < 2; k++) memcpy(out.data() + 8 + 32 * (k + 1), rec[k], 28);
+    memcpy(out.data() + sizeof(idx_hdr), img.data() + sizeof(idx_hdr), 4 * (size_t)h.video.sample_count);   // the main's samples as added
+    memcpy(out.data() + sizeof(idx_hdr) + 4 * (size_t)h.video.sample_count, smp[0].data(), 4 * smp[0].size());
+    memcpy(out.data() + sizeof(idx_hdr) + 4 * ((size_t)h.video.sample_count + smp[0].size()), smp[1].data(), 4 * smp[1].size());
+    if (out.size() >> 32 || fwd.size() >> 32) return fail(EF_EINVAL, "title %d: its trick files or video.idx reach 4 GiB", title);
+    uint8_t* p = nullptr;
+    TRY(dev_alloc(c, &p, out.size()));
+    CK(cudaMemcpy(p, out.data(), out.size(), cudaMemcpyHostToDevice));
+    t.idx = p; t.idx_bytes = (uint32_t)out.size();
+    const std::vector<uint8_t>* files[3] = { &rwd, nullptr, &fwd };
+    for (int f = 0; f < 3; f += 2) {
+        TRY(dev_alloc(c, &p, files[f]->size()));
+        CK(cudaMemcpy(p, files[f]->data(), files[f]->size(), cudaMemcpyHostToDevice));
+        t.ts[f] = p; t.bytes[f] = (uint32_t)files[f]->size();
+    }
+    t.f_first = h.fwd.first_pts; t.f_last = h.fwd.last_pts; t.r_first = h.rev.first_pts; t.r_last = h.rev.last_pts;
+    t.f_bin = t.r_bin = bin; t.f_trick = t.r_trick = 15; t.f_n = h.fwd.sample_count; t.r_n = h.rev.sample_count;
+    CK(cudaMemcpy(c->d_lib_titles + title, &t, sizeof(t), cudaMemcpyHostToDevice));
+    c->lib_titles[title] = t;
+    return EF_OK;
+}
+
+int ef_library_read(ef_ctx* c, int title, int what, uint8_t* dst, uint64_t cap, uint64_t* bytes)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c || !bytes) return fail(EF_EINVAL, "null argument");
+    if (!c->d_lib) return fail(EF_ESTATE, "ef_library_read before the first ef_library_add");
+    if (title < 0 || title >= (int)c->lib_titles.size() || what < -1 || what > 2) return fail(EF_EINVAL, "no title %d or part %d", title, what);
+    const EfLibTitle& t = c->lib_titles[title];
+    const uint8_t* src = what < 0 ? t.idx : t.ts[what];
+    *bytes = what < 0 ? t.idx_bytes : t.bytes[what];
+    if (!*bytes) return EF_OK;
+    if (!dst || cap < *bytes) return fail(EF_ENOMEM, "part %d of title %d has %llu bytes", what, title, (unsigned long long)*bytes);
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(dst, src, *bytes, cudaMemcpyDeviceToHost));
+    return EF_OK;
+}
+
+int ef_trick_stage_ms(float* decode_ms, float* gather_ms, float* encode_ms, float* mux_ms)
+{
+    if (decode_ms) *decode_ms = g_trick_ms[0];
+    if (gather_ms) *gather_ms = g_trick_ms[1];
+    if (encode_ms) *encode_ms = g_trick_ms[2];
+    if (mux_ms) *mux_ms = g_trick_ms[3];
     return EF_OK;
 }
 

@@ -289,6 +289,18 @@ struct __align__(16) EfLibStream {   // layout of ef_library_status (include/esp
     int64_t pos;                 // _info[_nav].pos: the main pts the next PLAY, SKIP, FAST_FORWARD or REWIND starts from
 };
 
+// trick streams (ef_trick_build, csrc/ef_trick.cu): every picture's 28 header bytes, the worst-case bytes of one intra slice (start
+// code + 6 bits + 22 macroblocks of 2 bits + 6 blocks of a 16-bit DC code, 63 28-bit escapes and the end of block, in whole words), and
+// one output picture of the mux: its ES bytes, its first packet among all output packets, its pts and its file's continuity counter
+constexpr int kTrickHeaderBytes = 28;
+constexpr int kTrickSliceBytes = 29440;
+static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (2 + 6 * (16 + 63 * 28 + 2)) + 31) / 32) * 4, "worst-case slice");
+struct EfTrickPic {
+    uint64_t es_off, pkt_first;
+    int64_t pts;
+    uint32_t es_len, cc0;
+};
+
 static inline __host__ __device__ int64_t ef_lib_pts2pts(const EfLibTitle& t, int64_t pts, int speed)
 {
     return ef_pts2pts(pts, speed, t.v_first, t.v_last, t.f_first, t.f_last, t.r_first, t.r_last);

@@ -1,0 +1,320 @@
+// csrc/ef_trick.cu — the trick streams of a title (video_fwd.ts, video_rwd.ts) made on the device: the reference's indexer makes them
+// with two ffmpeg re-encodes (indexer/indexer.cpp:308-309); here the decoded frames of every 15th main picture are intra-coded and
+// muxed. The rule, byte for byte, is tests/trick_cases.py. The host side (segmenting, the decode, the plan) is ef_trick_build in
+// ef_capi.cu. Kernels:
+//   ef_trick_gather_kernel    after K1b of a picture index: copies the frames of the selected pictures out of the frame stores
+//   ef_trick_encode_kernel    one warp per slice (macroblock row): FDCT, quantiser, code lengths, a warp prefix sum for the bit
+//                             offsets, codes OR-ed into a shared window and flushed to a per-slice region of kTrickSliceBytes
+//   ef_trick_assemble_kernel  one CTA per picture: header + its 12 slices, back to back, at the picture's offset in the ES
+//   ef_trick_mux_kernel       one warp per output TS packet, fwd and rwd of every file in one launch
+#include <stdint.h>
+#include <string.h>
+
+#include "ef_common.cuh"
+#include "ef_iso11172_tables.h"
+
+namespace {
+
+// FDCT_C of tests/trick_cases.py: round(4096 c_k cos((2n + 1) k pi / 16)); rows sum to at most 11,585 in magnitude, so with pixels
+// 0..255 the row pass stays below 2^22 and the column pass below 2^28 (int32).
+__constant__ int c_fdct[64] = {
+    1448, 1448, 1448, 1448, 1448, 1448, 1448, 1448,
+    2009, 1703, 1138, 400, -400, -1138, -1703, -2009,
+    1892, 784, -784, -1892, -1892, -784, 784, 1892,
+    1703, -400, -2009, -1138, 1138, 2009, 400, -1703,
+    1448, -1448, -1448, 1448, 1448, -1448, -1448, 1448,
+    1138, -2009, 400, 1703, -1703, -400, 2009, -1138,
+    784, -1892, 1892, -784, -784, 1892, -1892, 784,
+    400, -1138, 1703, -2009, 2009, -1703, 1138, -400,
+};
+
+struct TrickTables {
+    uint32_t ac[32 * 41];      // run 0..31 x level 0..40: (code << 8) | length, without the sign bit; 0 = escape
+    uint32_t dc[2][9];         // luma / chroma dct_dc_size: (code << 8) | length
+    uint8_t zz[64];            // zig-zag index -> raster index
+    uint8_t q[64];             // default intra matrix, raster index
+};
+__constant__ TrickTables c_trick;
+
+constexpr int kWarps = 4;
+constexpr int kWin = 64;       // window words: one block's codes (at most 1,784 bits) plus 31 carried bits
+static_assert(kWin * 32 >= 31 + 2 + 16 + 63 * 28 + 2, "window holds a macroblock header and a worst-case block");
+
+__device__ __forceinline__ void put_bits(uint32_t* win, uint32_t q, uint32_t code, uint32_t len)
+{
+    if (!len) return;
+    const uint32_t w = q >> 5, off = q & 31;
+    if (off + len <= 32) atomicOr(&win[w], code << (32 - off - len));
+    else {
+        atomicOr(&win[w], code >> (off + len - 32));
+        atomicOr(&win[w + 1], code << (64 - off - len));
+    }
+}
+
+__device__ __forceinline__ void code_of(int i, int lv, uint64_t mask, const uint32_t* ac, uint32_t* code, uint32_t* len)
+{
+    *code = 0; *len = 0;
+    if (i == 0 || lv == 0) return;
+    const int prev = 63 - __clzll((long long)(mask & ((1ull << i) - 1)));
+    const int run = i - prev - 1, a = lv < 0 ? -lv : lv;
+    const uint32_t e = (a <= 40 && run <= 31) ? ac[run * 41 + a] : 0u;
+    if (e & 0xFF) { *code = ((e >> 8) << 1) | (lv < 0 ? 1u : 0u); *len = (e & 0xFF) + 1; return; }
+    uint32_t L, bits;
+    if (lv >= -127 && lv <= 127) { L = 8; bits = (uint32_t)lv & 0xFF; }
+    else if (lv > 0) { L = 16; bits = (uint32_t)lv; }
+    else { L = 16; bits = (128u << 8) | ((uint32_t)(lv + 256) & 0xFF); }
+    *code = (1u << (6 + L)) | ((uint32_t)run << L) | bits;
+    *len = 12 + L;
+}
+
+// bit i of m -> bit 2 i
+__device__ __forceinline__ uint64_t spread_bits(uint32_t m)
+{
+    uint64_t x = m;
+    x = (x | (x << 16)) & 0x0000FFFF0000FFFFull;
+    x = (x | (x << 8)) & 0x00FF00FF00FF00FFull;
+    x = (x | (x << 4)) & 0x0F0F0F0F0F0F0F0Full;
+    x = (x | (x << 2)) & 0x3333333333333333ull;
+    return (x | (x << 1)) & 0x5555555555555555ull;
+}
+
+__device__ __forceinline__ int quant(int i, const int* F, int qscale)
+{
+    const int z = c_trick.zz[i], f = F[z];
+    if (i == 0) { const int dc = (f + 4) >> 3; return dc > 255 ? 255 : dc; }
+    const int den = qscale * c_trick.q[z], num = 8 * (f < 0 ? -f : f);
+    int lv = (2 * num + den) / (2 * den);
+    lv = lv > 255 ? 255 : lv;
+    return f < 0 ? -lv : lv;
+}
+
+}  // namespace
+
+__global__ void ef_trick_gather_kernel(const uint8_t* __restrict__ frames, const uint32_t* __restrict__ streams, const uint32_t* __restrict__ slots,
+                                       int count, int fb, uint8_t* __restrict__ dst)
+{
+    constexpr uint32_t per = EF_FRAME / 16;
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t k = (uint32_t)(t / per), w = (uint32_t)(t % per);
+    if (k >= (uint32_t)count) return;
+    const uint4* src = (const uint4*)(frames + ef_frame_offset((int)streams[k], fb));
+    ((uint4*)(dst + (size_t)slots[k] * EF_FRAME))[w] = src[w];
+}
+
+__global__ void __launch_bounds__(kWarps * 32) ef_trick_encode_kernel(const uint8_t* __restrict__ in, int n_pics, int qscale, uint32_t* __restrict__ slots,
+                                                                     uint32_t* __restrict__ slice_len)
+{
+    __shared__ uint32_t s_ac[32 * 41];
+    __shared__ int s_t[kWarps][64], s_f[kWarps][64];
+    __shared__ uint32_t s_win[kWarps][kWin + 2];
+    for (int i = threadIdx.x; i < 32 * 41; i += blockDim.x) s_ac[i] = c_trick.ac[i];
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int gw = blockIdx.x * kWarps + warp;
+    if (gw >= n_pics * EF_MBH_MAX) return;
+    const int pic = gw / EF_MBH_MAX, row = gw % EF_MBH_MAX;
+    uint32_t* out = slots + (size_t)gw * (kTrickSliceBytes / 4);
+    const uint8_t* frame = in + (size_t)pic * EF_FRAME;
+    uint32_t* win = s_win[warp];
+    int* T = s_t[warp];
+    int* F = s_f[warp];
+    for (int i = lane; i < kWin + 2; i += 32) win[i] = 0;
+    __syncwarp();
+    if (lane == 0) { win[0] = 0x00000100u | (uint32_t)(row + 1); win[1] = (uint32_t)qscale << 27; }   // slice start code, quantiser, extra bit
+    uint32_t P = 38, wbase = 0;              // bit position in the slice, slice word held in win[0]
+    int pred[3] = { 128, 128, 128 };
+    const int r = lane >> 2, k0 = (lane & 3) * 2;
+    for (int mb = 0; mb < EF_MBW_MAX; mb++) {
+        const uint8_t* tile = frame + ef_tile_offset(mb, row);
+        __syncwarp();
+        if (lane == 0) put_bits(win, P - wbase * 32, 3u, 2);    // address increment 1, intra macroblock type
+        P += 2;
+        for (int b = 0; b < 6; b++) {
+            // row pass: lane = (row r, outputs k0, k0 + 1)
+            const int po = b < 4 ? ((b >> 1) * 8 + r) * 16 + (b & 1) * 8 : 256 + (b - 4) * 64 + r * 8;
+            const uint2 px = *(const uint2*)(tile + po);
+            int x[8];
+            #pragma unroll
+            for (int n = 0; n < 4; n++) { x[n] = (px.x >> (8 * n)) & 0xFF; x[n + 4] = (px.y >> (8 * n)) & 0xFF; }
+            #pragma unroll
+            for (int kk = 0; kk < 2; kk++) {
+                int acc = 0;
+                #pragma unroll
+                for (int n = 0; n < 8; n++) acc += c_fdct[(k0 + kk) * 8 + n] * x[n];
+                T[r * 8 + k0 + kk] = (acc + 128) >> 8;
+            }
+            __syncwarp();
+            // column pass: lane = (column r, outputs k0, k0 + 1)
+            #pragma unroll
+            for (int kk = 0; kk < 2; kk++) {
+                int acc = 0;
+                #pragma unroll
+                for (int n = 0; n < 8; n++) acc += c_fdct[(k0 + kk) * 8 + n] * T[n * 8 + r];
+                F[(k0 + kk) * 8 + r] = (acc + 32768) >> 16;
+            }
+            __syncwarp();
+            // quantise zig-zag indices 2 lane and 2 lane + 1 (so the lanes' codes follow each other in bitstream order); the DC
+            // counts as coded
+            const int lv0 = quant(2 * lane, F, qscale), lv1 = quant(2 * lane + 1, F, qscale);
+            const uint32_t ev = __ballot_sync(0xFFFFFFFFu, lane == 0 || lv0 != 0), od = __ballot_sync(0xFFFFFFFFu, lv1 != 0);
+            const uint64_t mask = spread_bits(ev) | (spread_bits(od) << 1);
+            uint32_t c0, n0, c1, n1;
+            code_of(2 * lane, lv0, mask, s_ac, &c0, &n0);
+            code_of(2 * lane + 1, lv1, mask, s_ac, &c1, &n1);
+            const int dc = __shfl_sync(0xFFFFFFFFu, lv0, 0);
+            const int comp = b < 4 ? 0 : b - 3;
+            if (lane == 0) {                 // DC difference: size code, then the difference bits
+                const int diff = dc - pred[comp], a = diff < 0 ? -diff : diff;
+                const uint32_t size = 32 - __clz(a);
+                const uint32_t e = c_trick.dc[comp ? 1 : 0][size];
+                c0 = ((e >> 8) << size) | (uint32_t)(diff > 0 ? diff : diff + (1 << size) - 1);
+                n0 = (e & 0xFF) + size;
+            }
+            pred[comp] = dc;
+            const uint32_t sum = n0 + n1;
+            uint32_t incl = sum;
+            #pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+                if (lane >= d) incl += v;
+            }
+            const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+            const uint32_t q = P - wbase * 32 + incl - sum;
+            put_bits(win, q, c0, n0);
+            put_bits(win, q + n0, c1, n1);
+            if (lane == 0) put_bits(win, P - wbase * 32 + total, 2u, 2);     // end of block "10"
+            P += total + 2;
+            __syncwarp();
+            // flush the complete words, keep the partial one
+            const uint32_t full = (P >> 5) - wbase;
+            for (uint32_t i = lane; i < full; i += 32) out[wbase + i] = __byte_perm(win[i], 0, 0x0123);
+            __syncwarp();
+            const uint32_t carry = win[full];
+            __syncwarp();
+            for (int i = lane; i < kWin + 2; i += 32) win[i] = 0;
+            __syncwarp();
+            if (lane == 0) win[0] = carry;
+            wbase += full;
+        }
+    }
+    __syncwarp();
+    const uint32_t words = ((P + 31) >> 5) - wbase;          // the slice ends on a byte boundary, zero-padded
+    for (uint32_t i = lane; i < words; i += 32) out[wbase + i] = __byte_perm(win[i], 0, 0x0123);
+    if (lane == 0) slice_len[gw] = (P + 7) >> 3;
+}
+
+// one CTA per picture: the 28 header bytes of its file, then its slices, at pic_dst[p] in es
+__global__ void ef_trick_assemble_kernel(const uint32_t* __restrict__ slots, const uint32_t* __restrict__ slice_len, const uint64_t* __restrict__ pic_dst,
+                                         const uint8_t* __restrict__ headers, uint8_t* __restrict__ es)
+{
+    const int p = blockIdx.x;
+    __shared__ uint32_t off[EF_MBH_MAX + 1];
+    if (threadIdx.x == 0) {
+        off[0] = kTrickHeaderBytes;
+        for (int s = 0; s < EF_MBH_MAX; s++) off[s + 1] = off[s] + slice_len[p * EF_MBH_MAX + s];
+    }
+    __syncthreads();
+    uint8_t* dst = es + pic_dst[p];
+    for (int i = threadIdx.x; i < kTrickHeaderBytes; i += blockDim.x) dst[i] = headers[(size_t)p * kTrickHeaderBytes + i];
+    for (int s = 0; s < EF_MBH_MAX; s++) {
+        const uint8_t* src = (const uint8_t*)(slots + (size_t)(p * EF_MBH_MAX + s) * (kTrickSliceBytes / 4));
+        const uint32_t n = off[s + 1] - off[s];
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) dst[off[s] + i] = src[i];
+    }
+}
+
+// one warp per output packet: out[k] is packet k of all the trick files back to back; pics[] (ascending pkt_first) says which picture
+// and which part of its PES the packet carries (efs_wrap_ts's layout: a 14-byte PES header, full packets, the last one stuffed)
+__global__ void ef_trick_mux_kernel(const uint8_t* __restrict__ es, const EfTrickPic* __restrict__ pics, int n_pics, uint64_t n_packets, uint8_t* __restrict__ out)
+{
+    const uint64_t k = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (k >= n_packets) return;
+    int lo = 0, hi = n_pics - 1;
+    while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (pics[m].pkt_first <= k) lo = m; else hi = m - 1; }
+    const EfTrickPic d = pics[lo];
+    const uint32_t j = (uint32_t)(k - d.pkt_first);
+    const uint32_t pes_len = 14 + d.es_len, pos = j * 184, left = pes_len - pos;
+    const uint32_t af = left >= 184 ? 0 : 184 - left;                   // adaptation field bytes, its length byte included
+    const uint64_t pts = (uint64_t)d.pts & ((1ull << 33) - 1);
+    uint8_t* pkt = out + k * 188;
+    for (int t = lane; t < 188; t += 32) {
+        uint8_t v;
+        if (t == 0) v = 0x47;
+        else if (t == 1) v = (uint8_t)((j == 0 ? 0x40 : 0) | 0x01);
+        else if (t == 2) v = 0x00;
+        else if (t == 3) v = (uint8_t)((af ? 0x30 : 0x10) | ((d.cc0 + j) & 15));
+        else if ((uint32_t)t < 4 + af) v = t == 4 ? (uint8_t)(af - 1) : t == 5 ? 0 : 0xFF;
+        else {
+            const uint32_t b = pos + (uint32_t)t - 4 - af;             // byte of the PES
+            if (b >= 14) v = es[d.es_off + b - 14];
+            else {
+                switch (b) {
+                case 2: v = 1; break;
+                case 3: v = 0xE0; break;
+                case 6: case 7: v = 0x80; break;
+                case 8: v = 5; break;
+                case 9: v = (uint8_t)(0x21 | ((pts >> 29) & 0x0E)); break;
+                case 10: v = (uint8_t)(pts >> 22); break;
+                case 11: v = (uint8_t)(0x01 | ((pts >> 14) & 0xFE)); break;
+                case 12: v = (uint8_t)(pts >> 7); break;
+                case 13: v = (uint8_t)(0x01 | ((pts << 1) & 0xFE)); break;
+                default: v = 0;
+                }
+            }
+        }
+        pkt[t] = v;
+    }
+}
+
+// ---- host side ----------------------------------------------------------------------------------------------------------------------
+static uint32_t vlc_entry(const char* code)
+{
+    uint32_t v = 0, n = 0;
+    for (; *code; code++, n++) v = (v << 1) | (uint32_t)(*code == '1');
+    return (v << 8) | n;
+}
+
+cudaError_t ef_trick_upload_tables()
+{
+    TrickTables t;
+    memset(&t, 0, sizeof(t));
+    for (int i = 0; i < EF_VLC_DCT_COUNT; i++) {
+        const int run = ef_vlc_dct[i].value >> 8, level = ef_vlc_dct[i].value & 0xFF;
+        if (run <= 31 && level <= 40) t.ac[run * 41 + level] = vlc_entry(ef_vlc_dct[i].code);
+    }
+    for (int i = 0; i < EF_VLC_DC_LUMA_COUNT; i++) t.dc[0][ef_vlc_dc_luma[i].value] = vlc_entry(ef_vlc_dc_luma[i].code);
+    for (int i = 0; i < EF_VLC_DC_CHROMA_COUNT; i++) t.dc[1][ef_vlc_dc_chroma[i].value] = vlc_entry(ef_vlc_dc_chroma[i].code);
+    memcpy(t.zz, ef_zigzag, 64);
+    memcpy(t.q, ef_default_intra_q, 64);
+    return cudaMemcpyToSymbol(c_trick, &t, sizeof(t));
+}
+
+cudaError_t ef_trick_launch_gather(const uint8_t* frames, const uint32_t* streams, const uint32_t* slots, int count, int fb, uint8_t* dst, cudaStream_t st)
+{
+    if (!count) return cudaSuccess;
+    const uint64_t threads = (uint64_t)count * (EF_FRAME / 16);
+    ef_trick_gather_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(frames, streams, slots, count, fb, dst);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st)
+{
+    const int warps = n_pics * EF_MBH_MAX;
+    ef_trick_encode_kernel<<<(warps + kWarps - 1) / kWarps, kWarps * 32, 0, st>>>(in, n_pics, qscale, slots, slice_len);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int n_pics,
+                                     uint8_t* es, cudaStream_t st)
+{
+    ef_trick_assemble_kernel<<<n_pics, 256, 0, st>>>(slots, slice_len, pic_dst, headers, es);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st)
+{
+    if (!n_packets) return cudaSuccess;
+    ef_trick_mux_kernel<<<(unsigned)((n_packets * 32 + 255) / 256), 256, 0, st>>>(es, pics, n_pics, n_packets, out);
+    return cudaGetLastError();
+}

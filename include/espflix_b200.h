@@ -38,6 +38,7 @@
  *   ef_video_set_scroll / _overlay  _hscroll video.cpp:1146-1154, composite() video.cpp:839-887
  *   ef_tsidx_scan                 make_index(const string&, vector<idx>&) indexer/indexer.cpp:90
  *   ef_tsidx_samples              pts2seq(idx&,int,int) + pts2pos indexer/indexer.cpp:193-228
+ *   ef_trick_build                the ffmpeg re-encodes of make_video() indexer/indexer.cpp:308-309: video_fwd.ts, video_rwd.ts
  *   ef_audio_demux_ts             MpegDecoder::demux() for the audio PIDs -> push_audio() player.cpp:381-432, video.cpp:1007
  *   ef_audio_decode               decode_audio() video.cpp:964, sbc_decoder() sbc_decoder.cpp:343, pdm_second_order()
  *                                 espflix.ino:73
@@ -59,7 +60,7 @@
  *   ef_carry_enable / ef_end_streams / ef_carry_info  the decoder pulling bytes on demand across the producer's Buffers
  *                                 (FILL_BITS -> more(), player.cpp:348-352, 459-493; espflix.cpp:723-737): TS submits cut at any
  *                                 packet boundary, and the len <= 0 Buffer that ends a stream (player.cpp:456, 469-473)
- *   ef_library_add / _command / _submit / _info  Streamer::get() + read() of a title (espflix.cpp:723-747) and ESPFlix's play, skip,
+ *   ef_library_add / _command / _submit / _info / _add_trick  Streamer::get() + read() of a title (espflix.cpp:723-747) and ESPFlix's play, skip,
  *                                 fast_forward, rewind, play_pause, get_index and save_pos (espflix.cpp:787-859): titles in HBM, every
  *                                 stream's seek resolved from video.idx and its bytes gathered on the device
  * Calls run on the context's device and restore the caller's current device.
@@ -211,6 +212,34 @@ int ef_tsidx_scan(int device, const uint8_t* ts, const uint64_t* off, int n_file
                   ef_tsidx_info* info, int64_t* seq_pts, uint32_t* seq_pos);
 int ef_tsidx_samples(int device, const int64_t* seq_pts, const uint32_t* seq_pos, int n_seq, int64_t first_pts, int64_t last_pts,
                      uint32_t bin_size, uint32_t* samples, uint32_t cap, uint32_t* n_samples);
+
+/* ---- trick streams: the fwd / rwd half of the reference's indexer (indexer/indexer.cpp:308-309), without ffmpeg ---------------
+ * Stateless (no context); host buffers; the decode, the encoder and the mux run on `device`. The rule, byte for byte, is
+ * tests/trick_cases.py.
+ * ef_trick_build  video_fwd.ts and video_rwd.ts of n_files mains packed back to back (off[n_files + 1], multiples of 188). Every
+ *                 main is decoded as the reference decodes it, cut at its sequence headers into segments decoded as one batch (a
+ *                 sequence header whose PES has no valid PTS or whose first picture is not intra joins the segment before it). fwd
+ *                 picture k is main picture 15 k (the trick_speed merge_index writes), with pts p_0 + (p_15k - p_0) / 15 (a C
+ *                 division; p_j = ef_picture_pts of main picture j); rwd holds the same pictures in reverse order with pts
+ *                 f_0 + (f_{n-1} - f_{n-1-j}) (setpts=PTS/15 and -vf reverse). Every picture is one random-access point: a sequence
+ *                 header (352 x 192, the aspect and picture-rate codes of the main's first one, default matrices), a closed GOP, an
+ *                 I picture of 12 slices of intra macroblocks at quantiser scale qscale (1..31; 8 is the project's default). The
+ *                 mux is efs_wrap_ts's: PID 0x100, one PES (stream id 0xE0, a PTS) per picture, the last packet of every PES
+ *                 padded with adaptation-field stuffing, one continuity counter per file. No audio (the reference uses -an).
+ *                 fwd_off / rwd_off[n_files + 1] receive the byte offsets of every file's output. A capacity below the total (or a
+ *                 NULL buffer) returns EF_ENOMEM with both offset arrays filled and nothing written: a sizing call.
+ *                 EF_EINVAL: qscale outside 1..31, offsets that are not non-decreasing multiples of 188, an empty main or one
+ *                 without a sequence header at the start of a video PES (make_index()'s table), and a main with more than 4,096
+ *                 pictures between two sequence headers that start a segment (or pictures of more than 16 slices).
+ *                 Device memory: the mains' TS, their encoded pictures and output packets are held for the call, plus one decode
+ *                 batch of at most 256 segments and 64 MB of TS and at most max(256, one batch's selected pictures) frames being
+ *                 encoded: pass a catalogue in calls of a size the card holds. A too-small capacity is found only after the whole
+ *                 build, so size the buffers generously (the mains' total is usually enough, but not at every qscale).
+ * ef_trick_stage_ms  device milliseconds of the last ef_trick_build on the calling thread: the decode (upload, K0, K1a, K1b), the
+ *                 gather of the selected frames, the encode (FDCT, quantiser, VLC and the picture assembly) and the mux. */
+int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_files, int qscale, uint8_t* fwd, uint64_t fwd_cap, uint64_t* fwd_off,
+                   uint8_t* rwd, uint64_t rwd_cap, uint64_t* rwd_off);
+int ef_trick_stage_ms(float* decode_ms, float* gather_ms, float* encode_ms, float* mux_ms);
 
 /* ---- audio (SURVEY.md 8f-3): the SBC decoder and the PDM modulator of the reference, batched ---------------------
  * Stateless (no context); host buffers; the kernels run on `device`.
@@ -540,6 +569,22 @@ int ef_library_add(ef_ctx* ctx, const uint8_t* idx, uint64_t idx_bytes, const ui
 int ef_library_command(ef_ctx* ctx, int first, int count, int cmd, int title, int64_t arg);
 int ef_library_submit(ef_ctx* ctx, uint32_t packets, const uint32_t* per_stream, void* stream);
 int ef_library_info(ef_ctx* ctx, int first, int count, ef_library_status* status);
+/* ef_library_add_trick  gives a title added with its main only (ts[0] and ts[2] NULL) its fast-forward and rewind files: ef_trick_build
+ *                     on the main already in device memory (read back once: the segment plan reads its packets on the host), then the
+ *                     fwd and rwd records and samples of the title's video.idx as merge_index() computes them for the built files
+ *                     (bin_size 7,500, trick_speed 15, pts2seq()'s samples); the header's video record, its padding bytes and the main's
+ *                     samples stay byte for byte as added. The image equals what ef_tsidx_scan + ef_tsidx_samples (capi.build_video_idx)
+ *                     give for (main, fwd, rwd) when the title's own records were built that way. From then on FAST_FORWARD and REWIND
+ *                     play the built files. Synchronous. EF_ESTATE before the first ef_library_add, or when the title already has either
+ *                     trick file (a second call); EF_EINVAL for an unknown title, qscale outside 1..31, the cases of ef_trick_build, or a
+ *                     main of fewer than 16 pictures (a one-picture trick file, whose record the reference divides by zero with). Nothing
+ *                     changes on an error. */
+int ef_library_add_trick(ef_ctx* ctx, int title, int qscale);
+/* ef_library_read     copies part `what` of a title to host memory: -1 its video.idx image, 0 / 1 / 2 its rwd / main / fwd file (after
+ *                     ef_library_add_trick: the built files and the rewritten image, for a service to store beside video.ts).
+ *                     *bytes = the part's size (0: no such file, nothing copied). EF_ENOMEM when dst is NULL or cap is below it (a
+ *                     sizing call). EF_ESTATE before the first ef_library_add; EF_EINVAL for an unknown title or part. Synchronous. */
+int ef_library_read(ef_ctx* ctx, int title, int what, uint8_t* dst, uint64_t cap, uint64_t* bytes);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
