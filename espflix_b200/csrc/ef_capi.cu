@@ -5,11 +5,15 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
+#include <atomic>
+#include <thread>
 #include <vector>
 
 #include "../../include/espflix_b200.h"
 #include "../host/ef_indexer.h"
 #include "ef_common.cuh"
+#include "ef_iso11172_tables.h"
 #include <stdlib.h>
 
 // from the other translation units
@@ -2303,31 +2307,209 @@ struct GrowBuf {                                 // device buffer that keeps its
     }
 };
 
-// The video ES of the first packets from packet `pkt` on (PID 0x100 payloads, as demux() reads them, player.cpp:381-432), at most
-// `cap` bytes; *pts_ok = packet `pkt` starts a video PES whose PTS parse_pts() accepts (player.cpp:299-306).
-void trick_video_es(const uint8_t* ts, uint64_t pkt, uint64_t end, size_t cap, std::vector<uint8_t>& es, bool* pts_ok)
+// Appends to es the video ES of packets pkt.. (PID 0x100 payloads, as demux() reads them, player.cpp:381-432) until es holds `cap`
+// bytes or packet `end`; returns the packet after the last one read. *pts_ok (unless null) = packet `pkt` starts a video PES whose
+// PTS parse_pts() accepts (player.cpp:299-306).
+uint64_t trick_video_es(const uint8_t* ts, uint64_t pkt, uint64_t end, size_t cap, std::vector<uint8_t>& es, bool* pts_ok)
 {
-    es.clear();
-    *pts_ok = false;
-    for (uint64_t k = pkt; k < end && es.size() < cap; k++) {
+    if (pts_ok) *pts_ok = false;
+    uint64_t k = pkt;
+    for (; k < end && es.size() < cap; k++) {
         const uint8_t* d = ts + k * 188;
         if (d[0] != 0x47 || (((d[1] << 8) | d[2]) & 0x1FFF) != 0x100 || !(d[3] & 0x10)) continue;
         int o = (d[3] & 0x20) ? 5 + d[4] : 4;
         if ((d[1] & 0x40) && o + 14 <= 188) {
             const int flags = (d[o + 6] << 8) | d[o + 7];
-            if (k == pkt) *pts_ok = (flags & 0x80) && (d[o + 9] & 0xF0) == ((flags >> 2) & 0x30);
+            if (k == pkt && pts_ok) *pts_ok = (flags & 0x80) && (d[o + 9] & 0xF0) == ((flags >> 2) & 0x30);
             o += 9 + d[o + 8];
         }
         if (o < 188) es.insert(es.end(), d + o, d + 188);
     }
+    return k;
 }
 
-// picture_coding_type of the first picture in es (0: none found)
-int trick_first_picture_type(const std::vector<uint8_t>& es)
+// VLC lookup of one ISO 11172-2 table, two levels so that it stays in cache: e[next `first` bits] = (code length << 16) |
+// (uint16_t)value, (1 << 31) | offset of a table of the next `bits` - `first` bits for longer codes, or 0 where no code starts
+struct TrickVlc {
+    std::vector<uint32_t> e;
+    int bits = 0, first = 0;
+    TrickVlc(const ef_vlc_code* c, int n, const char* extra = nullptr, int extra_value = 0)
+    {
+        for (int i = 0; i < n; i++) bits = std::max(bits, (int)strlen(c[i].code));
+        first = std::min(bits, 10);
+        const int sub = bits - first;
+        e.assign((size_t)1 << first, 0);
+        for (int i = 0; i <= n; i++) {
+            const char* code = i < n ? c[i].code : extra;
+            if (!code) break;
+            const int len = (int)strlen(code);
+            const uint32_t val = ((uint32_t)len << 16) | (uint16_t)(i < n ? c[i].value : extra_value);
+            uint32_t v = 0;
+            for (int k = 0; k < len; k++) v = (v << 1) | (uint32_t)(code[k] == '1');
+            if (len <= first) {
+                for (uint32_t t = 0; t < (1u << (first - len)); t++) e[(v << (first - len)) | t] = val;
+                continue;
+            }
+            const uint32_t pre = v >> (len - first);
+            if (!(e[pre] >> 31)) { e[pre] = (1u << 31) | (uint32_t)e.size(); e.resize(e.size() + ((size_t)1 << sub), 0); }
+            const uint32_t off = e[pre] & 0x7FFFFFFFu, rest = v & ((1u << (len - first)) - 1);
+            for (uint32_t t = 0; t < (1u << (bits - len)); t++) e[off + ((rest << (bits - len)) | t)] = val;
+        }
+    }
+};
+
+struct TrickBits {                               // MSB-first reader; bytes past the end read as 0
+    const uint8_t* p; size_t n, pos;
+    uint32_t peek(int k) const                   // k <= 25
+    {
+        const size_t b = pos >> 3;
+        uint64_t w = 0;
+        if (b + 8 <= n) { memcpy(&w, p + b, 8); w = __builtin_bswap64(w); }
+        else for (size_t i = 0; i < 8; i++) w = (w << 8) | (b + i < n ? p[b + i] : 0);
+        return (uint32_t)((w << (pos & 7)) >> (64 - k));
+    }
+    uint32_t get(int k) { const uint32_t v = k ? peek(k) : 0; pos += k; return v; }
+    bool vlc(const TrickVlc& t, int* v)
+    {
+        uint32_t e = t.e[peek(t.first)];
+        if (e >> 31) e = t.e[(e & 0x7FFFFFFFu) + (peek(t.bits) & ((1u << (t.bits - t.first)) - 1))];
+        if (!e) return false;
+        pos += e >> 16; *v = (int16_t)(e & 0xFFFF);
+        return true;
+    }
+};
+
+// one block's codes (block(), player.cpp:999-1148); false on a code the tables do not hold or a run past the block
+bool trick_skip_block(TrickBits& r, int blk, bool intra)
 {
-    for (size_t i = 0; i + 5 < es.size(); i++)
-        if (es[i] == 0 && es[i + 1] == 0 && es[i + 2] == 1 && es[i + 3] == 0) return (es[i + 5] >> 3) & 7;
-    return 0;
+    static const TrickVlc dct(ef_vlc_dct, EF_VLC_DCT_COUNT, "000001", 0), dcl(ef_vlc_dc_luma, EF_VLC_DC_LUMA_COUNT),
+        dcc(ef_vlc_dc_chroma, EF_VLC_DC_CHROMA_COUNT);
+    int n = 0, v;
+    if (intra) {
+        if (!r.vlc(blk < 4 ? dcl : dcc, &v)) return false;
+        r.get(v);
+        n = 1;
+    }
+    for (;;) {
+        const uint32_t p = r.peek(2);
+        if (n && p == 2) { r.pos += 2; return true; }
+        int run = 0;
+        if (p >> 1) r.pos += n ? 3 : 2;                          // run 0 level 1 and its sign
+        else {
+            if (!r.vlc(dct, &v)) return false;
+            if (v == 0) { run = (int)r.get(6); const uint32_t l = r.get(8); if (l == 0 || l == 128) r.get(8); }
+            else { run = v >> 8; r.pos += 1; }
+        }
+        n += run;
+        if (n >= 64) return false;
+        n++;
+    }
+}
+
+// Whether a segment may start at es, which begins with a sequence header: a decode from the cleared frame stores then gives
+// the frames of a continuous decode. The two stores alternate, so the first picture must write every macroblock of the
+// picture from its own codes, and the second every one, coded or skipped (a skip copies from the first). The slices are
+// walked as the decoder walks them (slice(), player.cpp:1238-1316): a slice starts at column 0 of its row whatever its first
+// increment, runs across rows, and an increment above 1 skips macroblocks, which an I picture copies from the other store.
+// The first picture must be intra and the second intra or predicted. 1 yes, 0 no, -1 es ends before the answer (`whole`: es
+// holds the rest of the main).
+int trick_pictures_whole(const std::vector<uint8_t>& es, bool whole)
+{
+    static const TrickVlc mba(ef_vlc_mba, EF_VLC_MBA_COUNT), type_i(ef_vlc_mbtype_i, EF_VLC_MBTYPE_I_COUNT),
+        type_p(ef_vlc_mbtype_p, EF_VLC_MBTYPE_P_COUNT), cbp(ef_vlc_cbp, EF_VLC_CBP_COUNT), mv(ef_vlc_mv, EF_VLC_MV_COUNT);
+    if (es.size() < 8 || es[0] || es[1] || es[2] != 1 || es[3] != 0xB3) return whole ? 0 : -1;
+    const int mbw = (((es[4] << 4) | (es[5] >> 4)) + 15) >> 4, mbh = ((((es[5] & 15) << 8) | es[6]) + 15) >> 4;
+    if (mbw < 1 || mbh < 1) return 0;
+    const int tw = std::min(mbw, EF_MBW_MAX), th = std::min(mbh, EF_MBH_MAX);
+    uint8_t mb[2][EF_MBW_MAX * EF_MBH_MAX] = {};    // per picture: 0 not written, 1 skipped, 2 coded (the last write counts)
+    int pics = 0, type = 0, r_size = 0;
+    bool done = false;
+    const uint8_t* d = es.data();
+    for (size_t j = 2; j + 1 < es.size(); j++) {                        // j: the 0x01 of a start code, found with memchr
+        const uint8_t* hit = (const uint8_t*)memchr(d + j, 1, es.size() - 1 - j);
+        if (!hit) break;
+        j = (size_t)(hit - d);
+        if (d[j - 1] || d[j - 2]) continue;
+        const size_t i = j - 2;
+        const uint8_t c = es[i + 3];
+        if (c == 0x00) {
+            if (pics == 2) { done = true; break; }
+            if (i + 9 > es.size()) return whole ? 0 : -1;
+            TrickBits h = { d + i + 4, 5, 0 };
+            h.get(10);
+            type = (int)h.get(3);
+            if (type != 1 && (pics == 0 || type != 2)) return 0;
+            h.get(16);
+            if (type == 2) { h.get(1); r_size = (int)h.get(3) - 1; if (r_size < 0) return 0; }
+            pics++;
+        } else if (c == 0xB7) { done = true; break; }
+        else if (pics && c >= 0x01 && c <= 0xAF) {
+            const uint8_t* nx = nullptr;                                 // the next start code ends the slice's bytes
+            for (size_t k = i + 4; k + 2 < es.size() && !nx; k++) {
+                const uint8_t* q = (const uint8_t*)memchr(d + k, 1, es.size() - k);
+                if (!q) break;
+                k = (size_t)(q - d);
+                if (k >= i + 6 && !q[-1] && !q[-2]) nx = q - 2;
+            }
+            if (!nx && !whole) return -1;
+            TrickBits r = { d + i + 4, (size_t)((nx ? nx : d + es.size()) - (d + i + 4)), 0 };
+            int x = mbw - 1, y = c - 2;
+            if (y >= mbh) continue;
+            r.get(5);
+            while (r.get(1)) r.get(8);
+            uint8_t* m = mb[pics - 1];
+            auto step = [&]() { if (++x >= mbw) { x -= mbw; y++; } };
+            for (int k = 0; r.peek(23) != 0; k++) {
+                int inc = 0, v;
+                if (!r.vlc(mba, &v)) return 0;
+                while (v == 34) if (!r.vlc(mba, &v)) return 0;
+                while (v == 35) { inc += 33; if (!r.vlc(mba, &v)) return 0; }
+                inc += v;
+                if (k) for (; inc > 1 && y < EF_MBH_MAX; inc--) { step(); if (y < EF_MBH_MAX && x < EF_MBW_MAX) m[y * EF_MBW_MAX + x] = 1; }
+                step();
+                if (y >= EF_MBH_MAX) break;
+                if (x < EF_MBW_MAX) m[y * EF_MBW_MAX + x] = 2;
+                int t;
+                if (!r.vlc(type == 1 ? type_i : type_p, &t)) return 0;
+                const bool intra = t & 0x01;
+                if (t & 0x10) r.get(5);
+                if (!intra && (t & 0x08))
+                    for (int a = 0; a < 2; a++) { if (!r.vlc(mv, &v)) return 0; if (v && r_size) r.get(r_size); }
+                int pat = intra ? 63 : 0;
+                if ((t & 0x02) && !r.vlc(cbp, &pat)) return 0;
+                for (int b = 0; b < 6; b++)
+                    if ((pat & (0x20 >> b)) && !trick_skip_block(r, b, intra)) return 0;
+            }
+        }
+    }
+    if (!done && !whole) return -1;
+    if (!pics) return 0;
+    for (int yy = 0; yy < th; yy++)
+        for (int xx = 0; xx < tw; xx++)
+            if (mb[0][yy * EF_MBW_MAX + xx] != 2 || (pics == 2 && !mb[1][yy * EF_MBW_MAX + xx])) return 0;
+    return 1;
+}
+
+// trick_pictures_whole for the sequence header at packet `pkt`, whose PES must have a PTS parse_pts() accepts: the main (to
+// packet `end`) is read on to its third picture start code first, so the pictures are walked once
+int trick_cut_ok(const uint8_t* ts, uint64_t pkt, uint64_t end)
+{
+    std::vector<uint8_t> es;
+    bool ok;
+    uint64_t next = trick_video_es(ts, pkt, end, 4096, es, &ok);
+    if (!ok) return 0;
+    for (;;) {
+        int pics = 0;
+        for (size_t j = 2; j + 1 < es.size() && pics < 3; j++) {
+            const uint8_t* hit = (const uint8_t*)memchr(es.data() + j, 1, es.size() - 1 - j);
+            if (!hit) break;
+            j = (size_t)(hit - es.data());
+            if (!es[j - 1] && !es[j - 2] && es[j + 1] == 0x00) pics++;
+        }
+        if (pics >= 3 || next == end) break;
+        next = trick_video_es(ts, next, end, es.size() * 2, es, nullptr);
+    }
+    return trick_pictures_whole(es, next == end) == 1;
 }
 
 void trick_bits(std::vector<uint8_t>& out, uint32_t& acc, int& n, uint32_t v, int bits)
@@ -2420,7 +2602,8 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     for (int f = 0; f <= n_files; f++) poff[f] = (off[f] - off[0]) / 188;
     const uint64_t n_packets = poff[n_files];
 
-    // sequence headers: make_index()'s table (ef_tsidx_scan); cut before each one that starts a PES with a PTS and an I picture
+    // sequence headers: make_index()'s table (ef_tsidx_scan); cut before each one that starts a PES with a PTS and whose first two
+    // pictures are whole (trick_pictures_whole), so that the segment decoded from reset frame stores gives a continuous decode's frames
     std::vector<ef_tsidx_info> info((size_t)n_files);
     std::vector<int64_t> spts(n_packets + 1);
     std::vector<uint32_t> spos(n_packets + 1);
@@ -2434,17 +2617,31 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     for (int f = 0; f < n_files; f++) {
         if (!info[f].n_seq) return fail(EF_EINVAL, "main %d has no sequence header", f);
         bool ok;
+        es.clear();
         trick_video_es(base, poff[f] + spos[poff[f]], poff[f + 1], 16, es, &ok);
         int i = 0;
         while (i + 8 <= (int)es.size() && !(es[i] == 0 && es[i + 1] == 0 && es[i + 2] == 1 && es[i + 3] == 0xB3)) i++;
         if (i + 8 > (int)es.size()) return fail(EF_EINVAL, "main %d: its first sequence header is cut short", f);
         headers[f] = trick_header(es[i + 7] >> 4, es[i + 7] & 15);
+    }
+    std::vector<std::pair<uint64_t, uint64_t>> cand;                    // (packet, end of its main) of every later sequence header
+    for (int f = 0; f < n_files; f++)
+        for (uint32_t k = 1; k < info[f].n_seq; k++) cand.push_back({ poff[f] + spos[poff[f] + k], poff[f + 1] });
+    std::vector<uint8_t> cut(cand.size(), 0);
+    {   // each check walks two pictures' macroblocks: spread them over the host's cores
+        std::atomic<size_t> next_cand{ 0 };
+        auto work = [&]() { for (size_t c; (c = next_cand++) < cand.size();) cut[c] = trick_cut_ok(base, cand[c].first, cand[c].second) == 1; };
+        std::vector<std::thread> pool;
+        const unsigned nt = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(cand.size() / 64 + 1, 32));
+        for (unsigned t = 1; t < nt; t++) pool.emplace_back(work);
+        work();
+        for (std::thread& t : pool) t.join();
+    }
+    for (int f = 0, c = 0; f < n_files; f++) {
         segs.push_back({ f, poff[f], poff[f + 1] });
-        for (uint32_t k = 1; k < info[f].n_seq; k++) {
-            const uint64_t p = poff[f] + spos[poff[f] + k];
-            if (p <= segs.back().pkt0) continue;
-            trick_video_es(base, p, poff[f + 1], 4096, es, &ok);
-            if (!ok || trick_first_picture_type(es) != 1) continue;    // joins the segment before it
+        for (uint32_t k = 1; k < info[f].n_seq; k++, c++) {
+            const uint64_t p = cand[c].first;
+            if (p <= segs.back().pkt0 || !cut[c]) continue;                // joins the segment before it
             segs.back().pkt1 = p;
             segs.push_back({ f, p, poff[f + 1] });
         }

@@ -217,8 +217,10 @@ int ef_tsidx_samples(int device, const int64_t* seq_pts, const uint32_t* seq_pos
  * Stateless (no context); host buffers; the decode, the encoder and the mux run on `device`. The rule, byte for byte, is
  * tests/trick_cases.py.
  * ef_trick_build  video_fwd.ts and video_rwd.ts of n_files mains packed back to back (off[n_files + 1], multiples of 188). Every
- *                 main is decoded as the reference decodes it, cut at its sequence headers into segments decoded as one batch (a
- *                 sequence header whose PES has no valid PTS or whose first picture is not intra joins the segment before it). fwd
+ *                 main is decoded as the reference decodes it, cut at its sequence headers into segments decoded as one batch. A
+ *                 sequence header starts a segment only when its PES has a valid PTS, its first picture is intra and codes every
+ *                 macroblock, and the next picture codes or skips every one (a host walk of their macroblocks); otherwise it joins
+ *                 the segment before it, so each segment, decoded from cleared frame stores, gives a continuous decode's frames. fwd
  *                 picture k is main picture 15 k (the trick_speed merge_index writes), with pts p_0 + (p_15k - p_0) / 15 (a C
  *                 division; p_j = ef_picture_pts of main picture j); rwd holds the same pictures in reverse order with pts
  *                 f_0 + (f_{n-1} - f_{n-1-j}) (setpts=PTS/15 and -vf reverse). Every picture is one random-access point: a sequence

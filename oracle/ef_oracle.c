@@ -229,9 +229,28 @@ static void sequence(dec_t* d)                         /* player.cpp:658 */
 
 static void gop(dec_t* d) { get_bits(d, 25); get_bits(d, 7); }   /* player.cpp:680 (Q9: values unused) */
 
+/* which macroblocks each of the first EFO_COV_PICTURES pictures of the last efo_decode_es call wrote: 2 decoded from its own
+   codes, 1 copied by a skip (the last write counts), 0 not written (tests of ef_trick_build's segment rule) */
+#define EFO_COV_PICTURES 8
+static uint8_t g_cov[EFO_COV_PICTURES][264];
+static int g_cov_n;
+
+static void cover(const dec_t* d, uint8_t how)
+{
+    if (g_cov_n >= 1 && g_cov_n <= EFO_COV_PICTURES && d->mb_x < 22 && d->mb_y < 12) g_cov[g_cov_n - 1][d->mb_y * 22 + d->mb_x] = how;
+}
+
+int efo_coverage(uint8_t* out, int max_pictures)
+{
+    const int n = g_cov_n < max_pictures ? g_cov_n : max_pictures;
+    memcpy(out, g_cov, (size_t)(n < EFO_COV_PICTURES ? n : EFO_COV_PICTURES) * 264);
+    return g_cov_n;
+}
+
 static void picture(dec_t* d)                          /* player.cpp:704 */
 {
     flush_picture(d, 0);
+    g_cov_n++;
     get_bits(d, 10);
     d->picture_coding_type = (int)get_bits(d, 3);
     g_stats.pictures[d->picture_coding_type & 7]++;
@@ -484,11 +503,13 @@ static int slice(dec_t* d, int s)
                 if (d->mb_y >= 12) return -1;             /* past the frame's 12 strips: the reference writes out of bounds */
                 g_stats.skipped++;
                 predict_zero(d);
+                cover(d, 1);
                 increment--;
             }
             inc_mb(d);
         }
         if (d->mb_y >= 12) return -1;                  /* past the frame's 12 strips: the reference writes out of bounds */
+        cover(d, 2);
 
         int mb_type = get_vlc(d, d->picture_coding_type == 1 ? &T_type_i : &T_type_p);
         int intra = mb_type & 0x01;
@@ -518,6 +539,8 @@ long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
                    uint8_t* out_i420, size_t cap_frames, uint8_t* strips_out)
 {
     tables_init();
+    g_cov_n = 0;
+    memset(g_cov, 0, sizeof(g_cov));
     dec_t* d = (dec_t*)calloc(1, sizeof(dec_t));
     d->es = es; d->len = len;
     d->fb[0] = (uint8_t*)calloc(1, EFO_FRAME_BYTES + 64);   /* Frame::init zero-fills (player.cpp:25) */

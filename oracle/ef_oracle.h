@@ -39,6 +39,10 @@ size_t efo_demux_ts(const uint8_t* ts, size_t len, uint8_t* es, size_t es_cap,
 long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
                    uint8_t* out_i420, size_t cap_frames, uint8_t* strips_out);
 
+/* Macroblocks the first 8 pictures of the last efo_decode_es call wrote, 264 bytes per picture (row * 22 + column): 2 decoded
+ * from the picture's own codes, 1 copied by a skip (the last write counts), 0 not written. Returns the pictures decoded. */
+int efo_coverage(uint8_t* out, int max_pictures);
+
 /* Coverage counters accumulated by efo_decode_es since the last reset (process-global; tests only). */
 typedef struct {
     uint64_t pictures[8];      /* by picture_coding_type */

@@ -48,6 +48,8 @@ class Oracle:
         L.efo_field.argtypes = [VP, VP, ctypes.c_int, VP]
         L.efo_field_ex.argtypes = [VP, VP, VP, ctypes.c_int, ctypes.c_int, VP, ctypes.c_int, ctypes.c_int, VP]
         L.efo_stats_get.argtypes = [VP]
+        L.efo_coverage.restype = ctypes.c_int
+        L.efo_coverage.argtypes = [VP, ctypes.c_int]
         L.efo_paced_schedule.restype = ctypes.c_long
         L.efo_paced_schedule.argtypes = [VP, VP, ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_long, VP, VP]
         L.efo_paced_schedule_ex.restype = ctypes.c_long
@@ -169,6 +171,13 @@ class Oracle:
         out = np.zeros(2 * 352 + 160, dtype=np.uint16)
         self.lib.efo_blit(ctypes.byref(v), strips.ctypes.data, out.ctypes.data, line, x, width, frame_counter)
         return out
+
+    def coverage(self, max_pictures):
+        """uint8 [pictures, 264]: the macroblocks (row * 22 + column) each of the first pictures of the last decode wrote: 2 from
+        its own codes, 1 by a skip's copy, 0 not at all"""
+        out = np.zeros((8, 264), dtype=np.uint8)
+        n = self.lib.efo_coverage(out.ctypes.data, min(max_pictures, 8))
+        return out[:min(n, max_pictures, 8)].copy()
 
     def stats_reset(self):
         self.lib.efo_stats_reset()

@@ -16,6 +16,8 @@ Transform: FDCT_C, an integer separable DCT with fixed rounding (fdct()); quanti
 0 .. 255, AC level = round-half-away-from-zero of 8 F / (qscale q_intra[zz]) clamped to +-255, both in integers.
 Mux: efs_wrap_ts's layout with these pts: PID 0x100, one PES per picture (stream id 0xE0, flags 0x8080, a 5-byte PTS), every
 PES starts a packet and its last packet is padded with adaptation-field stuffing, one continuity counter through the file."""
+import collections
+import hashlib
 import os
 import re
 
@@ -234,12 +236,26 @@ def source(ts, oracle):
     return frames, pts, main_codes(es)
 
 
+_ENCODED = collections.OrderedDict()        # (frame digest, qscale, header) -> picture: mains repeat frames, the encoder is slow
+
+
+def _encode_cached(frame, qscale, header):
+    key = (hashlib.sha256(bytes(frame)).digest(), qscale, header)
+    if key in _ENCODED:
+        _ENCODED.move_to_end(key)
+    else:
+        _ENCODED[key] = encode_picture(frame, qscale, header)
+        if len(_ENCODED) > 512:
+            _ENCODED.popitem(last=False)
+    return _ENCODED[key]
+
+
 def restate(ts, oracle, qscale=DEFAULT_QSCALE, src=None):
     """video.ts -> (video_fwd.ts, video_rwd.ts, fwd source picture indices)"""
     frames, pts, codes = src if src is not None else source(ts, oracle)
     sel, f, r = select(pts)
     hdr = header_bytes(*codes)
-    pics = [encode_picture(frames[j], qscale, hdr) for j in sel]
+    pics = [_encode_cached(frames[j], qscale, hdr) for j in sel]
     return mux(pics, f), mux(pics[::-1], r), sel
 
 
