@@ -24,11 +24,17 @@
 // accepted frame's subband samples, the last 9 V rows and the modulator state. The whole-stream ef_audio_decode is
 // the same kernels with a zeroed state and every stream ended (DESIGN.md §4).
 // Quirks kept: decode_audio() decodes the first frame twice (once to learn the frame size, video.cpp:971), so the
-// filter memory already holds it when the real decode starts; a frame it rejects (bad sync byte, joint stereo,
-// 4 subbands) re-synthesises the previous frame's samples; 32-bit wrap-around of the accumulators. Domain: mono,
-// 8 subbands, 16 blocks (write_pcm_16(mono,128,1) passes 128 samples whatever the header says); a frame size that
-// does not divide the reference's 4 KB ring makes it read past the ring on the straddling frame (undefined there;
-// here the stream is simply linear).
+// filter memory already holds it when the real decode starts; a frame it rejects (bad sync byte, 4 subbands)
+// re-synthesises the previous frame's samples; 32-bit wrap-around of the accumulators. Domain: mono, 8 subbands,
+// 16 blocks, bit pool <= EF_SBC_MAX_BITPOOL (128) (write_pcm_16(mono,128,1) passes 128 samples whatever the header
+// says; the reference's bit allocation never ends above 128). Joint stereo (mode 3) is outside it: the reference sets
+// two channels and the header's block count before it rejects the frame, then synthesises both channels' blocks.
+// Out of the domain at frame 0: the stream reports -2 and decodes nothing; a later out-of-domain frame re-synthesises
+// the previous accepted samples, exactly like a rejected frame. A 4-subband frame (and a bad-sync frame right after it,
+// which leaves that header in force) makes the reference synthesise nothing and emit whatever its mono[128] held: that
+// frame is undefined there; the re-synthesised samples write the V rows the filter already ends with, so every later
+// frame agrees. A frame size that does not divide the reference's 4 KB ring makes it read past the ring on the
+// straddling frame (undefined there; here the stream is simply linear).
 #include "../../include/espflix_b200.h"
 #include "ef_common.cuh"
 #include "ef_sbc_tables.h"
@@ -40,15 +46,17 @@ __constant__ int c_window[10][8];
 __constant__ signed char c_offset8[4][8];
 
 // header + scale factors + bit allocation of one frame (get_samples / bit_allocation, sbc_decoder.cpp:141-305).
-// Returns the sum of bits over the 8 subbands, or -1 for a frame the reference rejects, -2 outside its domain.
+// Returns the sum of bits over the 8 subbands, or -1 for a frame the reference rejects, -2 outside its domain. A bit
+// pool above EF_SBC_MAX_BITPOOL is outside it: the slice loop below never reaches such a pool (each subband adds 16 over
+// the whole descent), so only the signed overflow of bitslice would end it.
 __device__ int sbc_frame_bits(const uint8_t* d, uint64_t avail, int* bits, int* sf)
 {
     if (avail < 4 || d[0] != 0x9C) return -1;
     const uint32_t b1 = d[1];
     const int frequency = (b1 >> 6) & 3, blocks = 4 * (((b1 >> 4) & 3) + 1), mode = (b1 >> 2) & 3;
     const int allocation = (b1 >> 1) & 1, subbands = (b1 & 1) ? 8 : 4, bitpool = avail > 2 ? d[2] : 0;
-    if (mode == 3 || subbands == 4) return -1;
-    if (mode != 0 || blocks != 16) return -2;
+    if (subbands == 4) return -1;
+    if (mode != 0 || blocks != 16 || bitpool > EF_SBC_MAX_BITPOOL) return -2;
     int bitneed[8], max_bitneed = 0;
 #pragma unroll
     for (int sb = 0; sb < 8; sb++) {

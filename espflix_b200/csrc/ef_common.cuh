@@ -176,7 +176,8 @@ struct EfCarryArgs {
 };
 
 // Per-stream audio state that one ef_decode_audio call hands to the next (ef_audio.cu). All zero = a fresh stream.
-#define EF_AUDIO_CARRY 264       // most bytes one SBC frame's bit loader reads: header + scale factors 8 + 16 blocks x 128 bits
+#define EF_SBC_MAX_BITPOOL 128   // 8 subbands x 16 bits: the bit allocation's slice loop cannot reach a larger pool (outside the domain)
+#define EF_AUDIO_CARRY (8 + 2 * EF_SBC_MAX_BITPOOL)   // most bytes one SBC frame's bit loader reads (264): header + scale factors 8 + 16 blocks x 128 bits
 struct __align__(16) EfAudioState {
     int32_t frame_size;      // 0 not learned yet, > 0 learned by the probe, -1 / -2 first frame rejected / outside the domain
     int32_t carry_len;       // bytes held back: [0, EF_AUDIO_CARRY)

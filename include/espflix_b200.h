@@ -255,8 +255,12 @@ int ef_trick_stage_ms(float* decode_ms, float* gather_ms, float* encode_ms, floa
  *                    int16 samples each at pcm + info[s].pcm_offset, and - when pdm is not NULL - every sample becomes
  *                    2 x 16 one-bit samples at pdm + 2 * pcm_offset (modulator state zero at the start of a stream).
  *                    pcm == NULL: sizing call, only info[] is filled. info[s].frame_size: > 0 bytes, 0 empty stream,
- *                    -1 first frame rejected by the reference (nothing decoded), -2 outside its domain (the reference
- *                    handles mono, 8 subbands, 16 blocks only). */
+ *                    -1 first frame rejected by the reference (bad sync byte or 4 subbands; nothing decoded), -2 first
+ *                    frame outside its domain (nothing decoded). The domain: mono, 8 subbands, 16 blocks, bit pool
+ *                    <= 128; joint stereo (mode 3) is outside it. A later frame that the reference rejects or that is
+ *                    outside the domain re-synthesises the previous accepted frame's samples. A 4-subband frame is the
+ *                    one rejected frame whose output the reference leaves undefined (it emits uninitialised samples and
+ *                    does not advance its filter; every later frame agrees with the re-synthesis). */
 typedef struct { int32_t frame_size; uint32_t n_frames; uint64_t pcm_offset; } ef_audio_info;
 int ef_audio_demux_ts(int device, const uint8_t* ts, const uint64_t* off, int n_files, uint8_t* es, uint64_t es_cap, uint64_t* es_off);
 int ef_audio_decode(int device, const uint8_t* sbc, const uint64_t* off, int n_streams, ef_audio_info* info,

@@ -113,13 +113,18 @@ size_t efo_build_idx(const uint8_t* const ts[3], const size_t len[3], uint8_t* o
 
 /* ---- audio (SURVEY.md 8f-3; oracle/ef_oracle_audio.c) ---------------------------------------------------------
  * efo_demux_audio_ts  payload of PID 0x101 / 0x102 as push_audio() receives it (player.cpp:381-432); returns the byte count
- * efo_sbc_frame       one SBC frame -> sb_sample[16][8] (get_samples, sbc_decoder.cpp:274-341); bytes consumed, -1 rejected,
- *                     -2 outside the reference's domain (not mono / not 16 blocks)
+ * efo_sbc_frame       one SBC frame -> sb_sample[16][8] (get_samples, sbc_decoder.cpp:274-341); bytes consumed, -1 rejected
+ *                     (bad sync, 4 subbands), -2 outside the reference's domain (not mono / not 16 blocks, joint stereo,
+ *                     bit pool > 128)
+ * efo_sbc_bits        the same frame's header, scale factors and bit allocation (sbc_decoder.cpp:142-233): the sum of the
+ *                     8 sample widths, -1 or -2 as efo_sbc_frame; bits[8] = the widths (zero unless the sum is >= 0)
  * efo_sbc_decode      decode_audio() + sbc_decoder() over the pushed bytes (video.cpp:964-986): PCM samples produced
- *                     (stores <= cap_samples), -2 outside the domain
+ *                     (stores <= cap_samples), -1 frame 0 rejected, -2 frame 0 outside the domain; a later out-of-domain
+ *                     frame re-synthesises the previous samples, like a rejected frame
  * efo_pdm             pdm_second_order (espflix.ino:73-107) from reset state: 2 n words of 16 one-bit samples */
 size_t efo_demux_audio_ts(const uint8_t* ts, size_t len, uint8_t* es, size_t cap);
 int efo_sbc_frame(const uint8_t* data, size_t len, int32_t sb_sample[16][8]);
+int efo_sbc_bits(const uint8_t* data, size_t len, int bits[8]);
 long efo_sbc_decode(const uint8_t* es, size_t len, int16_t* pcm, size_t cap_samples);
 void efo_pdm(const int16_t* pcm, size_t n, uint16_t* out);
 

@@ -7,9 +7,12 @@
  *   efo_sbc_decode       decode_audio() driving sbc_decoder()                  src/video.cpp:964-986, sbc_decoder.cpp:343-373
  *   efo_pdm              pdm_second_order()                                    espflix.ino:73-107
  * Parity status: PINNED against the unmodified reference (oracle/_ref/efref_audio) on the audio of the reference's
- * own splash.ts / vmedia.ts (tests/golden/audio_pins.json) and on synthetic SBC streams (tests/test_audio.py).
- * Domain: mono, 8 subbands, 16 blocks (what the reference's ffmpeg line produces; write_pcm_16(mono,128,1) passes 128
- * samples whatever the header says, so other shapes read uninitialised stack there), first audio payload >= 64 bytes
+ * own splash.ts / vmedia.ts (tests/golden/audio_pins.json), on synthetic SBC streams (tests/test_audio.py) and on
+ * directed frames across the whole header domain (tests/golden/sbc_pins.json, tests/test_sbc_domain.py).
+ * Domain: mono, 8 subbands, 16 blocks, bit pool <= 128 (what the reference's ffmpeg line produces; write_pcm_16(mono,
+ * 128,1) passes 128 samples whatever the header says, so other shapes read uninitialised stack there, and the bit
+ * allocation never ends above 128); joint stereo is outside it, since the reference synthesises two channels' blocks
+ * for such a frame; first audio payload >= 64 bytes
  * (decode_audio probes the frame size on the first 64 bytes of its ring). Constant tables: espflix_b200/csrc/ef_sbc_tables.h
  * (spec constants, checked against the reference's arrays by tests/test_tables.py). */
 #include <stdlib.h>
@@ -63,7 +66,9 @@ size_t efo_demux_audio_ts(const uint8_t* ts, size_t len, uint8_t* es, size_t cap
 }
 
 /* ---- one SBC frame -> 16 x 8 subband samples (sbc_decoder.cpp:141-341). Returns the bytes the bit loader consumed
- * (what the reference uses as the frame size), -1 for a frame it rejects (bad sync, joint stereo, 4 subbands). */
+ * (what the reference uses as the frame size), or sbc_header's -1 / -2. */
+#define EFO_SBC_MAX_BITPOOL 128                            /* EF_SBC_MAX_BITPOOL of espflix_b200/csrc/ef_common.cuh */
+
 static void bit_allocation8(int frequency, int allocation, int bitpool, const uint8_t* sf, int* bits)
 {
     int bitneed[8], max_bitneed = 0;
@@ -101,17 +106,38 @@ static void bit_allocation8(int frequency, int allocation, int bitpool, const ui
         if (bits[sb] < 16) { bits[sb]++; bitcount++; }
 }
 
-int efo_sbc_frame(const uint8_t* data, size_t len, int32_t sb_sample[16][8])
+/* header + scale factors + bit allocation: the sum of the 8 widths, or -1 for a frame the reference rejects (bad sync,
+ * 4 subbands), -2 outside its domain (see the header comment): not mono / 16 blocks, joint stereo (the reference sets
+ * two channels and the header's block count before it rejects such a frame, then synthesises both channels), or a bit
+ * pool above EFO_SBC_MAX_BITPOOL, which bit_allocation8's slice loop never reaches (each subband adds 16 over the whole
+ * descent: only the signed overflow of bitslice would end it) */
+static int sbc_header(const uint8_t* data, size_t len, uint8_t sf[8], int bits[8])
 {
     if (len < 4 || data[0] != 0x9C) return -1;
     const int frequency = (data[1] >> 6) & 3, blocks = 4 * (((data[1] >> 4) & 3) + 1), mode = (data[1] >> 2) & 3;
     const int allocation = (data[1] >> 1) & 1, subbands = (data[1] & 1) ? 8 : 4, bitpool = data[2];
-    if (mode == 3 || subbands == 4) return -1;
-    if (mode != 0 || blocks != 16) return -2;                  /* outside the reference's own domain (see the header comment) */
-    uint8_t sf[8];
+    if (subbands == 4) return -1;
+    if (mode != 0 || blocks != 16 || bitpool > EFO_SBC_MAX_BITPOOL) return -2;
     for (int sb = 0; sb < 8; sb += 2) { uint8_t a = 4 + (size_t)(sb >> 1) < len ? data[4 + (sb >> 1)] : 0; sf[sb] = a >> 4; sf[sb + 1] = a & 15; }
-    int bits[8];
     bit_allocation8(frequency, allocation, bitpool, sf, bits);
+    int total = 0;
+    for (int sb = 0; sb < 8; sb++) total += bits[sb];
+    return total;
+}
+
+int efo_sbc_bits(const uint8_t* data, size_t len, int bits[8])
+{
+    uint8_t sf[8];
+    for (int sb = 0; sb < 8; sb++) bits[sb] = 0;
+    return sbc_header(data, len, sf, bits);
+}
+
+int efo_sbc_frame(const uint8_t* data, size_t len, int32_t sb_sample[16][8])
+{
+    uint8_t sf[8];
+    int bits[8];
+    const int total = sbc_header(data, len, sf, bits);
+    if (total < 0) return total;
     const uint8_t* p = data + 8;
     uint32_t acc = 0;
     int have = 0;
@@ -166,7 +192,8 @@ static void efo_sbc_synth(efo_sbc_state* s, const int32_t* src, int16_t* dst)
 
 /* decode_audio() over everything push_audio() received (video.cpp:964-986), "instant audio thread": the first call
  * decodes the first 64 bytes once to learn the frame size (and leaves that frame in the filter memory), then whole
- * frames are decoded in order; a rejected frame re-synthesises the previous frame's subband samples. */
+ * frames are decoded in order; a rejected frame re-synthesises the previous frame's subband samples. Frame 0 outside
+ * the domain: -2, nothing decoded; a later frame outside it re-synthesises like a rejected frame. */
 long efo_sbc_decode(const uint8_t* es, size_t len, int16_t* pcm, size_t cap_samples)
 {
     if (!len) return 0;
@@ -181,8 +208,7 @@ long efo_sbc_decode(const uint8_t* es, size_t len, int16_t* pcm, size_t cap_samp
     if (frame_size <= 0) return frame_size == 0 ? 0 : -1;      /* the reference stalls / misbehaves here: outside the domain */
     long n = 0;
     for (size_t r = 0; r + (size_t)frame_size <= len; r += (size_t)frame_size) {
-        int fs = efo_sbc_frame(es + r, len - r, sb);           /* a rejected frame leaves sb[] as it was */
-        if (fs == -2) return -2;
+        efo_sbc_frame(es + r, len - r, sb);                    /* a rejected or out-of-domain frame leaves sb[] as it was */
         for (int blk = 0; blk < 16; blk++) {
             int16_t out[8];
             efo_sbc_synth(&st, sb[blk], out);

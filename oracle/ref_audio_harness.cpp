@@ -10,7 +10,11 @@
 //   * write_pcm_16 (an ESP-only hook, espflix.ino:123) records the PCM and runs pdm_second_order, whose text the
 //     Makefile extracts from espflix.ino into _ref/pdm_extract.inc at build time (the sketch itself needs the Arduino SDK).
 // CLI (one run per process: decoder scratch, _sbc and the modulator state are process globals):
-//   efref_audio <in.ts> <out.bin>   out = u64 es_bytes, u64 pcm_samples, es bytes, pcm int16[], pdm uint16[2*pcm]
+//   efref_audio <in.ts> <out.bin>       out = u64 es_bytes, u64 pcm_samples, es bytes, pcm int16[], pdm uint16[2*pcm]
+//   efref_audio -es <in.sbc> <out.bin>  the SBC bytes handed to the REAL push_audio in one call, then decode_audio until
+//                                       it stops: every byte a frame's bit loader reads is in the ring when the frame
+//                                       is decoded (a stream of at most 4 KB - 264 bytes never wraps the ring, and the
+//                                       bytes after its end are the ring's initial zeros); same output file
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -55,17 +59,42 @@ void efref_hook_push_audio(const uint8_t* data, int len, int64_t pts, bool pes_c
 }
 void efref_hook_push_video(Frame*, int, int64_t, int) {}
 
+static void write_out(const char* path)
+{
+    FILE* o = fopen(path, "wb");
+    if (!o) { perror(path); _exit(2); }
+    uint64_t hdr[2] = { g_es.size(), g_pcm.size() };
+    fwrite(hdr, 8, 2, o);
+    fwrite(g_es.data(), 1, g_es.size(), o);
+    fwrite(g_pcm.data(), 2, g_pcm.size(), o);
+    fwrite(g_pdm.data(), 2, g_pdm.size(), o);
+    fclose(o);
+    fprintf(stdout, "{\"es_bytes\": %zu, \"pcm_samples\": %zu, \"pdm_words\": %zu}\n", g_es.size(), g_pcm.size(), g_pdm.size());
+    fflush(stdout);
+}
+
 int main(int argc, char** argv)
 {
-    if (argc < 3) { fprintf(stderr, "usage: %s in.ts out.bin\n", argv[0]); return 2; }
-    FILE* f = fopen(argv[1], "rb");
-    if (!f) { perror(argv[1]); return 2; }
+    const bool es_mode = argc >= 4 && !strcmp(argv[1], "-es");
+    if (argc < 3) { fprintf(stderr, "usage: %s [-es] in.ts|in.sbc out.bin\n", argv[0]); return 2; }
+    const char* in = argv[es_mode ? 2 : 1];
+    const char* out = argv[es_mode ? 3 : 2];
+    FILE* f = fopen(in, "rb");
+    if (!f) { perror(in); return 2; }
     std::vector<uint8_t> ts;
     uint8_t tmp[65536]; size_t n;
     while ((n = fread(tmp, 1, sizeof(tmp), f)) > 0) ts.insert(ts.end(), tmp, tmp + n);
     fclose(f);
 
     video_init(1);                    // sbc_init(&_sbc), video.cpp:595
+    if (es_mode) {
+        if (ts.size() + 264 > 4096) { fprintf(stderr, "%s: more than 4 KB - 264 bytes\n", in); return 2; }
+        g_es = ts;
+        if (!ts.empty()) push_audio(ts.data(), (int)ts.size(), 0, true);
+        while (decode_audio()) {}
+        write_out(out);
+        _exit(0);
+    }
     Frame* fb = new Frame[2];
     fb[0].init(); fb[1].init();
     MpegDecoder* dec = new MpegDecoder(&fb[0], &fb[1]);
@@ -91,15 +120,6 @@ int main(int argc, char** argv)
     while (!(get_events() & DECODER_PAUSED)) std::this_thread::sleep_for(std::chrono::microseconds(200));
     th->detach();
 
-    FILE* o = fopen(argv[2], "wb");
-    if (!o) { perror(argv[2]); _exit(2); }
-    uint64_t hdr[2] = { g_es.size(), g_pcm.size() };
-    fwrite(hdr, 8, 2, o);
-    fwrite(g_es.data(), 1, g_es.size(), o);
-    fwrite(g_pcm.data(), 2, g_pcm.size(), o);
-    fwrite(g_pdm.data(), 2, g_pdm.size(), o);
-    fclose(o);
-    fprintf(stdout, "{\"es_bytes\": %zu, \"pcm_samples\": %zu, \"pdm_words\": %zu}\n", g_es.size(), g_pcm.size(), g_pdm.size());
-    fflush(stdout);
+    write_out(out);
     _exit(0);
 }

@@ -63,6 +63,8 @@ class Oracle:
         L.efo_demux_audio_ts.restype = ctypes.c_size_t
         L.efo_demux_audio_ts.argtypes = [VP, ctypes.c_size_t, VP, ctypes.c_size_t]
         L.efo_sbc_decode.restype = ctypes.c_long
+        L.efo_sbc_bits.restype = ctypes.c_int
+        L.efo_sbc_bits.argtypes = [VP, ctypes.c_size_t, VP]
         L.efo_sbc_decode.argtypes = [VP, ctypes.c_size_t, VP, ctypes.c_size_t]
         L.efo_pdm.argtypes = [VP, ctypes.c_size_t, VP]
         self._video = {}
@@ -81,6 +83,15 @@ class Oracle:
         pcm = np.zeros(cap, dtype=np.int16)
         n = self.lib.efo_sbc_decode(es.ctypes.data if es.size else pcm.ctypes.data, es.size, pcm.ctypes.data, cap)
         return int(n) if n < 0 else pcm[:n].copy()
+
+    def sbc_bits(self, frame):
+        """-> (sum of the 8 sample widths or -1 / -2, the 8 widths) of one SBC frame's header, scale factors and bit allocation"""
+        d = np.ascontiguousarray(np.frombuffer(bytes(frame), dtype=np.uint8))
+        buf = np.zeros(max(d.size, 1), dtype=np.uint8)
+        buf[:d.size] = d
+        bits = np.zeros(8, dtype=np.int32)
+        total = self.lib.efo_sbc_bits(buf.ctypes.data, d.size, bits.ctypes.data)
+        return int(total), [int(b) for b in bits]
 
     def pdm(self, pcm):
         pcm = np.ascontiguousarray(pcm, dtype=np.int16)

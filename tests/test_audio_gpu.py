@@ -42,7 +42,7 @@ def test_reference_fixture_audio(oracle):
 
 def test_batch_of_synthetic_streams(oracle):
     """many streams of different shape in one call: both allocation modes, all frequencies, bit pools 2..120 (sample
-    widths 0, 2..16), inconsistent scale factors (the bit loader runs into the next frame / past the end), rejected
+    widths 0..16: the allocation's last loop gives width 1 too), inconsistent scale factors (the bit loader runs into the next frame / past the end), rejected
     frames (re-synthesis of the previous samples), empty and sub-frame streams, loud streams (32-bit wrap-around)."""
     streams = []
     for i in range(48):
