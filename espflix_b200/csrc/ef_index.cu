@@ -7,6 +7,12 @@
 // start codes are byte aligned in every stream it accepts (Q8), so here a warp sweeps 512 bytes of
 // one stream per step with 128-bit loads, finds "00 00 01 xx" with byte permutes, and orders the
 // hits with a ballot + popcount prefix so the picture/slice tables come out in stream order.
+// One exception to "every byte-aligned 00 00 01 xx is a start code": sequence() reads its quantiser
+// matrices with get_bits and run() searches on from the end of the header (player.cpp:666-671,
+// 1360-1363), so a hit inside a sequence header's 8 / 72 / 136 bytes (code included: 12 + 64 per
+// loaded matrix) is not one. Zero matrix entries make such hits (the non-intra matrix starts byte
+// aligned: entries 0, 0, 1, c are the bytes 00 00 01 c); the sweep skips them with a warp-uniform
+// skip_to set at every 0xB3 hit.
 //   ef_scan_kernel    one warp per stream   -> seq[], pics[], slice_off[], slice_code[], n_pics[]
 //   ef_prefix_kernel  one CTA               -> per picture index: exclusive prefix over streams
 //   ef_fill_kernel    one thread per (picture, stream) -> flat EfWork list per picture index
@@ -81,6 +87,7 @@ ef_scan_kernel(EfDev* __restrict__ Dp, EfCarryArgs C)
     uint32_t n_pic = 0, n_slice = 0, n_seq = 0;           // warp-uniform running counts
     // fp_rs: full_pel | r_size << 1 of the last P header (stale state a B/D picture would see)
     bool stop = false;
+    uint64_t skip_to = 0;                                 // end of the last sequence header: hits before it are matrix bytes
     // kCarry: the open unit (0 none, 1 headers only, 2 with its picture header), where it starts, its picture's code byte,
     // and the counts and P-vector state as of the last complete unit
     int open = 0;
@@ -135,6 +142,7 @@ ef_scan_kernel(EfDev* __restrict__ Dp, EfCarryArgs C)
                 h &= h - 1;
                 if (obase + i < misalign || obase + i - misalign + 4 > len) continue;   // window bytes outside the stream (alignment slack, tail)
                 const uint64_t pos = obase + i - misalign;                    // first 00 of the start code
+                if (pos < skip_to) continue;                                  // inside a sequence header (warp-uniform)
                 // the start-code value is byte i + 3 of the owning lane's 20-byte window: a shuffle, not another
                 // dependent global load per start code (the sweep is latency bound, ~170 start codes per stream)
                 const int bi = i + 3;
@@ -171,13 +179,14 @@ ef_scan_kernel(EfDev* __restrict__ Dp, EfCarryArgs C)
                         if (j < (uint32_t)D.max_slices && lane == 0) { soff[j] = (uint32_t)(pos + 4); scode[j] = (uint8_t)code; }
                     }
                 } else if (code == 0xB3) {                                    // sequence(), player.cpp:658
+                    const uint64_t hb = (pos + 4) * 8;
+                    const uint32_t load_intra = bits_at(es, len, hb + 62, 1);
+                    const uint64_t after_intra = hb + 63 + (load_intra ? 512 : 0);
+                    const uint32_t load_inter = bits_at(es, len, after_intra, 1);
+                    skip_to = pos + 12 + (load_intra ? 64 : 0) + (load_inter ? 64 : 0);
                     const uint32_t k = ++n_seq;
                     if (k <= (uint32_t)D.max_seq) {
-                        const uint64_t hb = (pos + 4) * 8;
                         const uint32_t hsize = bits_at(es, len, hb, 12), vsize = bits_at(es, len, hb + 12, 12);
-                        const uint32_t load_intra = bits_at(es, len, hb + 62, 1);
-                        const uint64_t after_intra = hb + 63 + (load_intra ? 512 : 0);
-                        const uint32_t load_inter = bits_at(es, len, after_intra, 1);
                         EfSeq* q = seqs + k;
                         for (int n = lane; n < 64; n += 32) {
                             // Q4: the decoder keeps the 64 bytes in stream order and indexes them with the raster

@@ -535,6 +535,11 @@ static int slice(dec_t* d, int s)
 /* ------------------------------------------------------------------------------------------
  * run / marker (player.cpp:1318-1367)
  * ---------------------------------------------------------------------------------------- */
+/* efo_walk's record of the markers efo_decode_es dispatches (NULL: not recording) */
+static uint64_t* g_walk_pos;
+static uint8_t* g_walk_code;
+static size_t g_walk_cap, g_walk_n;
+
 long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
                    uint8_t* out_i420, size_t cap_frames, uint8_t* strips_out)
 {
@@ -555,8 +560,11 @@ long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
     size_t limit = (len + 16) * 8;
     while (!d->ended && d->bitpos < limit) {
         while (peek_bits(d, 24) == 0 && d->bitpos < limit) d->bitpos++;
+        const size_t at = d->bitpos;
         get_bits(d, 24);
         int m = (int)get_bits(d, 8);
+        if (g_walk_n < g_walk_cap) { g_walk_pos[g_walk_n] = at; g_walk_code[g_walk_n] = (uint8_t)m; }
+        g_walk_n++;
         switch (m) {
             case 0xB3: sequence(d); break;
             case 0xB8: gop(d); break;
@@ -570,6 +578,22 @@ long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
     if (strips_out) { memcpy(strips_out, d->fb[0], EFO_FRAME_BYTES); memcpy(strips_out + EFO_FRAME_BYTES, d->fb[1], EFO_FRAME_BYTES); }
     long n = (long)d->n_out;
     free(d->fb[0]); free(d->fb[1]); free(d);
+    return n;
+}
+
+long efo_walk(const uint8_t* es, size_t len, uint64_t* pos, uint8_t* code, size_t cap, long counts[3])
+{
+    g_walk_pos = pos; g_walk_code = code; g_walk_cap = pos && code ? cap : 0; g_walk_n = 0;
+    efo_decode_es(es, len, 1, NULL, 0, NULL);
+    const long n = (long)g_walk_n;
+    if (counts) {
+        counts[0] = counts[1] = counts[2] = 0;
+        for (size_t i = 0; i < g_walk_n && i < g_walk_cap; i++) {
+            const uint8_t m = code[i];
+            counts[0] += m == 0x00; counts[1] += m >= 0x01 && m <= 0xAF; counts[2] += m == 0xB3;
+        }
+    }
+    g_walk_pos = NULL; g_walk_code = NULL; g_walk_cap = 0; g_walk_n = 0;
     return n;
 }
 

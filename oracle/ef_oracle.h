@@ -39,6 +39,12 @@ size_t efo_demux_ts(const uint8_t* ts, size_t len, uint8_t* es, size_t es_cap,
 long efo_decode_es(const uint8_t* es, size_t len, int has_pts,
                    uint8_t* out_i420, size_t cap_frames, uint8_t* strips_out);
 
+/* The marker walk of efo_decode_es (run(), player.cpp:1355-1366) over an elementary stream: every marker it dispatches,
+ * in order, as the bit position of its 24-bit prefix (pos[], may lie in the end-of-stream padding the reader appends) and
+ * its code byte (code[]), the first cap of them. counts[3] (optional) = the picture, slice (codes 0x01-0xAF) and
+ * sequence-header markers dispatched. Returns the number of markers dispatched. */
+long efo_walk(const uint8_t* es, size_t len, uint64_t* pos, uint8_t* code, size_t cap, long counts[3]);
+
 /* Macroblocks the first 8 pictures of the last efo_decode_es call wrote, 264 bytes per picture (row * 22 + column): 2 decoded
  * from the picture's own codes, 1 copied by a skip (the last write counts), 0 not written. Returns the pictures decoded. */
 int efo_coverage(uint8_t* out, int max_pictures);

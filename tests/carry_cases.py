@@ -14,7 +14,7 @@ import bisect
 
 import numpy as np
 
-from tests import pts_cases
+from tests import pts_cases, scan_cases
 
 UNIT_CODES = (0x00, 0xB3, 0xB8, 0xB7)
 
@@ -22,14 +22,8 @@ UNIT_CODES = (0x00, 0xB3, 0xB8, 0xB7)
 def scan(region, end=False):
     """K0 with carry over one stream's region -> (code byte offsets of the complete pictures, held bytes, code byte offset of
     the held picture or None)"""
-    region = bytes(region)
     pics, c_pic, open_, unit, unit_code, stop = [], 0, 0, 0, None, False
-    i = 0
-    while True:
-        i = region.find(b"\x00\x00\x01", i)
-        if i < 0 or i + 4 > len(region):
-            break
-        code = region[i + 3]
+    for i, code in scan_cases.start_codes(region):
         if code in UNIT_CODES:
             if open_ == 2 or code == 0xB7:
                 c_pic = len(pics)
@@ -44,7 +38,6 @@ def scan(region, end=False):
                 open_ = 1
         if code == 0x00:
             pics.append(i + 3)
-        i += 1
     if stop or end:
         return pics, 0, None
     if open_:

