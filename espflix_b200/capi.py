@@ -105,6 +105,8 @@ _SIGNATURES = {
     "ef_trick_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 4),
     "ef_library_add_trick": (_I, [_VP, _I, _I]),
     "ef_library_read": (_I, [_VP, _I, _I, _VP, ctypes.c_uint64, _U64P]),
+    "ef_encode_build": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
+    "ef_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 5),
 }
 
 # ef_library_command's commands and ef_library_info's stream states (include/espflix_b200.h)
@@ -656,6 +658,53 @@ def trick_build(mains, qscale=TRICK_QSCALE, device=0):
         cap = need
     _check_rc(lib, rc)
     return [(fwd[int(fo[i]):int(fo[i + 1])].tobytes(), rwd[int(ro[i]):int(ro[i + 1])].tobytes()) for i in range(n)]
+
+
+class EncodeParams(ctypes.Structure):
+    """ef_encode_params (include/espflix_b200.h)"""
+    _fields_ = [("gop", ctypes.c_int), ("qscale_i", ctypes.c_int), ("qscale_p", ctypes.c_int), ("search", ctypes.c_int),
+                ("aspect", ctypes.c_int), ("rate", ctypes.c_int), ("pts0", ctypes.c_int64), ("pts_step", ctypes.c_uint32)]
+
+
+# ef_encode_build's defaults (tests/encode_cases.DEFAULT_PARAMS, where the measurement behind the quantisers is): GOP 12 as ffmpeg's
+# mpeg1video and both fixtures; qscale 8 / 8, the largest that keeps every picture of both fixtures at or above 35 dB; search 7:
+# forward_f_code 1 reaches -8..7.5 pixels; aspect 1 (square samples), rate 2 and a pts step of 3,750: 24 pictures per second on the
+# 90 kHz clock.
+ENCODE_DEFAULTS = dict(gop=12, qscale_i=8, qscale_p=8, search=7, aspect=1, rate=2, pts0=0, pts_step=3750)
+PICTURE_BYTES = 101376
+
+
+def encode_build(titles, device=0, **params):
+    """ef_encode_build: video.ts of every title (a uint8 array of shape (n, 101376): 352 x 192 I420 pictures in display order)
+    -> [bytes, ...]"""
+    lib = load_library()
+    p = dict(ENCODE_DEFAULTS, **params)
+    arrs = [np.ascontiguousarray(np.asarray(t, dtype=np.uint8).reshape(-1, PICTURE_BYTES)) for t in titles]
+    n = len(arrs)
+    off = np.zeros(n + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([a.shape[0] for a in arrs])
+    blob = np.concatenate(arrs) if n else np.zeros((1, PICTURE_BYTES), np.uint8)
+    if blob.size == 0:
+        blob = np.zeros((1, PICTURE_BYTES), np.uint8)
+    par = EncodeParams(**{k: int(v) for k, v in p.items()})
+    to = np.zeros(n + 1, dtype=np.uint64)
+    cap = int(off[-1]) * 16384 + 188 * 64    # about twice the bytes per picture of the defaults on the fixtures; retried once when short
+    for _ in range(2):
+        ts = np.zeros(cap, dtype=np.uint8)
+        rc = lib.ef_encode_build(device, blob.ctypes.data, off.ctypes.data, n, ctypes.byref(par), ts.ctypes.data, ts.size, to.ctypes.data)
+        if rc != EF_ENOMEM or int(to[-1]) <= cap:
+            break
+        cap = int(to[-1])
+    _check_rc(lib, rc)
+    return [ts[int(to[i]):int(to[i + 1])].tobytes() for i in range(n)]
+
+
+def encode_stage_ms():
+    """(upload, search, code, reconstruction, mux) device milliseconds of the last encode_build on this thread"""
+    lib = load_library()
+    v = [ctypes.c_float() for _ in range(5)]
+    _check_rc(lib, lib.ef_encode_stage_ms(*[ctypes.byref(x) for x in v]))
+    return tuple(x.value for x in v)
 
 
 def trick_stage_ms():

@@ -45,6 +45,14 @@ cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, ui
 cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int n_pics,
                                      uint8_t* es, cudaStream_t st);
 cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st);
+cudaError_t ef_encode_upload_tables();
+cudaError_t ef_encode_launch_tile(const uint8_t* i420, const uint32_t* src, int count, uint8_t* tiled, cudaStream_t st);
+cudaError_t ef_encode_launch_search(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
+                                    const uint32_t* n_pics, int search, uint32_t* mbinfo, cudaStream_t st);
+cudaError_t ef_encode_launch_p(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
+                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st);
+cudaError_t ef_encode_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* header, int n_pics,
+                                      uint8_t* es, cudaStream_t st);
 __global__ void ef_tsidx_packet_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, int64_t* pkt_pts, uint8_t* pkt_kind);
 __global__ void ef_tsidx_compact_kernel(const uint64_t* pkt_off, const int64_t* pkt_pts, const uint8_t* pkt_kind, int64_t* seq_pts, uint32_t* seq_pos, int64_t* info);
 __global__ void ef_tsidx_sample_kernel(const int64_t* seq_pts, const uint32_t* seq_pos, int n, int64_t first_pts, uint32_t bin_size, uint32_t n_samples, uint32_t* samples);
@@ -2841,6 +2849,202 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     }
     return EF_OK;
 }
+
+}  // extern "C"
+
+// ---- encoded titles: video.ts of many titles from raw pictures (csrc/ef_encode.cu; the rule is tests/encode_cases.py) -------------
+namespace {
+
+// GOPs of one batch: every one is a stream of the decode context that reconstructs them (about 1.5 MB of device memory each at GOP
+// 12: its source pictures, two frame stores, one tiled picture, its slice regions and its share of the submit buffers). Longer GOPs
+// make smaller batches, so that a batch's source pictures stay at most 6,144 (620 MB).
+constexpr int kEncodeBatchGops = 512;
+constexpr int kEncodeBatchPictures = 6144;
+constexpr int kEncodeMaxGop = 1024;                // the 10-bit temporal reference of a picture counts within its GOP
+constexpr size_t kEncodeSubmitBytes = 32u << 20;   // ES bytes of one reconstruction submit (a larger round is split)
+thread_local float g_encode_ms[5] = { 0, 0, 0, 0, 0 };
+
+// the 9 bytes of a P picture header: temporal reference tref, vbv_delay 0xFFFF, full_pel_forward 0, forward_f_code 1
+std::vector<uint8_t> encode_p_header(int tref)
+{
+    std::vector<uint8_t> h = { 0, 0, 1, 0x00 };
+    uint32_t acc = 0; int n = 0;
+    trick_bits(h, acc, n, (uint32_t)tref, 10); trick_bits(h, acc, n, 2, 3); trick_bits(h, acc, n, 0xFFFF, 16);
+    trick_bits(h, acc, n, 0, 1); trick_bits(h, acc, n, 1, 3); trick_bits(h, acc, n, 0, 1); trick_bits(h, acc, n, 0, 6);
+    return h;
+}
+
+}  // namespace
+
+extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p, uint8_t* ts,
+                               uint64_t ts_cap, uint64_t* ts_off)
+{
+    if (!pic_off || n_titles < 1 || !p || !ts_off || !i420) return fail(EF_EINVAL, "null argument");
+    if (p->gop < 1 || p->gop > kEncodeMaxGop) return fail(EF_EINVAL, "gop %d outside 1..%d", p->gop, kEncodeMaxGop);
+    if (p->qscale_i < 1 || p->qscale_i > 31 || p->qscale_p < 1 || p->qscale_p > 31)
+        return fail(EF_EINVAL, "qscale_i %d / qscale_p %d outside 1..31", p->qscale_i, p->qscale_p);
+    if (p->search < 0 || p->search > 15) return fail(EF_EINVAL, "search %d outside 0..15", p->search);
+    if (p->aspect < 1 || p->aspect > 14 || p->rate < 1 || p->rate > 8) return fail(EF_EINVAL, "aspect %d / rate %d outside 1..14 / 1..8", p->aspect, p->rate);
+    for (int t = 0; t < n_titles; t++) {
+        if (pic_off[t + 1] <= pic_off[t]) return fail(EF_EINVAL, "title %d is empty (pictures %llu..%llu)", t, (unsigned long long)pic_off[t],
+                                                       (unsigned long long)pic_off[t + 1]);
+        const uint64_t n = pic_off[t + 1] - pic_off[t];
+        const __int128 last = (__int128)p->pts0 + (__int128)(n - 1) * p->pts_step;
+        if (p->pts0 < 0 || last >= ((__int128)1 << 33)) return fail(EF_EINVAL, "title %d: the pts of its %llu pictures leave 0..2^33 - 1", t, (unsigned long long)n);
+    }
+    if (pic_off[n_titles] - pic_off[0] > (1ull << 32)) return fail(EF_EINVAL, "more than 2^32 pictures in one call");
+    TRY(usable_device(device));
+    DeviceScope scope_(device);
+
+    // GOPs: (first picture relative to pic_off[0], pictures); every batch of GOPs is a contiguous run of pictures
+    struct Gop { uint64_t first; int n; };
+    std::vector<Gop> gops;
+    for (int t = 0; t < n_titles; t++)
+        for (uint64_t k = pic_off[t]; k < pic_off[t + 1]; k += (uint64_t)p->gop)
+            gops.push_back({ k - pic_off[0], (int)std::min<uint64_t>((uint64_t)p->gop, pic_off[t + 1] - k) });
+    const int B = (int)std::min<size_t>(gops.size(), std::min(kEncodeBatchGops, std::max(1, kEncodeBatchPictures / p->gop)));
+    const std::vector<uint8_t> i_hdr = trick_header(p->aspect, p->rate);
+
+    CK(ef_trick_upload_tables());
+    CK(ef_encode_upload_tables());
+    cudaStream_t st = 0;
+    TrickTimer timer;
+    GrowBuf d_src, d_tiled, d_list, d_info, d_slots, d_len, d_es, d_dst, d_hdr, d_off;
+    CK(d_tiled.reserve((size_t)B * EF_FRAME));
+    CK(d_list.reserve((size_t)B * 8));
+    CK(d_info.reserve((size_t)B * EF_MBW_MAX * EF_MBH_MAX * 4));
+    CK(d_slots.reserve((size_t)B * EF_MBH_MAX * std::max(kEncSliceBytes, kTrickSliceBytes)));
+    CK(d_len.reserve((size_t)B * EF_MBH_MAX * 4));
+    CK(d_dst.reserve((size_t)B * 8));
+    CK(d_hdr.reserve((size_t)B * kTrickHeaderBytes));
+    CK(d_off.reserve(((size_t)B + 1) * 8));
+    ef_ctx* ctx = nullptr;
+    struct CtxGuard { ef_ctx** c; ~CtxGuard() { if (*c) ef_destroy(*c); } } ctx_guard{ &ctx };
+    ef_config cfg = { device, B, 1, EF_MBH_MAX, kEncodeSubmitBytes, 0 };
+    TRY(ef_create(&ctx, &cfg));
+
+    std::vector<uint64_t> es_off(pic_off[n_titles] - pic_off[0]);      // every picture's bytes in d_es
+    std::vector<uint32_t> es_len(es_off.size());
+    uint64_t es_total = 0;
+    for (size_t g0 = 0; g0 < gops.size(); g0 += (size_t)B) {
+        const int nb = (int)std::min<size_t>((size_t)B, gops.size() - g0);
+        const uint64_t p0 = gops[g0].first, np = gops[g0 + nb - 1].first + gops[g0 + nb - 1].n - p0;
+        if (g0) TRY(ef_reset(ctx));
+        CK(d_src.reserve(np * EF_FRAME));
+        CK(timer.begin(st));
+        CK(cudaMemcpyAsync(d_src.p, i420 + (pic_off[0] + p0) * EF_FRAME, np * EF_FRAME, cudaMemcpyHostToDevice, st));
+        CK(timer.end(0, st));
+        for (int k = 0; k < p->gop; k++) {
+            // round k: picture k of every GOP of the batch that has one (all GOPs but a title's last are whole)
+            std::vector<uint32_t> act, src;
+            for (int g = 0; g < nb; g++)
+                if (gops[g0 + g].n > k) { act.push_back((uint32_t)g); src.push_back((uint32_t)(gops[g0 + g].first + k - p0)); }
+            if (act.empty()) break;
+            const int na = (int)act.size();
+            CK(cudaMemcpyAsync(d_list.p, act.data(), (size_t)na * 4, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_list.p + (size_t)B * 4, src.data(), (size_t)na * 4, cudaMemcpyHostToDevice, st));
+            const uint32_t* d_act = (const uint32_t*)d_list.p;
+            CK(timer.begin(st));
+            CK(ef_encode_launch_tile(d_src.p, (const uint32_t*)(d_list.p + (size_t)B * 4), na, d_tiled.p, st));
+            ctx->launches++;
+            if (k) {
+                CK(ef_encode_launch_search(d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, p->search, (uint32_t*)d_info.p, st));
+                ctx->launches++;
+                CK(timer.end(1, st));
+                CK(timer.begin(st));
+                CK(ef_encode_launch_p(d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, (const uint32_t*)d_info.p, p->qscale_p,
+                                      (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
+            } else CK(ef_trick_launch_encode(d_tiled.p, na, p->qscale_i, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
+            ctx->launches++;
+            std::vector<uint32_t> len((size_t)na * EF_MBH_MAX);
+            CK(cudaMemcpyAsync(len.data(), d_len.p, len.size() * 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            const uint32_t hb = k ? kEncPHeaderBytes : kTrickHeaderBytes;
+            std::vector<uint64_t> dst((size_t)na);
+            const uint64_t round0 = es_total;
+            for (int a = 0; a < na; a++) {
+                uint32_t bytes = hb;
+                for (int s = 0; s < EF_MBH_MAX; s++) bytes += len[(size_t)a * EF_MBH_MAX + s];
+                const uint64_t pic = p0 + src[a];
+                dst[a] = es_off[pic] = es_total; es_len[pic] = bytes;
+                es_total += bytes;
+            }
+            if (es_total + 16 > d_es.cap) CK(d_es.reserve(std::max<size_t>(es_total + 16, d_es.cap * 2), round0));
+            CK(cudaMemcpyAsync(d_dst.p, dst.data(), dst.size() * 8, cudaMemcpyHostToDevice, st));
+            if (k) {
+                const std::vector<uint8_t> h = encode_p_header(k);
+                CK(cudaMemcpyAsync(d_hdr.p, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+                CK(ef_encode_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, na, d_es.p, st));
+            } else {
+                std::vector<uint8_t> h((size_t)na * kTrickHeaderBytes);
+                for (int a = 0; a < na; a++) memcpy(&h[(size_t)a * kTrickHeaderBytes], i_hdr.data(), kTrickHeaderBytes);
+                CK(cudaMemcpyAsync(d_hdr.p, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+                CK(ef_trick_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, na, d_es.p, st));
+            }
+            ctx->launches++;
+            CK(timer.end(2, st));
+            // the decoder's reconstruction of round k: each GOP's picture in its own stream, in submits of at most kEncodeSubmitBytes
+            CK(timer.begin(st));
+            for (int a0 = 0; a0 < na;) {
+                int a1 = a0 + 1;
+                while (a1 < na && dst[a1] + es_len[p0 + src[a1]] - dst[a0] <= kEncodeSubmitBytes) a1++;
+                std::vector<uint64_t> off((size_t)B + 1);
+                for (int g = 0, a = a0; g <= B; g++) {
+                    while (a < a1 && (int)act[a] < g) a++;
+                    off[g] = (a < a1 ? dst[a] : dst[a1 - 1] + es_len[p0 + src[a1 - 1]]) - dst[a0];
+                }
+                CK(cudaMemcpyAsync(d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice, st));
+                TRY(ef_submit_es_device(ctx, d_es.p + dst[a0], (const uint64_t*)d_off.p, st));
+                TRY(ef_index(ctx, st));
+                TRY(decode_range(ctx, 0, 1, st));
+                a0 = a1;
+            }
+            CK(timer.end(3, st));
+        }
+    }
+    TRY(ef_index_info(ctx, nullptr, nullptr, nullptr, nullptr));
+
+    // one TS per title: a PES per picture with pts0 + k pts_step, one continuity counter per file
+    std::vector<EfTrickPic> plan;
+    uint64_t pk = 0;
+    ts_off[0] = 0;
+    for (int t = 0; t < n_titles; t++) {
+        uint32_t cc = 0;
+        for (uint64_t k = pic_off[t]; k < pic_off[t + 1]; k++) {
+            const uint64_t pic = k - pic_off[0];
+            plan.push_back({ es_off[pic], pk, p->pts0 + (int64_t)(k - pic_off[t]) * (int64_t)p->pts_step, es_len[pic], cc });
+            const uint32_t pkts = (14 + es_len[pic] + 183) / 184;
+            pk += pkts; cc += pkts;
+        }
+        ts_off[t + 1] = ts_off[t] + (uint64_t)cc * 188;
+    }
+    if (ts_cap < ts_off[n_titles] || !ts) return fail(EF_ENOMEM, "the titles need %llu bytes", (unsigned long long)ts_off[n_titles]);
+    GrowBuf d_plan, d_out;
+    CK(d_plan.reserve(plan.size() * sizeof(EfTrickPic)));
+    CK(d_out.reserve(pk * 188 + 16));
+    CK(cudaMemcpy(d_plan.p, plan.data(), plan.size() * sizeof(EfTrickPic), cudaMemcpyHostToDevice));
+    CK(timer.begin(st));
+    CK(ef_trick_launch_mux(d_es.p, (const EfTrickPic*)d_plan.p, (int)plan.size(), pk, d_out.p, st));
+    CK(timer.end(4, st));
+    CK(cudaMemcpy(ts, d_out.p, pk * 188, cudaMemcpyDeviceToHost));
+    CK(cudaDeviceSynchronize());
+    for (float& m : g_encode_ms) m = 0;
+    for (auto& s : timer.spans) {
+        float ms = 0;
+        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
+        g_encode_ms[s.first] += ms;
+    }
+    return EF_OK;
+}
+
+extern "C" int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* code_ms, float* recon_ms, float* mux_ms)
+{
+    float* o[5] = { upload_ms, search_ms, code_ms, recon_ms, mux_ms };
+    for (int i = 0; i < 5; i++) if (o[i]) *o[i] = g_encode_ms[i];
+    return EF_OK;
+}
+
+extern "C" {
 
 // ef_library_add_trick: ef_trick_build on a title's main, then merge_index()'s fwd and rwd records and samples for the built files
 int ef_library_add_trick(ef_ctx* c, int title, int qscale)

@@ -296,6 +296,12 @@ struct __align__(16) EfLibStream {   // layout of ef_library_status (include/esp
 constexpr int kTrickHeaderBytes = 28;
 constexpr int kTrickSliceBytes = 29440;
 static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (2 + 6 * (16 + 63 * 28 + 2)) + 31) / 32) * 4, "worst-case slice");
+// encoded titles (ef_encode_build, csrc/ef_encode.cu): the worst-case bytes of one P slice (start code + 6 bits + 22 macroblocks of an
+// 11-bit address increment, a 5-bit type, two 11-bit vector codes, a 9-bit pattern and 6 non-intra blocks of 64 28-bit escapes and
+// the end of block, in whole words; an intra macroblock's blocks are shorter) and a P picture's header bytes
+constexpr int kEncSliceBytes = 29736;
+static_assert(kEncSliceBytes >= ((32 + 6 + 22 * (11 + 5 + 2 * 11 + 9 + 6 * (64 * 28 + 2)) + 31) / 32) * 4, "worst-case P slice");
+constexpr int kEncPHeaderBytes = 9;
 struct EfTrickPic {
     uint64_t es_off, pkt_first;
     int64_t pts;

@@ -243,6 +243,37 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
                    uint8_t* rwd, uint64_t rwd_cap, uint64_t* rwd_off);
 int ef_trick_stage_ms(float* decode_ms, float* gather_ms, float* encode_ms, float* mux_ms);
 
+/* ---- encoded titles: make_video()'s video step (indexer/indexer.cpp:306) without ffmpeg -----------------------------------------
+ * Stateless (no context); host buffers; the encoder, its reconstruction and the mux run on `device`. The rule, byte for byte, is
+ * tests/encode_cases.py.
+ * ef_encode_build  video.ts of n_titles titles from raw pictures: i420 holds 352 x 192 I420 pictures (101,376 bytes each) back to
+ *                  back in display order, title t being pictures pic_off[t] .. pic_off[t + 1] - 1. Every title is cut into GOPs of
+ *                  p->gop pictures (the last may be shorter): a sequence header (352 x 192, p->aspect, p->rate, default matrices), a
+ *                  closed GOP header and an I picture coded as ef_trick_build codes its pictures at p->qscale_i, then P pictures at
+ *                  p->qscale_p predicted from the decoder's own reconstruction of the picture before them, with a full-pel search of
+ *                  radius p->search (vectors stay inside forward_f_code 1's range, -8..7.5 pixels) and a half-pel refinement. Picture
+ *                  k of a title has pts p->pts0 + k p->pts_step. The mux is ef_trick_build's: PID 0x100, one PES per picture, one
+ *                  continuity counter per file; no audio. ts_off[n_titles + 1] receives the byte offsets of every title's output.
+ *                  A capacity below the total (or a NULL ts) returns EF_ENOMEM with ts_off filled and nothing written: a sizing call.
+ *                  EF_EINVAL: NULL arguments, gop outside 1..1024 (the temporal reference has 10 bits), a quantiser outside 1..31,
+ *                  search outside 0..15, aspect outside 1..14, rate outside 1..8, an empty title, a pts outside 0..2^33 - 1.
+ *                  Device memory: the encoded pictures and output packets of the whole call, plus one batch of at most 512 GOPs
+ *                  and 6,144 source pictures (two frame stores and the slice regions of one picture per GOP, about 1.5 MB per GOP
+ *                  of 12).
+ * ef_encode_stage_ms  device milliseconds of the last ef_encode_build on the calling thread: the upload of the pictures, the tiling
+ *                  and motion search, the coding (FDCT, quantiser, VLC, assembly), the reconstruction (submit, K0, K1a, K1b) and the mux. */
+typedef struct {
+    int gop;                     /* pictures per GOP, 1..1024 (12: ffmpeg's mpeg1video default) */
+    int qscale_i, qscale_p;      /* 1..31: the slice quantiser of I and of P pictures */
+    int search;                  /* full-pel search radius 0..15 */
+    int aspect, rate;            /* sequence-header codes: aspect 1..14, picture_rate 1..8 */
+    int64_t pts0;                /* pts of picture k of a title = pts0 + k * pts_step */
+    uint32_t pts_step;
+} ef_encode_params;
+int ef_encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p,
+                    uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off);
+int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* code_ms, float* recon_ms, float* mux_ms);
+
 /* ---- audio (SURVEY.md 8f-3): the SBC decoder and the PDM modulator of the reference, batched ---------------------
  * Stateless (no context); host buffers; the kernels run on `device`.
  * ef_audio_demux_ts  MpegDecoder::demux() for PID 0x101 / 0x102 (src/player.cpp:381-432): the payload bytes that reach
