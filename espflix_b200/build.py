@@ -16,7 +16,7 @@ ORACLE_LIB = os.path.join(ROOT, "oracle", "libef_oracle.so")
 REF_DECODE = os.path.join(ROOT, "oracle", "_ref", "efref_decode")
 REF_VIDEO = os.path.join(ROOT, "oracle", "_ref", "libefref_vid.so")
 
-CUDA_SOURCES = ["ef_capi.cu", "ef_decode.cu", "ef_index.cu", "ef_composite.cu", "ef_tsindex.cu", "ef_audio.cu", "ef_library.cu", "ef_trick.cu", "ef_encode.cu", "ef_idct_tc.cu", "ef_tables.cpp"]
+CUDA_SOURCES = ["ef_capi.cu", "ef_decode.cu", "ef_index.cu", "ef_composite.cu", "ef_tsindex.cu", "ef_audio.cu", "ef_library.cu", "ef_trick.cu", "ef_encode.cu", "ef_audio_encode.cu", "ef_idct_tc.cu", "ef_tables.cpp"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

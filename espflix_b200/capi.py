@@ -107,6 +107,9 @@ _SIGNATURES = {
     "ef_library_read": (_I, [_VP, _I, _I, _VP, ctypes.c_uint64, _U64P]),
     "ef_encode_build": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 5),
+    "ef_sbc_encode": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
+    "ef_mux_audio": (_I, [_I, _VP, _VP, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
+    "ef_audio_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 4),
 }
 
 # ef_library_command's commands and ef_library_info's stream states (include/espflix_b200.h)
@@ -705,6 +708,76 @@ def encode_stage_ms():
     v = [ctypes.c_float() for _ in range(5)]
     _check_rc(lib, lib.ef_encode_stage_ms(*[ctypes.byref(x) for x in v]))
     return tuple(x.value for x in v)
+
+
+class AudioParams(ctypes.Structure):
+    """ef_audio_params (include/espflix_b200.h)"""
+    _fields_ = [("frequency", ctypes.c_int), ("allocation", ctypes.c_int), ("bitpool", ctypes.c_int), ("frames_per_pes", ctypes.c_int),
+                ("pts0", ctypes.c_int64)]
+
+
+# ef_sbc_encode / ef_mux_audio defaults: the reference's make_video() audio (48 kHz, mono, 192 kbit/s: bit pool 28 makes 64-byte frames,
+# 375 a second; loudness allocation as ffmpeg's encoder; -pes_payload_size 512: 8 frames per PES)
+AUDIO_ENCODE_DEFAULTS = dict(frequency=3, allocation=0, bitpool=28, frames_per_pes=0, pts0=0)
+
+
+def sbc_encode(pcms, device=0, **params):
+    """ef_sbc_encode: SBC of every mono int16 PCM stream -> [bytes, ...]"""
+    lib = load_library()
+    par = AudioParams(**{k: int(v) for k, v in dict(AUDIO_ENCODE_DEFAULTS, **params).items()})
+    arrs = [np.ascontiguousarray(np.asarray(x, dtype=np.int16).reshape(-1)) for x in pcms]
+    off = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([a.size for a in arrs])
+    blob = np.concatenate(arrs + [np.zeros(1, np.int16)])
+    so = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    rc = lib.ef_sbc_encode(device, blob.ctypes.data, off.ctypes.data, len(arrs), ctypes.byref(par), None, 0, so.ctypes.data)
+    if rc != EF_ENOMEM:
+        _check_rc(lib, rc)
+    out = np.zeros(max(int(so[-1]), 1), dtype=np.uint8)
+    _check_rc(lib, lib.ef_sbc_encode(device, blob.ctypes.data, off.ctypes.data, len(arrs), ctypes.byref(par), out.ctypes.data, out.size,
+                                     so.ctypes.data))
+    return [out[int(so[i]):int(so[i + 1])].tobytes() for i in range(len(arrs))]
+
+
+def mux_audio(videos, sbcs, device=0, **params):
+    """ef_mux_audio: every video transport stream with its SBC interleaved on PID 0x102 -> [bytes, ...]"""
+    lib = load_library()
+    if len(videos) != len(sbcs):
+        raise ValueError("one SBC stream per video")
+    par = AudioParams(**{k: int(v) for k, v in dict(AUDIO_ENCODE_DEFAULTS, **params).items()})
+    tb, to = Context.pack(videos)
+    sb, so = Context.pack(sbcs)
+    oo = np.zeros(len(videos) + 1, dtype=np.uint64)
+    args = (device, tb.ctypes.data, to.ctypes.data, sb.ctypes.data, so.ctypes.data, len(videos), ctypes.byref(par))
+    rc = lib.ef_mux_audio(*args, None, 0, oo.ctypes.data)
+    if rc != EF_ENOMEM:
+        _check_rc(lib, rc)
+    out = np.zeros(max(int(oo[-1]), 1), dtype=np.uint8)
+    _check_rc(lib, lib.ef_mux_audio(*args, out.ctypes.data, out.size, oo.ctypes.data))
+    return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(videos))]
+
+
+def audio_encode_stage_ms():
+    """(upload, encode, download) device milliseconds of the last sbc_encode and the host milliseconds of the last mux_audio on this
+    thread"""
+    lib = load_library()
+    v = [ctypes.c_float() for _ in range(4)]
+    _check_rc(lib, lib.ef_audio_encode_stage_ms(*[ctypes.byref(x) for x in v]))
+    return tuple(x.value for x in v)
+
+
+def encode_title(pictures, pcm, device=0, **params):
+    """a title's video.ts with audio: encode_build of its pictures, sbc_encode of its PCM and mux_audio of both. params: those of
+    ENCODE_DEFAULTS and AUDIO_ENCODE_DEFAULTS (pts0 is the video's; the audio's is audio_pts0, default the same)"""
+    vp = {k: v for k, v in params.items() if k in ENCODE_DEFAULTS}
+    ap = {k: v for k, v in params.items() if k in AUDIO_ENCODE_DEFAULTS and k != "pts0"}
+    unknown = set(params) - set(ENCODE_DEFAULTS) - set(AUDIO_ENCODE_DEFAULTS) - {"audio_pts0"}
+    if unknown:
+        raise TypeError("unknown parameters %s" % sorted(unknown))
+    ap["pts0"] = params.get("audio_pts0", vp.get("pts0", 0))
+    video = encode_build([pictures], device=device, **vp)[0]
+    sbc = sbc_encode([pcm], device=device, **ap)[0]
+    return mux_audio([video], [sbc], device=device, **ap)[0]
 
 
 def trick_stage_ms():

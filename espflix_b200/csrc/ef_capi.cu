@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <thread>
 #include <vector>
 
@@ -46,6 +47,10 @@ cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slic
                                      uint8_t* es, cudaStream_t st);
 cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st);
 cudaError_t ef_encode_upload_tables();
+cudaError_t ef_sbc_encode_upload_tables();
+cudaError_t ef_sbc_launch_encode(const int16_t* pcm, uint64_t pcm_base, uint64_t pcm_len, const uint64_t* pcm_off, const uint64_t* frame_first,
+                                 int n_streams, uint64_t frame0, uint64_t n_frames, int frequency, int allocation, int bitpool, uint8_t* out,
+                                 cudaStream_t st);
 cudaError_t ef_encode_launch_tile(const uint8_t* i420, const uint32_t* src, int count, uint8_t* tiled, cudaStream_t st);
 cudaError_t ef_encode_launch_search(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
                                     const uint32_t* n_pics, int search, uint32_t* mbinfo, cudaStream_t st);
@@ -3041,6 +3046,168 @@ extern "C" int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* cod
 {
     float* o[5] = { upload_ms, search_ms, code_ms, recon_ms, mux_ms };
     for (int i = 0; i < 5; i++) if (o[i]) *o[i] = g_encode_ms[i];
+    return EF_OK;
+}
+
+// ---- encoded titles, audio: SBC from PCM (csrc/ef_audio_encode.cu) and its interleave (the rule is tests/sbc_encode_cases.py) --------
+namespace {
+
+constexpr uint64_t kSbcChunkFrames = 1u << 18;     // frames of one launch: 64 MB of PCM, at most 66 MB of SBC
+thread_local float g_audio_enc_ms[4] = { 0, 0, 0, 0 };
+const int kSbcRate[4] = { 16000, 32000, 44100, 48000 };
+
+}  // namespace
+
+extern "C" int ef_sbc_encode(int device, const int16_t* pcm, const uint64_t* pcm_off, int n_streams, const ef_audio_params* p, uint8_t* sbc,
+                             uint64_t cap, uint64_t* sbc_off)
+{
+    if (!pcm_off || n_streams < 1 || !p || !sbc_off) return fail(EF_EINVAL, "null argument");
+    if (p->frequency < 0 || p->frequency > 3 || p->allocation < 0 || p->allocation > 1 || p->bitpool < 2 || p->bitpool > EF_SBC_MAX_BITPOOL)
+        return fail(EF_EINVAL, "frequency %d / allocation %d / bit pool %d outside 0..3 / 0..1 / 2..%d", p->frequency, p->allocation, p->bitpool,
+                    EF_SBC_MAX_BITPOOL);
+    for (int s = 0; s < n_streams; s++) if (pcm_off[s + 1] < pcm_off[s]) return fail(EF_EINVAL, "pcm offsets must not decrease");
+    if (pcm_off[n_streams] > pcm_off[0] && !pcm) return fail(EF_EINVAL, "null argument");
+    const uint64_t fbytes = 8 + 2 * (uint64_t)p->bitpool;
+    std::vector<uint64_t> first((size_t)n_streams + 1, 0);
+    sbc_off[0] = 0;
+    for (int s = 0; s < n_streams; s++) {
+        first[s + 1] = first[s] + (pcm_off[s + 1] - pcm_off[s] + 127) / 128;
+        sbc_off[s + 1] = first[s + 1] * fbytes;
+    }
+    const uint64_t total = first[n_streams];
+    if (cap < sbc_off[n_streams] || (total && !sbc)) return fail(EF_ENOMEM, "the SBC needs %llu bytes", (unsigned long long)sbc_off[n_streams]);
+    for (float& m : g_audio_enc_ms) m = 0;
+    if (!total) return EF_OK;
+    TRY(usable_device(device));
+    DeviceScope scope_(device);
+    CK(ef_sbc_encode_upload_tables());
+    cudaStream_t st = 0;
+    TrickTimer timer;
+    const uint64_t chunk = std::min(total, kSbcChunkFrames);
+    GrowBuf d_pcm, d_off, d_out;
+    CK(d_pcm.reserve((chunk * 128 + 72) * 2 + 16));
+    CK(d_out.reserve(chunk * fbytes + 16));
+    CK(d_off.reserve((size_t)(2 * n_streams + 1) * 8));
+    CK(cudaMemcpy(d_off.p, pcm_off, ((size_t)n_streams + 1) * 8, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_off.p + ((size_t)n_streams + 1) * 8, first.data(), (size_t)n_streams * 8, cudaMemcpyHostToDevice));
+    const uint64_t* d_pcm_off = (const uint64_t*)d_off.p;
+    const uint64_t* d_first = d_pcm_off + n_streams + 1;
+    for (uint64_t f0 = 0; f0 < total; f0 += chunk) {
+        const uint64_t nf = std::min(chunk, total - f0);
+        // the samples the chunk's frames read: from 72 before its first frame to the end of its last, inside the call's PCM
+        const int s0 = (int)(std::upper_bound(first.begin(), first.begin() + n_streams, f0) - first.begin()) - 1;
+        const int s1 = (int)(std::upper_bound(first.begin(), first.begin() + n_streams, f0 + nf - 1) - first.begin()) - 1;
+        const uint64_t a = pcm_off[s0] + (f0 - first[s0]) * 128, lo = a >= pcm_off[0] + 72 ? a - 72 : pcm_off[0];
+        const uint64_t hi = std::min(pcm_off[s1] + (f0 + nf - first[s1]) * 128, pcm_off[n_streams]);
+        CK(timer.begin(st));
+        CK(cudaMemcpyAsync(d_pcm.p, pcm + lo, (hi - lo) * 2, cudaMemcpyHostToDevice, st));
+        CK(timer.end(0, st));
+        CK(timer.begin(st));
+        CK(ef_sbc_launch_encode((const int16_t*)d_pcm.p, lo, hi - lo, d_pcm_off, d_first, n_streams, f0, nf, p->frequency, p->allocation,
+                                p->bitpool, d_out.p, st));
+        CK(timer.end(1, st));
+        CK(timer.begin(st));
+        CK(cudaMemcpyAsync(sbc + f0 * fbytes, d_out.p, nf * fbytes, cudaMemcpyDeviceToHost, st));
+        CK(timer.end(2, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    for (auto& s : timer.spans) {
+        float ms = 0;
+        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
+        g_audio_enc_ms[s.first] += ms;
+    }
+    return EF_OK;
+}
+
+extern "C" int ef_mux_audio(int device, const uint8_t* ts, const uint64_t* ts_off, const uint8_t* sbc, const uint64_t* sbc_off, int n_titles,
+                            const ef_audio_params* p, uint8_t* out, uint64_t cap, uint64_t* out_off)
+{
+    (void)device;
+    if (!ts_off || !sbc_off || n_titles < 1 || !p || !out_off) return fail(EF_EINVAL, "null argument");
+    if (p->frequency < 0 || p->frequency > 3 || p->bitpool < 2 || p->bitpool > EF_SBC_MAX_BITPOOL)
+        return fail(EF_EINVAL, "frequency %d / bit pool %d outside 0..3 / 2..%d", p->frequency, p->bitpool, EF_SBC_MAX_BITPOOL);
+    const uint64_t fbytes = 8 + 2 * (uint64_t)p->bitpool;
+    if (p->frames_per_pes < 0 || (uint64_t)p->frames_per_pes > (65535 - 8) / fbytes)
+        return fail(EF_EINVAL, "frames_per_pes %d outside 0..%llu", p->frames_per_pes, (unsigned long long)((65535 - 8) / fbytes));
+    const uint64_t fpp = p->frames_per_pes ? (uint64_t)p->frames_per_pes : 512 / fbytes;
+    for (int t = 0; t < n_titles; t++) {
+        if (ts_off[t] % 188 || ts_off[t + 1] % 188 || ts_off[t + 1] < ts_off[t]) return fail(EF_EINVAL, "ts offsets must be non-decreasing multiples of 188");
+        if (sbc_off[t + 1] < sbc_off[t] || (sbc_off[t + 1] - sbc_off[t]) % fbytes) return fail(EF_EINVAL, "title %d: its SBC is not whole %llu-byte frames", t,
+                                                                                                (unsigned long long)fbytes);
+    }
+    if ((ts_off[n_titles] > ts_off[0] && !ts) || (sbc_off[n_titles] > sbc_off[0] && !sbc)) return fail(EF_EINVAL, "null argument");
+    const auto t_start = std::chrono::steady_clock::now();
+    // per title: the audio PES (pts, first frame, frames) and the input packet each goes before
+    struct Pes { int64_t pts; uint64_t frame, n, before; uint32_t pkts; };
+    std::vector<std::vector<Pes>> plan((size_t)n_titles);
+    out_off[0] = 0;
+    for (int t = 0; t < n_titles; t++) {
+        const uint8_t* d0 = ts + ts_off[t];
+        const uint64_t n_pk = (ts_off[t + 1] - ts_off[t]) / 188, n_fr = (sbc_off[t + 1] - sbc_off[t]) / fbytes;
+        std::vector<std::pair<uint64_t, int64_t>> starts;                  // (packet, pts) of every video PES start
+        for (uint64_t k = 0; k < n_pk; k++) {
+            const uint8_t* d = d0 + k * 188;
+            const int pid = ((d[1] << 8) | d[2]) & 0x1FFF;
+            if (pid == 0x101 || pid == 0x102) return fail(EF_EINVAL, "title %d packet %llu is on audio PID 0x%x", t, (unsigned long long)k, pid);
+            if (pid != 0x100 || !(d[1] & 0x40)) continue;
+            const int o = (d[3] & 0x20) ? 5 + d[4] : 4;
+            if (!(d[3] & 0x10) || o + 14 > 188 || d[o] || d[o + 1] || d[o + 2] != 1 || !(d[o + 7] & 0x80))
+                return fail(EF_EINVAL, "title %d packet %llu: a video PES start without a PTS", t, (unsigned long long)k);
+            const uint8_t* q = d + o + 9;
+            starts.push_back({ k, (int64_t)((q[0] >> 1) & 7) << 30 | (int64_t)q[1] << 22 | (int64_t)(q[2] >> 1) << 15 | (int64_t)q[3] << 7 | (q[4] >> 1) });
+        }
+        // a_k rises with k, so the first start with v_j >= a_k never moves back: one pass over the starts for all the PES
+        uint64_t pk = n_pk;
+        size_t j = 0;
+        for (uint64_t k = 0, f = 0; f < n_fr; k++, f += fpp) {
+            const __int128 pts = (__int128)p->pts0 + (__int128)k * fpp * 128 * 90000 / kSbcRate[p->frequency];
+            if (p->pts0 < 0 || pts >= ((__int128)1 << 33)) return fail(EF_EINVAL, "title %d: audio pts beyond 2^33 - 1", t);
+            Pes e = { (int64_t)pts, f, std::min(fpp, n_fr - f), n_pk, 0 };
+            e.pkts = (uint32_t)((14 + e.n * fbytes + 183) / 184);
+            while (j < starts.size() && starts[j].second < e.pts) j++;
+            if (j < starts.size()) e.before = starts[j].first;
+            pk += e.pkts;
+            plan[t].push_back(e);
+        }
+        out_off[t + 1] = out_off[t] + pk * 188;
+    }
+    if (cap < out_off[n_titles] || (out_off[n_titles] && !out)) return fail(EF_ENOMEM, "the titles need %llu bytes", (unsigned long long)out_off[n_titles]);
+    for (int t = 0; t < n_titles; t++) {
+        const uint8_t* d0 = ts + ts_off[t];
+        const uint8_t* a0 = sbc + sbc_off[t];
+        const uint64_t n_pk = (ts_off[t + 1] - ts_off[t]) / 188;
+        uint8_t* o = out + out_off[t];
+        uint32_t cc = 0;
+        size_t e = 0;
+        for (uint64_t k = 0; k <= n_pk; k++) {
+            for (; e < plan[t].size() && plan[t][e].before == k; e++) {  // the audio PES that go before input packet k
+                const Pes& a = plan[t][e];
+                const uint64_t pay = a.n * fbytes, len = 14 + pay;
+                uint8_t h[14] = { 0, 0, 1, 0xBD, (uint8_t)((8 + pay) >> 8), (uint8_t)(8 + pay), 0x80, 0x80, 5 };
+                const uint64_t v = (uint64_t)a.pts;
+                h[9] = (uint8_t)(0x21 | ((v >> 29) & 0x0E)); h[10] = (uint8_t)(v >> 22); h[11] = (uint8_t)(0x01 | ((v >> 14) & 0xFE));
+                h[12] = (uint8_t)(v >> 7); h[13] = (uint8_t)(0x01 | ((v << 1) & 0xFE));
+                for (uint64_t pos = 0; pos < len; pos += 184, cc++, o += 188) {
+                    const uint64_t left = len - pos, af = left >= 184 ? 0 : 184 - left;
+                    o[0] = 0x47; o[1] = (uint8_t)((pos ? 0 : 0x40) | 0x01); o[2] = 0x02; o[3] = (uint8_t)((af ? 0x30 : 0x10) | (cc & 15));
+                    if (af) { o[4] = (uint8_t)(af - 1); if (af > 1) { o[5] = 0; memset(o + 6, 0xFF, af - 2); } }
+                    for (uint64_t b = 4 + af; b < 188; b++) {
+                        const uint64_t x = pos + b - 4 - af;
+                        o[b] = x < 14 ? h[x] : a0[a.frame * fbytes + x - 14];
+                    }
+                }
+            }
+            if (k < n_pk) { memcpy(o, d0 + k * 188, 188); o += 188; }
+        }
+    }
+    g_audio_enc_ms[3] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    return EF_OK;
+}
+
+extern "C" int ef_audio_encode_stage_ms(float* upload_ms, float* encode_ms, float* download_ms, float* mux_ms)
+{
+    float* o[4] = { upload_ms, encode_ms, download_ms, mux_ms };
+    for (int i = 0; i < 4; i++) if (o[i]) *o[i] = g_audio_enc_ms[i];
     return EF_OK;
 }
 

@@ -6,6 +6,9 @@
 // ef_indexer_cli --encode pictures.i420 title_dir [qscale_i qscale_p] — the whole make_video() from decoded pictures: the 352 x 192
 // I420 pictures of pictures.i420 are encoded on the GPU (ef_encode_build at espflix_b200.capi.ENCODE_DEFAULTS, no ffmpeg) into
 // title_dir/video.ts, then the title_dir path above writes video_fwd.ts, video_rwd.ts and video.idx.
+//   --audio pcm.s16le (last) gives the title its sound: mono 16-bit little-endian PCM at 48 kHz, encoded to SBC (ef_sbc_encode at
+//   espflix_b200.capi.AUDIO_ENCODE_DEFAULTS: the reference's 48 kHz, 192 kbit/s) and interleaved on PID 0x102 (ef_mux_audio). The
+//   trick files stay audio-free, as the reference's "-an" makes them.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -53,8 +56,31 @@ static void make_trick_files(const std::string& dir, int qscale)
     write_file(dir + "/video_rwd.ts", rwd.data(), ro[1]);
 }
 
-// title_dir/video.ts of the pictures in `pictures` (I420, 101,376 bytes each)
-static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p)
+// the video transport stream `ts` with the SBC of the PCM in `pcm_path` interleaved
+static std::vector<uint8_t> add_audio(const std::vector<uint8_t>& ts, const std::string& pcm_path)
+{
+    const std::vector<uint8_t> raw = read_file(pcm_path);
+    if (raw.size() % 2) throw std::runtime_error(pcm_path + ": not a whole number of 16-bit samples");
+    std::vector<int16_t> pcm(raw.size() / 2 + 1, 0);
+    for (size_t i = 0; i + 1 < pcm.size(); i++) pcm[i] = (int16_t)(raw[2 * i] | raw[2 * i + 1] << 8);
+    const ef_audio_params p = { 3, 0, 28, 0, 0 };
+    const uint64_t po[2] = { 0, raw.size() / 2 };
+    uint64_t so[2] = { 0, 0 };
+    if (ef_sbc_encode(0, pcm.data(), po, 1, &p, nullptr, 0, so) != EF_ENOMEM && so[1]) throw std::runtime_error("ef_sbc_encode: sizing failed");
+    std::vector<uint8_t> sbc(so[1] + 1);
+    if (ef_sbc_encode(0, pcm.data(), po, 1, &p, sbc.data(), so[1], so) != EF_OK) throw std::runtime_error(std::string("ef_sbc_encode: ") + ef_last_error());
+    const uint64_t to[2] = { 0, ts.size() };
+    uint64_t oo[2] = { 0, 0 };
+    const int rc = ef_mux_audio(0, ts.data(), to, sbc.data(), so, 1, &p, nullptr, 0, oo);
+    if (rc != EF_ENOMEM) throw std::runtime_error(std::string("ef_mux_audio: ") + ef_last_error());
+    std::vector<uint8_t> out(oo[1]);
+    if (ef_mux_audio(0, ts.data(), to, sbc.data(), so, 1, &p, out.data(), out.size(), oo) != EF_OK)
+        throw std::runtime_error(std::string("ef_mux_audio: ") + ef_last_error());
+    return out;
+}
+
+// title_dir/video.ts of the pictures in `pictures` (I420, 101,376 bytes each), with the sound of `pcm_path` when it is not empty
+static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p, const std::string& pcm_path)
 {
     const std::vector<uint8_t> pics = read_file(pictures);
     if (pics.empty() || pics.size() % 101376) throw std::runtime_error(pictures + ": not a whole number of 352 x 192 I420 pictures");
@@ -68,15 +94,19 @@ static void make_video(const std::string& pictures, const std::string& dir, int 
         rc = ef_encode_build(0, pics.data(), off, 1, &p, ts.data(), ts.size(), to);
     }
     if (rc != EF_OK) throw std::runtime_error(std::string("ef_encode_build: ") + ef_last_error());
-    write_file(dir + "/video.ts", ts.data(), to[1]);
+    ts.resize(to[1]);
+    if (!pcm_path.empty()) ts = add_audio(ts, pcm_path);
+    write_file(dir + "/video.ts", ts.data(), ts.size());
 }
 
 int main(int argc, char** argv)
 {
     const bool encode = argc >= 2 && std::string(argv[1]) == "--encode";
+    std::string pcm_path;
+    if (encode && argc >= 6 && std::string(argv[argc - 2]) == "--audio") { pcm_path = argv[argc - 1]; argc -= 2; }
     if (encode ? (argc != 4 && argc != 6) : (argc != 5 && argc != 2 && argc != 3)) {
         fprintf(stderr, "usage: %s video.ts fwd.ts rev.ts out_dir\n       %s title_dir [qscale]   (title_dir/video.ts -> video_fwd.ts, video_rwd.ts, video.idx)\n"
-                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p]   (-> title_dir/video.ts, then as title_dir)\n",
+                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p] [--audio pcm.s16le]   (-> title_dir/video.ts, then as title_dir)\n",
                 argv[0], argv[0], argv[0]);
         return 2;
     }
@@ -90,7 +120,7 @@ int main(int argc, char** argv)
         } else {
             const std::string dir = encode ? argv[3] : argv[1];
             const int qscale = !encode && argc == 3 ? atoi(argv[2]) : 8;
-            if (encode) make_video(argv[2], dir, argc == 6 ? atoi(argv[4]) : 8, argc == 6 ? atoi(argv[5]) : 8);
+            if (encode) make_video(argv[2], dir, argc == 6 ? atoi(argv[4]) : 8, argc == 6 ? atoi(argv[5]) : 8, pcm_path);
             make_trick_files(dir, qscale);
             make_index(dir + "/video.ts", all);
             make_index(dir + "/video_fwd.ts", all);

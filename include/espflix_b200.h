@@ -274,6 +274,43 @@ int ef_encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, in
                     uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off);
 int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* code_ms, float* recon_ms, float* mux_ms);
 
+/* ---- encoded titles, audio: SBC from PCM and its interleave into video.ts ----------------------------------------------------------
+ * The audio of the reference's make_video() (indexer/indexer.cpp:306-309: ffmpeg's "-codec:a sbc -ar 48000 -b:a 192k -ac 1
+ * -streamid 1:258 -pes_payload_size 512"). Stateless; host buffers. The rule, byte for byte, is tests/sbc_encode_cases.py.
+ * ef_sbc_encode   mono / 16-block / 8-subband SBC (the frames decode_audio() plays, video.cpp:964-986) of n_streams mono int16 PCM
+ *                 streams at the header's rate, stream s being pcm[pcm_off[s] .. pcm_off[s + 1]): ceil(n / 128) frames of
+ *                 8 + 2 p->bitpool bytes each (the bit allocation spends exactly the bit pool in every block), samples outside
+ *                 the stream read as zero. The A2DP analysis filterbank in integers, gain 1 through the decoder's synthesis
+ *                 (sbc_decoder.cpp:70-139), scale factors, the decoder's bit allocation (sbc_decoder.cpp:141-231), a quantiser that
+ *                 never reaches IQUANT's 32-bit wrap (sbc_decoder.cpp:257), and the CRC-8 ffmpeg checks. Runs on `device`.
+ *                 sbc_off[n_streams + 1] receives the byte offsets; a capacity below the total (or a NULL sbc) returns EF_ENOMEM
+ *                 with sbc_off filled and nothing written. EF_EINVAL: NULL arguments, decreasing offsets, frequency outside 0..3,
+ *                 allocation outside 0..1, bit pool outside 2..128.
+ * ef_mux_audio    each title's video transport stream (ts_off[n_titles + 1], multiples of 188) with its SBC (sbc_off, whole frames
+ *                 of p->bitpool) interleaved: PES of p->frames_per_pes frames (0: floor(512 / frame bytes), ffmpeg's
+ *                 -pes_payload_size 512) on PID 0x102, stream_id 0xBD, a PTS on every one (player.cpp:423-432 plays audio only
+ *                 after one), PES k at pts p->pts0 + floor(k frames_per_pes 128 90000 / fs); PES k goes right before the first
+ *                 video PES start whose pts is >= its own, or at the end. Input packets keep their bytes and order. out_off
+ *                 receives the offsets; EF_ENOMEM as above. EF_EINVAL: NULL arguments, offsets not multiples of 188, an input
+ *                 packet on PID 0x101 / 0x102, a video PES start without a PTS, SBC that is not whole frames, frames_per_pes
+ *                 outside 0..(65535 - 8) / frame bytes, an audio pts outside 0..2^33 - 1. The mux runs on the host: it moves every
+ *                 byte once, between host buffers, and a device mux would add two host-link crossings of the whole file to that.
+ * ef_audio_encode_stage_ms  milliseconds of the last ef_sbc_encode / ef_mux_audio on the calling thread: the upload of the PCM, the
+ *                 encode kernel (filterbank, allocation, quantiser, packing), the download of the SBC (device events), and the
+ *                 mux (host clock). */
+typedef struct {
+    int frequency;               /* header code 0..3: 16, 32, 44.1, 48 kHz (the PCM is taken at that rate; no resampling) */
+    int allocation;              /* 0 loudness (ffmpeg's), 1 SNR */
+    int bitpool;                 /* 2..128 */
+    int frames_per_pes;          /* 0 = floor(512 / (8 + 2 bitpool)) */
+    int64_t pts0;                /* pts of the first audio PES */
+} ef_audio_params;
+int ef_sbc_encode(int device, const int16_t* pcm, const uint64_t* pcm_off, int n_streams, const ef_audio_params* p,
+                  uint8_t* sbc, uint64_t cap, uint64_t* sbc_off);
+int ef_mux_audio(int device, const uint8_t* ts, const uint64_t* ts_off, const uint8_t* sbc, const uint64_t* sbc_off, int n_titles,
+                 const ef_audio_params* p, uint8_t* out, uint64_t cap, uint64_t* out_off);
+int ef_audio_encode_stage_ms(float* upload_ms, float* encode_ms, float* download_ms, float* mux_ms);
+
 /* ---- audio (SURVEY.md 8f-3): the SBC decoder and the PDM modulator of the reference, batched ---------------------
  * Stateless (no context); host buffers; the kernels run on `device`.
  * ef_audio_demux_ts  MpegDecoder::demux() for PID 0x101 / 0x102 (src/player.cpp:381-432): the payload bytes that reach
