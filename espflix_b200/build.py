@@ -70,8 +70,8 @@ def build_host(force=False):
     srcs = [os.path.join(hdir, f) for f in ("player_gpu.cpp", "video_gpu.cpp", "indexer_gpu.cpp")]
     if not all(os.path.exists(s) for s in srcs):
         return
-    deps = srcs + [os.path.join(hdir, f) for f in os.listdir(hdir) if f.endswith(".h")]
-    if force or _newer(HOST_LIB, deps + [LIB]):
+    deps = srcs + [os.path.join(hdir, f) for f in os.listdir(hdir) if f.endswith(".h") or f.endswith("_cli.cpp")]
+    if force or _newer(HOST_LIB, deps + [LIB]) or _newer(INDEXER_CLI, deps + [LIB]) or _newer(HOST_CLI, deps + [LIB]):
         common = ["-O2", "-std=c++17", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", hdir]
         link = ["-L", PKG, "-lespflix_b200", "-lpthread"]
         _run(["g++"] + common + ["-shared", "-o", HOST_LIB] + srcs + link + ["-Wl,-rpath,$ORIGIN/.."])

@@ -107,6 +107,7 @@ _SIGNATURES = {
     "ef_library_read": (_I, [_VP, _I, _I, _VP, ctypes.c_uint64, _U64P]),
     "ef_encode_build": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 5),
+    "ef_encode_build_rate": (_I, [_I, _VP, _VP, _I, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP, _VP]),
     "ef_sbc_encode": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_mux_audio": (_I, [_I, _VP, _VP, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_audio_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 4),
@@ -702,6 +703,46 @@ def encode_build(titles, device=0, **params):
     return [ts[int(to[i]):int(to[i + 1])].tobytes() for i in range(n)]
 
 
+class RateParams(ctypes.Structure):
+    """ef_rate_params (include/espflix_b200.h)"""
+    _fields_ = [("bit_rate", ctypes.c_uint32), ("vbv_bits", ctypes.c_uint32), ("qmin", ctypes.c_int), ("qmax", ctypes.c_int)]
+
+
+# ef_encode_build_rate's defaults: the reference's make_video() "-b:v 1500k -maxrate 1500k -bufsize 0.25M -qmin 3" (the quantisers
+# up to 31, MPEG-1's largest)
+ENCODE_RATE_DEFAULTS = dict(bit_rate=1500000, vbv_bits=250000, qmin=3, qmax=31)
+
+
+def encode_build_rate(titles, device=0, **params):
+    """ef_encode_build_rate: video.ts of every title encoded to a bit rate and buffer size -> [(ts bytes, pic_q uint8 [n], pic_bytes
+    uint32 [n]), ...]; params: those of ENCODE_DEFAULTS (qscale_i / qscale_p are not read) and ENCODE_RATE_DEFAULTS"""
+    lib = load_library()
+    unknown = set(params) - set(ENCODE_DEFAULTS) - set(ENCODE_RATE_DEFAULTS)
+    if unknown:
+        raise TypeError("unknown parameters %s" % sorted(unknown))
+    par = EncodeParams(**{k: int(v) for k, v in dict(ENCODE_DEFAULTS, **{k: v for k, v in params.items() if k in ENCODE_DEFAULTS}).items()})
+    rp = RateParams(**{k: int(v) for k, v in dict(ENCODE_RATE_DEFAULTS, **{k: v for k, v in params.items() if k in ENCODE_RATE_DEFAULTS}).items()})
+    arrs = [np.ascontiguousarray(np.asarray(t, dtype=np.uint8).reshape(-1, PICTURE_BYTES)) for t in titles]
+    n = len(arrs)
+    off = np.zeros(n + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([a.shape[0] for a in arrs])
+    blob = np.concatenate(arrs) if n and off[-1] else np.zeros((1, PICTURE_BYTES), np.uint8)
+    to = np.zeros(n + 1, dtype=np.uint64)
+    q = np.zeros(max(int(off[-1]), 1), dtype=np.uint8)
+    nb = np.zeros(max(int(off[-1]), 1), dtype=np.uint32)
+    cap = int(off[-1]) * 16384 + 188 * 64
+    for _ in range(2):
+        ts = np.zeros(cap, dtype=np.uint8)
+        rc = lib.ef_encode_build_rate(device, blob.ctypes.data, off.ctypes.data, n, ctypes.byref(par), ctypes.byref(rp), ts.ctypes.data, ts.size,
+                                      to.ctypes.data, q.ctypes.data, nb.ctypes.data)
+        if rc != EF_ENOMEM or int(to[-1]) <= cap:
+            break
+        cap = int(to[-1])
+    _check_rc(lib, rc)
+    return [(ts[int(to[i]):int(to[i + 1])].tobytes(), q[int(off[i]):int(off[i + 1])].copy(), nb[int(off[i]):int(off[i + 1])].copy())
+            for i in range(n)]
+
+
 def encode_stage_ms():
     """(upload, search, code, reconstruction, mux) device milliseconds of the last encode_build on this thread"""
     lib = load_library()
@@ -766,16 +807,24 @@ def audio_encode_stage_ms():
     return tuple(x.value for x in v)
 
 
-def encode_title(pictures, pcm, device=0, **params):
+def encode_title(pictures, pcm, rate=None, device=0, **params):
     """a title's video.ts with audio: encode_build of its pictures, sbc_encode of its PCM and mux_audio of both. params: those of
-    ENCODE_DEFAULTS and AUDIO_ENCODE_DEFAULTS (pts0 is the video's; the audio's is audio_pts0, default the same)"""
+    ENCODE_DEFAULTS and AUDIO_ENCODE_DEFAULTS (pts0 is the video's; the audio's is audio_pts0, default the same). rate: None for the
+    fixed quantisers, else a dict of ENCODE_RATE_DEFAULTS' fields ({} for the defaults) for encode_build_rate; the audio is not
+    counted in the video's bucket, as ffmpeg's -b:v does not count it. An integer rate is the sequence header's picture-rate code, as
+    it was before rate control existed."""
+    if rate is not None and not isinstance(rate, dict):
+        params["rate"], rate = rate, None
     vp = {k: v for k, v in params.items() if k in ENCODE_DEFAULTS}
     ap = {k: v for k, v in params.items() if k in AUDIO_ENCODE_DEFAULTS and k != "pts0"}
     unknown = set(params) - set(ENCODE_DEFAULTS) - set(AUDIO_ENCODE_DEFAULTS) - {"audio_pts0"}
     if unknown:
         raise TypeError("unknown parameters %s" % sorted(unknown))
     ap["pts0"] = params.get("audio_pts0", vp.get("pts0", 0))
-    video = encode_build([pictures], device=device, **vp)[0]
+    if rate is None:
+        video = encode_build([pictures], device=device, **vp)[0]
+    else:
+        video = encode_build_rate([pictures], device=device, **vp, **dict(rate))[0][0]
     sbc = sbc_encode([pcm], device=device, **ap)[0]
     return mux_audio([video], [sbc], device=device, **ap)[0]
 

@@ -42,7 +42,8 @@ cudaError_t ef_decode_configure();
 int ef_decode_resident_ctas(int which);
 cudaError_t ef_trick_upload_tables();
 cudaError_t ef_trick_launch_gather(const uint8_t* frames, const uint32_t* streams, const uint32_t* slots, int count, int fb, uint8_t* dst, cudaStream_t st);
-cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st);
+cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st,
+                                  const uint8_t* qpic = nullptr);
 cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int n_pics,
                                      uint8_t* es, cudaStream_t st);
 cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st);
@@ -55,7 +56,12 @@ cudaError_t ef_encode_launch_tile(const uint8_t* i420, const uint32_t* src, int 
 cudaError_t ef_encode_launch_search(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
                                     const uint32_t* n_pics, int search, uint32_t* mbinfo, cudaStream_t st);
 cudaError_t ef_encode_launch_p(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
-                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st);
+                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, const uint8_t* qpic, uint32_t* slots, uint32_t* slice_len,
+                               cudaStream_t st);
+cudaError_t ef_encode_launch_census(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
+                                    const uint32_t* n_pics, const uint32_t* mbinfo, int ipic, int qmin, int nq, uint32_t* census, cudaStream_t st);
+cudaError_t ef_encode_launch_choose(const uint32_t* census, const uint32_t* streams, int count, int j, int qmin, int qmax, const EfRateBucket& rb,
+                                    const uint32_t* gop_n, int64_t* bucket, uint8_t* qpic, uint32_t* pic_bytes, cudaStream_t st);
 cudaError_t ef_encode_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* header, int n_pics,
                                       uint8_t* es, cudaStream_t st);
 __global__ void ef_tsidx_packet_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, int64_t* pkt_pts, uint8_t* pkt_kind);
@@ -2534,13 +2540,14 @@ void trick_bits(std::vector<uint8_t>& out, uint32_t& acc, int& n, uint32_t v, in
 }
 
 // sequence header (352 x 192, the main's aspect and picture-rate codes, bit_rate 0x3FFFF, vbv 20, default matrices), closed GOP
-// header, I picture header: tests/trick_cases.header_bytes()
-std::vector<uint8_t> trick_header(int aspect, int rate)
+// header, I picture header: tests/trick_cases.header_bytes(); a rate-controlled title's carries its own bit_rate and vbv_buffer_size
+// fields (tests/rate_cases.header_bytes())
+std::vector<uint8_t> trick_header(int aspect, int rate, uint32_t bit_rate = 0x3FFFF, uint32_t vbv = 20)
 {
     std::vector<uint8_t> h = { 0, 0, 1, 0xB3 };
     uint32_t acc = 0; int n = 0;
     trick_bits(h, acc, n, 352, 12); trick_bits(h, acc, n, 192, 12); trick_bits(h, acc, n, aspect, 4); trick_bits(h, acc, n, rate, 4);
-    trick_bits(h, acc, n, 0x3FFFF, 18); trick_bits(h, acc, n, 1, 1); trick_bits(h, acc, n, 20, 10); trick_bits(h, acc, n, 0, 3);
+    trick_bits(h, acc, n, bit_rate, 18); trick_bits(h, acc, n, 1, 1); trick_bits(h, acc, n, vbv, 10); trick_bits(h, acc, n, 0, 3);
     h.insert(h.end(), { 0, 0, 1, 0xB8 });
     trick_bits(h, acc, n, 1u << 12, 25); trick_bits(h, acc, n, 1, 1); trick_bits(h, acc, n, 0, 6);
     h.insert(h.end(), { 0, 0, 1, 0x00 });
@@ -2879,15 +2886,62 @@ std::vector<uint8_t> encode_p_header(int tref)
     return h;
 }
 
+// the bits of a VLC table's code for `value` (0 when absent)
+int vlc_len(const ef_vlc_code* t, int count, int value)
+{
+    for (int i = 0; i < count; i++) if (t[i].value == value) return (int)strlen(t[i].code);
+    return 0;
+}
+
+// the rate rule's fallback sizes (tests/rate_cases.py), from the code tables. P_MIN: a P picture with every macroblock not coded (per
+// slice: start code and quantiser, the first macroblock as 0x08 with vector (0, 0), 20 skipped, the last likewise). D_MAX: the I
+// fallback at its worst, every block's DC difference at the longest size-8 code and an end of block, every macroblock "1" "1".
+uint32_t rate_p_min_bytes()
+{
+    const int mb = vlc_len(ef_vlc_mbtype_p, EF_VLC_MBTYPE_P_COUNT, 0x08) + 2 * vlc_len(ef_vlc_mv, EF_VLC_MV_COUNT, 0);
+    const int slice = 38 + vlc_len(ef_vlc_mba, EF_VLC_MBA_COUNT, 1) + mb + vlc_len(ef_vlc_mba, EF_VLC_MBA_COUNT, EF_MBW_MAX - 1) + mb;
+    return kEncPHeaderBytes + EF_MBH_MAX * (uint32_t)((slice + 7) / 8);
+}
+
+uint32_t rate_d_max_bytes()
+{
+    const int luma = vlc_len(ef_vlc_dc_luma, EF_VLC_DC_LUMA_COUNT, 8) + 8 + 2, chroma = vlc_len(ef_vlc_dc_chroma, EF_VLC_DC_CHROMA_COUNT, 8) + 8 + 2;
+    const int slice = 38 + EF_MBW_MAX * (2 + 4 * luma + 2 * chroma);
+    return kTrickHeaderBytes + EF_MBH_MAX * (uint32_t)((slice + 7) / 8);
+}
+
+int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p, const ef_rate_params* rc,
+                 uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off, uint8_t* pic_q, uint32_t* pic_bytes);
+
 }  // namespace
 
 extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p, uint8_t* ts,
                                uint64_t ts_cap, uint64_t* ts_off)
 {
     if (!pic_off || n_titles < 1 || !p || !ts_off || !i420) return fail(EF_EINVAL, "null argument");
-    if (p->gop < 1 || p->gop > kEncodeMaxGop) return fail(EF_EINVAL, "gop %d outside 1..%d", p->gop, kEncodeMaxGop);
     if (p->qscale_i < 1 || p->qscale_i > 31 || p->qscale_p < 1 || p->qscale_p > 31)
         return fail(EF_EINVAL, "qscale_i %d / qscale_p %d outside 1..31", p->qscale_i, p->qscale_p);
+    return encode_build(device, i420, pic_off, n_titles, p, nullptr, ts, ts_cap, ts_off, nullptr, nullptr);
+}
+
+extern "C" int ef_encode_build_rate(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p,
+                                    const ef_rate_params* rc, uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off, uint8_t* pic_q, uint32_t* pic_bytes)
+{
+    if (!pic_off || n_titles < 1 || !p || !rc || !ts_off || !i420) return fail(EF_EINVAL, "null argument");
+    if (rc->bit_rate < 400 || rc->bit_rate > 400u * 0x3FFFE) return fail(EF_EINVAL, "bit_rate %u outside 400..%u", rc->bit_rate, 400u * 0x3FFFE);
+    if (rc->vbv_bits < 1 || rc->vbv_bits > 1023u * 16384) return fail(EF_EINVAL, "vbv_bits %u outside 1..%u", rc->vbv_bits, 1023u * 16384);
+    if (rc->qmin < 1 || rc->qmax > 31 || rc->qmin > rc->qmax) return fail(EF_EINVAL, "qmin %d / qmax %d: not 1 <= qmin <= qmax <= 31", rc->qmin, rc->qmax);
+    return encode_build(device, i420, pic_off, n_titles, p, rc, ts, ts_cap, ts_off, pic_q, pic_bytes);
+}
+
+namespace {
+
+// ef_encode_build (rc NULL: every picture at the fixed quantisers) and ef_encode_build_rate (rc: each picture's quantiser chosen on the
+// device from the census of every candidate, ef_encode_census_kernel and ef_encode_choose_kernel, before it is coded)
+int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p, const ef_rate_params* rc,
+                 uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off, uint8_t* pic_q, uint32_t* pic_bytes)
+{
+    if (p->gop < 1 || p->gop > kEncodeMaxGop) return fail(EF_EINVAL, "gop %d outside 1..%d", p->gop, kEncodeMaxGop);
     if (p->search < 0 || p->search > 15) return fail(EF_EINVAL, "search %d outside 0..15", p->search);
     if (p->aspect < 1 || p->aspect > 14 || p->rate < 1 || p->rate > 8) return fail(EF_EINVAL, "aspect %d / rate %d outside 1..14 / 1..8", p->aspect, p->rate);
     for (int t = 0; t < n_titles; t++) {
@@ -2898,23 +2952,50 @@ extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* 
         if (p->pts0 < 0 || last >= ((__int128)1 << 33)) return fail(EF_EINVAL, "title %d: the pts of its %llu pictures leave 0..2^33 - 1", t, (unsigned long long)n);
     }
     if (pic_off[n_titles] - pic_off[0] > (1ull << 32)) return fail(EF_EINVAL, "more than 2^32 pictures in one call");
+    EfRateBucket rb = { 0, 0, 0 };
+    if (rc) {
+        // a full GOP that ends full must have room for its I picture at the fallback's worst size and for every picture after it
+        rb.full = (int64_t)rc->vbv_bits * kRateUnit;
+        rb.r = std::min<int64_t>((int64_t)rc->bit_rate * p->pts_step, rb.full);
+        rb.fb_p = (int64_t)rate_p_min_bytes() * 8 * kRateUnit;
+        int64_t need = rb.full;
+        for (int m = p->gop - 1; m >= 1; m--) need = std::max(rb.fb_p, rb.fb_p + need - rb.r);
+        const int64_t d_max = (int64_t)rate_d_max_bytes() * 8 * kRateUnit;
+        if (d_max > std::min(rb.full, rb.full + rb.r - need))
+            return fail(EF_EINVAL, "bit_rate %u / vbv_bits %u cannot hold a GOP of %d: its I picture's fallback (%u bytes) does not fit", rc->bit_rate,
+                        rc->vbv_bits, p->gop, rate_d_max_bytes());
+    }
     TRY(usable_device(device));
     DeviceScope scope_(device);
 
     // GOPs: (first picture relative to pic_off[0], pictures); every batch of GOPs is a contiguous run of pictures
-    struct Gop { uint64_t first; int n; };
+    struct Gop { uint64_t first; int n; bool last; };   // last: the title's last GOP
     std::vector<Gop> gops;
     for (int t = 0; t < n_titles; t++)
         for (uint64_t k = pic_off[t]; k < pic_off[t + 1]; k += (uint64_t)p->gop)
-            gops.push_back({ k - pic_off[0], (int)std::min<uint64_t>((uint64_t)p->gop, pic_off[t + 1] - k) });
+            gops.push_back({ k - pic_off[0], (int)std::min<uint64_t>((uint64_t)p->gop, pic_off[t + 1] - k), k + (uint64_t)p->gop >= pic_off[t + 1] });
     const int B = (int)std::min<size_t>(gops.size(), std::min(kEncodeBatchGops, std::max(1, kEncodeBatchPictures / p->gop)));
-    const std::vector<uint8_t> i_hdr = trick_header(p->aspect, p->rate);
+    const std::vector<uint8_t> i_hdr = rc ? trick_header(p->aspect, p->rate, (rc->bit_rate + 399) / 400, (rc->vbv_bits + 16383) / 16384)
+                                          : trick_header(p->aspect, p->rate);
 
     CK(ef_trick_upload_tables());
     CK(ef_encode_upload_tables());
     cudaStream_t st = 0;
     TrickTimer timer;
-    GrowBuf d_src, d_tiled, d_list, d_info, d_slots, d_len, d_es, d_dst, d_hdr, d_off;
+    GrowBuf d_src, d_tiled, d_list, d_info, d_slots, d_len, d_es, d_dst, d_hdr, d_off, d_census, d_rate;
+    const int qmin = rc ? rc->qmin : 0, nq = rc ? rc->qmax - rc->qmin + 1 : 0;
+    // rate: census [B][32][12] u32; d_rate: bucket [B] i64, choice bytes [B] u32, GOP lengths [B] u32, quantisers [B] u8
+    int64_t* d_bucket = nullptr;
+    uint32_t *d_pbytes = nullptr, *d_gopn = nullptr;
+    uint8_t* d_qpic = nullptr;
+    if (rc) {
+        CK(d_census.reserve((size_t)B * 32 * EF_MBH_MAX * 4));
+        CK(d_rate.reserve((size_t)B * 17));
+        d_bucket = (int64_t*)d_rate.p;
+        d_pbytes = (uint32_t*)(d_rate.p + (size_t)B * 8);
+        d_gopn = (uint32_t*)(d_rate.p + (size_t)B * 12);
+        d_qpic = d_rate.p + (size_t)B * 16;
+    }
     CK(d_tiled.reserve((size_t)B * EF_FRAME));
     CK(d_list.reserve((size_t)B * 8));
     CK(d_info.reserve((size_t)B * EF_MBW_MAX * EF_MBH_MAX * 4));
@@ -2939,6 +3020,11 @@ extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* 
         CK(timer.begin(st));
         CK(cudaMemcpyAsync(d_src.p, i420 + (pic_off[0] + p0) * EF_FRAME, np * EF_FRAME, cudaMemcpyHostToDevice, st));
         CK(timer.end(0, st));
+        std::vector<uint32_t> gopn((size_t)nb);
+        if (rc) {                                        // every GOP's length, and whether it is its title's last (it ends at 0)
+            for (int g = 0; g < nb; g++) gopn[g] = (uint32_t)gops[g0 + g].n | (gops[g0 + g].last ? 1u << 16 : 0u);
+            CK(cudaMemcpyAsync(d_gopn, gopn.data(), gopn.size() * 4, cudaMemcpyHostToDevice, st));
+        }
         for (int k = 0; k < p->gop; k++) {
             // round k: picture k of every GOP of the batch that has one (all GOPs but a title's last are whole)
             std::vector<uint32_t> act, src;
@@ -2957,12 +3043,25 @@ extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* 
                 ctx->launches++;
                 CK(timer.end(1, st));
                 CK(timer.begin(st));
+            }
+            if (rc) {                                    // the census of every candidate, then each GOP's choice, on the device
+                CK(ef_encode_launch_census(d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, (const uint32_t*)d_info.p, k == 0,
+                                           qmin, nq, (uint32_t*)d_census.p, st));
+                CK(ef_encode_launch_choose((const uint32_t*)d_census.p, d_act, na, k, qmin, rc->qmax, rb, d_gopn, d_bucket, d_qpic, d_pbytes, st));
+                ctx->launches += 2;
+            }
+            if (k)
                 CK(ef_encode_launch_p(d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, (const uint32_t*)d_info.p, p->qscale_p,
-                                      (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
-            } else CK(ef_trick_launch_encode(d_tiled.p, na, p->qscale_i, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
+                                      d_qpic, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
+            else CK(ef_trick_launch_encode(d_tiled.p, na, p->qscale_i, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st, d_qpic));
             ctx->launches++;
-            std::vector<uint32_t> len((size_t)na * EF_MBH_MAX);
+            std::vector<uint32_t> len((size_t)na * EF_MBH_MAX), chosen_bytes(rc ? (size_t)na : 0);
+            std::vector<uint8_t> chosen_q(chosen_bytes.size());
             CK(cudaMemcpyAsync(len.data(), d_len.p, len.size() * 4, cudaMemcpyDeviceToHost, st));
+            if (rc) {
+                CK(cudaMemcpyAsync(chosen_bytes.data(), d_pbytes, (size_t)na * 4, cudaMemcpyDeviceToHost, st));
+                CK(cudaMemcpyAsync(chosen_q.data(), d_qpic, (size_t)na, cudaMemcpyDeviceToHost, st));
+            }
             CK(cudaStreamSynchronize(st));
             const uint32_t hb = k ? kEncPHeaderBytes : kTrickHeaderBytes;
             std::vector<uint64_t> dst((size_t)na);
@@ -2973,6 +3072,13 @@ extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* 
                 const uint64_t pic = p0 + src[a];
                 dst[a] = es_off[pic] = es_total; es_len[pic] = bytes;
                 es_total += bytes;
+                if (rc) {                                // the bucket counted the census's size: it must be the coder's
+                    if (chosen_bytes[a] != bytes)
+                        return fail(EF_ECUDA, "picture %llu: the census gave %u bytes at its quantiser, the coder %u", (unsigned long long)pic,
+                                    chosen_bytes[a], bytes);
+                    if (pic_q) pic_q[pic] = chosen_q[a] & kQFallback ? 0 : chosen_q[a];
+                }
+                if (pic_bytes) pic_bytes[pic] = bytes;
             }
             if (es_total + 16 > d_es.cap) CK(d_es.reserve(std::max<size_t>(es_total + 16, d_es.cap * 2), round0));
             CK(cudaMemcpyAsync(d_dst.p, dst.data(), dst.size() * 8, cudaMemcpyHostToDevice, st));
@@ -3041,6 +3147,8 @@ extern "C" int ef_encode_build(int device, const uint8_t* i420, const uint64_t* 
     }
     return EF_OK;
 }
+
+}  // namespace
 
 extern "C" int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* code_ms, float* recon_ms, float* mux_ms)
 {

@@ -302,6 +302,19 @@ static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (2 + 6 * (16 + 63 * 28 + 2)) +
 constexpr int kEncSliceBytes = 29736;
 static_assert(kEncSliceBytes >= ((32 + 6 + 22 * (11 + 5 + 2 * 11 + 9 + 6 * (64 * 28 + 2)) + 31) / 32) * 4, "worst-case P slice");
 constexpr int kEncPHeaderBytes = 9;
+// rate-controlled titles (ef_encode_build_rate): a picture's quantiser byte is q, or qmax | kQFallback for its fallback coding (P: every
+// macroblock not coded; I: the DC levels alone); the census holds every slice's bytes at up to 31 candidates and the fallback in slot
+// kCensusFallback
+constexpr int kQFallback = 0x80;
+constexpr int kCensusFallback = 31;
+constexpr int64_t kRateUnit = 90000;       // bucket fullness is counted in 1/90000 bit, so that a refill R * pts_step is exact
+// The I picture's share of a GOP's budget against one P picture's (tests/rate_cases.I_WEIGHT, where the measurement behind it is)
+constexpr int kIWeight = 3;
+struct EfRateBucket {
+    int64_t full;                          // B * kRateUnit
+    int64_t r;                             // min(R * pts_step, full): a refill beyond a full buffer changes no choice
+    int64_t fb_p;                          // the P fallback's bits * kRateUnit
+};
 struct EfTrickPic {
     uint64_t es_off, pkt_first;
     int64_t pts;

@@ -9,6 +9,9 @@
 //                              neighbours and the intra decision
 //   ef_encode_p_kernel         one warp per slice of a P picture: prediction, FDCT, quantiser, then the macroblock header and block
 //                              codes placed by a warp prefix sum in a shared window, flushed to a per-slice region of kEncSliceBytes
+//   ef_encode_census_kernel    ef_encode_build_rate: one warp per slice, the slice's exact bytes at every candidate quantiser and as
+//                              its fallback, from one FDCT per block
+//   ef_encode_choose_kernel    ef_encode_build_rate: one thread per GOP, its bucket and the choice of the picture's quantiser
 //   ef_encode_assemble_kernel  one CTA per P picture: its 9 header bytes and 12 slices at the picture's offset in the ES
 #include <stdint.h>
 
@@ -161,8 +164,8 @@ __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_search_kernel(const 
 
 __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_p_kernel(const uint8_t* __restrict__ src, const uint32_t* __restrict__ streams, int count,
                                                                     const uint8_t* __restrict__ frames, const uint32_t* __restrict__ base_pics,
-                                                                    const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ mbinfo, int qscale,
-                                                                    uint32_t* __restrict__ slots, uint32_t* __restrict__ slice_len)
+                                                                    const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ mbinfo, int qscale_all,
+                                                                    const uint8_t* __restrict__ qpic, uint32_t* __restrict__ slots, uint32_t* __restrict__ slice_len)
 {
     __shared__ uint32_t s_ac[32 * 41];
     __shared__ int s_t[kEncWarps][64], s_f[kEncWarps][64];
@@ -173,6 +176,8 @@ __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_p_kernel(const uint8
     const int gw = blockIdx.x * kEncWarps + warp;
     if (gw >= count * EF_MBH_MAX) return;
     const int k = gw / EF_MBH_MAX, row = gw % EF_MBH_MAX;
+    const int qv = qpic ? (int)qpic[k] : qscale_all, qscale = qv & 31;
+    const bool fallback = qv & kQFallback;               // every macroblock not coded: vector (0, 0), no levels
     const int s = (int)streams[k];
     const uint8_t* ref = frames + ef_frame_offset(s, (int)((base_pics[s] + n_pics[s]) & 1u));
     const uint8_t* frame = src + (size_t)k * EF_FRAME;
@@ -200,7 +205,7 @@ __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_p_kernel(const uint8
         wbase += full;
     };
     for (int mx = 0; mx < EF_MBW_MAX; mx++) {
-        const uint32_t info = info_row[mx];
+        const uint32_t info = fallback ? 0u : info_row[mx];
         const bool intra = (info >> 16) & 1;
         const int h = (int8_t)(info & 0xFF), v = (int8_t)((info >> 8) & 0xFF);
         const uint8_t* tile = frame + ef_tile_offset(mx, row);
@@ -233,6 +238,7 @@ __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_p_kernel(const uint8
             fdct_block(x, T, F, r, k0);
             lv0[b] = intra ? quant(2 * lane, F, qscale) : quant_inter(2 * lane, F, qscale);
             lv1[b] = intra ? quant(2 * lane + 1, F, qscale) : quant_inter(2 * lane + 1, F, qscale);
+            if (fallback) lv0[b] = lv1[b] = 0;
             if (!intra && __any_sync(0xFFFFFFFFu, lv0[b] != 0 || lv1[b] != 0)) cbp |= 0x20u >> b;
             __syncwarp();
         }
@@ -313,6 +319,175 @@ __global__ void __launch_bounds__(kEncWarps * 32) ef_encode_p_kernel(const uint8
     if (lane == 0) slice_len[gw] = (P + 7) >> 3;
 }
 
+// the exact bytes of slice `row` of picture k of the round coded at every candidate q = qmin + lane (lane < nq) and as its fallback
+// (lane kCensusFallback): census[(k * 32 + lane) * 12 + row]. One warp per slice; the FDCT of a block does not depend on q, so each
+// block is transformed once and then quantised and its codes counted at every candidate, the lanes splitting the coefficients as
+// ef_encode_p_kernel does. Lane q then walks the slice's macroblock headers for its own q: address increments and skips (they depend
+// on q through the coded block pattern), the predictor resets, vector, type and pattern codes, DC differences. ipic: the round's
+// pictures are I pictures (every macroblock intra, the trick encoder's 2-bit header); else P pictures with their search's mbinfo.
+__global__ void __launch_bounds__(kEncWarps * 32) ef_encode_census_kernel(const uint8_t* __restrict__ src, const uint32_t* __restrict__ streams, int count,
+                                                                         const uint8_t* __restrict__ frames, const uint32_t* __restrict__ base_pics,
+                                                                         const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ mbinfo, int ipic,
+                                                                         int qmin, int nq, uint32_t* __restrict__ census)
+{
+    __shared__ uint32_t s_ac[32 * 41];
+    __shared__ int s_t[kEncWarps][64], s_f[kEncWarps][64];
+    for (int i = threadIdx.x; i < 32 * 41; i += blockDim.x) s_ac[i] = c_trick.ac[i];
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int gw = blockIdx.x * kEncWarps + warp;
+    if (gw >= count * EF_MBH_MAX) return;
+    const int k = gw / EF_MBH_MAX, row = gw % EF_MBH_MAX;
+    const uint8_t* frame = src + (size_t)k * EF_FRAME;
+    const uint8_t* ref = nullptr;
+    const uint32_t* info_row = nullptr;
+    if (!ipic) {
+        const int s = (int)streams[k];
+        ref = frames + ef_frame_offset(s, (int)((base_pics[s] + n_pics[s]) & 1u));
+        info_row = mbinfo + (size_t)k * EF_MBW_MAX * EF_MBH_MAX + row * EF_MBW_MAX;
+    }
+    int* T = s_t[warp];
+    int* F = s_f[warp];
+    const int r = lane >> 2, k0 = (lane & 3) * 2;
+    const bool fb_lane = lane == kCensusFallback;
+    const int my_q = qmin + lane;                        // this lane's candidate (lanes nq .. 30 count nothing of use)
+    uint32_t P = 38;
+    int pred[3] = { 128, 128, 128 }, mvp[2] = { 0, 0 }, pending = 0;
+    for (int mx = 0; mx < EF_MBW_MAX; mx++) {
+        const uint32_t info = ipic ? (1u << 16) : info_row[mx];
+        const bool intra = (info >> 16) & 1;
+        const int h = (int8_t)(info & 0xFF), v = (int8_t)((info >> 8) & 0xFF);
+        const uint8_t* tile = frame + ef_tile_offset(mx, row);
+        uint32_t cbp = 0, blk = 0;                       // this lane's q: coded blocks, their run / level and end-of-block bits
+        int dcl[6];
+        #pragma unroll 1
+        for (int b = 0; b < 6; b++) {
+            const int po = b < 4 ? ((b >> 1) * 8 + r) * 16 + (b & 1) * 8 : 256 + (b - 4) * 64 + r * 8;
+            const uint2 px = *(const uint2*)(tile + po);
+            int x[8];
+            #pragma unroll
+            for (int n = 0; n < 4; n++) { x[n] = (px.x >> (8 * n)) & 0xFF; x[n + 4] = (px.y >> (8 * n)) & 0xFF; }
+            if (!intra) {
+                if (b < 4) {
+                    const int X = 2 * (mx * 16 + (b & 1) * 8) + h, Y = 2 * (row * 16 + (b >> 1) * 8 + r) + v;
+                    const int x0 = X >> 1, y0 = Y >> 1, xh = X & 1, yh = Y & 1;
+                    #pragma unroll
+                    for (int n = 0; n < 8; n++)
+                        x[n] -= mc_pel(ref + ef_luma_offset(x0 + n, y0), ref + ef_luma_offset(x0 + n + xh, y0), ref + ef_luma_offset(x0 + n, y0 + yh),
+                                       ref + ef_luma_offset(x0 + n + xh, y0 + yh), xh, yh);
+                } else {
+                    const int hx = (32 * mx + h) >> 1, hy = (32 * row + v) >> 1, p = b - 4;
+                    const int x0 = hx >> 1, y0 = (hy >> 1) + r, xh = hx & 1, yh = hy & 1;
+                    #pragma unroll
+                    for (int n = 0; n < 8; n++)
+                        x[n] -= mc_pel(ref + ef_chroma_offset(p, x0 + n, y0), ref + ef_chroma_offset(p, x0 + n + xh, y0),
+                                       ref + ef_chroma_offset(p, x0 + n, y0 + yh), ref + ef_chroma_offset(p, x0 + n + xh, y0 + yh), xh, yh);
+                }
+            }
+            fdct_block(x, T, F, r, k0);
+            dcl[b] = intra ? quant(0, F, 1) : 0;         // an intra DC level does not depend on q
+            // every candidate, lowest first; levels only shrink as q grows, so once a block has no level left (intra: no AC
+            // level) it has none at any later candidate
+            int qi = 0;
+            for (; qi < nq; qi++) {
+                const int q = qmin + qi;
+                const int a0 = intra ? (lane ? quant(2 * lane, F, q) : 0) : quant_inter(2 * lane, F, q);
+                const int a1 = intra ? quant(2 * lane + 1, F, q) : quant_inter(2 * lane + 1, F, q);
+                const uint32_t ev = __ballot_sync(0xFFFFFFFFu, (intra && lane == 0) || a0 != 0), od = __ballot_sync(0xFFFFFFFFu, a1 != 0);
+                if (!(od | (intra ? ev & ~1u : ev))) break;
+                const uint64_t mask = spread_bits(ev) | (spread_bits(od) << 1);
+                uint32_t c0, n0, c1, n1;
+                code_of(2 * lane, a0, mask, s_ac, &c0, &n0);
+                code_of(2 * lane + 1, a1, mask, s_ac, &c1, &n1);
+                if (lane == 0 && !intra) {
+                    if (a0 == 1 || a0 == -1) n0 = 2;
+                    else if (a0) code_of(1, a0, 1, s_ac, &c0, &n0);
+                }
+                const uint32_t bits = (uint32_t)__reduce_add_sync(0xFFFFFFFFu, (int)(n0 + n1));
+                if (lane == qi) { blk += bits + 2; cbp |= 0x20u >> b; }
+            }
+            if (intra && lane >= qi && !fb_lane) { blk += 2; cbp |= 0x20u >> b; }
+            __syncwarp();
+        }
+        // the fallback: P every macroblock not coded; I the DC levels and end of block of every block
+        const bool my_intra = intra && !(fb_lane && !ipic);
+        const bool zero = (h == 0 && v == 0) || fb_lane;
+        if (fb_lane) { cbp = ipic ? 63u : 0u; blk = ipic ? 12u : 0u; }
+        if (!my_intra && zero && !cbp && mx > 0 && mx < EF_MBW_MAX - 1) { pending++; continue; }
+        if (pending) { pred[0] = pred[1] = pred[2] = 128; mvp[0] = mvp[1] = 0; }
+        P += c_enc.mba[pending + 1] & 0xFF;
+        pending = 0;
+        const int type = my_intra ? 0x01 : !zero ? (cbp ? 0x0A : 0x08) : (cbp ? 0x02 : 0x08);
+        P += ipic ? 1 : c_enc.type[type] & 0xFF;
+        if (my_intra) {
+            mvp[0] = mvp[1] = 0;
+            #pragma unroll
+            for (int b = 0; b < 6; b++) {
+                const int comp = b < 4 ? 0 : b - 3;
+                const int diff = dcl[b] - pred[comp], size = 32 - __clz(diff < 0 ? -diff : diff);
+                P += (c_trick.dc[comp ? 1 : 0][size] & 0xFF) + size;
+                pred[comp] = dcl[b];
+            }
+        } else {
+            pred[0] = pred[1] = pred[2] = 128;
+            if (type & 0x08) {
+                #pragma unroll
+                for (int c = 0; c < 2; c++) {
+                    const int val = fb_lane ? 0 : c ? v : h;
+                    int d = val - mvp[c];
+                    d = d < -16 ? d + 32 : d > 15 ? d - 32 : d;
+                    P += c_enc.mv[d + 16] & 0xFF;
+                    mvp[c] = val;
+                }
+            } else mvp[0] = mvp[1] = 0;
+            if (type & 0x02) P += c_enc.cbp[cbp] & 0xFF;
+        }
+        P += blk;
+    }
+    if (lane < nq || fb_lane) census[((size_t)k * 32 + lane) * EF_MBH_MAX + row] = (P + 7) >> 3;
+}
+
+// one thread per GOP of the round: the GOP's bucket (fullness in 1/90000 bit, bucket[g]) and the choice of picture j's quantiser from
+// the census (tests/rate_cases.py): the smallest candidate within the soft target and the hard bound, else the smallest within the
+// hard bound, else the fallback. gop_n[g] = pictures of GOP g | 1 << 16 when it is its title's last (it must end at 0, not full).
+// qpic[k] receives the choice, pic_bytes[k] its ES bytes.
+__global__ void ef_encode_choose_kernel(const uint32_t* __restrict__ census, const uint32_t* __restrict__ streams, int count, int j, int qmin, int nq,
+                                        int qmax, EfRateBucket rb, const uint32_t* __restrict__ gop_n, int64_t* __restrict__ bucket,
+                                        uint8_t* __restrict__ qpic, uint32_t* __restrict__ pic_bytes)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const int g = (int)streams[k];
+    const int n = (int)(gop_n[g] & 0xFFFF);
+    const int64_t E = (gop_n[g] >> 16) ? 0 : rb.full;
+    int64_t need = E;                                    // need_{j + 1}: every picture after j is a P picture
+    for (int m = n - 1; m > j; m--) need = max(rb.fb_p, rb.fb_p + need - rb.r);
+    const int64_t f = j ? bucket[g] : rb.full;
+    const int64_t hard = min(f, f + rb.r - need);
+    const int64_t L = f + (int64_t)(n - j) * rb.r - E;
+    const int64_t soft = j ? L / (n - j) : L * kIWeight / (kIWeight + n - 1);
+    const uint32_t hb = j ? kEncPHeaderBytes : kTrickHeaderBytes;
+    const uint32_t* c = census + (size_t)k * 32 * EF_MBH_MAX;
+    auto bytes = [&](int slot) {
+        uint32_t s = hb;
+        for (int row = 0; row < EF_MBH_MAX; row++) s += c[slot * EF_MBH_MAX + row];
+        return s;
+    };
+    int pick = -1;
+    uint32_t s = 0;
+    for (int pass = 0; pass < 2 && pick < 0; pass++) {
+        const int64_t cap = pass ? hard : min(soft, hard);
+        for (int qi = 0; qi < nq; qi++) {
+            s = bytes(qi);
+            if ((int64_t)s * 8 * kRateUnit <= cap) { pick = qi; break; }
+        }
+    }
+    if (pick < 0) s = bytes(kCensusFallback);
+    qpic[k] = (uint8_t)(pick < 0 ? (qmax | kQFallback) : qmin + pick);
+    pic_bytes[k] = s;
+    bucket[g] = min(rb.full, f - (int64_t)s * 8 * kRateUnit + rb.r);
+}
+
 // one CTA per P picture: the round's header (all pictures of a round share their temporal reference), then its 12 slices
 __global__ void ef_encode_assemble_kernel(const uint32_t* __restrict__ slots, const uint32_t* __restrict__ slice_len, const uint64_t* __restrict__ pic_dst,
                                           const uint8_t* __restrict__ header, uint8_t* __restrict__ es)
@@ -364,11 +539,29 @@ cudaError_t ef_encode_launch_search(const uint8_t* src, const uint32_t* streams,
 }
 
 cudaError_t ef_encode_launch_p(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
-                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st)
+                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, const uint8_t* qpic, uint32_t* slots, uint32_t* slice_len,
+                               cudaStream_t st)
 {
     const int warps = count * EF_MBH_MAX;
     ef_encode_p_kernel<<<(warps + kEncWarps - 1) / kEncWarps, kEncWarps * 32, 0, st>>>(src, streams, count, frames, base_pics, n_pics, mbinfo, qscale,
-                                                                                      slots, slice_len);
+                                                                                      qpic, slots, slice_len);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_encode_launch_census(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
+                                    const uint32_t* n_pics, const uint32_t* mbinfo, int ipic, int qmin, int nq, uint32_t* census, cudaStream_t st)
+{
+    const int warps = count * EF_MBH_MAX;
+    ef_encode_census_kernel<<<(warps + kEncWarps - 1) / kEncWarps, kEncWarps * 32, 0, st>>>(src, streams, count, frames, base_pics, n_pics, mbinfo, ipic,
+                                                                                           qmin, nq, census);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_encode_launch_choose(const uint32_t* census, const uint32_t* streams, int count, int j, int qmin, int qmax, const EfRateBucket& rb,
+                                    const uint32_t* gop_n, int64_t* bucket, uint8_t* qpic, uint32_t* pic_bytes, cudaStream_t st)
+{
+    ef_encode_choose_kernel<<<(count + 127) / 128, 128, 0, st>>>(census, streams, count, j, qmin, qmax - qmin + 1, qmax, rb, gop_n, bucket, qpic,
+                                                                 pic_bytes);
     return cudaGetLastError();
 }
 

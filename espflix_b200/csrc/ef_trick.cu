@@ -26,7 +26,8 @@ __global__ void ef_trick_gather_kernel(const uint8_t* __restrict__ frames, const
     ((uint4*)(dst + (size_t)slots[k] * EF_FRAME))[w] = src[w];
 }
 
-__global__ void __launch_bounds__(kWarps * 32) ef_trick_encode_kernel(const uint8_t* __restrict__ in, int n_pics, int qscale, uint32_t* __restrict__ slots,
+__global__ void __launch_bounds__(kWarps * 32) ef_trick_encode_kernel(const uint8_t* __restrict__ in, int n_pics, int qscale_all,
+                                                                     const uint8_t* __restrict__ qpic, uint32_t* __restrict__ slots,
                                                                      uint32_t* __restrict__ slice_len)
 {
     __shared__ uint32_t s_ac[32 * 41];
@@ -38,6 +39,8 @@ __global__ void __launch_bounds__(kWarps * 32) ef_trick_encode_kernel(const uint
     const int gw = blockIdx.x * kWarps + warp;
     if (gw >= n_pics * EF_MBH_MAX) return;
     const int pic = gw / EF_MBH_MAX, row = gw % EF_MBH_MAX;
+    const int qv = qpic ? (int)qpic[pic] : qscale_all, qscale = qv & 31;
+    const bool fallback = qv & kQFallback;   // every AC level zero: the DC levels alone
     uint32_t* out = slots + (size_t)gw * (kTrickSliceBytes / 4);
     const uint8_t* frame = in + (size_t)pic * EF_FRAME;
     uint32_t* win = s_win[warp];
@@ -64,7 +67,8 @@ __global__ void __launch_bounds__(kWarps * 32) ef_trick_encode_kernel(const uint
             fdct_block(x, T, F, r, k0);
             // quantise zig-zag indices 2 lane and 2 lane + 1 (so the lanes' codes follow each other in bitstream order); the DC
             // counts as coded
-            const int lv0 = quant(2 * lane, F, qscale), lv1 = quant(2 * lane + 1, F, qscale);
+            int lv0 = quant(2 * lane, F, qscale), lv1 = quant(2 * lane + 1, F, qscale);
+            if (fallback) { lv1 = 0; if (lane) lv0 = 0; }
             const uint32_t ev = __ballot_sync(0xFFFFFFFFu, lane == 0 || lv0 != 0), od = __ballot_sync(0xFFFFFFFFu, lv1 != 0);
             const uint64_t mask = spread_bits(ev) | (spread_bits(od) << 1);
             uint32_t c0, n0, c1, n1;
@@ -187,10 +191,11 @@ cudaError_t ef_trick_launch_gather(const uint8_t* frames, const uint32_t* stream
     return cudaGetLastError();
 }
 
-cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st)
+cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st,
+                                  const uint8_t* qpic)
 {
     const int warps = n_pics * EF_MBH_MAX;
-    ef_trick_encode_kernel<<<(warps + kWarps - 1) / kWarps, kWarps * 32, 0, st>>>(in, n_pics, qscale, slots, slice_len);
+    ef_trick_encode_kernel<<<(warps + kWarps - 1) / kWarps, kWarps * 32, 0, st>>>(in, n_pics, qscale, qpic, slots, slice_len);
     return cudaGetLastError();
 }
 

@@ -6,6 +6,8 @@
 // ef_indexer_cli --encode pictures.i420 title_dir [qscale_i qscale_p] — the whole make_video() from decoded pictures: the 352 x 192
 // I420 pictures of pictures.i420 are encoded on the GPU (ef_encode_build at espflix_b200.capi.ENCODE_DEFAULTS, no ffmpeg) into
 // title_dir/video.ts, then the title_dir path above writes video_fwd.ts, video_rwd.ts and video.idx.
+// ef_indexer_cli --encode pictures.i420 title_dir --rate bit_rate vbv_bits — the same, with video.ts encoded to a bit rate and buffer
+// size (ef_encode_build_rate at espflix_b200.capi.ENCODE_RATE_DEFAULTS' quantisers 3..31) in place of the fixed quantisers.
 //   --audio pcm.s16le (last) gives the title its sound: mono 16-bit little-endian PCM at 48 kHz, encoded to SBC (ef_sbc_encode at
 //   espflix_b200.capi.AUDIO_ENCODE_DEFAULTS: the reference's 48 kHz, 192 kbit/s) and interleaved on PID 0x102 (ef_mux_audio). The
 //   trick files stay audio-free, as the reference's "-an" makes them.
@@ -80,7 +82,8 @@ static std::vector<uint8_t> add_audio(const std::vector<uint8_t>& ts, const std:
 }
 
 // title_dir/video.ts of the pictures in `pictures` (I420, 101,376 bytes each), with the sound of `pcm_path` when it is not empty
-static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p, const std::string& pcm_path)
+static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p, const ef_rate_params* rate,
+                       const std::string& pcm_path)
 {
     const std::vector<uint8_t> pics = read_file(pictures);
     if (pics.empty() || pics.size() % 101376) throw std::runtime_error(pictures + ": not a whole number of 352 x 192 I420 pictures");
@@ -88,12 +91,16 @@ static void make_video(const std::string& pictures, const std::string& dir, int 
     const ef_encode_params p = { 12, qscale_i, qscale_p, 7, 1, 2, 0, 3750 };
     uint64_t to[2] = { 0, 0 };
     std::vector<uint8_t> ts(pics.size() / 4);
-    int rc = ef_encode_build(0, pics.data(), off, 1, &p, ts.data(), ts.size(), to);
+    auto build = [&]() {
+        return rate ? ef_encode_build_rate(0, pics.data(), off, 1, &p, rate, ts.data(), ts.size(), to, nullptr, nullptr)
+                    : ef_encode_build(0, pics.data(), off, 1, &p, ts.data(), ts.size(), to);
+    };
+    int rc = build();
     if (rc == EF_ENOMEM && to[1] > ts.size()) {
         ts.resize(to[1]);
-        rc = ef_encode_build(0, pics.data(), off, 1, &p, ts.data(), ts.size(), to);
+        rc = build();
     }
-    if (rc != EF_OK) throw std::runtime_error(std::string("ef_encode_build: ") + ef_last_error());
+    if (rc != EF_OK) throw std::runtime_error(std::string(rate ? "ef_encode_build_rate: " : "ef_encode_build: ") + ef_last_error());
     ts.resize(to[1]);
     if (!pcm_path.empty()) ts = add_audio(ts, pcm_path);
     write_file(dir + "/video.ts", ts.data(), ts.size());
@@ -104,9 +111,16 @@ int main(int argc, char** argv)
     const bool encode = argc >= 2 && std::string(argv[1]) == "--encode";
     std::string pcm_path;
     if (encode && argc >= 6 && std::string(argv[argc - 2]) == "--audio") { pcm_path = argv[argc - 1]; argc -= 2; }
-    if (encode ? (argc != 4 && argc != 6) : (argc != 5 && argc != 2 && argc != 3)) {
+    const bool rated = encode && argc == 7 && std::string(argv[4]) == "--rate";
+    ef_rate_params rate = { 1500000, 250000, 3, 31 };
+    if (rated) {
+        rate.bit_rate = (uint32_t)strtoul(argv[5], nullptr, 10);
+        rate.vbv_bits = (uint32_t)strtoul(argv[6], nullptr, 10);
+    }
+    if (encode ? (argc != 4 && argc != 6 && !rated) : (argc != 5 && argc != 2 && argc != 3)) {
         fprintf(stderr, "usage: %s video.ts fwd.ts rev.ts out_dir\n       %s title_dir [qscale]   (title_dir/video.ts -> video_fwd.ts, video_rwd.ts, video.idx)\n"
-                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p] [--audio pcm.s16le]   (-> title_dir/video.ts, then as title_dir)\n",
+                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p | --rate bit_rate vbv_bits] [--audio pcm.s16le]   "
+                        "(-> title_dir/video.ts, then as title_dir)\n",
                 argv[0], argv[0], argv[0]);
         return 2;
     }
@@ -120,7 +134,7 @@ int main(int argc, char** argv)
         } else {
             const std::string dir = encode ? argv[3] : argv[1];
             const int qscale = !encode && argc == 3 ? atoi(argv[2]) : 8;
-            if (encode) make_video(argv[2], dir, argc == 6 ? atoi(argv[4]) : 8, argc == 6 ? atoi(argv[5]) : 8, pcm_path);
+            if (encode) make_video(argv[2], dir, argc == 6 ? atoi(argv[4]) : 8, argc == 6 ? atoi(argv[5]) : 8, rated ? &rate : nullptr, pcm_path);
             make_trick_files(dir, qscale);
             make_index(dir + "/video.ts", all);
             make_index(dir + "/video_fwd.ts", all);

@@ -274,6 +274,31 @@ int ef_encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, in
                     uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off);
 int ef_encode_stage_ms(float* upload_ms, float* search_ms, float* code_ms, float* recon_ms, float* mux_ms);
 
+/* ---- encoded titles to a bit rate: make_video()'s "-b:v 1500k -maxrate 1500k -bufsize 0.25M -qmin 3" (indexer/indexer.cpp:307) --------
+ * Stateless; host buffers. The rule, byte for byte, is tests/rate_cases.py.
+ * ef_encode_build_rate  ef_encode_build with each picture's quantiser chosen on the device so that every GOP fits a leaky bucket of
+ *                  rc->vbv_bits filled at rc->bit_rate: each GOP starts with a full buffer, no picture takes more bits than the buffer
+ *                  holds, and every GOP but a title's last hands on a full buffer, so a player may start at any GOP after buffering
+ *                  vbv_bits. The quantiser of picture j is the smallest of qmin..qmax whose exact coded size (a census of every
+ *                  candidate, on the device) fits the picture's share of what the GOP may still spend and keeps the rest of the GOP
+ *                  feasible; else the smallest that keeps it feasible; else a fallback (P: every macroblock not coded, a copy of the
+ *                  reference picture; I: the DC levels alone) that always fits. p supplies gop, search, aspect, rate and the pts; its
+ *                  qscale_i and qscale_p are not read. Every sequence header carries bit_rate = ceil(bit_rate / 400) and
+ *                  vbv_buffer_size = ceil(vbv_bits / 16384), vbv_delay stays 0xFFFF (variable rate, bit_rate the peak); the audio is
+ *                  not counted, as ffmpeg's -b:v does not count it. pic_q[i] (may be NULL) receives input picture i's quantiser, 0 for
+ *                  a fallback, and pic_bytes[i] (may be NULL) its ES bytes; both are filled by a sizing call too.
+ *                  ts, ts_cap, ts_off, the sizing call, the batch limits and the EF_EINVAL cases are ef_encode_build's, and further
+ *                  EF_EINVAL: bit_rate outside 400 .. 400 * 0x3FFFE, vbv_bits outside 1 .. 1023 * 16384, not 1 <= qmin <= qmax <= 31,
+ *                  or a bucket too small for any guarantee: the I fallback's worst case (3,592 bytes) does not fit a full GOP that must
+ *                  end full. The census and the choice count in ef_encode_stage_ms's coding stage. */
+typedef struct {
+    uint32_t bit_rate;           /* bits per second, 400 .. 400 * 0x3FFFE (1,500,000: -b:v / -maxrate 1500k) */
+    uint32_t vbv_bits;           /* the buffer, 1 .. 1023 * 16384 bits (250,000: -bufsize 0.25M) */
+    int qmin, qmax;              /* the candidate quantisers, 1 <= qmin <= qmax <= 31 (3 .. 31: -qmin 3) */
+} ef_rate_params;
+int ef_encode_build_rate(int device, const uint8_t* i420, const uint64_t* pic_off, int n_titles, const ef_encode_params* p,
+                         const ef_rate_params* rc, uint8_t* ts, uint64_t ts_cap, uint64_t* ts_off, uint8_t* pic_q, uint32_t* pic_bytes);
+
 /* ---- encoded titles, audio: SBC from PCM and its interleave into video.ts ----------------------------------------------------------
  * The audio of the reference's make_video() (indexer/indexer.cpp:306-309: ffmpeg's "-codec:a sbc -ar 48000 -b:a 192k -ac 1
  * -streamid 1:258 -pes_payload_size 512"). Stateless; host buffers. The rule, byte for byte, is tests/sbc_encode_cases.py.
