@@ -40,30 +40,25 @@ __global__ void ef_pts_packet_kernel(const uint8_t* ts, const uint64_t* ts_off, 
 size_t ef_recon_smem_bytes();
 cudaError_t ef_decode_configure();
 int ef_decode_resident_ctas(int which);
-cudaError_t ef_trick_upload_tables();
 cudaError_t ef_trick_launch_gather(const uint8_t* frames, const uint32_t* streams, const uint32_t* slots, int count, int fb, uint8_t* dst, cudaStream_t st);
-cudaError_t ef_trick_launch_encode(const uint8_t* in, int n_pics, int qscale, uint32_t* slots, uint32_t* slice_len, cudaStream_t st,
-                                  const uint8_t* qpic = nullptr);
-cudaError_t ef_trick_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int n_pics,
-                                     uint8_t* es, cudaStream_t st);
 cudaError_t ef_trick_launch_mux(const uint8_t* es, const EfTrickPic* pics, int n_pics, uint64_t n_packets, uint8_t* out, cudaStream_t st);
-cudaError_t ef_encode_upload_tables();
 cudaError_t ef_sbc_encode_upload_tables();
 cudaError_t ef_sbc_launch_encode(const int16_t* pcm, uint64_t pcm_base, uint64_t pcm_len, const uint64_t* pcm_off, const uint64_t* frame_first,
                                  int n_streams, uint64_t frame0, uint64_t n_frames, int frequency, int allocation, int bitpool, uint8_t* out,
                                  cudaStream_t st);
+cudaError_t ef_encode_upload_tables();
 cudaError_t ef_encode_launch_tile(const uint8_t* i420, const uint32_t* src, int count, uint8_t* tiled, cudaStream_t st);
 cudaError_t ef_encode_launch_search(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
                                     const uint32_t* n_pics, int search, uint32_t* mbinfo, cudaStream_t st);
-cudaError_t ef_encode_launch_p(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
-                               const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, const uint8_t* qpic, uint32_t* slots, uint32_t* slice_len,
-                               cudaStream_t st);
+cudaError_t ef_encode_launch_slices(bool ipic, const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
+                                    const uint32_t* n_pics, const uint32_t* mbinfo, int qscale, const uint8_t* qpic, uint32_t* slots, uint32_t* slice_len,
+                                    cudaStream_t st);
 cudaError_t ef_encode_launch_census(const uint8_t* src, const uint32_t* streams, int count, const uint8_t* frames, const uint32_t* base_pics,
                                     const uint32_t* n_pics, const uint32_t* mbinfo, int ipic, int qmin, int nq, uint32_t* census, cudaStream_t st);
 cudaError_t ef_encode_launch_choose(const uint32_t* census, const uint32_t* streams, int count, int j, int qmin, int qmax, const EfRateBucket& rb,
                                     const uint32_t* gop_n, int64_t* bucket, uint8_t* qpic, uint32_t* pic_bytes, cudaStream_t st);
-cudaError_t ef_encode_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* header, int n_pics,
-                                      uint8_t* es, cudaStream_t st);
+cudaError_t ef_encode_launch_assemble(const uint32_t* slots, const uint32_t* slice_len, const uint64_t* pic_dst, const uint8_t* headers, int hb,
+                                      bool per_picture, int n_pics, uint8_t* es, cudaStream_t st);
 __global__ void ef_tsidx_packet_kernel(const uint8_t* ts, const uint64_t* pkt_off, int n_files, uint64_t n_packets, int64_t* pkt_pts, uint8_t* pkt_kind);
 __global__ void ef_tsidx_compact_kernel(const uint64_t* pkt_off, const int64_t* pkt_pts, const uint8_t* pkt_kind, int64_t* seq_pts, uint32_t* seq_pos, int64_t* info);
 __global__ void ef_tsidx_sample_kernel(const int64_t* seq_pts, const uint32_t* seq_pos, int n, int64_t first_pts, uint32_t bin_size, uint32_t n_samples, uint32_t* samples);
@@ -2307,7 +2302,7 @@ namespace {
 constexpr int kTrickSpeed = 15;                  // merge_index's trick_speed
 constexpr int kTrickChunkStreams = 256;          // segments decoded in one batch (about 2.2 MB of device memory each)
 constexpr uint64_t kTrickChunkBytes = 64u << 20; // TS bytes of one batch (a longer segment is a batch of its own)
-constexpr int kTrickEncodeBatch = 256;           // pictures per encode launch (26 MB of frames, 90 MB of slice regions)
+constexpr int kTrickEncodeBatch = 256;           // pictures per encode launch (26 MB of frames, 91 MB of slice regions)
 
 struct GrowBuf {                                 // device buffer that keeps its contents when it grows
     uint8_t* p = nullptr;
@@ -2575,8 +2570,114 @@ struct TrickTimer {                              // CUDA event pairs per phase, 
         open_ev = nullptr;
         return cudaEventRecord(b, st);
     }
+    template <int N>
+    cudaError_t collect(float (&ms)[N])          // every phase's spans summed into ms[phase], once they have ended
+    {
+        for (float& m : ms) m = 0;
+        for (auto& s : spans) {
+            float t = 0;
+            const cudaError_t e = cudaEventElapsedTime(&t, s.second.first, s.second.second);
+            if (e != cudaSuccess) return e;
+            ms[s.first] += t;
+        }
+        return cudaSuccess;
+    }
 };
 thread_local float g_trick_ms[4] = { 0, 0, 0, 0 };
+
+// The ES of coded pictures in device memory. The slice coder writes n pictures' slices to `slots` and their bytes to `len`; place()
+// reads the lengths back, puts the pictures back to back at the end of the ES (`es` grows and keeps what it holds) and assembles
+// each there behind its header: hdr holds hb bytes per picture, or one header for all when `shared`. dst[p] and bytes[p] receive
+// where picture p went and its bytes.
+struct CodedEs {
+    GrowBuf slots, len, es, d_dst, d_hdr;
+    uint64_t total = 0;
+    std::vector<uint64_t> dst;
+    std::vector<uint32_t> bytes;
+
+    cudaError_t reserve(size_t n)                // room for the slices of n pictures
+    {
+        const cudaError_t e = slots.reserve(n * EF_MBH_MAX * kTrickSliceBytes);
+        return e != cudaSuccess ? e : len.reserve(n * EF_MBH_MAX * 4);
+    }
+    int place(int n, const uint8_t* hdr, int hb, bool shared, cudaStream_t st)
+    {
+        std::vector<uint32_t> l((size_t)n * EF_MBH_MAX);
+        CK(cudaMemcpyAsync(l.data(), len.p, l.size() * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        dst.resize((size_t)n); bytes.resize((size_t)n);
+        const uint64_t es0 = total;
+        for (int p = 0; p < n; p++) {
+            uint32_t b = (uint32_t)hb;
+            for (int s = 0; s < EF_MBH_MAX; s++) b += l[(size_t)p * EF_MBH_MAX + s];
+            dst[p] = total; bytes[p] = b;
+            total += b;
+        }
+        if (total + 16 > es.cap) CK(es.reserve(std::max<size_t>(total + 16, es.cap * 2), es0));     // grows geometrically
+        const size_t hdr_bytes = (size_t)hb * (shared ? 1 : n);
+        CK(d_dst.reserve((size_t)n * 8)); CK(d_hdr.reserve(hdr_bytes));
+        CK(cudaMemcpyAsync(d_dst.p, dst.data(), (size_t)n * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_hdr.p, hdr, hdr_bytes, cudaMemcpyHostToDevice, st));
+        CK(ef_encode_launch_assemble((const uint32_t*)slots.p, (const uint32_t*)len.p, (const uint64_t*)d_dst.p, d_hdr.p, hb, !shared, n, es.p, st));
+        return EF_OK;
+    }
+};
+
+// The TS of coded pictures: output sets of files back to back, each file one PES per picture (add(), in order) with its own continuity
+// counter; begin_set() and end_file() fill the set's off[n_files + 1]. run() answers EF_ENOMEM ("<what> need <bytes> (<name>) and
+// ... bytes") when a set does not fit its dst, else muxes every set from the ES in one launch and copies each to its dst.
+struct TsMux {
+    struct Set { uint8_t* dst; uint64_t cap; uint64_t* off; const char* name; int files; };
+    std::vector<Set> sets;
+    std::vector<EfTrickPic> plan;
+    uint64_t packets = 0;
+    uint32_t cc = 0;
+
+    void begin_set(uint8_t* dst, uint64_t cap, uint64_t* off, const char* name = nullptr)
+    {
+        sets.push_back({ dst, cap, off, name, 0 });
+        off[0] = 0;
+    }
+    void add(uint64_t es_off, uint32_t es_len, int64_t pts)
+    {
+        plan.push_back({ es_off, packets, pts, es_len, cc });
+        const uint32_t pkts = (14 + es_len + 183) / 184;
+        packets += pkts; cc += pkts;
+    }
+    void end_file()
+    {
+        Set& s = sets.back();
+        s.off[s.files + 1] = s.off[s.files] + (uint64_t)cc * 188;
+        s.files++; cc = 0;
+    }
+    int run(const uint8_t* es, const char* what, TrickTimer& timer, int phase, cudaStream_t st)
+    {
+        bool fits = true;
+        char need[256] = "";
+        for (const Set& s : sets) {
+            const uint64_t n = s.off[s.files];
+            fits = fits && s.cap >= n && (!n || s.dst);
+            const size_t l = strlen(need);
+            snprintf(need + l, sizeof(need) - l, s.name ? "%s%llu (%s)" : "%s%llu", l ? " and " : "", (unsigned long long)n, s.name);
+        }
+        if (!fits) return fail(EF_ENOMEM, "%s need %s bytes", what, need);
+        GrowBuf d_plan, d_out;
+        CK(d_plan.reserve(std::max<size_t>(plan.size(), 1) * sizeof(EfTrickPic)));
+        CK(d_out.reserve(packets * 188 + 16));
+        CK(cudaMemcpy(d_plan.p, plan.data(), plan.size() * sizeof(EfTrickPic), cudaMemcpyHostToDevice));
+        CK(timer.begin(st));
+        CK(ef_trick_launch_mux(es, (const EfTrickPic*)d_plan.p, (int)plan.size(), packets, d_out.p, st));
+        CK(timer.end(phase, st));
+        uint64_t o = 0;
+        for (const Set& s : sets) {
+            const uint64_t n = s.off[s.files];
+            if (n) CK(cudaMemcpy(s.dst, d_out.p + o, n, cudaMemcpyDeviceToHost));
+            o += n;
+        }
+        CK(cudaDeviceSynchronize());
+        return EF_OK;
+    }
+};
 
 // the state of one decode batch, for the K1b hook: after picture index p, gather the frames of the selected pictures with that index
 struct TrickGather {
@@ -2689,10 +2790,11 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
         max_pusi = std::max(max_pusi, n);
     }
 
-    CK(ef_trick_upload_tables());
+    CK(ef_encode_upload_tables());
     cudaStream_t st = 0;
     TrickTimer timer;
-    GrowBuf d_ts, d_off, d_list, d_in, d_slots, d_len, d_es, d_dst, d_hdr;
+    GrowBuf d_ts, d_off, d_list, d_in;
+    CodedEs ces;
     CK(d_ts.reserve(n_packets * 188 + 16));
     CK(cudaMemcpy(d_ts.p, base, n_packets * 188, cudaMemcpyHostToDevice));
     CK(d_off.reserve(((size_t)max_streams + 1) * 8));
@@ -2700,13 +2802,12 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     ef_ctx* ctx = nullptr;
     struct CtxGuard { ef_ctx** c; ~CtxGuard() { if (*c) ef_destroy(*c); } } ctx_guard{ &ctx };
 
-    // every encoded picture: its file, its main pts, where its bytes are in d_es
+    // every encoded picture: its file, its main pts, where its bytes are in the ES
     struct Enc { int file; int64_t main_pts; uint64_t es_off; uint32_t es_len; };
     std::vector<Enc> enc;
     std::vector<std::vector<uint32_t>> fwd_of((size_t)n_files);   // encoded picture ids of every file's fwd pictures, in order
     std::vector<uint64_t> seen((size_t)n_files, 0);                 // main pictures of every file so far
     std::vector<int64_t> p0((size_t)n_files, -1);
-    uint64_t es_total = 0;
     size_t pending = 0;                                             // gathered, not yet encoded: enc[enc.size() - pending ..)
     size_t in_cap = 0;
 
@@ -2714,31 +2815,15 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
         if (!pending) return EF_OK;
         const int n = (int)pending;
         const size_t e0 = enc.size() - pending;
-        CK(d_slots.reserve((size_t)n * EF_MBH_MAX * kTrickSliceBytes));
-        CK(d_len.reserve((size_t)n * EF_MBH_MAX * 4));
+        CK(ces.reserve((size_t)n));
         CK(timer.begin(st));
-        CK(ef_trick_launch_encode(d_in.p, n, qscale, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
-        std::vector<uint32_t> len((size_t)n * EF_MBH_MAX);
-        CK(cudaMemcpyAsync(len.data(), d_len.p, len.size() * 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        std::vector<uint64_t> dst((size_t)n);
+        CK(ef_encode_launch_slices(true, d_in.p, nullptr, n, nullptr, nullptr, nullptr, nullptr, qscale, nullptr, (uint32_t*)ces.slots.p,
+                                   (uint32_t*)ces.len.p, st));
         std::vector<uint8_t> hdr((size_t)n * kTrickHeaderBytes);
-        const uint64_t es0 = es_total;
-        for (int p = 0; p < n; p++) {
-            uint32_t bytes = kTrickHeaderBytes;
-            for (int s = 0; s < EF_MBH_MAX; s++) bytes += len[(size_t)p * EF_MBH_MAX + s];
-            Enc& e = enc[e0 + p];
-            e.es_off = dst[p] = es_total; e.es_len = bytes;
-            es_total += bytes;
-            memcpy(&hdr[(size_t)p * kTrickHeaderBytes], headers[e.file].data(), kTrickHeaderBytes);
-        }
-        if (es_total + 16 > d_es.cap) CK(d_es.reserve(std::max<size_t>(es_total + 16, d_es.cap * 2), es0));   // grows geometrically
-        CK(d_dst.reserve(dst.size() * 8)); CK(d_hdr.reserve(hdr.size()));
-        CK(cudaMemcpyAsync(d_dst.p, dst.data(), dst.size() * 8, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_hdr.p, hdr.data(), hdr.size(), cudaMemcpyHostToDevice, st));
-        CK(ef_trick_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, n, d_es.p, st));
+        for (int p = 0; p < n; p++) memcpy(&hdr[(size_t)p * kTrickHeaderBytes], headers[enc[e0 + p].file].data(), kTrickHeaderBytes);
+        TRY(ces.place(n, hdr.data(), kTrickHeaderBytes, false, st));
+        for (int p = 0; p < n; p++) { enc[e0 + p].es_off = ces.dst[p]; enc[e0 + p].es_len = ces.bytes[p]; }
         CK(timer.end(2, st));
-        CK(cudaStreamSynchronize(st));                    // the host buffers above go out of scope
         pending = 0;
         return EF_OK;
     };
@@ -2817,48 +2902,25 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     }
     TRY(encode_pending());
 
-    // the plan of both outputs: every file's fwd pictures, then every file's rwd pictures
-    std::vector<EfTrickPic> plan;
-    uint64_t pk = 0;
+    // both outputs in one mux: every file's fwd pictures, then every file's rwd pictures
+    TsMux mux;
     for (int dir = 0; dir < 2; dir++) {
-        uint64_t* o = dir ? rwd_off : fwd_off;
-        o[0] = 0;
+        if (dir) mux.begin_set(rwd, rwd_cap, rwd_off, "rwd");
+        else mux.begin_set(fwd, fwd_cap, fwd_off, "fwd");
         for (int f = 0; f < n_files; f++) {
             const std::vector<uint32_t>& ids = fwd_of[f];
             const size_t n = ids.size();
             std::vector<int64_t> fp(n);
             for (size_t k = 0; k < n; k++) fp[k] = p0[f] + (enc[ids[k]].main_pts - p0[f]) / kTrickSpeed;
-            uint32_t cc = 0;
             for (size_t k = 0; k < n; k++) {
-                const size_t src = dir ? n - 1 - k : k;
-                const Enc& e = enc[ids[src]];
-                const int64_t t = dir ? fp[0] + (fp[n - 1] - fp[n - 1 - k]) : fp[k];
-                plan.push_back({ e.es_off, pk, t, e.es_len, cc });
-                const uint32_t pkts = (14 + e.es_len + 183) / 184;
-                pk += pkts; cc += pkts;
+                const Enc& e = enc[ids[dir ? n - 1 - k : k]];
+                mux.add(e.es_off, e.es_len, dir ? fp[0] + (fp[n - 1] - fp[n - 1 - k]) : fp[k]);
             }
-            o[f + 1] = o[f] + (uint64_t)cc * 188;
+            mux.end_file();
         }
     }
-    const uint64_t fwd_need = fwd_off[n_files], rwd_need = rwd_off[n_files];
-    if (fwd_cap < fwd_need || rwd_cap < rwd_need || (fwd_need && !fwd) || (rwd_need && !rwd))
-        return fail(EF_ENOMEM, "the trick files need %llu (fwd) and %llu (rwd) bytes", (unsigned long long)fwd_need, (unsigned long long)rwd_need);
-    GrowBuf d_plan, d_out;
-    CK(d_plan.reserve(std::max<size_t>(plan.size(), 1) * sizeof(EfTrickPic)));
-    CK(d_out.reserve(pk * 188 + 16));
-    CK(cudaMemcpy(d_plan.p, plan.data(), plan.size() * sizeof(EfTrickPic), cudaMemcpyHostToDevice));
-    CK(timer.begin(st));
-    CK(ef_trick_launch_mux(d_es.p, (const EfTrickPic*)d_plan.p, (int)plan.size(), pk, d_out.p, st));
-    CK(timer.end(3, st));
-    if (fwd_need) CK(cudaMemcpy(fwd, d_out.p, fwd_need, cudaMemcpyDeviceToHost));
-    if (rwd_need) CK(cudaMemcpy(rwd, d_out.p + fwd_need, rwd_need, cudaMemcpyDeviceToHost));
-    CK(cudaDeviceSynchronize());
-    for (float& m : g_trick_ms) m = 0;
-    for (auto& s : timer.spans) {
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
-        g_trick_ms[s.first] += ms;
-    }
+    TRY(mux.run(ces.es.p, "the trick files", timer, 3, st));
+    CK(timer.collect(g_trick_ms));
     return EF_OK;
 }
 
@@ -2978,11 +3040,11 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
     const std::vector<uint8_t> i_hdr = rc ? trick_header(p->aspect, p->rate, (rc->bit_rate + 399) / 400, (rc->vbv_bits + 16383) / 16384)
                                           : trick_header(p->aspect, p->rate);
 
-    CK(ef_trick_upload_tables());
     CK(ef_encode_upload_tables());
     cudaStream_t st = 0;
     TrickTimer timer;
-    GrowBuf d_src, d_tiled, d_list, d_info, d_slots, d_len, d_es, d_dst, d_hdr, d_off, d_census, d_rate;
+    GrowBuf d_src, d_tiled, d_list, d_info, d_off, d_census, d_rate;
+    CodedEs ces;
     const int qmin = rc ? rc->qmin : 0, nq = rc ? rc->qmax - rc->qmin + 1 : 0;
     // rate: census [B][32][12] u32; d_rate: bucket [B] i64, choice bytes [B] u32, GOP lengths [B] u32, quantisers [B] u8
     int64_t* d_bucket = nullptr;
@@ -2999,19 +3061,15 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
     CK(d_tiled.reserve((size_t)B * EF_FRAME));
     CK(d_list.reserve((size_t)B * 8));
     CK(d_info.reserve((size_t)B * EF_MBW_MAX * EF_MBH_MAX * 4));
-    CK(d_slots.reserve((size_t)B * EF_MBH_MAX * std::max(kEncSliceBytes, kTrickSliceBytes)));
-    CK(d_len.reserve((size_t)B * EF_MBH_MAX * 4));
-    CK(d_dst.reserve((size_t)B * 8));
-    CK(d_hdr.reserve((size_t)B * kTrickHeaderBytes));
+    CK(ces.reserve((size_t)B));
     CK(d_off.reserve(((size_t)B + 1) * 8));
     ef_ctx* ctx = nullptr;
     struct CtxGuard { ef_ctx** c; ~CtxGuard() { if (*c) ef_destroy(*c); } } ctx_guard{ &ctx };
     ef_config cfg = { device, B, 1, EF_MBH_MAX, kEncodeSubmitBytes, 0 };
     TRY(ef_create(&ctx, &cfg));
 
-    std::vector<uint64_t> es_off(pic_off[n_titles] - pic_off[0]);      // every picture's bytes in d_es
+    std::vector<uint64_t> es_off(pic_off[n_titles] - pic_off[0]);      // every picture's bytes in the ES
     std::vector<uint32_t> es_len(es_off.size());
-    uint64_t es_total = 0;
     for (size_t g0 = 0; g0 < gops.size(); g0 += (size_t)B) {
         const int nb = (int)std::min<size_t>((size_t)B, gops.size() - g0);
         const uint64_t p0 = gops[g0].first, np = gops[g0 + nb - 1].first + gops[g0 + nb - 1].n - p0;
@@ -3050,28 +3108,23 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
                 CK(ef_encode_launch_choose((const uint32_t*)d_census.p, d_act, na, k, qmin, rc->qmax, rb, d_gopn, d_bucket, d_qpic, d_pbytes, st));
                 ctx->launches += 2;
             }
-            if (k)
-                CK(ef_encode_launch_p(d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, (const uint32_t*)d_info.p, p->qscale_p,
-                                      d_qpic, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st));
-            else CK(ef_trick_launch_encode(d_tiled.p, na, p->qscale_i, (uint32_t*)d_slots.p, (uint32_t*)d_len.p, st, d_qpic));
+            CK(ef_encode_launch_slices(k == 0, d_tiled.p, d_act, na, ctx->h.frames, ctx->h.base_pics, ctx->h.n_pics, (const uint32_t*)d_info.p,
+                                       k ? p->qscale_p : p->qscale_i, d_qpic, (uint32_t*)ces.slots.p, (uint32_t*)ces.len.p, st));
             ctx->launches++;
-            std::vector<uint32_t> len((size_t)na * EF_MBH_MAX), chosen_bytes(rc ? (size_t)na : 0);
+            std::vector<uint32_t> chosen_bytes(rc ? (size_t)na : 0);
             std::vector<uint8_t> chosen_q(chosen_bytes.size());
-            CK(cudaMemcpyAsync(len.data(), d_len.p, len.size() * 4, cudaMemcpyDeviceToHost, st));
-            if (rc) {
+            if (rc) {                                    // read back with the slice lengths
                 CK(cudaMemcpyAsync(chosen_bytes.data(), d_pbytes, (size_t)na * 4, cudaMemcpyDeviceToHost, st));
                 CK(cudaMemcpyAsync(chosen_q.data(), d_qpic, (size_t)na, cudaMemcpyDeviceToHost, st));
             }
-            CK(cudaStreamSynchronize(st));
-            const uint32_t hb = k ? kEncPHeaderBytes : kTrickHeaderBytes;
-            std::vector<uint64_t> dst((size_t)na);
-            const uint64_t round0 = es_total;
+            const std::vector<uint8_t> hdr = k ? encode_p_header(k) : i_hdr;      // all pictures of a round share their header
+            TRY(ces.place(na, hdr.data(), k ? kEncPHeaderBytes : kTrickHeaderBytes, true, st));
+            ctx->launches++;
+            const std::vector<uint64_t>& dst = ces.dst;
             for (int a = 0; a < na; a++) {
-                uint32_t bytes = hb;
-                for (int s = 0; s < EF_MBH_MAX; s++) bytes += len[(size_t)a * EF_MBH_MAX + s];
                 const uint64_t pic = p0 + src[a];
-                dst[a] = es_off[pic] = es_total; es_len[pic] = bytes;
-                es_total += bytes;
+                const uint32_t bytes = ces.bytes[a];
+                es_off[pic] = dst[a]; es_len[pic] = bytes;
                 if (rc) {                                // the bucket counted the census's size: it must be the coder's
                     if (chosen_bytes[a] != bytes)
                         return fail(EF_ECUDA, "picture %llu: the census gave %u bytes at its quantiser, the coder %u", (unsigned long long)pic,
@@ -3080,19 +3133,6 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
                 }
                 if (pic_bytes) pic_bytes[pic] = bytes;
             }
-            if (es_total + 16 > d_es.cap) CK(d_es.reserve(std::max<size_t>(es_total + 16, d_es.cap * 2), round0));
-            CK(cudaMemcpyAsync(d_dst.p, dst.data(), dst.size() * 8, cudaMemcpyHostToDevice, st));
-            if (k) {
-                const std::vector<uint8_t> h = encode_p_header(k);
-                CK(cudaMemcpyAsync(d_hdr.p, h.data(), h.size(), cudaMemcpyHostToDevice, st));
-                CK(ef_encode_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, na, d_es.p, st));
-            } else {
-                std::vector<uint8_t> h((size_t)na * kTrickHeaderBytes);
-                for (int a = 0; a < na; a++) memcpy(&h[(size_t)a * kTrickHeaderBytes], i_hdr.data(), kTrickHeaderBytes);
-                CK(cudaMemcpyAsync(d_hdr.p, h.data(), h.size(), cudaMemcpyHostToDevice, st));
-                CK(ef_trick_launch_assemble((const uint32_t*)d_slots.p, (const uint32_t*)d_len.p, (const uint64_t*)d_dst.p, d_hdr.p, na, d_es.p, st));
-            }
-            ctx->launches++;
             CK(timer.end(2, st));
             // the decoder's reconstruction of round k: each GOP's picture in its own stream, in submits of at most kEncodeSubmitBytes
             CK(timer.begin(st));
@@ -3105,7 +3145,7 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
                     off[g] = (a < a1 ? dst[a] : dst[a1 - 1] + es_len[p0 + src[a1 - 1]]) - dst[a0];
                 }
                 CK(cudaMemcpyAsync(d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice, st));
-                TRY(ef_submit_es_device(ctx, d_es.p + dst[a0], (const uint64_t*)d_off.p, st));
+                TRY(ef_submit_es_device(ctx, ces.es.p + dst[a0], (const uint64_t*)d_off.p, st));
                 TRY(ef_index(ctx, st));
                 TRY(decode_range(ctx, 0, 1, st));
                 a0 = a1;
@@ -3115,36 +3155,16 @@ int encode_build(int device, const uint8_t* i420, const uint64_t* pic_off, int n
     }
     TRY(ef_index_info(ctx, nullptr, nullptr, nullptr, nullptr));
 
-    // one TS per title: a PES per picture with pts0 + k pts_step, one continuity counter per file
-    std::vector<EfTrickPic> plan;
-    uint64_t pk = 0;
-    ts_off[0] = 0;
+    // one TS per title: a PES per picture with pts0 + k pts_step
+    TsMux mux;
+    mux.begin_set(ts, ts_cap, ts_off);
     for (int t = 0; t < n_titles; t++) {
-        uint32_t cc = 0;
-        for (uint64_t k = pic_off[t]; k < pic_off[t + 1]; k++) {
-            const uint64_t pic = k - pic_off[0];
-            plan.push_back({ es_off[pic], pk, p->pts0 + (int64_t)(k - pic_off[t]) * (int64_t)p->pts_step, es_len[pic], cc });
-            const uint32_t pkts = (14 + es_len[pic] + 183) / 184;
-            pk += pkts; cc += pkts;
-        }
-        ts_off[t + 1] = ts_off[t] + (uint64_t)cc * 188;
+        for (uint64_t k = pic_off[t]; k < pic_off[t + 1]; k++)
+            mux.add(es_off[k - pic_off[0]], es_len[k - pic_off[0]], p->pts0 + (int64_t)(k - pic_off[t]) * (int64_t)p->pts_step);
+        mux.end_file();
     }
-    if (ts_cap < ts_off[n_titles] || !ts) return fail(EF_ENOMEM, "the titles need %llu bytes", (unsigned long long)ts_off[n_titles]);
-    GrowBuf d_plan, d_out;
-    CK(d_plan.reserve(plan.size() * sizeof(EfTrickPic)));
-    CK(d_out.reserve(pk * 188 + 16));
-    CK(cudaMemcpy(d_plan.p, plan.data(), plan.size() * sizeof(EfTrickPic), cudaMemcpyHostToDevice));
-    CK(timer.begin(st));
-    CK(ef_trick_launch_mux(d_es.p, (const EfTrickPic*)d_plan.p, (int)plan.size(), pk, d_out.p, st));
-    CK(timer.end(4, st));
-    CK(cudaMemcpy(ts, d_out.p, pk * 188, cudaMemcpyDeviceToHost));
-    CK(cudaDeviceSynchronize());
-    for (float& m : g_encode_ms) m = 0;
-    for (auto& s : timer.spans) {
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
-        g_encode_ms[s.first] += ms;
-    }
+    TRY(mux.run(ces.es.p, "the titles", timer, 4, st));
+    CK(timer.collect(g_encode_ms));
     return EF_OK;
 }
 
@@ -3219,11 +3239,7 @@ extern "C" int ef_sbc_encode(int device, const int16_t* pcm, const uint64_t* pcm
         CK(timer.end(2, st));
     }
     CK(cudaStreamSynchronize(st));
-    for (auto& s : timer.spans) {
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, s.second.first, s.second.second));
-        g_audio_enc_ms[s.first] += ms;
-    }
+    CK(timer.collect(g_audio_enc_ms));
     return EF_OK;
 }
 

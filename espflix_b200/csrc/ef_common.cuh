@@ -290,17 +290,16 @@ struct __align__(16) EfLibStream {   // layout of ef_library_status (include/esp
     int64_t pos;                 // _info[_nav].pos: the main pts the next PLAY, SKIP, FAST_FORWARD or REWIND starts from
 };
 
-// trick streams (ef_trick_build, csrc/ef_trick.cu): every picture's 28 header bytes, the worst-case bytes of one intra slice (start
-// code + 6 bits + 22 macroblocks of 2 bits + 6 blocks of a 16-bit DC code, 63 28-bit escapes and the end of block, in whole words), and
-// one output picture of the mux: its ES bytes, its first packet among all output packets, its pts and its file's continuity counter
+// coded pictures (csrc/ef_encode.cu): an I picture's 28 header bytes (sequence, GOP and picture headers), a P picture's 9, and the
+// slice region of one coded slice, the larger of two worst cases in whole words: an intra slice (start code + 6 bits + 22 macroblocks
+// of 2 bits + 6 blocks of a 16-bit DC code, 63 28-bit escapes and the end of block) and a P slice (22 macroblocks of an 11-bit
+// address increment, a 5-bit type, two 11-bit vector codes, a 9-bit pattern and 6 non-intra blocks of 64 28-bit escapes and the end
+// of block; an intra macroblock's blocks are shorter). One output picture of the mux: its ES bytes, its first packet among all output
+// packets, its pts and its file's continuity counter.
 constexpr int kTrickHeaderBytes = 28;
-constexpr int kTrickSliceBytes = 29440;
-static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (2 + 6 * (16 + 63 * 28 + 2)) + 31) / 32) * 4, "worst-case slice");
-// encoded titles (ef_encode_build, csrc/ef_encode.cu): the worst-case bytes of one P slice (start code + 6 bits + 22 macroblocks of an
-// 11-bit address increment, a 5-bit type, two 11-bit vector codes, a 9-bit pattern and 6 non-intra blocks of 64 28-bit escapes and
-// the end of block, in whole words; an intra macroblock's blocks are shorter) and a P picture's header bytes
-constexpr int kEncSliceBytes = 29736;
-static_assert(kEncSliceBytes >= ((32 + 6 + 22 * (11 + 5 + 2 * 11 + 9 + 6 * (64 * 28 + 2)) + 31) / 32) * 4, "worst-case P slice");
+constexpr int kTrickSliceBytes = 29736;
+static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (2 + 6 * (16 + 63 * 28 + 2)) + 31) / 32) * 4, "worst-case I slice");
+static_assert(kTrickSliceBytes >= ((32 + 6 + 22 * (11 + 5 + 2 * 11 + 9 + 6 * (64 * 28 + 2)) + 31) / 32) * 4, "worst-case P slice");
 constexpr int kEncPHeaderBytes = 9;
 // rate-controlled titles (ef_encode_build_rate): a picture's quantiser byte is q, or qmax | kQFallback for its fallback coding (P: every
 // macroblock not coded; I: the DC levels alone); the census holds every slice's bytes at up to 31 candidates and the fallback in slot
