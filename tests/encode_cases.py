@@ -52,11 +52,6 @@ P_HEADER_BYTES = 9
 # bytes and 42.5 dB lowest; at 16 / 16 vmedia's worst picture falls to 31.6 dB.
 DEFAULT_PARAMS = dict(gop=12, qscale_i=8, qscale_p=8, search=7, aspect=1, rate=2, pts0=0, pts_step=3750)
 
-MBA = tc._vlc("ef_vlc_mba")
-MBTYPE_P = tc._vlc("ef_vlc_mbtype_p")
-MV = tc._vlc("ef_vlc_mv")
-CBP = tc._vlc("ef_vlc_cbp")
-
 
 def planes(i420):
     f = np.frombuffer(bytes(i420), dtype=np.uint8).astype(np.int64)
@@ -144,113 +139,41 @@ def inter_levels(F, qscale):
     return np.sign(f) * np.minimum((8 * np.abs(f)) // (16 * qscale), 255)
 
 
-class Bits:
-    def __init__(self):
-        self.v, self.n = [], []
-
-    def put(self, val, n):
-        self.v.append(int(val)); self.n.append(int(n))
-
-    def code(self, s):
-        self.put(int(s, 2), len(s))
+def p_header(tref):
+    """a P picture's header (P_HEADER_BYTES) of temporal reference tref"""
+    return b"\x00\x00\x01\x00" + tc.pack([tref, 2, 0xFFFF, 0, 1, 0], [10, 3, 16, 1, 3, 1])
 
 
-def ac_code(run, lv):
-    a = abs(int(lv))
-    if a <= 40 and tc.AC_LEN[run, a]:
-        return (int(tc.AC_CODE[run, a]) << 1) | (lv < 0), int(tc.AC_LEN[run, a]) + 1
-    if -127 <= lv <= 127:
-        L, bits = 8, lv & 0xFF
-    elif lv > 0:
-        L, bits = 16, lv
-    else:
-        L, bits = 16, (128 << 8) | ((lv + 256) & 0xFF)
-    return (1 << (6 + L)) | (run << L) | bits, 12 + L
-
-
-def put_block(bw, lv, intra, comp, pred):
-    """one coded block's codes; intra: returns the new DC predictor"""
-    start = 0
-    if intra:
-        dc = int(lv[0])
-        bw.put(*tc._dc_code(min(comp, 1), dc - pred))
-        pred, start = dc, 1
-    prev = start - 1
-    for i in range(start, 64):
-        if lv[i]:
-            run = i - prev - 1
-            if not intra and i == 0 and abs(int(lv[0])) == 1:
-                bw.put(2 | (lv[0] < 0), 2)
-            else:
-                bw.put(*ac_code(run, int(lv[i])))
-            prev = i
-    bw.code("10")
-    return pred
-
-
-def p_picture(src, ref, k, gop, qscale, search_px):
-    """-> (picture bytes, per-macroblock (h, v, intra, skipped, cbp))"""
+def analyse(src, ref, search_px):
+    """the quantiser-independent part of a P picture: the search, the mode decision and both transforms"""
     y, cb, cr = src
     h, v, best, intra = search(y, ref[0], search_px)
     h, v = np.where(intra, 0, h), np.where(intra, 0, v)
     blocks = mb_blocks(y, cb, cr)
-    pred = predictions(ref, h, v)
-    Fi = tc.fdct(blocks)
-    Fp = tc.fdct(blocks - pred)
-    Li = tc.quantise(Fi, qscale)
-    Lp = inter_levels(Fp, qscale)
-    L = np.where(intra[:, None, None], Li, Lp)
-    cbp = np.where(intra, 63, ((L != 0).any(axis=2) * (0x20 >> np.arange(6))).sum(axis=1))
-    hdr = tc.pack([k % gop, 2, 0xFFFF, 0, 1, 0], [10, 3, 16, 1, 3, 1])
-    out = [b"\x00\x00\x01\x00" + hdr]
-    skipped = np.zeros(264, bool)
-    for row in range(MBH):
-        bw = Bits()
-        bw.put(qscale << 1, 6)
-        pending, dcp, mvp = 0, [128, 128, 128], [0, 0]
-        for mx in range(MBW):
-            a = row * MBW + mx
-            zero = h[a] == 0 and v[a] == 0
-            if not intra[a] and zero and cbp[a] == 0 and 0 < mx < MBW - 1:
-                pending += 1
-                skipped[a] = True
-                continue
-            if pending:
-                dcp, mvp = [128, 128, 128], [0, 0]
-            bw.code(MBA[pending + 1])
-            pending = 0
-            if intra[a]:
-                t = 0x01
-            elif not zero:
-                t = 0x0A if cbp[a] else 0x08
-            else:
-                t = 0x02 if cbp[a] else 0x08
-            bw.code(MBTYPE_P[t])
-            if intra[a]:
-                mvp = [0, 0]
-            else:
-                dcp = [128, 128, 128]
-                if t & 0x08:
-                    for c, val in enumerate((int(h[a]), int(v[a]))):
-                        d = val - mvp[c]
-                        d = d + 32 if d < -16 else d - 32 if d > 15 else d
-                        bw.code(MV[d])
-                        mvp[c] = val
-                else:
-                    mvp = [0, 0]
-                if t & 0x02:
-                    bw.code(CBP[int(cbp[a])])
-            for b in range(6):
-                if cbp[a] & (0x20 >> b):
-                    comp = 0 if b < 4 else b - 3
-                    dcp[comp] = put_block(bw, L[a, b], bool(intra[a]), comp, dcp[comp])
-        out.append(bytes([0, 0, 1, row + 1]) + tc.pack(bw.v, bw.n))
-    info = dict(h=h, v=v, intra=intra, skipped=skipped, cbp=cbp)
-    return b"".join(out), info
+    return dict(h=h, v=v, intra=intra, Fi=tc.fdct(blocks), Fp=tc.fdct(blocks - predictions(ref, h, v)))
 
 
-def i_picture(i420, qscale, aspect, rate):
-    return tc.encode_picture(i420, qscale, tc.header_bytes(aspect, rate))
+def p_levels(an, q):
+    """[264, 6, 64] zig-zag levels at quantiser q"""
+    return np.where(an["intra"][:, None, None], tc.quantise(an["Fi"], q), inter_levels(an["Fp"], q))
+
+
+def p_codes(an, qs, fallback):
+    """a P picture's slice codes [candidates, 12, slots] at each candidate quantiser of qs; fallback [candidates]: every macroblock not
+    intra, with vector (0, 0) and all levels zero"""
+    fb = np.asarray(fallback, bool)
+    L = np.stack([p_levels(an, q) for q in qs])
+    L[fb] = 0
+    intra, h, v = (np.where(fb[:, None], d, an[k]).reshape(-1, MBH, MBW) for k, d in (("intra", False), ("h", 0), ("v", 0)))
+    return tc.slice_codes(True, tc.ROWS, intra, h, v, L.reshape(-1, MBH, MBW, 6, 64), np.asarray(qs)[:, None])
+
+
+def p_picture(an, tref, qscale):
+    """-> (picture bytes, per-macroblock (h, v, intra, skipped, cbp)); skipped: the slice writes no address increment for it"""
+    codes = p_codes(an, [qscale], [False])
+    skipped = codes[1][0, :, 2::tc.MB_SLOTS].ravel() == 0
+    cbp = np.where(an["intra"], 63, ((p_levels(an, qscale) != 0).any(axis=2) * (0x20 >> np.arange(6))).sum(axis=1))
+    return tc.picture(p_header(tref), codes), dict(h=an["h"], v=an["v"], intra=an["intra"], skipped=skipped, cbp=cbp)
 
 
 def encode_title(pictures, oracle, **params):
@@ -262,12 +185,10 @@ def encode_title(pictures, oracle, **params):
     gop_es = b""
     for k in range(len(pictures)):
         if k % gop == 0:
-            es = i_picture(pictures[k], p["qscale_i"], p["aspect"], p["rate"])
-            info = None
+            es, info = tc.encode_picture(pictures[k], p["qscale_i"], tc.header_bytes(p["aspect"], p["rate"])), None
             gop_es = b""
         else:
-            ref = planes(recon[-1])
-            es, info = p_picture(planes(pictures[k]), ref, k, gop, p["qscale_p"], p["search"])
+            es, info = p_picture(analyse(planes(pictures[k]), planes(recon[-1]), p["search"]), k % gop, p["qscale_p"])
         gop_es += es
         frames = oracle.decode_es(gop_es, max_frames=gop)
         assert len(frames) == k % gop + 1, (k, len(frames))

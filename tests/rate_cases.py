@@ -35,23 +35,10 @@ RATE_DEFAULTS = dict(bit_rate=1500000, vbv_bits=250000, qmin=3, qmax=31)
 # leave less to the P pictures after it.
 I_WEIGHT = 3
 
-MBA_LEN = np.array([len(ec.MBA.get(i, "")) for i in range(34)], np.int64)
-TYPE_LEN = {k: len(v) for k, v in ec.MBTYPE_P.items()}
-MV_LEN = np.array([len(ec.MV[d]) for d in range(-16, 16)] + [len(ec.MV[16])], np.int64)   # [d + 16]
-CBP_LEN = np.array([len(ec.CBP.get(c, "")) for c in range(64)], np.int64)
-DC_LEN = [np.array([len(tc.DC_CODES[c][s]) + s for s in range(9)], np.int64) for c in (0, 1)]
-
-
-def _slice_bytes(bits):
-    return (bits + 7) // 8
-
-
-def _p_min_slice_bits():
-    return 38 + 2 * (MBA_LEN[1] + TYPE_LEN[8] + 2 * MV_LEN[16]) + MBA_LEN[21] - MBA_LEN[1]
-
-
-P_MIN = ec.P_HEADER_BYTES + 12 * int(_slice_bytes(_p_min_slice_bits()))
-D_MAX = tc.HEADER_BYTES + 12 * int(_slice_bytes(38 + 22 * (2 + 4 * (DC_LEN[0][8] + 2) + 2 * (DC_LEN[1][8] + 2))))
+# The fallbacks' sizes from the code tables: P_MIN, every slice (start code and quantiser, 38 bits) two 0x08 macroblocks of vector (0, 0)
+# around a skip run of 20; D_MAX, the worst I fallback: 22 intra macroblocks a slice, every DC difference at the longest size-8 code.
+P_MIN = ec.P_HEADER_BYTES + 12 * ((38 + 2 * (len(tc.MBTYPE[1][8]) + 2 * len(tc.MV[0])) + len(tc.MBA[1]) + len(tc.MBA[21]) + 7) // 8)
+D_MAX = tc.HEADER_BYTES + 12 * ((38 + 22 * (2 + sum(len(tc.DC_CODES[c][8]) + 8 + 2 for c in (0, 0, 0, 0, 1, 1))) + 7) // 8)
 
 
 def header_bytes(aspect, rate, bit_rate, vbv_bits):
@@ -61,172 +48,18 @@ def header_bytes(aspect, rate, bit_rate, vbv_bits):
 
 
 # -- sizes at every q ----------------------------------------------------------------------------------------------------------------
-def ac_bits(L, intra):
-    """[..., 64] zig-zag levels -> [...] bits of their run / level codes (intra: from index 1, the DC counted as coded; non-intra:
-    from index 0, a first coefficient of +-1 as "1s")"""
-    idx = np.arange(64)
-    nz = L != 0
-    if intra:
-        nz[..., 0] = True
-    mark = np.where(nz, idx, -1)
-    prev = np.concatenate([np.full(L.shape[:-1] + (1,), -1), np.maximum.accumulate(mark, axis=-1)[..., :-1]], axis=-1)
-    run = idx - prev - 1
-    a = np.minimum(np.abs(L), 255)
-    alen = tc.AC_LEN[np.clip(run, 0, 63), a]
-    n = np.where((a <= 40) & (alen > 0), alen + 1, np.where(a <= 127, 20, 28))
-    if not intra:
-        n[..., 0] = np.where(a[..., 0] == 1, 2, n[..., 0])
-    else:
-        nz[..., 0] = False
-    return np.where(nz, n, 0).sum(axis=-1)
+def take_census(code, x, qs, head_bytes):
+    """(codes, bytes) of a picture at every candidate q of qs and, last, at its fallback (slices at qs[-1]), from one coder call:
+    code is tc.i_codes (x: the coefficients) or ec.p_codes (x: the analysis)"""
+    qs = list(qs)
+    codes = code(x, qs + qs[-1:], [False] * len(qs) + [True])
+    return codes, tc.picture_bytes(head_bytes, codes)
 
 
 def i_sizes(i420, qs):
     """-> {q: ES bytes of the I picture coded at q}, and its fallback's bytes"""
-    F = tc.fdct(tc.picture_blocks(i420))                           # [12, 22, 6, 8, 8], the same at every q
-    L0 = tc.quantise(F, 1)
-    dc = L0[..., 0]
-    dcb = np.zeros(12, np.int64)
-    comp = [0, 0, 0, 0, 1, 2]
-    for row in range(12):
-        pred = [128, 128, 128]
-        for mb in range(22):
-            for b in range(6):
-                c = comp[b]
-                dcb[row] += DC_LEN[min(c, 1)][abs(int(dc[row, mb, b]) - pred[c]).bit_length()]
-                pred[c] = int(dc[row, mb, b])
-    fixed = 38 + 22 * 2 + dcb + 132 * 2
-    out = {}
-    for q in qs:
-        out[q] = tc.HEADER_BYTES + int(_slice_bytes(fixed + ac_bits(tc.quantise(F, q), True).sum(axis=(1, 2))).sum())
-    return out, tc.HEADER_BYTES + int(_slice_bytes(fixed).sum())
-
-
-def p_analysis(src, ref, search_px):
-    """the q-independent part of a P picture: the search and both transforms"""
-    y, cb, cr = src
-    h, v, best, intra = ec.search(y, ref[0], search_px)
-    h, v = np.where(intra, 0, h), np.where(intra, 0, v)
-    blocks = ec.mb_blocks(y, cb, cr)
-    return dict(h=h, v=v, intra=intra, Fi=tc.fdct(blocks), Fp=tc.fdct(blocks - ec.predictions(ref, h, v)))
-
-
-def p_levels(an, q):
-    return np.where(an["intra"][:, None, None], tc.quantise(an["Fi"], q), ec.inter_levels(an["Fp"], q))
-
-
-def p_sizes(an, qs):
-    """-> {q: ES bytes of the P picture coded at q}: the slice walk of encode_cases.p_picture counting bits, vectorised over q"""
-    qs = list(qs)
-    nq = len(qs)
-    L = np.stack([p_levels(an, q) for q in qs])                     # [nq, 264, 6, 64]
-    intra, h, v = an["intra"], an["h"], an["v"]
-    coded = (L != 0).any(axis=3)                                    # [nq, 264, 6]
-    coded[:, intra] = True
-    cbp = (coded * (0x20 >> np.arange(6))).sum(axis=2)
-    blk = np.where(intra[None, :, None], ac_bits(L, True), ac_bits(L, False)) + 2
-    blk = np.where(coded, blk, 0).sum(axis=2)                       # [nq, 264]: run / level and end-of-block bits
-    dcl = L[:, :, :, 0]
-    total = np.full(nq, ec.P_HEADER_BYTES, np.int64)
-    for row in range(12):
-        bits = np.full(nq, 38, np.int64)
-        pending = np.zeros(nq, np.int64)
-        dcp = np.full((nq, 3), 128, np.int64)
-        mvp = np.zeros((nq, 2), np.int64)
-        for mx in range(22):
-            a = row * 22 + mx
-            zero = h[a] == 0 and v[a] == 0
-            c = cbp[:, a]
-            skip = (not intra[a]) & zero & (c == 0) & (0 < mx < 21)
-            go = ~skip
-            reset = go & (pending > 0)
-            dcp[reset] = 128
-            mvp[reset] = 0
-            bits += np.where(go, MBA_LEN[np.minimum(pending + 1, 33)], 0)
-            pending = np.where(go, 0, pending + 1)
-            if intra[a]:
-                t = np.full(nq, 0x01)
-            elif not zero:
-                t = np.where(c != 0, 0x0A, 0x08)
-            else:
-                t = np.where(c != 0, 0x02, 0x08)
-            bits += np.where(go, [TYPE_LEN[int(x)] for x in t], 0)
-            if intra[a]:
-                mvp[go] = 0
-                for b in range(6):
-                    cp = 0 if b < 4 else b - 3
-                    d = np.abs(dcl[:, a, b] - dcp[:, cp])
-                    nb = DC_LEN[min(cp, 1)][np.array([int(x).bit_length() for x in d])]
-                    bits += np.where(go, nb, 0)
-                    dcp[go, cp] = dcl[go, a, b]
-            else:
-                dcp[go] = 128
-                mv = go & ((t & 0x08) != 0)
-                for cc, val in enumerate((int(h[a]), int(v[a]))):
-                    d = val - mvp[:, cc]
-                    d = np.where(d < -16, d + 32, np.where(d > 15, d - 32, d))
-                    bits += np.where(mv, MV_LEN[d + 16], 0)
-                    mvp[mv, cc] = val
-                mvp[go & ~mv] = 0
-                bits += np.where(go & ((t & 0x02) != 0), CBP_LEN[c], 0)
-            bits += np.where(go, blk[:, a], 0)
-        total += _slice_bytes(bits)
-    return {q: int(total[i]) for i, q in enumerate(qs)}
-
-
-# -- the coder at one q --------------------------------------------------------------------------------------------------------------
-def i_picture(i420, q, hdr, fallback):
-    levels = tc.quantise(tc.fdct(tc.picture_blocks(i420)), q)
-    if fallback:
-        levels[..., 1:] = 0
-    return hdr + b"".join(tc.slice_codes(levels[r], r, q) for r in range(12))
-
-
-def p_picture(an, k, gop, q, fallback):
-    """encode_cases.p_picture from a precomputed analysis; the fallback codes every macroblock as not coded"""
-    if fallback:
-        z = np.zeros(264, np.int64)
-        h, v, intra, L = z, z, np.zeros(264, bool), np.zeros((264, 6, 64), np.int64)
-    else:
-        h, v, intra, L = an["h"], an["v"], an["intra"], p_levels(an, q)
-    cbp = np.where(intra, 63, ((L != 0).any(axis=2) * (0x20 >> np.arange(6))).sum(axis=1))
-    out = [b"\x00\x00\x01\x00" + tc.pack([k % gop, 2, 0xFFFF, 0, 1, 0], [10, 3, 16, 1, 3, 1])]
-    for row in range(12):
-        bw = ec.Bits()
-        bw.put(q << 1, 6)
-        pending, dcp, mvp = 0, [128, 128, 128], [0, 0]
-        for mx in range(22):
-            a = row * 22 + mx
-            zero = h[a] == 0 and v[a] == 0
-            if not intra[a] and zero and cbp[a] == 0 and 0 < mx < 21:
-                pending += 1
-                continue
-            if pending:
-                dcp, mvp = [128, 128, 128], [0, 0]
-            bw.code(ec.MBA[pending + 1])
-            pending = 0
-            t = 0x01 if intra[a] else (0x0A if cbp[a] else 0x08) if not zero else (0x02 if cbp[a] else 0x08)
-            bw.code(ec.MBTYPE_P[t])
-            if intra[a]:
-                mvp = [0, 0]
-            else:
-                dcp = [128, 128, 128]
-                if t & 0x08:
-                    for c, val in enumerate((int(h[a]), int(v[a]))):
-                        d = val - mvp[c]
-                        d = d + 32 if d < -16 else d - 32 if d > 15 else d
-                        bw.code(ec.MV[d])
-                        mvp[c] = val
-                else:
-                    mvp = [0, 0]
-                if t & 0x02:
-                    bw.code(ec.CBP[int(cbp[a])])
-            for b in range(6):
-                if cbp[a] & (0x20 >> b):
-                    comp = 0 if b < 4 else b - 3
-                    dcp[comp] = ec.put_block(bw, L[a, b], bool(intra[a]), comp, dcp[comp])
-        out.append(bytes([0, 0, 1, row + 1]) + tc.pack(bw.v, bw.n))
-    return b"".join(out)
+    size = take_census(tc.i_codes, tc.fdct(tc.picture_blocks(i420)), qs, tc.HEADER_BYTES)[1].tolist()
+    return dict(zip(qs, size)), size[-1]
 
 
 # -- the bucket ----------------------------------------------------------------------------------------------------------------------
@@ -290,12 +123,13 @@ def encode_title(pictures, oracle, **params):
             n = min(gop, N - k)
             E = 0 if k + n == N else BU
             need, f, gop_es = needs(n, r, E), BU, b""
-            sizes, fb = i_sizes(pictures[k], qs)
+            head, code, x = hdr, tc.i_codes, tc.fdct(tc.picture_blocks(pictures[k]))
         else:
-            an = p_analysis(ec.planes(pictures[k]), ec.planes(recon[-1]), p["search"])
-            sizes, fb = p_sizes(an, qs), P_MIN
-        q, s = choose(sizes, fb, f, j, n, r, E, need[j + 1], qmin, qmax)
-        es = i_picture(pictures[k], q or qmax, hdr, not q) if j == 0 else p_picture(an, k, gop, q or qmax, not q)
+            head, code, x = ec.p_header(j), ec.p_codes, ec.analyse(ec.planes(pictures[k]), ec.planes(recon[-1]), p["search"])
+        codes, size = take_census(code, x, qs, len(head))
+        sizes = dict(zip(qs, size.tolist()))
+        q, s = choose(sizes, int(size[-1]), f, j, n, r, E, need[j + 1], qmin, qmax)
+        es = tc.picture(head, [c[q - qmin if q else -1] for c in codes])
         assert len(es) == s, (k, q, len(es), s)
         f = min(BU, f - s * 8 * U + r)
         gop_es += es

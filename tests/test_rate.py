@@ -145,7 +145,7 @@ def test_fallback_sizes_from_the_tables():
     """P_MIN: 12 slices of start code, quantiser, two 0x08 macroblocks and an increment of 21; D_MAX: 22 macroblocks of 106 bits"""
     assert 2 + 4 * (len(tc.DC_CODES[0][8]) + 8 + 2) + 2 * (len(tc.DC_CODES[1][8]) + 8 + 2) == 106
     assert rc.D_MAX == 28 + 12 * ((38 + 22 * 106 + 7) // 8) == 3592
-    assert rc.P_MIN == 9 + 12 * ((38 + 2 * (1 + 3 + 1 + 1) + len(ec.MBA[21]) + 7) // 8)
+    assert rc.P_MIN == 9 + 12 * ((38 + 2 * (1 + 3 + 1 + 1) + len(tc.MBA[21]) + 7) // 8)
     # the I fallback of a picture of 8 x 8 blocks alternating 0 and 255: many DC differences take the size-8 code
     i420 = np.zeros(ec.PICTURE_BYTES, np.uint8)
     i420[:67584] = np.kron((np.add.outer(np.arange(24), np.arange(44)) & 1) * 255, np.ones((8, 8), np.int64)).ravel()

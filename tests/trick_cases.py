@@ -61,15 +61,29 @@ def _u8(name):
     return np.array([int(x) for x in re.findall(r"\d+", s[s.index("{", i):s.index("};", i)])], dtype=np.int64)
 
 
+def _lut(table, n, offset=0):
+    """VLC table -> (codes, lengths) indexed by value + offset, length 0 where the table has no code"""
+    code, length = np.zeros(n, np.int64), np.zeros(n, np.int64)
+    for v, c in table.items():
+        code[v + offset], length[v + offset] = int(c, 2), len(c)
+    return code, length
+
+
 ZIGZAG = _u8("ef_zigzag")                  # zig-zag index -> raster index
 INTRA_Q = _u8("ef_default_intra_q")        # indexed by the raster index, as efsynth and the decoder index it
 _DCT = _vlc("ef_vlc_dct")
+MBA = _vlc("ef_vlc_mba")
+MBTYPE = [_vlc("ef_vlc_mbtype_i"), _vlc("ef_vlc_mbtype_p")]    # [P picture][macroblock type]
+MV = _vlc("ef_vlc_mv")
+CBP = _vlc("ef_vlc_cbp")
 DC_CODES = [_vlc("ef_vlc_dc_luma"), _vlc("ef_vlc_dc_chroma")]
 # run / level table: code and length without the sign bit, length 0 = escape
 AC_CODE = np.zeros((64, 256), dtype=np.int64)
 AC_LEN = np.zeros((64, 256), dtype=np.int64)
 for _v, _c in _DCT.items():
     AC_CODE[_v >> 8, _v & 0xFF], AC_LEN[_v >> 8, _v & 0xFF] = int(_c, 2), len(_c)
+_MBA, _MBTYPE, _MV, _CBP = _lut(MBA, 36), [_lut(t, 32) for t in MBTYPE], _lut(MV, 33, 16), _lut(CBP, 64)
+_DC = np.array([_lut(t, 9) for t in DC_CODES])             # [luma / chroma, code / length, size]
 
 
 # -- selection and timestamps --------------------------------------------------------------------------------------------------
@@ -128,52 +142,70 @@ def pack(vals, lens):
     return np.packbits(np.concatenate([bits, np.zeros((-total) % 8, dtype=np.int64)]).astype(np.uint8)).tobytes()
 
 
-def _dc_code(comp, diff):
-    size = int(abs(diff)).bit_length()
-    c = DC_CODES[comp][size]
-    return (int(c, 2) << size) | (diff if diff > 0 else diff + (1 << size) - 1), len(c) + size
+def _before(x, fill, axis=-1):
+    """x of the element before each one along `axis` (the macroblock before, the coded coefficient before), `fill` before the first"""
+    x = np.moveaxis(np.asarray(x), axis, -1)
+    y = np.concatenate([np.full(x.shape[:-1] + (1,), fill, x.dtype), x[..., :-1]], axis=-1)
+    return np.moveaxis(y, -1, axis)
 
 
-def slice_codes(levels, row, qscale):
-    """levels int64 [22, 6, 64] of macroblock row `row` -> the slice's bytes"""
-    L = levels.reshape(132, 64)
-    keys, vals, lens = [], [], []
-    # macroblock headers: address increment 1 ("1") and intra type ("1") before block 0
-    mb = np.arange(0, 132, 6)
-    keys += [mb * 128, mb * 128 + 1]; vals += [np.ones(22, np.int64)] * 2; lens += [np.ones(22, np.int64)] * 2
-    # DC differences: one predictor per component, 128 at the start of the slice
-    comp = np.tile([0, 0, 0, 0, 1, 2], 22)
-    pred, dvals, dlens = [128, 128, 128], [], []
-    for b in range(132):
-        d = int(L[b, 0]) - pred[comp[b]]
-        pred[comp[b]] = int(L[b, 0])
-        v, n = _dc_code(min(comp[b], 1), d)
-        dvals.append(v); dlens.append(n)
-    keys.append(np.arange(132) * 128 + 2); vals.append(np.array(dvals, np.int64)); lens.append(np.array(dlens, np.int64))
-    # AC: run since the previous coded coefficient (the DC counts as coded)
-    b, i = np.nonzero(L[:, 1:])
-    i = i + 1
-    same = np.concatenate([[False], b[1:] == b[:-1]])
-    prev = np.where(same, np.concatenate([[0], i[:-1]]), 0)
-    run = i - prev - 1
-    lv = L[b, i]
+ROWS = np.arange(12)                       # the slice rows of a picture, for slice_codes' leading row axis
+MB_SLOTS = 5 + 6 * 65                      # a macroblock's code slots: increment, type, two vector codes, pattern, 6 x (64 + end of block)
+
+
+def slice_codes(p, row, intra, h, v, levels, q):
+    """one macroblock row's decisions -> its slice's codes in bitstream order, as (values, lengths) [..., 2 + 22 MB_SLOTS]: the slice
+    start code and quantiser, then MB_SLOTS per macroblock, length 0 where nothing is written (a skipped macroblock writes nothing).
+    p: a P picture (else I); intra, h, v [..., 22]: per macroblock; levels [..., 22, 6, 64] in zig-zag order; q: the quantiser. Leading
+    axes (candidates, rows) broadcast, so every candidate quantiser and every row is one call."""
+    L = np.asarray(levels)
+    mb_shape, lead = L.shape[:-2], L.shape[:-3]
+    intra, h, v = (np.broadcast_to(x, mb_shape) for x in (intra, h, v))
+    mx = np.arange(mb_shape[-1])
+    nz = L != 0
+    cbp = np.where(intra, 63, (nz.any(axis=-1) * (0x20 >> np.arange(6))).sum(axis=-1))
+    zero = (h == 0) & (v == 0)
+    # skipped: not intra, vector (0, 0), no coded block, and neither the first nor the last macroblock of the slice
+    coded = intra | ~zero | (cbp != 0) | (mx == 0) | (mx == mx[-1])
+    inc = mx - _before(np.maximum.accumulate(np.where(coded, mx, -1), axis=-1), -1)
+    follows = (inc == 1) & (mx > 0)                         # the macroblock before is coded: no predictor reset by a skip
+    t = np.where(intra, 0x01, np.where(cbp != 0, 0x02, 0) | np.where(zero & (cbp != 0), 0, 0x08))
+    fwd = coded & ((t & 0x08) != 0)
+    vals, lens = np.zeros((2,) + lead + (2 + mb_shape[-1] * MB_SLOTS,), np.int64)
+    vals[..., 0], vals[..., 1], lens[..., 0], lens[..., 1] = 0x101 + np.asarray(row), np.asarray(q) << 1, 32, 6
+    mb_v, mb_l = (x[..., 2:].reshape(mb_shape + (MB_SLOTS,)) for x in (vals, lens))           # views [..., 22, MB_SLOTS]
+    mb_v[..., 0], mb_l[..., 0] = _MBA[0][inc], np.where(coded, _MBA[1][inc], 0)
+    mb_v[..., 1], mb_l[..., 1] = _MBTYPE[p][0][t], np.where(coded, _MBTYPE[p][1][t], 0)
+    for k, mv in ((2, h), (3, v)):                          # the vector predictor: the macroblock before's vector if it had one
+        d = (mv - np.where(follows & _before(fwd, False), _before(mv, 0), 0) + 16) % 32      # the delta wrapped into -16..15, + 16
+        mb_v[..., k], mb_l[..., k] = _MV[0][d], np.where(fwd, _MV[1][d], 0)
+    mb_v[..., 4], mb_l[..., 4] = _CBP[0][cbp], np.where(coded & ((t & 0x02) != 0), _CBP[1][cbp], 0)
+    blk_v, blk_l = (x[..., 5:].reshape(L.shape[:-1] + (65,)) for x in (mb_v, mb_l))
+    blk_v[..., 64], blk_l[..., 64] = 2, 2 * (coded[..., None] & ((cbp[..., None] & (0x20 >> np.arange(6))) != 0))  # end of block "10"
+    # DC differences of intra blocks: predictors from the macroblock before when it is intra and coded, else 128
+    dc = L[..., 0]
+    carried = np.where((follows & _before(intra, False))[..., None], _before(dc[..., 3:], 128, axis=-2), 128)
+    diff = np.where(intra[..., None], dc - np.concatenate([carried[..., :1], dc[..., :3], carried[..., 1:]], axis=-1), 0)
+    size = np.frexp(np.abs(diff))[1]                        # bit length of |diff|
+    table = np.array([0, 0, 0, 0, 1, 1])                    # luma, chroma
+    dc_v = (_DC[table, 0, size] << size) | np.where(diff > 0, diff, diff + (1 << size) - 1)
+    dc_l = _DC[table, 1, size] + size
+    # every other coded coefficient: run / level code, escape, or a non-intra block's first coefficient of +-1 as "1s"; the run counts
+    # from the coded coefficient before in the block (an intra block's DC counts as coded)
+    first = intra[..., None, None] & (np.arange(64) == 0)
+    mark = nz | first
+    at = np.flatnonzero(mark)
+    blk, i, lv = at // 64, at % 64, L.reshape(-1)[at]
+    run = i - np.where(_before(blk, -1) == blk, _before(i, -1), -1) - 1
     a = np.abs(lv)
-    alen = AC_LEN[run, np.minimum(a, 255)]
-    coded = (a <= 40) & (alen > 0)
-    sign = (lv < 0).astype(np.int64)
-    esc8 = (lv >= -127) & (lv <= 127)
-    esc_level = np.where(esc8, lv & 0xFF, np.where(lv > 0, lv, (128 << 8) | ((lv + 256) & 0xFF)))
-    esc_len = np.where(esc8, 8, 16)
-    v = np.where(coded, (AC_CODE[run, np.minimum(a, 255)] << 1) | sign, (1 << (6 + esc_len)) | (run << esc_len) | esc_level)
-    n = np.where(coded, alen + 1, 12 + esc_len)
-    keys.append(b * 128 + 2 + i); vals.append(v); lens.append(n)
-    # end of block
-    keys.append(np.arange(132) * 128 + 127); vals.append(np.full(132, 2, np.int64)); lens.append(np.full(132, 2, np.int64))
-    keys, vals, lens = np.concatenate(keys), np.concatenate(vals), np.concatenate(lens)
-    o = np.argsort(keys, kind="stable")
-    head = [(qscale << 1), ]
-    body = pack(np.concatenate([head, vals[o]]), np.concatenate([[6], lens[o]]))
-    return bytes([0, 0, 1, row + 1]) + body
+    tab = AC_LEN[run, a]
+    wide = np.where(a > 127, 16, 8)                         # escape: 6-bit run, then an 8- or 16-bit level
+    esc = (1 << (6 + wide)) | (run << wide) | np.where(a > 127, np.where(lv > 0, lv, 0x8000 | (lv + 256)), lv & 0xFF)
+    ones = (i == 0) & (a == 1)
+    blk_v[..., :64][mark] = np.where(ones, 2 | (lv < 0), np.where(tab > 0, (AC_CODE[run, a] << 1) | (lv < 0), esc))
+    blk_l[..., :64][mark] = np.where(ones, 2, np.where(tab > 0, tab + 1, 12 + wide))
+    blk_v[..., 0], blk_l[..., 0] = np.where(intra[..., None], dc_v, blk_v[..., 0]), np.where(intra[..., None], dc_l, blk_l[..., 0])
+    return vals, lens
 
 
 def header_bytes(aspect, rate):
@@ -184,10 +216,27 @@ def header_bytes(aspect, rate):
     return b"\x00\x00\x01\xb3" + seq + b"\x00\x00\x01\xb8" + gop + b"\x00\x00\x01\x00" + pic
 
 
+def picture(header, codes):
+    """a picture's bytes: its header, then every slice's codes (one candidate's, [slices, slots]) packed"""
+    vals, lens = (c.reshape(-1, c.shape[-1]) for c in codes)
+    return header + b"".join(pack(v, n) for v, n in zip(vals, lens))
+
+
+def picture_bytes(head_bytes, codes):
+    """[candidates, slices, slots] codes -> [candidates] picture bytes: the header's, then every slice to a whole byte"""
+    return head_bytes + ((codes[1].sum(axis=-1) + 7) // 8).sum(axis=-1)
+
+
+def i_codes(F, qs, fallback):
+    """an I picture's slice codes [candidates, 12, slots] from its coefficients F [12, 22, 6, 8, 8] at each candidate quantiser of qs;
+    fallback [candidates]: AC levels zeroed"""
+    L = np.stack([quantise(F, q) for q in qs])
+    L[np.asarray(fallback, bool), ..., 1:] = 0
+    return slice_codes(False, ROWS, True, 0, 0, L, np.asarray(qs)[:, None])
+
+
 def encode_picture(i420, qscale, header):
-    F = fdct(picture_blocks(i420))
-    levels = quantise(F, qscale)
-    return header + b"".join(slice_codes(levels[r], r, qscale) for r in range(12))
+    return picture(header, i_codes(fdct(picture_blocks(i420)), [qscale], [False]))
 
 
 def main_codes(es):
