@@ -202,47 +202,26 @@ __global__ void __launch_bounds__(1024)
 ef_audio_size_kernel(const int4* __restrict__ plan, int n_streams, uint64_t pcm_cap, uint64_t* __restrict__ slot_base, uint64_t* __restrict__ pcm_off,
                      ef_audio_info* __restrict__ info, int* __restrict__ verdict)
 {
-    __shared__ uint64_t warp_sum[2][32];
-    __shared__ uint64_t carry[2];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry[0] = carry[1] = 0;
-    __syncthreads();
+    __shared__ EfBlockScan<uint64_t, 1024> slots, samples;
+    slots.init();
+    samples.init();
     for (int base = 0; base < n_streams; base += 1024) {
         const int k = base + threadIdx.x;
         const int4 p = k < n_streams ? plan[k] : make_int4(0, 0, 0, 0);
         const uint32_t frames = (uint32_t)p.z;
         // history rows (+ the probe decode of frame 0) + frames; a rejected probe of a restarted stream (y set, size < 0) its two rows
-        const uint64_t v0 = frames || (p.y && p.x < 0) ? 1 + (uint64_t)p.y + frames : 0, v1 = (uint64_t)frames * 128;
-        uint64_t x0 = v0, x1 = v1;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint64_t y0 = __shfl_up_sync(0xFFFFFFFFu, x0, d), y1 = __shfl_up_sync(0xFFFFFFFFu, x1, d);
-            if (lane >= d) { x0 += y0; x1 += y1; }
-        }
-        if (lane == 31) { warp_sum[0][warp] = x0; warp_sum[1][warp] = x1; }
-        __syncthreads();
-        if (warp < 2) {                                    // warp 0 scans the slot sums, warp 1 the sample sums
-            const uint64_t t = warp_sum[warp][lane];
-            uint64_t z = t;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
-            warp_sum[warp][lane] = z - t;
-        }
-        __syncthreads();
-        const uint64_t e0 = carry[0] + warp_sum[0][warp] + x0 - v0, e1 = carry[1] + warp_sum[1][warp] + x1 - v1;
+        const uint64_t e0 = slots.exclusive(frames || (p.y && p.x < 0) ? 1 + (uint64_t)p.y + frames : 0);
+        const uint64_t e1 = samples.exclusive((uint64_t)frames * 128);
         if (k < n_streams) {
             slot_base[k] = e0;
             pcm_off[k] = e1;
             info[k].frame_size = p.x; info[k].n_frames = frames; info[k].pcm_offset = e1;
         }
-        __syncthreads();
-        if (threadIdx.x == 1023) { carry[0] = e0 + v0; carry[1] = e1 + v1; }
-        __syncthreads();
     }
-    const bool over = carry[1] > pcm_cap;
+    const bool over = samples.carry > pcm_cap;
     if (over)                                              // the same thread wrote these entries above
         for (int i = threadIdx.x; i <= n_streams; i += 1024) { slot_base[i] = 0; pcm_off[i] = 0; }
-    else if (threadIdx.x == 0) { slot_base[n_streams] = carry[0]; pcm_off[n_streams] = carry[1]; }
+    else if (threadIdx.x == 0) { slot_base[n_streams] = slots.carry; pcm_off[n_streams] = samples.carry; }
     if (threadIdx.x == 0) *verdict = over;
 }
 

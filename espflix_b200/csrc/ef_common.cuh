@@ -351,3 +351,57 @@ static inline __host__ __device__ int ef_strips_to_tiled(int b)
     const int r = row & 15;
     return ef_chroma_offset(r >> 3, x - EF_W, (row >> 4) * 8 + (r & 7));
 }
+
+#ifdef __CUDACC__    // device code only: ef_tables.cpp reads this header through the host compiler
+// Integer prefix sums over one CTA of a 1-D launch (lane = threadIdx.x & 31).
+// Lane i of a full warp gets x_0 + ... + x_i; all 32 lanes must call it.
+template <typename T>
+__device__ __forceinline__ T ef_warp_inclusive_scan(T x)
+{
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const T y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
+    return x;
+}
+
+// The exclusive scan of a sequence longer than a CTA of kThreads threads, one tile of kThreads values at a time: thread t holds
+// value base + t, and base steps by kThreads. Declare it __shared__. init() zeroes the carry (the sum of the tiles before);
+// exclusive(v) returns the carry plus the v of the threads below the caller in this tile, then adds the tile's sum to the carry.
+// Both end on a barrier, so `carry` may be read after either. Every thread of the CTA must call both, the same number of times:
+// a thread past the end of the sequence passes 0. Four barriers per tile: warp totals written, warp totals scanned, the carry
+// and the offsets read, the carry advanced.
+template <typename T, int kThreads>
+struct EfBlockScan {
+    static_assert(kThreads % 32 == 0 && kThreads <= 1024, "whole warps, one CTA");
+    T warp_sum[kThreads / 32];
+    T carry;
+
+    __device__ __forceinline__ void init()
+    {
+        if (threadIdx.x == 0) carry = 0;
+        __syncthreads();
+    }
+
+    __device__ __forceinline__ T exclusive(T v)
+    {
+        constexpr int kWarps = kThreads / 32;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        const T x = ef_warp_inclusive_scan(v);
+        if (lane == 31) warp_sum[warp] = x;
+        __syncthreads();
+        // warp 0: the exclusive offsets of the warps. The vote makes the branch warp-uniform to the compiler; on `warp == 0` it
+        // keeps a divergent fallback path for the shuffles, which costs registers (and spills in ef_audio_size_kernel).
+        if (__all_sync(0xFFFFFFFFu, warp == 0)) {
+            const T t = lane < kWarps ? warp_sum[lane] : T(0);
+            const T z = ef_warp_inclusive_scan(t);
+            if (lane < kWarps) warp_sum[lane] = z - t;
+        }
+        __syncthreads();
+        const T excl = carry + warp_sum[warp] + x - v;
+        __syncthreads();
+        if (threadIdx.x == kThreads - 1) carry = excl + v;
+        __syncthreads();
+        return excl;
+    }
+};
+#endif

@@ -520,35 +520,16 @@ __global__ void __launch_bounds__(1024)
 ef_pace_size_kernel(const EfPaceOut* __restrict__ out, int n_streams, uint64_t cap, uint64_t* __restrict__ first, EfPaceOut* __restrict__ info,
                     uint64_t* __restrict__ total, int* __restrict__ chain, uint32_t* __restrict__ rec)
 {
-    __shared__ uint64_t warp_sum[32];
-    __shared__ uint64_t carry;
+    __shared__ EfBlockScan<uint64_t, 1024> scan;
     __shared__ int skip;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) { carry = 0; skip = *chain; }
-    __syncthreads();
+    if (threadIdx.x == 0) skip = *chain;
+    scan.init();
     for (int base = 0; base < n_streams; base += 1024) {
         const int k = base + threadIdx.x;
-        const uint64_t v = k < n_streams ? out[k].n_fields : 0;
-        uint64_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            const uint64_t t = warp_sum[lane];
-            uint64_t z = t;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
-            warp_sum[lane] = z - t;
-        }
-        __syncthreads();
-        const uint64_t e = carry + warp_sum[warp] + x - v;
+        const uint64_t e = scan.exclusive(k < n_streams ? out[k].n_fields : 0);
         if (k < n_streams) first[k] = e;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = e + v;
-        __syncthreads();
     }
-    const bool fits = !skip && carry <= cap;
+    const bool fits = !skip && scan.carry <= cap;
     for (int k = threadIdx.x; k < n_streams; k += 1024) {   // the same thread wrote first[k] above
         EfPaceOut o = out[k];
         o.first = skip ? 0 : first[k];
@@ -562,7 +543,7 @@ ef_pace_size_kernel(const EfPaceOut* __restrict__ out, int n_streams, uint64_t c
         for (size_t i = threadIdx.x; i < n; i += 1024) r[i] = make_uint4(0, 0, 0, 0);
     }
     if (threadIdx.x == 0) {
-        *total = fits ? carry : 0;
+        *total = fits ? scan.carry : 0;
         if (fits) chain[1] += 1; else chain[0] = 1;
     }
 }

@@ -284,12 +284,7 @@ struct SliceOut {
             pred[comp] = __shfl_sync(0xFFFFFFFFu, a0, 0);
         }
         const uint32_t sum = n0 + n1;
-        uint32_t incl = sum;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-            if (lane >= d) incl += t;
-        }
+        const uint32_t incl = ef_warp_inclusive_scan(sum);
         const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
         const uint32_t q = P - wbase * 32 + incl - sum;
         put_bits(win, q, c0, n0);

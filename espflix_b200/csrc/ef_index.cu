@@ -266,40 +266,22 @@ __global__ void __launch_bounds__(1024)
 ef_prefix_kernel(EfDev* __restrict__ Dp)
 {
     EfDev& D = *Dp;
-    __shared__ uint32_t warp_sum[32];
-    __shared__ uint32_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __shared__ EfBlockScan<uint32_t, 1024> scan;
     const int p = blockIdx.x;
     const int pmax = min((int)D.info[0], D.max_pictures);
     if (p >= pmax) {
         if (threadIdx.x == 0) { D.pic_total[p] = 0; D.cursor[p] = 0; }
         return;
     }
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
+    scan.init();
     for (int base = 0; base < D.n_streams; base += 1024) {
         const int s = base + threadIdx.x;
         uint32_t v = 0;
         if (s < D.n_streams && (uint32_t)p < D.n_pics[s]) v = D.pics[(size_t)s * D.max_pictures + p].n_slices;
-        uint32_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t t = warp_sum[lane], z = t;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
-            warp_sum[lane] = z - t;                   // exclusive offsets of the warps
-        }
-        __syncthreads();
-        const uint32_t excl = carry + warp_sum[warp] + x - v;
+        const uint32_t excl = scan.exclusive(v);
         if (s < D.n_streams) D.pic_pref[(size_t)p * D.n_streams + s] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
     }
-    if (threadIdx.x == 0) { D.pic_total[p] = carry; D.cursor[p] = 0; }
+    if (threadIdx.x == 0) { D.pic_total[p] = scan.carry; D.cursor[p] = 0; }
 }
 
 __global__ void __launch_bounds__(256)
@@ -378,63 +360,32 @@ __global__ void __launch_bounds__(256)
 ef_ts_scan_kernel(const uint32_t* __restrict__ len, const uint64_t* __restrict__ ts_off, uint32_t* __restrict__ local_off, uint16_t* __restrict__ pkt_stream,
                   uint64_t* __restrict__ stream_total)
 {
-    __shared__ uint32_t warp_sum[8];
-    __shared__ uint32_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, s = blockIdx.x;
+    __shared__ EfBlockScan<uint32_t, 256> scan;
+    const int s = blockIdx.x;
     const uint64_t p0 = ts_off[s] / 188, p1 = ts_off[s + 1] / 188;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
+    scan.init();
     for (uint64_t base = p0; base < p1; base += 256) {
         const uint64_t k = base + threadIdx.x;
-        const uint32_t v = k < p1 ? len[k] : 0;
-        uint32_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[warp] = x;
-        __syncthreads();
-        uint32_t before = carry;
-        for (int w = 0; w < warp; w++) before += warp_sum[w];
-        if (k < p1) { local_off[k] = before + x - v; pkt_stream[k] = (uint16_t)s; }
-        __syncthreads();
-        if (threadIdx.x == 255) carry = before + x;
-        __syncthreads();
+        const uint32_t excl = scan.exclusive(k < p1 ? len[k] : 0);
+        if (k < p1) { local_off[k] = excl; pkt_stream[k] = (uint16_t)s; }
     }
-    if (threadIdx.x == 0) stream_total[s] = carry;
+    if (threadIdx.x == 0) stream_total[s] = scan.carry;
 }
 
 // ES offset of every stream = exclusive scan of the stream totals (n_streams <= 65,535: one CTA), zero padding behind the ES
 __global__ void __launch_bounds__(1024)
 ef_ts_offsets_kernel(const uint64_t* __restrict__ stream_total, int n_streams, uint64_t* __restrict__ es_off, uint8_t* __restrict__ es)
 {
-    __shared__ uint64_t warp_sum[32];
-    __shared__ uint64_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
+    __shared__ EfBlockScan<uint64_t, 1024> scan;
+    scan.init();
     for (int base = 0; base < n_streams; base += 1024) {
         const int k = base + threadIdx.x;
-        const uint64_t v = k < n_streams ? stream_total[k] : 0;
-        uint64_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint64_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint64_t t = warp_sum[lane], z = t;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
-            warp_sum[lane] = z - t;
-        }
-        __syncthreads();
-        const uint64_t excl = carry + warp_sum[warp] + x - v;
+        const uint64_t excl = scan.exclusive(k < n_streams ? stream_total[k] : 0);
         if (k < n_streams) es_off[k] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
     }
-    if (threadIdx.x == 0) es_off[n_streams] = carry;
+    if (threadIdx.x == 0) es_off[n_streams] = scan.carry;
     // K1's bit reader runs a few bytes past the last slice: zero the 256 bytes behind the elementary stream
-    if (threadIdx.x < 256) es[carry + threadIdx.x] = 0;
+    if (threadIdx.x < 256) es[scan.carry + threadIdx.x] = 0;
 }
 
 // ---- TS submits cut anywhere (ef_carry_enable) ------------------------------------------------------------------------
@@ -534,30 +485,20 @@ __global__ void __launch_bounds__(256)
 ef_pts_packet_kernel(const uint8_t* __restrict__ ts, const uint64_t* __restrict__ ts_off, const uint32_t* __restrict__ local_off,
                      uint32_t* __restrict__ list_off, int64_t* __restrict__ list_pts, uint2* __restrict__ span)
 {
-    __shared__ uint32_t warp_cnt[8];
-    __shared__ uint32_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, s = blockIdx.x;
+    __shared__ EfBlockScan<uint32_t, 256> scan;
+    const int s = blockIdx.x;
     const uint64_t p0 = ts_off[s] / 188, p1 = ts_off[s + 1] / 188;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
+    scan.init();
     for (uint64_t base = p0; base < p1; base += 256) {
         const uint64_t k = base + threadIdx.x;
         const int64_t pts = k < p1 ? ts_video_pes_pts(ts + k * 188) : -1;
-        const unsigned m = __ballot_sync(0xFFFFFFFFu, pts >= 0);
-        if (lane == 0) warp_cnt[warp] = __popc(m);
-        __syncthreads();
-        uint32_t before = carry;
-        for (int w = 0; w < warp; w++) before += warp_cnt[w];
+        const uint64_t j = p0 + scan.exclusive(pts >= 0);
         if (pts >= 0) {
-            const uint64_t j = p0 + before + __popc(m & ((1u << lane) - 1u));
             list_off[j] = local_off[k];
             list_pts[j] = pts;
         }
-        __syncthreads();
-        if (threadIdx.x == 255) carry = before + __popc(m);
-        __syncthreads();
     }
-    if (threadIdx.x == 0) span[s] = make_uint2((uint32_t)p0, carry);
+    if (threadIdx.x == 0) span[s] = make_uint2((uint32_t)p0, scan.carry);
 }
 
 // Resolve pass after ef_fill_kernel, one warp per stream, lanes over pictures: upper-bound search for code byte + 2 in the

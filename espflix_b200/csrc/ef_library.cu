@@ -80,18 +80,15 @@ __global__ void ef_library_resolve_kernel(EfLibStream* __restrict__ ls, const Ef
 }
 
 // One CTA: every PLAYING stream takes min(its budget, packets left in its file) packets from its cursor; the exclusive prefix of the
-// run lengths gives each stream's place in the submit (off[n_streams + 1], the ef_ts_offsets_kernel pattern). A stream whose cursor
+// run lengths gives each stream's place in the submit (off[n_streams + 1], EfBlockScan). A stream whose cursor
 // reaches the end of its file ends with this submit: end[s] = 1, state ENDED, pos = pts2pts(0, _speed) (save_pos(0) at DONE,
 // espflix.cpp:906-911). src[s] = where the stream's run starts.
 __global__ void __launch_bounds__(1024)
 ef_library_count_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restrict__ titles, const uint32_t* __restrict__ budget, uint32_t packets,
                         int n_streams, const uint8_t** __restrict__ src, uint64_t* __restrict__ off, uint8_t* __restrict__ end)
 {
-    __shared__ uint64_t warp_sum[32];
-    __shared__ uint64_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
+    __shared__ EfBlockScan<uint64_t, 1024> scan;
+    scan.init();
     for (int base = 0; base < n_streams; base += 1024) {
         const int k = base + threadIdx.x;
         uint64_t v = 0;
@@ -116,25 +113,10 @@ ef_library_count_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restri
             }
             end[k] = e;
         }
-        uint64_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint64_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            uint64_t t = warp_sum[lane], z = t;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint64_t y = __shfl_up_sync(0xFFFFFFFFu, z, d); if (lane >= d) z += y; }
-            warp_sum[lane] = z - t;
-        }
-        __syncthreads();
-        const uint64_t excl = carry + warp_sum[warp] + x - v;
+        const uint64_t excl = scan.exclusive(v);
         if (k < n_streams) off[k] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + v;
-        __syncthreads();
     }
-    if (threadIdx.x == 0) off[n_streams] = carry;
+    if (threadIdx.x == 0) off[n_streams] = scan.carry;
 }
 
 // The gather: the submit is one flat range of 16-byte units, EF_LIB_UNITS of them per thread, a CTA's units contiguous. Every stream's

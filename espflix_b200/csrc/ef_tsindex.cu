@@ -5,7 +5,7 @@
 //   ef_tsidx_packet_kernel   one thread per 188-byte packet: PID, payload-unit-start, PES header -> pts and
 //                            "payload starts with a sequence header" (parse()/parse_pts(), indexer.cpp:43-75)
 //   ef_tsidx_compact_kernel  one CTA per file: ordered compaction of the sequence-header packets into the
-//                            (pts, packet number) table, first / last pts (block-wide ballot + prefix counts)
+//                            (pts, packet number) table, first / last pts (block-wide exclusive scan of the flags)
 //   ef_tsidx_sample_kernel   one thread per 1/12 s bin: nearest table entry in pts with the reference's exact
 //                            tie-breaking and its int-cast distance (pts2pos(), indexer.cpp:193-207)
 // All integer; the table and the samples are bit-identical to the reference's vectors.
@@ -59,36 +59,27 @@ ef_tsidx_compact_kernel(const uint64_t* __restrict__ pkt_off /* [n_files + 1], i
                         const uint8_t* __restrict__ pkt_kind, int64_t* __restrict__ seq_pts, uint32_t* __restrict__ seq_pos,
                         int64_t* __restrict__ info)
 {
-    __shared__ uint32_t warp_cnt[8];
-    __shared__ uint32_t base_s;
+    __shared__ EfBlockScan<uint32_t, 256> scan;
     __shared__ unsigned long long last_video;                             // 1 + packet index of the last video PES start
-    const int f = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int f = blockIdx.x;
     const uint64_t p0 = pkt_off[f], p1 = pkt_off[f + 1];
-    if (threadIdx.x == 0) { base_s = 0; last_video = 0; }
-    __syncthreads();
+    if (threadIdx.x == 0) last_video = 0;
+    scan.init();
     unsigned long long my_last = 0;
     for (uint64_t c = p0; c < p1; c += 256) {
         const uint64_t k = c + threadIdx.x;
         const uint32_t kind = k < p1 ? pkt_kind[k] : 0u;
         if (kind) my_last = k - p0 + 1;
-        const unsigned m = __ballot_sync(0xFFFFFFFFu, kind == 2);
-        if (lane == 0) warp_cnt[warp] = __popc(m);
-        __syncthreads();
-        uint32_t before = base_s;
-        for (int w = 0; w < warp; w++) before += warp_cnt[w];
+        const uint32_t j = scan.exclusive(kind == 2);
         if (kind == 2) {
-            const uint32_t j = before + __popc(m & ((1u << lane) - 1));
             seq_pts[p0 + j] = pkt_pts[k];                                 // the table of a file lives at its packet offset (n_seq <= n_packets)
             seq_pos[p0 + j] = (uint32_t)(k - p0);
         }
-        __syncthreads();
-        if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < 8; w++) t += warp_cnt[w]; base_s += t; }
-        __syncthreads();
     }
     atomicMax(&last_video, my_last);
     __syncthreads();
     if (threadIdx.x == 0) {
-        const uint32_t n = base_s;
+        const uint32_t n = scan.carry;
         int64_t origin = -1;                                              // "if (origin == -1) origin = pts" (indexer.cpp:136): the first
         for (uint32_t j = 0; j < n && origin == -1; j++) origin = seq_pts[p0 + j];   // entry whose pts is not -1 (a malformed PTS reads as -1)
         info[f * 3 + 0] = origin;
