@@ -3273,9 +3273,10 @@ extern "C" int ef_mux_audio(int device, const uint8_t* ts, const uint64_t* ts_of
             const uint8_t* d = d0 + k * 188;
             const int pid = ((d[1] << 8) | d[2]) & 0x1FFF;
             if (pid == 0x101 || pid == 0x102) return fail(EF_EINVAL, "title %d packet %llu is on audio PID 0x%x", t, (unsigned long long)k, pid);
-            if (pid != 0x100 || !(d[1] & 0x40)) continue;
+            if (pid != 0x100 || !(d[1] & 0x40) || !(d[3] & 0x10)) continue;     // more() demuxes only packets with a payload
             const int o = (d[3] & 0x20) ? 5 + d[4] : 4;
-            if (!(d[3] & 0x10) || o + 14 > 188 || d[o] || d[o + 1] || d[o + 2] != 1 || !(d[o + 7] & 0x80))
+            // the PTS must parse as parse_pts() reads it (player.cpp:299): a malformed prefix nibble is no PTS to the decoder
+            if (o + 14 > 188 || d[o] || d[o + 1] || d[o + 2] != 1 || !(d[o + 7] & 0x80) || (d[o + 9] & 0xF0) != ((d[o + 7] >> 2) & 0x30))
                 return fail(EF_EINVAL, "title %d packet %llu: a video PES start without a PTS", t, (unsigned long long)k);
             const uint8_t* q = d + o + 9;
             starts.push_back({ k, (int64_t)((q[0] >> 1) & 7) << 30 | (int64_t)q[1] << 22 | (int64_t)(q[2] >> 1) << 15 | (int64_t)q[3] << 7 | (q[4] >> 1) });

@@ -193,10 +193,10 @@ def video_starts(ts):
         pid = ((d[1] << 8) | d[2]) & 0x1FFF
         if pid in (0x101, 0x102):
             raise ValueError("packet %d is on audio PID 0x%x" % (k, pid))
-        if pid != 0x100 or not d[1] & 0x40:
+        if pid != 0x100 or not d[1] & 0x40 or not d[3] & 0x10:          # more() demuxes only packets with a payload
             continue
         o = 5 + d[4] if d[3] & 0x20 else 4
-        if not d[3] & 0x10 or o + 14 > 188 or d[o:o + 3] != b"\x00\x00\x01" or not d[o + 7] & 0x80:
+        if o + 14 > 188 or d[o:o + 3] != b"\x00\x00\x01" or not d[o + 7] & 0x80 or (d[o + 9] & 0xF0) != ((d[o + 7] >> 2) & 0x30):
             raise ValueError("video PES start at packet %d without a PTS" % k)
         p = d[o + 9:o + 14]
         out.append((k, ((p[0] >> 1) & 7) << 30 | p[1] << 22 | (p[2] >> 1) << 15 | p[3] << 7 | p[4] >> 1))

@@ -224,7 +224,7 @@ def _check_mux(video, sbc, oracle, **params):
             if vids_seen:
                 assert starts[vids_seen - 1][1] < a
             k += 1
-        elif q == 0x100 and d[1] & 0x40:
+        elif q == 0x100 and d[1] & 0x40 and d[3] & 0x10:               # a video PES start as se.video_starts() counts them
             vids_seen += 1
     assert k == len(se.audio_pes(sbc, **p))
     return out
