@@ -105,6 +105,9 @@ _SIGNATURES = {
     "ef_trick_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 4),
     "ef_library_add_trick": (_I, [_VP, _I, _I]),
     "ef_library_read": (_I, [_VP, _I, _I, _VP, ctypes.c_uint64, _U64P]),
+    "ef_library_add_poster": (_I, [_VP, _I, _VP, ctypes.c_uint64]),
+    "ef_library_nv_read": (_I, [_VP, _I, _I, _I, _VP]),
+    "ef_library_nv_write": (_I, [_VP, _I, _I, _I, _VP]),
     "ef_encode_build": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 5),
     "ef_encode_build_rate": (_I, [_I, _VP, _VP, _I, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP, _VP]),
@@ -114,8 +117,9 @@ _SIGNATURES = {
 }
 
 # ef_library_command's commands and ef_library_info's stream states (include/espflix_b200.h)
-LIB_PLAY_AT, LIB_PLAY, LIB_SKIP, LIB_FAST_FORWARD, LIB_REWIND, LIB_PAUSE, LIB_RESUME, LIB_STOP = range(8)
-LIB_IDLE, LIB_PLAYING, LIB_PAUSED, LIB_STOPPED, LIB_ENDED = range(5)
+LIB_PLAY_AT, LIB_PLAY, LIB_SKIP, LIB_FAST_FORWARD, LIB_REWIND, LIB_PAUSE, LIB_RESUME, LIB_STOP, LIB_NAV, LIB_NAV_STEP, LIB_MENU = range(11)
+LIB_IDLE, LIB_PLAYING, LIB_PAUSED, LIB_STOPPED, LIB_ENDED, LIB_POSTER = range(6)
+LIB_POSTER_FILE = 3              # ef_library_status.file of a stream on its poster, ef_library_read's part for poster.ts
 LIBRARY_STATUS = np.dtype([("title", "<i4"), ("speed", "<i4"), ("state", "<i4"), ("file", "<i4"), ("cursor", "<u8"), ("pos", "<i8")])
 
 
@@ -553,7 +557,8 @@ class Context:
         self._check(self.lib.ef_library_add_trick(self._h, int(title), TRICK_QSCALE if qscale is None else int(qscale)))
 
     def library_read(self, title, what):
-        """ef_library_read: a title's video.idx image (what -1) or its rwd / main / fwd file (0 / 1 / 2) as bytes (b"" when absent)"""
+        """ef_library_read: a title's video.idx image (what -1), its rwd / main / fwd file (0 / 1 / 2) or its poster.ts (3) as bytes
+        (b"" when absent)"""
         n = ctypes.c_uint64()
         rc = self.lib.ef_library_read(self._h, int(title), int(what), None, 0, ctypes.byref(n))
         if rc != EF_ENOMEM:
@@ -563,9 +568,26 @@ class Context:
         self._check(self.lib.ef_library_read(self._h, int(title), int(what), out.ctypes.data, out.size, ctypes.byref(n)))
         return out.tobytes()
 
+    def library_add_poster(self, title, poster):
+        """ef_library_add_poster: attach a title's poster.ts (capi.encode_poster makes one) as its file 3"""
+        a = np.frombuffer(bytes(poster), dtype=np.uint8)
+        self._check(self.lib.ef_library_add_poster(self._h, int(title), a.ctypes.data if a.size else None, a.size))
+
+    def library_nv_read(self, title, first=0, count=None):
+        """ef_library_nv_read -> int64 saved positions of streams [first, first + count) on `title` (0: none saved)"""
+        count = self.n_streams - first if count is None else count
+        out = np.zeros(max(count, 1), dtype=np.int64)
+        self._check(self.lib.ef_library_nv_read(self._h, int(title), first, count, out.ctypes.data))
+        return out[:count]
+
+    def library_nv_write(self, title, pos, first=0):
+        """ef_library_nv_write: saved positions of streams [first, first + len(pos)) on `title`, e.g. kept by a service across sessions"""
+        a = np.ascontiguousarray(pos, dtype=np.int64).reshape(-1)
+        self._check(self.lib.ef_library_nv_write(self._h, int(title), first, a.size, a.ctypes.data if a.size else None))
+
     def library_command(self, cmd, first=0, count=1, title=0, arg=0):
-        """ef_library_command: cmd (LIB_PLAY_AT ... LIB_STOP) on streams [first, first + count); title and arg (main pts for
-        PLAY_AT, seconds for SKIP) as the header describes"""
+        """ef_library_command: cmd (LIB_PLAY_AT ... LIB_MENU) on streams [first, first + count); title (PLAY_AT, NAV) and arg (main
+        pts for PLAY_AT, seconds for SKIP, the step of NAV_STEP) as the header describes"""
         self._check(self.lib.ef_library_command(self._h, first, count, int(cmd), int(title), int(arg)))
 
     def library_submit(self, packets=0, per_stream=None, stream=0):
@@ -701,6 +723,19 @@ def encode_build(titles, device=0, **params):
         cap = int(to[-1])
     _check_rc(lib, rc)
     return [ts[int(to[i]):int(to[i + 1])].tobytes() for i in range(n)]
+
+
+# make_video()'s poster: ffmpeg ... -bf 0 -q 2 poster.ts (indexer.cpp:306), one I picture at quantiser scale 2
+POSTER_PARAMS = dict(gop=1, qscale_i=2)
+
+
+def encode_poster(picture_i420, device=0):
+    """poster.ts of one 352 x 192 I420 picture (101,376 bytes): ef_encode_build of that picture with gop 1 and qscale_i 2, the
+    other parameters ENCODE_DEFAULTS -> bytes"""
+    pic = np.asarray(picture_i420, dtype=np.uint8).reshape(-1)
+    if pic.size != PICTURE_BYTES:
+        raise EspflixError(EF_EINVAL, "a poster is one picture of %d bytes, not %d" % (PICTURE_BYTES, pic.size))
+    return encode_build([pic.reshape(1, PICTURE_BYTES)], device=device, **POSTER_PARAMS)[0]
 
 
 class RateParams(ctypes.Structure):

@@ -86,8 +86,8 @@ cudaError_t ef_launch_blit(const EfDev* dev, int stream_index, int fb, int line,
 cudaError_t ef_launch_composite_paced(const EfDev* dev, const EfGeometry& g, const EfFieldDesc* desc, uint64_t n_fields, uint8_t* dst, bool dac8,
                                       cudaStream_t stream, uint64_t* launches, const EfFieldOverlay* fovl, const uint8_t* bitmaps, const uint64_t* total);
 __global__ void ef_pace_kernel(const EfPaceState* st, EfPaceState* next, EfPaceRun* run, EfPaceOut* out, const int64_t* pic_pts, const uint32_t* n_pics,
-                               const uint32_t* base_pics, const uint8_t* modes, const uint32_t* idle_n, int pic, int max_pictures, int n_streams, int ntsc,
-                               const EfOverlayState* ovl, EfOverlayState* ovl_next);
+                               const uint32_t* base_pics, const uint8_t* modes, const uint8_t* lib_modes, const uint32_t* idle_n, int pic, int max_pictures,
+                               int n_streams, int ntsc, const EfOverlayState* ovl, EfOverlayState* ovl_next);
 cudaError_t ef_launch_pace_fill(EfPaceState* st, const EfPaceState* next, const EfPaceRun* run, const uint64_t* first, EfFieldDesc* desc, EfOverlayState* ovl,
                                 const EfOverlayState* ovl_next, EfFieldOverlay* fovl, int n_streams, const int* chain, cudaStream_t stream);
 __global__ void ef_pace_size_kernel(const EfPaceOut* out, int n_streams, uint64_t cap, uint64_t* first, EfPaceOut* info, uint64_t* total, int* chain,
@@ -98,10 +98,10 @@ __global__ void ef_clock_kernel(EfClockState* clk, const EfOverlayState* ovl, Ef
 cudaError_t ef_launch_clock_commit(EfClockState* clk, const EfOverlayState* ovl_clk, const uint8_t* bm, uint8_t* slots, int n_streams, const int* chain,
                                    cudaStream_t stream);
 cudaError_t ef_launch_library_resolve(EfLibStream* ls, const EfLibTitle* titles, const int64_t* pts_last, int first, int count, int cmd, int title,
-                                      int64_t arg);
+                                      int64_t arg, uint8_t* mode, int64_t* nv, int n_streams, int n_titles, EfOverlayState* ovl);
 cudaError_t ef_launch_library_gather(EfLibStream* ls, const EfLibTitle* titles, const uint32_t* budget, uint32_t packets, int n_streams,
-                                     const uint8_t** src, uint64_t* off, uint8_t* end, uint8_t* dst, uint64_t max_bytes, cudaStream_t st,
-                                     uint64_t* launches);
+                                     const uint8_t** src, uint64_t* off, uint8_t* end, const uint8_t* mode, uint8_t* smode, uint8_t* dst,
+                                     uint64_t max_bytes, cudaStream_t st, uint64_t* launches);
 static_assert(sizeof(idx_hdr) == 104, "video.idx header: the reference's idx_hdr");
 static_assert(sizeof(EfLibStream) == sizeof(ef_library_status), "EfLibStream mirrors ef_library_status");
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
@@ -404,6 +404,11 @@ struct ef_ctx {
     uint32_t* d_lib_budget = nullptr;             // [n_streams] per-stream packet budgets of a submit
     cudaEvent_t ev_lib_staged = nullptr;          // the upload has copied the staging buffer
     bool lib_submit = false;                      // the pending submit is a library submit (its ends are the library's)
+    int64_t* d_lib_nv = nullptr;                  // [lib_cap][n_streams] the saved positions (NVS), 0 until written
+    // the poster menu, allocated by the first ef_library_add_poster; until then submits and present calls run as before
+    uint8_t* d_lib_mode = nullptr;                // [n_streams] the scroll mode of every stream's latest nav
+    uint8_t* d_lib_smode = nullptr;               // [n_streams] the modes a library submit carries (its posters that end in it)
+    uint8_t* d_lib_mode2[2] = { nullptr, nullptr };   // per ES buffer: the modes its submit carries, 0 for a submit of the host
 };
 
 namespace {
@@ -854,6 +859,7 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
             CK(cudaMemsetAsync(c->d_end2[b], 0, (size_t)n, up));
             c->h_end2[b].assign((size_t)n, 0);
         }
+        if (c->d_lib_mode) CK(cudaMemsetAsync(c->d_lib_mode2[b], 0, (size_t)n, up));   // a library submit copies its own over it
     }
     if (c->pts) {                                         // the video PES starts of this submit, into its ES buffer's list
         if (ts) {
@@ -1865,8 +1871,9 @@ static int present_schedule(ef_ctx* c, int pic, const uint8_t* modes, const uint
         c->launches++;
     }
     ef_pace_kernel<<<(n + 127) / 128, 128, 0, st>>>(c->d_pace, c->d_pace_next, c->d_pace_run, c->d_pace_out, c->d_pic_pts, c->h.n_pics, c->h.base_pics,
-                                                   pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, (const uint32_t*)c->d_pace_arg, pic,
-                                                   c->cfg.max_pictures, n, c->pace_ntsc, c->d_clk ? c->d_ovl_clk : c->d_ovl, c->d_ovl_next);
+                                                   pic >= 0 && modes ? (const uint8_t*)c->d_pace_arg : nullptr, c->d_lib_mode2[c->active],
+                                                   (const uint32_t*)c->d_pace_arg, pic, c->cfg.max_pictures, n, c->pace_ntsc,
+                                                   c->d_clk ? c->d_ovl_clk : c->d_ovl, c->d_ovl_next);
     CK(cudaGetLastError());
     c->launches++;
     return EF_OK;
@@ -2189,6 +2196,8 @@ int ef_library_add(ef_ctx* c, const uint8_t* idx, uint64_t idx_bytes, const uint
         const size_t cap = c->lib_cap ? 2 * c->lib_cap : 16;
         CK(cudaDeviceSynchronize());                      // a command or a submit may still read the title table
         TRY(dev_grow(c, &c->d_lib_titles, c->lib_cap, cap, c->lib_cap > 0));
+        TRY(dev_grow(c, &c->d_lib_nv, c->lib_cap * n, cap * n, c->lib_cap > 0));   // title-major: the new titles' rows follow
+        if (!c->lib_cap) CK(cudaMemset(c->d_lib_nv, 0, cap * n * sizeof(int64_t)));
         c->lib_cap = cap;
     }
     EfLibTitle t;
@@ -2228,30 +2237,48 @@ int ef_library_command(ef_ctx* c, int first, int count, int cmd, int title, int6
     if (!c) return fail(EF_EINVAL, "null context");
     TRY(library_ready(c, "ef_library_command"));
     TRY(stream_range(c, first, count));
-    if (cmd < EF_LIB_PLAY_AT || cmd > EF_LIB_STOP) return fail(EF_EINVAL, "unknown command %d", cmd);
-    if (cmd == EF_LIB_PLAY_AT && (title < 0 || (size_t)title >= c->lib_titles.size())) return fail(EF_EINVAL, "unknown title %d", title);
-    if (cmd == EF_LIB_SKIP && (arg < INT32_MIN || arg > INT32_MAX)) return fail(EF_EINVAL, "skip of %lld seconds is not an int", (long long)arg);
+    if (cmd < EF_LIB_PLAY_AT || cmd > EF_LIB_MENU) return fail(EF_EINVAL, "unknown command %d", cmd);
+    const int n_titles = (int)c->lib_titles.size();
+    if ((cmd == EF_LIB_PLAY_AT || cmd == EF_LIB_NAV) && (title < 0 || title >= n_titles)) return fail(EF_EINVAL, "unknown title %d", title);
+    if ((cmd == EF_LIB_SKIP || cmd == EF_LIB_NAV_STEP) && (arg < INT32_MIN || arg > INT32_MAX))
+        return fail(EF_EINVAL, "%s of %lld is not an int", cmd == EF_LIB_SKIP ? "skip" : "step", (long long)arg);
     TRY(restart_ready(c, "ef_library_command"));
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());                          // a library submit may still move the cursors
     std::vector<EfLibStream> st((size_t)count);
     CK(cudaMemcpy(st.data(), c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
+    // the restart op of every stream: play() and load_poster() reset (1), video_pause(0) (2); NAV_STEP and MENU differ per stream
+    std::vector<uint8_t> ops((size_t)count, cmd <= EF_LIB_REWIND || cmd == EF_LIB_NAV ? 1 : cmd == EF_LIB_RESUME ? 2 : 0);
     for (int i = 0; i < count; i++) {
         const EfLibStream& v = st[(size_t)i];
+        int nav_to = -1;                                  // the title whose poster the command shows
         if (cmd == EF_LIB_PLAY_AT) continue;
-        if (v.state == EF_LIB_IDLE) return fail(EF_EINVAL, "stream %d has never played: start it with EF_LIB_PLAY_AT", first + i);
+        if (cmd == EF_LIB_NAV) {
+            if (v.state != EF_LIB_IDLE && v.state != EF_LIB_POSTER) return fail(EF_EINVAL, "EF_LIB_NAV on stream %d, which is not idle or on a poster", first + i);
+            nav_to = title;
+        } else if (v.state == EF_LIB_IDLE) {
+            return fail(EF_EINVAL, "stream %d has never played: start it with EF_LIB_PLAY_AT or EF_LIB_NAV", first + i);
+        } else if (cmd == EF_LIB_NAV_STEP) {
+            if (v.state != EF_LIB_POSTER) return fail(EF_EINVAL, "EF_LIB_NAV_STEP on stream %d, which is not on a poster", first + i);
+            const int64_t to = (int64_t)v.title + arg;
+            if (to >= 0 && to < n_titles) { nav_to = (int)to; ops[(size_t)i] = 1; }
+        } else if (cmd == EF_LIB_MENU) {
+            if (v.state != EF_LIB_POSTER) ops[(size_t)i] = 1;
+            if (v.state != EF_LIB_POSTER && !(v.state == EF_LIB_PLAYING && v.speed)) nav_to = v.title;
+        }
+        if (nav_to >= 0 && !c->lib_titles[(size_t)nav_to].ts[EF_LIB_POSTER_FILE])
+            return fail(EF_EINVAL, "stream %d: title %d has no poster", first + i, nav_to);
         if (cmd == EF_LIB_RESUME && v.state != EF_LIB_PAUSED) return fail(EF_EINVAL, "EF_LIB_RESUME on stream %d, which is not paused", first + i);
+        if (v.title < 0) continue;
         const EfLibTitle& t = c->lib_titles[(size_t)v.title];
         if ((cmd == EF_LIB_FAST_FORWARD && !t.ts[2]) || (cmd == EF_LIB_REWIND && !t.ts[0]))
             return fail(EF_EINVAL, "stream %d: title %d has no %s file", first + i, v.title, cmd == EF_LIB_REWIND ? "rewind" : "fast-forward");
     }
-    CK(ef_launch_library_resolve(c->d_lib, c->d_lib_titles, c->d_pts_last, first, count, cmd, title, arg));
+    EfOverlayState* ovl = c->paced ? c->d_ovl : nullptr;  // hide_progress(): without an overlay nothing is drawn anyway
+    CK(ef_launch_library_resolve(c->d_lib, c->d_lib_titles, c->d_pts_last, first, count, cmd, title, arg, c->d_lib_mode, c->d_lib_nv,
+                                 c->cfg.n_streams, n_titles, ovl));
     c->launches++;
-    const uint8_t op = cmd <= EF_LIB_REWIND ? 1 : cmd == EF_LIB_RESUME ? 2 : 0;   // play(): reset + video_reset; video_pause(0)
-    if (op) {
-        const std::vector<uint8_t> ops((size_t)count, op);
-        return restart_apply(c, first, count, ops.data());
-    }
+    for (uint8_t op : ops) if (op) return restart_apply(c, first, count, ops.data());
     CK(cudaDeviceSynchronize());
     return EF_OK;
 }
@@ -2272,10 +2299,11 @@ int ef_library_submit(ef_ctx* c, uint32_t packets, const uint32_t* per_stream, v
     CK(cudaStreamWaitEvent(st, c->ev_lib_staged, 0));   // the upload of the previous library submit has copied the staging buffer
     if (per_stream) CK(cudaMemcpyAsync(c->d_lib_budget, per_stream, (size_t)n * 4, cudaMemcpyHostToDevice, st));
     CK(ef_launch_library_gather(c->d_lib, c->d_lib_titles, per_stream ? c->d_lib_budget : nullptr, packets, n, c->d_lib_src, c->d_lib_off,
-                                c->d_lib_end, c->d_lib_stage, bound * 188, st, &c->launches));
+                                c->d_lib_end, c->d_lib_mode, c->d_lib_smode, c->d_lib_stage, bound * 188, st, &c->launches));
     TRY(submit_common(c, c->d_lib_stage, c->d_lib_off, false, true, st));
     const int b = c->pending;                             // the streams whose file ends with this submit, as ef_end_streams marks them
     CK(cudaMemcpyAsync(c->d_end2[b], c->d_lib_end, (size_t)n, cudaMemcpyDeviceToDevice, c->up_stream));
+    if (c->d_lib_mode) CK(cudaMemcpyAsync(c->d_lib_mode2[b], c->d_lib_smode, (size_t)n, cudaMemcpyDeviceToDevice, c->up_stream));   // the modes travel with it
     CK(cudaEventRecord(c->ev_up_done[b], c->up_stream));
     CK(cudaEventRecord(c->ev_lib_staged, c->up_stream));
     c->lib_submit = true;
@@ -2291,6 +2319,62 @@ int ef_library_info(ef_ctx* c, int first, int count, ef_library_status* status)
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(status, c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
+    return EF_OK;
+}
+
+// ---- the poster menu: load_poster() (espflix.cpp:1060-1069) and the NVS of nav() / save_pos() (espflix.cpp:719, 856-858) --------
+int ef_library_add_poster(ef_ctx* c, int title, const uint8_t* ts, uint64_t bytes)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->d_lib) return fail(EF_ESTATE, "ef_library_add_poster before the first ef_library_add");
+    if (title < 0 || title >= (int)c->lib_titles.size()) return fail(EF_EINVAL, "no title %d", title);
+    if (!ts || !bytes || bytes % 188 || bytes >> 32) return fail(EF_EINVAL, "a poster of %llu bytes: whole 188-byte packets below 4 GiB", (unsigned long long)bytes);
+    EfLibTitle t = c->lib_titles[title];
+    if (t.ts[EF_LIB_POSTER_FILE]) return fail(EF_ESTATE, "title %d already has a poster", title);
+    const int n = c->cfg.n_streams;
+    if (!c->d_lib_mode) {                                 // the first poster: the modes a library submit carries
+        TRY(dev_alloc(c, &c->d_lib_mode, (size_t)n)); TRY(dev_alloc(c, &c->d_lib_smode, (size_t)n));
+        for (int b = 0; b < 2; b++) TRY(dev_alloc(c, &c->d_lib_mode2[b], (size_t)n));
+        CK(cudaDeviceSynchronize());                      // no submit or present call may be in flight when they appear
+        CK(cudaMemset(c->d_lib_mode, 0, (size_t)n));
+        for (int b = 0; b < 2; b++) CK(cudaMemset(c->d_lib_mode2[b], 0, (size_t)n));
+    }
+    uint8_t* p = nullptr;
+    TRY(dev_alloc(c, &p, bytes));
+    CK(cudaMemcpy(p, ts, bytes, cudaMemcpyHostToDevice));
+    t.ts[EF_LIB_POSTER_FILE] = p; t.bytes[EF_LIB_POSTER_FILE] = (uint32_t)bytes;
+    CK(cudaDeviceSynchronize());                          // a command or a submit may still read the title table
+    CK(cudaMemcpy(c->d_lib_titles + title, &t, sizeof(t), cudaMemcpyHostToDevice));
+    c->lib_titles[title] = t;
+    return EF_OK;
+}
+
+static int library_nv_check(ef_ctx* c, int title, int first, int count, const void* pos, const char* what)
+{
+    if (!c) return fail(EF_EINVAL, "null context");
+    if (!c->d_lib) return fail(EF_ESTATE, "%s before the first ef_library_add", what);
+    if (title < 0 || title >= (int)c->lib_titles.size()) return fail(EF_EINVAL, "no title %d", title);
+    return stream_range(c, first, count, pos);
+}
+
+int ef_library_nv_read(ef_ctx* c, int title, int first, int count, int64_t* pos)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    TRY(library_nv_check(c, title, first, count, pos, "ef_library_nv_read"));
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(pos, c->d_lib_nv + (size_t)title * c->cfg.n_streams + first, (size_t)count * sizeof(int64_t), cudaMemcpyDeviceToHost));
+    return EF_OK;
+}
+
+int ef_library_nv_write(ef_ctx* c, int title, int first, int count, const int64_t* pos)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    TRY(library_nv_check(c, title, first, count, pos, "ef_library_nv_write"));
+    if (!count) return EF_OK;
+    CK(cudaDeviceSynchronize());                          // a command may still read or write the table
+    CK(cudaMemcpy(c->d_lib_nv + (size_t)title * c->cfg.n_streams + first, pos, (size_t)count * sizeof(int64_t), cudaMemcpyHostToDevice));
     return EF_OK;
 }
 
@@ -3419,7 +3503,7 @@ int ef_library_read(ef_ctx* c, int title, int what, uint8_t* dst, uint64_t cap, 
     DeviceScope scope_(c ? c->cfg.device : -1);
     if (!c || !bytes) return fail(EF_EINVAL, "null argument");
     if (!c->d_lib) return fail(EF_ESTATE, "ef_library_read before the first ef_library_add");
-    if (title < 0 || title >= (int)c->lib_titles.size() || what < -1 || what > 2) return fail(EF_EINVAL, "no title %d or part %d", title, what);
+    if (title < 0 || title >= (int)c->lib_titles.size() || what < -1 || what > EF_LIB_POSTER_FILE) return fail(EF_EINVAL, "no title %d or part %d", title, what);
     const EfLibTitle& t = c->lib_titles[title];
     const uint8_t* src = what < 0 ? t.idx : t.ts[what];
     *bytes = what < 0 ? t.idx_bytes : t.bytes[what];

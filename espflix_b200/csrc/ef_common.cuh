@@ -270,13 +270,14 @@ static inline __host__ __device__ int64_t ef_pts2pts(int64_t pts, int speed, int
 }
 
 // The title library (ef_library_*, ef_library.cu): titles held in device memory and every stream's place in one of them.
-// A title is its video.idx image and its three transport streams in the reference's _vid_names order (espflix.cpp:641):
-// 0 video_rwd.ts, 1 video.ts, 2 video_fwd.ts; a missing trick file has ts NULL and bytes 0. Stream states and commands: EF_LIB_* of
-// include/espflix_b200.h.
+// A title is its video.idx image and its transport streams: the three in the reference's _vid_names order (espflix.cpp:641),
+// 0 video_rwd.ts, 1 video.ts, 2 video_fwd.ts, then 3 poster.ts (load_poster, espflix.cpp:1060-1069); a missing file has ts NULL
+// and bytes 0. Stream states and commands: EF_LIB_* of include/espflix_b200.h.
+#define EF_LIB_POSTER_FILE 3
 struct __align__(16) EfLibTitle {
     const uint8_t* idx;          // the video.idx image: idx_hdr (104 bytes), then the main, fwd and rwd sample arrays (uint32)
-    const uint8_t* ts[3];
-    uint32_t bytes[3];           // file sizes, multiples of 188 below 4 GiB
+    const uint8_t* ts[4];
+    uint32_t bytes[4];           // file sizes, multiples of 188 below 4 GiB
     uint32_t idx_bytes;
     int64_t v_first, v_last, f_first, f_last, r_first, r_last;   // the header's records
     uint32_t v_bin, f_bin, r_bin, f_trick, r_trick, v_n, f_n, r_n;
@@ -284,8 +285,8 @@ struct __align__(16) EfLibTitle {
 struct __align__(16) EfLibStream {   // layout of ef_library_status (include/espflix_b200.h)
     int32_t title;               // -1 before the first PLAY_AT
     int32_t speed;               // _speed: -1, 0, 1
-    int32_t state;               // EF_LIB_IDLE ... EF_LIB_ENDED
-    int32_t file;                // speed + 1: the file the cursor is in
+    int32_t state;               // EF_LIB_IDLE ... EF_LIB_POSTER
+    int32_t file;                // speed + 1, or EF_LIB_POSTER_FILE: the file the cursor is in
     uint64_t cursor;             // byte offset of the next packet in that file
     int64_t pos;                 // _info[_nav].pos: the main pts the next PLAY, SKIP, FAST_FORWARD or REWIND starts from
 };

@@ -403,12 +403,13 @@ __device__ __forceinline__ int pace_hscroll(int ai) { return ai < 0 ? -c_easd[-a
 }  // namespace
 
 // pic >= 0: every stream with a picture `pic` pushes it (pts from pic_pts, modes[s] or 0); pic < 0: every stream idles until
-// it has emitted idle_n[s] fields. ovl (NULL unless the context stages overlays): the staged overlay changes latch, into
-// ovl_next, when the call draws line 0 of their latch field
+// it has emitted idle_n[s] fields. lib_modes (NULL unless the context has library posters): the poster mode the current submit
+// carries for each stream (ef_library_submit), used for the stream's last picture of the submit where modes[s] is 0. ovl (NULL
+// unless the context stages overlays): the staged overlay changes latch, into ovl_next, when the call draws line 0 of their latch field
 __global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* __restrict__ next, EfPaceRun* __restrict__ run, EfPaceOut* __restrict__ out,
                                const int64_t* __restrict__ pic_pts, const uint32_t* __restrict__ n_pics, const uint32_t* __restrict__ base_pics,
-                               const uint8_t* __restrict__ modes, const uint32_t* __restrict__ idle_n, int pic, int max_pictures, int n_streams, int ntsc,
-                               const EfOverlayState* __restrict__ ovl, EfOverlayState* __restrict__ ovl_next)
+                               const uint8_t* __restrict__ modes, const uint8_t* __restrict__ lib_modes, const uint32_t* __restrict__ idle_n, int pic,
+                               int max_pictures, int n_streams, int ntsc, const EfOverlayState* __restrict__ ovl, EfOverlayState* __restrict__ ovl_next)
 {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_streams) return;
@@ -428,7 +429,8 @@ __global__ void ef_pace_kernel(const EfPaceState* __restrict__ st, EfPaceState* 
         }
     } else if ((uint32_t)pic < n_pics[s]) {
         const int64_t pts = pic_pts[(size_t)s * max_pictures + pic];
-        const int mode = modes ? modes[s] : 0;
+        int mode = modes ? modes[s] : 0;
+        if (!mode && lib_modes && (uint32_t)pic + 1u == n_pics[s]) mode = lib_modes[s];   // load_poster's flush_picture(mode)
         if (pts == -1 && mode == 0) q.flags |= 1u;                         // flush_picture() pushes nothing (player.cpp:692-702)
         else {
             const uint32_t vp = (uint32_t)(pts / (ntsc ? 1500 : 1800));

@@ -4,6 +4,8 @@
 // The reference's player reads a title through Streamer::get(url, offset) and 8-packet Buffers (espflix.cpp:723-747, 787-798) and
 // seeks with the video.idx sample at idx_hdr::pts2offset (espflix.cpp:607-629, 823-829). Here the titles live in HBM: a command is
 // a few bytes from the host, the offset arithmetic and the sample read run on the device, and a submit is a device-to-device gather.
+// The poster menu (nav(), menu(), load_poster(), espflix.cpp:704-720, 778-785, 1060-1069) runs here too: the scroll mode of each
+// stream's latest nav, the saved positions nv_read() / nv_write() keep in NVS, and the mode a submit carries to the present calls.
 #include "../../include/espflix_b200.h"
 #include "ef_common.cuh"
 
@@ -44,13 +46,34 @@ __device__ __forceinline__ void lib_play(EfLibStream& v, const EfLibTitle& t, in
     v.state = EF_LIB_PLAYING;
 }
 
+// nav(s, i) (espflix.cpp:704-720, 1060-1069): the scroll mode load_poster() flushes the poster's last picture with, from the old title
+// (_nav - i; 0 before the first nav), pos = nv_read() of title i, and the poster's bytes from byte 0. hide_progress() stages a blend of
+// 0 on a presenting context (ovl), as ef_present_overlay stages it. _speed stays.
+__device__ __forceinline__ void lib_nav(EfLibStream& v, int s, int i, uint8_t* mode, const int64_t* nv, int n_streams, EfOverlayState* ovl)
+{
+    const int dir = v.title == -1 ? 0 : v.title - i;
+    mode[s] = dir == 0 ? 1 : dir < 0 ? 2 : 3;
+    v.title = i;
+    v.pos = nv[(size_t)i * n_streams + s];
+    v.state = EF_LIB_POSTER;
+    v.file = EF_LIB_POSTER_FILE;
+    v.cursor = 0;
+    if (ovl) {
+        ovl[s].p_blend = 0;
+        ovl[s].pending |= 2u;
+    }
+}
+
 }  // namespace
 
-// One thread per commanded stream of [first, first + count): the ESPFlix method the command names (espflix.cpp:800-859). Every command
-// but PLAY_AT and RESUME first saves pos = pts2pts(get_pts(), _speed) on a PLAYING stream (save_pos, espflix.cpp:843-852); get_pts()
-// is the stream's last_pts after the current submit. The host has checked the arguments against every stream's state.
+// One thread per commanded stream of [first, first + count): the ESPFlix method the command names (espflix.cpp:704-720, 778-859,
+// 906-939). Every command but PLAY_AT, RESUME, NAV and NAV_STEP first saves pos = pts2pts(get_pts(), _speed) on a PLAYING stream
+// (save_pos, espflix.cpp:843-852); get_pts() is the stream's last_pts after the current submit. The host has checked the arguments
+// against every stream's state. mode / nv / ovl: the poster modes, the saved positions (nv[title][stream]) and the overlay states
+// (NULL off a presenting context); only the poster commands use them.
 __global__ void ef_library_resolve_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restrict__ titles, const int64_t* __restrict__ pts_last,
-                                          int first, int count, int cmd, int title, int64_t arg)
+                                          int first, int count, int cmd, int title, int64_t arg, uint8_t* __restrict__ mode, int64_t* __restrict__ nv,
+                                          int n_streams, int n_titles, EfOverlayState* __restrict__ ovl)
 {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= count) return;
@@ -60,6 +83,12 @@ __global__ void ef_library_resolve_kernel(EfLibStream* __restrict__ ls, const Ef
         v.title = title;
         v.pos = arg;
         lib_play(v, titles[title], 0);
+    } else if (cmd == EF_LIB_NAV) {
+        lib_nav(v, s, title, mode, nv, n_streams, ovl);
+    } else if (cmd == EF_LIB_NAV_STEP) {                                // the left / right keys in NAV: nav(_nav +- 1)
+        const int64_t i = (int64_t)v.title + arg;
+        if (i < 0 || i >= n_titles) return;                             // nav()'s early return
+        lib_nav(v, s, (int)i, mode, nv, n_streams, ovl);
     } else {
         const EfLibTitle& t = titles[v.title];
         if (cmd != EF_LIB_RESUME && v.state == EF_LIB_PLAYING) v.pos = ef_lib_pts2pts(t, pts_last[s], v.speed);
@@ -73,19 +102,30 @@ __global__ void ef_library_resolve_kernel(EfLibStream* __restrict__ ls, const Ef
         case EF_LIB_REWIND: lib_play(v, t, -1); break;
         case EF_LIB_PAUSE: if (v.state == EF_LIB_PLAYING) v.state = EF_LIB_PAUSED; break;
         case EF_LIB_RESUME: v.state = EF_LIB_PLAYING; break;
+        case EF_LIB_MENU:                                               // menu(), then loop()'s pending-NAV branch
+            if (v.state == EF_LIB_POSTER) break;                        // set_state(NAV) from NAV
+            if (v.state == EF_LIB_PLAYING) {                            // save_pos(pts, true)
+                nv[(size_t)v.title * n_streams + s] = v.pos;
+                if (v.speed) { lib_play(v, t, 0); break; }              // trick mode: play_pause() from NAV, no poster
+            }
+            lib_nav(v, s, v.title, mode, nv, n_streams, ovl);           // set_state(NAV): nav(_nav), mode 1
+            break;
         default: v.state = EF_LIB_STOPPED; break;                           // STOP
         }
     }
     ls[s] = v;
 }
 
-// One CTA: every PLAYING stream takes min(its budget, packets left in its file) packets from its cursor; the exclusive prefix of the
-// run lengths gives each stream's place in the submit (off[n_streams + 1], EfBlockScan). A stream whose cursor
-// reaches the end of its file ends with this submit: end[s] = 1, state ENDED, pos = pts2pts(0, _speed) (save_pos(0) at DONE,
-// espflix.cpp:906-911). src[s] = where the stream's run starts.
+// One CTA: every PLAYING stream, and every POSTER stream with poster bytes left, takes min(its budget, packets left in its file)
+// packets from its cursor; the exclusive prefix of the run lengths gives each stream's place in the submit (off[n_streams + 1],
+// EfBlockScan). A stream whose cursor reaches the end of its file ends with this submit: end[s] = 1. A PLAYING stream becomes ENDED
+// with pos = pts2pts(0, _speed) (save_pos(0) at DONE, espflix.cpp:906-911); a POSTER stream stays POSTER with its pos (the poster
+// stays on screen), and its mode travels with the submit: smode[s] (NULL on a context without posters) = mode[s] there, else 0.
+// src[s] = where the stream's run starts.
 __global__ void __launch_bounds__(1024)
 ef_library_count_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restrict__ titles, const uint32_t* __restrict__ budget, uint32_t packets,
-                        int n_streams, const uint8_t** __restrict__ src, uint64_t* __restrict__ off, uint8_t* __restrict__ end)
+                        int n_streams, const uint8_t** __restrict__ src, uint64_t* __restrict__ off, uint8_t* __restrict__ end,
+                        const uint8_t* __restrict__ mode, uint8_t* __restrict__ smode)
 {
     __shared__ EfBlockScan<uint64_t, 1024> scan;
     scan.init();
@@ -94,24 +134,30 @@ ef_library_count_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restri
         uint64_t v = 0;
         if (k < n_streams) {
             EfLibStream q = ls[k];
-            uint8_t e = 0;
-            if (q.state == EF_LIB_PLAYING) {
+            uint8_t e = 0, m = 0;
+            if (q.state == EF_LIB_PLAYING || q.state == EF_LIB_POSTER) {
                 const EfLibTitle& t = titles[q.title];
                 const uint64_t size = t.bytes[q.file];
-                const uint64_t left = q.cursor < size ? (size - q.cursor) / 188u : 0;
-                const uint64_t b = budget ? budget[k] : packets;
-                const uint64_t take = b < left ? b : left;
-                v = take * 188u;
-                src[k] = t.ts[q.file] + (q.cursor < size ? q.cursor : 0);
-                q.cursor += v;
-                if (take == left) {
-                    e = 1;
-                    q.state = EF_LIB_ENDED;
-                    q.pos = ef_lib_pts2pts(t, 0, q.speed);
+                if (q.state == EF_LIB_PLAYING || q.cursor < size) {
+                    const uint64_t left = q.cursor < size ? (size - q.cursor) / 188u : 0;
+                    const uint64_t b = budget ? budget[k] : packets;
+                    const uint64_t take = b < left ? b : left;
+                    v = take * 188u;
+                    src[k] = t.ts[q.file] + (q.cursor < size ? q.cursor : 0);
+                    q.cursor += v;
+                    if (take == left) {
+                        e = 1;
+                        if (q.state == EF_LIB_POSTER) m = mode[k];
+                        else {
+                            q.state = EF_LIB_ENDED;
+                            q.pos = ef_lib_pts2pts(t, 0, q.speed);
+                        }
+                    }
+                    ls[k] = q;
                 }
-                ls[k] = q;
             }
             end[k] = e;
+            if (smode) smode[k] = m;
         }
         const uint64_t excl = scan.exclusive(v);
         if (k < n_streams) off[k] = excl;
@@ -168,18 +214,18 @@ ef_library_gather_kernel(const uint8_t* const* __restrict__ src, const uint64_t*
 }
 
 cudaError_t ef_launch_library_resolve(EfLibStream* ls, const EfLibTitle* titles, const int64_t* pts_last, int first, int count, int cmd, int title,
-                                      int64_t arg)
+                                      int64_t arg, uint8_t* mode, int64_t* nv, int n_streams, int n_titles, EfOverlayState* ovl)
 {
-    ef_library_resolve_kernel<<<(count + 127) / 128, 128>>>(ls, titles, pts_last, first, count, cmd, title, arg);
+    ef_library_resolve_kernel<<<(count + 127) / 128, 128>>>(ls, titles, pts_last, first, count, cmd, title, arg, mode, nv, n_streams, n_titles, ovl);
     return cudaGetLastError();
 }
 
 // count, then gather over at most max_bytes of submit (the host's bound: its grid follows it, CTAs past the submit's end exit)
 cudaError_t ef_launch_library_gather(EfLibStream* ls, const EfLibTitle* titles, const uint32_t* budget, uint32_t packets, int n_streams,
-                                     const uint8_t** src, uint64_t* off, uint8_t* end, uint8_t* dst, uint64_t max_bytes, cudaStream_t st,
-                                     uint64_t* launches)
+                                     const uint8_t** src, uint64_t* off, uint8_t* end, const uint8_t* mode, uint8_t* smode, uint8_t* dst,
+                                     uint64_t max_bytes, cudaStream_t st, uint64_t* launches)
 {
-    ef_library_count_kernel<<<1, 1024, 0, st>>>(ls, titles, budget, packets, n_streams, src, off, end);
+    ef_library_count_kernel<<<1, 1024, 0, st>>>(ls, titles, budget, packets, n_streams, src, off, end, mode, smode);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     ++*launches;

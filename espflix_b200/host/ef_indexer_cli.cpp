@@ -11,6 +11,9 @@
 //   --audio pcm.s16le (last) gives the title its sound: mono 16-bit little-endian PCM at 48 kHz, encoded to SBC (ef_sbc_encode at
 //   espflix_b200.capi.AUDIO_ENCODE_DEFAULTS: the reference's 48 kHz, 192 kbit/s) and interleaved on PID 0x102 (ef_mux_audio). The
 //   trick files stay audio-free, as the reference's "-an" makes them.
+//   --poster poster.i420 (last) also writes title_dir/poster.ts, what make_video()'s "ffmpeg ... -bf 0 -q 2 poster.ts" makes
+//   (indexer.cpp:306): the one 352 x 192 I420 picture of poster.i420 as an I picture at quantiser scale 2 (ef_encode_build with gop 1
+//   and qscale_i 2, the rest as video.ts; espflix_b200.capi.encode_poster).
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -81,14 +84,10 @@ static std::vector<uint8_t> add_audio(const std::vector<uint8_t>& ts, const std:
     return out;
 }
 
-// title_dir/video.ts of the pictures in `pictures` (I420, 101,376 bytes each), with the sound of `pcm_path` when it is not empty
-static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p, const ef_rate_params* rate,
-                       const std::string& pcm_path)
+// the transport stream of the I420 pictures `pics` encoded with `p` (and to `rate` when it is not NULL)
+static std::vector<uint8_t> encode(const std::vector<uint8_t>& pics, const ef_encode_params& p, const ef_rate_params* rate)
 {
-    const std::vector<uint8_t> pics = read_file(pictures);
-    if (pics.empty() || pics.size() % 101376) throw std::runtime_error(pictures + ": not a whole number of 352 x 192 I420 pictures");
     const uint64_t off[2] = { 0, pics.size() / 101376 };
-    const ef_encode_params p = { 12, qscale_i, qscale_p, 7, 1, 2, 0, 3750 };
     uint64_t to[2] = { 0, 0 };
     std::vector<uint8_t> ts(pics.size() / 4);
     auto build = [&]() {
@@ -102,14 +101,34 @@ static void make_video(const std::string& pictures, const std::string& dir, int 
     }
     if (rc != EF_OK) throw std::runtime_error(std::string(rate ? "ef_encode_build_rate: " : "ef_encode_build: ") + ef_last_error());
     ts.resize(to[1]);
+    return ts;
+}
+
+// title_dir/video.ts of the pictures in `pictures` (I420, 101,376 bytes each), with the sound of `pcm_path` when it is not empty
+static void make_video(const std::string& pictures, const std::string& dir, int qscale_i, int qscale_p, const ef_rate_params* rate,
+                       const std::string& pcm_path)
+{
+    const std::vector<uint8_t> pics = read_file(pictures);
+    if (pics.empty() || pics.size() % 101376) throw std::runtime_error(pictures + ": not a whole number of 352 x 192 I420 pictures");
+    std::vector<uint8_t> ts = encode(pics, ef_encode_params{ 12, qscale_i, qscale_p, 7, 1, 2, 0, 3750 }, rate);
     if (!pcm_path.empty()) ts = add_audio(ts, pcm_path);
     write_file(dir + "/video.ts", ts.data(), ts.size());
+}
+
+// title_dir/poster.ts of the one picture in `picture`: gop 1, qscale_i 2 (ffmpeg's -q 2)
+static void make_poster(const std::string& picture, const std::string& dir)
+{
+    const std::vector<uint8_t> pic = read_file(picture);
+    if (pic.size() != 101376) throw std::runtime_error(picture + ": not one 352 x 192 I420 picture");
+    const std::vector<uint8_t> ts = encode(pic, ef_encode_params{ 1, 2, 8, 7, 1, 2, 0, 3750 }, nullptr);
+    write_file(dir + "/poster.ts", ts.data(), ts.size());
 }
 
 int main(int argc, char** argv)
 {
     const bool encode = argc >= 2 && std::string(argv[1]) == "--encode";
-    std::string pcm_path;
+    std::string pcm_path, poster_path;
+    if (encode && argc >= 6 && std::string(argv[argc - 2]) == "--poster") { poster_path = argv[argc - 1]; argc -= 2; }
     if (encode && argc >= 6 && std::string(argv[argc - 2]) == "--audio") { pcm_path = argv[argc - 1]; argc -= 2; }
     const bool rated = encode && argc == 7 && std::string(argv[4]) == "--rate";
     ef_rate_params rate = { 1500000, 250000, 3, 31 };
@@ -119,7 +138,7 @@ int main(int argc, char** argv)
     }
     if (encode ? (argc != 4 && argc != 6 && !rated) : (argc != 5 && argc != 2 && argc != 3)) {
         fprintf(stderr, "usage: %s video.ts fwd.ts rev.ts out_dir\n       %s title_dir [qscale]   (title_dir/video.ts -> video_fwd.ts, video_rwd.ts, video.idx)\n"
-                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p | --rate bit_rate vbv_bits] [--audio pcm.s16le]   "
+                        "       %s --encode pictures.i420 title_dir [qscale_i qscale_p | --rate bit_rate vbv_bits] [--audio pcm.s16le] [--poster poster.i420]   "
                         "(-> title_dir/video.ts, then as title_dir)\n",
                 argv[0], argv[0], argv[0]);
         return 2;
@@ -135,6 +154,7 @@ int main(int argc, char** argv)
             const std::string dir = encode ? argv[3] : argv[1];
             const int qscale = !encode && argc == 3 ? atoi(argv[2]) : 8;
             if (encode) make_video(argv[2], dir, argc == 6 ? atoi(argv[4]) : 8, argc == 6 ? atoi(argv[5]) : 8, rated ? &rate : nullptr, pcm_path);
+            if (!poster_path.empty()) make_poster(poster_path, dir);
             make_trick_files(dir, qscale);
             make_index(dir + "/video.ts", all);
             make_index(dir + "/video_fwd.ts", all);

@@ -63,6 +63,9 @@
  *   ef_library_add / _command / _submit / _info / _add_trick  Streamer::get() + read() of a title (espflix.cpp:723-747) and ESPFlix's play, skip,
  *                                 fast_forward, rewind, play_pause, get_index and save_pos (espflix.cpp:787-859): titles in HBM, every
  *                                 stream's seek resolved from video.idx and its bytes gathered on the device
+ *   ef_library_add_poster / _nv_read / _nv_write, EF_LIB_NAV / _NAV_STEP / _MENU  ESPFlix::nav(), menu() and load_poster()
+ *                                 (espflix.cpp:704-720, 778-785, 1060-1069) and the NVS resume (espflix.cpp:851-859; espflix.ino:160-178):
+ *                                 the poster menu, its scroll mode pushed on the device, and one saved position per title and stream
  * Calls run on the context's device and restore the caller's current device.
  */
 #ifndef ESPFLIX_B200_H
@@ -658,11 +661,15 @@ int ef_carry_info(ef_ctx* ctx, int first, int count, uint32_t* held_bytes, uint8
 #define EF_LIB_PAUSE        5
 #define EF_LIB_RESUME       6
 #define EF_LIB_STOP         7
+#define EF_LIB_NAV          8    /* the poster menu: ef_library_add_poster below */
+#define EF_LIB_NAV_STEP     9
+#define EF_LIB_MENU         10
 #define EF_LIB_IDLE    0         /* stream states: never played */
 #define EF_LIB_PLAYING 1
 #define EF_LIB_PAUSED  2
 #define EF_LIB_STOPPED 3
 #define EF_LIB_ENDED   4         /* its cursor reached the end of its file */
+#define EF_LIB_POSTER  5         /* the reference's NAV: the title's poster.ts is streamed (file 3) or shown */
 typedef struct { int32_t title, speed, state, file; uint64_t cursor; int64_t pos; } ef_library_status;
 int ef_library_add(ef_ctx* ctx, const uint8_t* idx, uint64_t idx_bytes, const uint8_t* const* ts, const uint64_t* bytes, int* title);
 int ef_library_command(ef_ctx* ctx, int first, int count, int cmd, int title, int64_t arg);
@@ -680,10 +687,45 @@ int ef_library_info(ef_ctx* ctx, int first, int count, ef_library_status* status
  *                     changes on an error. */
 int ef_library_add_trick(ef_ctx* ctx, int title, int qscale);
 /* ef_library_read     copies part `what` of a title to host memory: -1 its video.idx image, 0 / 1 / 2 its rwd / main / fwd file (after
- *                     ef_library_add_trick: the built files and the rewritten image, for a service to store beside video.ts).
- *                     *bytes = the part's size (0: no such file, nothing copied). EF_ENOMEM when dst is NULL or cap is below it (a
- *                     sizing call). EF_ESTATE before the first ef_library_add; EF_EINVAL for an unknown title or part. Synchronous. */
+ *                     ef_library_add_trick: the built files and the rewritten image, for a service to store beside video.ts), 3 its
+ *                     poster.ts. *bytes = the part's size (0: no such file, nothing copied). EF_ENOMEM when dst is NULL or cap is below
+ *                     it (a sizing call). EF_ESTATE before the first ef_library_add; EF_EINVAL for an unknown title or part. Synchronous. */
 int ef_library_read(ef_ctx* ctx, int title, int what, uint8_t* dst, uint64_t cap, uint64_t* bytes);
+
+/* ---- the poster menu: ESPFlix::nav(), menu(), load_poster() and the NVS resume (espflix.cpp:704-720, 763-785, 851-859, 906-939,
+ * 1060-1069; espflix.ino:160-178) ---------------------------------------------------------------------------------------------------
+ * ef_library_add_poster  attaches a title's poster.ts (what the reference's make_video() writes with ffmpeg -bf 0 -q 2, indexer.cpp:306;
+ *                     capi.encode_poster makes it) as the title's file 3. Synchronous. EF_EINVAL for an unknown title, a NULL poster or a
+ *                     size that is 0, not whole packets or >= 4 GiB; EF_ESTATE before the first ef_library_add or when the title has a
+ *                     poster already. Nothing changes on an error.
+ * The saved positions (the reference's NVS, one int64 per title and stream): nv[title x n_streams + s], title-major, every entry 0 at
+ * first (nv_read's default for a missing key); it grows with the title table. ef_library_nv_read / _nv_write copy entries
+ * [first, first + count) of one title to / from host memory, synchronously, so that a service can keep its viewers' places across
+ * sessions as NVS survives a reboot. EF_ESTATE before the first ef_library_add; EF_EINVAL for an unknown title or a bad stream range.
+ * Commands of ef_library_command, where nav(s, i) is the reference's nav(i) for stream s: dir = (title == -1) ? 0 : title - i from the
+ * old title, mode = dir == 0 ? 1 : dir < 0 ? 2 : 3; title = i, pos = nv[i][s], state EF_LIB_POSTER, file 3 from byte 0, restart op 1
+ * (load_poster's _decoder.reset()), and on a presenting context a blend of 0 staged as ef_present_overlay stages it (hide_progress()).
+ * speed is kept (nav() leaves _speed alone).
+ *   EF_LIB_NAV (title i)                 from IDLE or POSTER: nav(s, i). The first nav(0) after init_service(), or any jump.
+ *   EF_LIB_NAV_STEP (arg = step, an int) from POSTER: nav(s, title + step); a stream whose target is outside [0, titles) is left as it
+ *                                        is, with no restart and no blend (nav()'s early return). The left / right keys.
+ *   EF_LIB_MENU                          menu() and then loop()'s pending-NAV branch. PLAYING at speed 0: pos = pts2pts(get_pts(), 0),
+ *                                        nv[title][s] = pos, nav(s, title) (mode 1). PLAYING at speed +-1: pos = pts2pts(get_pts(),
+ *                                        speed), nv[title][s] = pos, then play at speed 0 from pos (op 1, no poster; espflix.cpp:911-913).
+ *                                        PAUSED, STOPPED, ENDED: nav(s, title) with no NVS write, so pos becomes the last saved value.
+ *                                        POSTER: nothing (set_state()'s early return).
+ * EF_EINVAL, nothing changed: NAV or NAV_STEP from any other state, MENU on IDLE, NAV to an unknown title, a nav to a title without a
+ * poster, a step outside int. The other commands treat a POSTER stream by their existing rules: PLAY plays the title at speed 0 from pos
+ * (play_pause() from NAV, so it resumes from the saved position), SKIP / FAST_FORWARD / REWIND start from pos, PAUSE does nothing,
+ * RESUME is EF_EINVAL, STOP stops the poster's bytes. The host reads back the commanded streams' states only, as for every command.
+ * ef_library_submit gives a POSTER stream packets of file 3 as it gives a PLAYING stream packets of its file; the submit that reaches
+ * the poster's end ends the stream (as ef_end_streams) and carries the stream's mode, but the stream stays POSTER with its pos and takes
+ * no more packets. On a presenting context the push of that stream's last picture of that submit (index n_pics - 1) uses the mode, in
+ * ef_present_picture and ef_present_picture_async alike, where the call's modes[s] is 0 or modes is NULL (a caller's mode wins);
+ * the poster's earlier pictures are pushed at mode 0. A later nav before the poster ended replaces the mode. */
+int ef_library_add_poster(ef_ctx* ctx, int title, const uint8_t* ts, uint64_t bytes);
+int ef_library_nv_read(ef_ctx* ctx, int title, int first, int count, int64_t* pos);
+int ef_library_nv_write(ef_ctx* ctx, int title, int first, int count, const int64_t* pos);
 
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
