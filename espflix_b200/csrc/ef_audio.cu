@@ -401,30 +401,16 @@ __global__ void ef_audio_commit_kernel(EfAudioState* __restrict__ st, const uint
 }
 
 // ---- TS -> audio bytes --------------------------------------------------------------------------------------
-// per packet: payload start (0 = none) and length of PID 0x101 / 0x102, and for PES starts whether the PTS parses
+// per packet of PID 0x101 / 0x102 with the payload flag: payload start (0 = none), and for PES starts whether the PTS parses. A packet
+// without the sync byte is skipped (more(), player.cpp:476-479).
 __global__ void ef_audio_ts_packet_kernel(const uint8_t* __restrict__ ts, uint64_t n_packets, uint8_t* __restrict__ start, uint8_t* __restrict__ kind)
 {
     const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_packets) return;
-    const uint8_t* d = ts + k * 188;
-    uint8_t st = 0, kd = 0;                                // kind: 0 continuation, 1 PES start with PTS, 2 PES start without
-    const int pid = ((d[1] << 8) | d[2]) & 0x1FFF;
-    if (d[0] == 0x47 && (pid == 0x101 || pid == 0x102) && (d[3] & 0x10)) {
-        int o = 4;
-        if (d[3] & 0x20) o = 5 + d[4];
-        if (d[1] & 0x40) {
-            kd = 2;
-            if (o + 9 <= 188) {
-                const int flags = (d[o + 6] << 8) | d[o + 7];
-                const int p = o + 9;
-                if ((flags & 0x80) && p < 188 && (d[p] & 0xF0) == ((flags >> 2) & 0x30)) kd = 1;   // parse_pts(), player.cpp:299
-                o = o + 9 + d[o + 8];
-            } else o = 188;
-        }
-        if (o < 188) st = (uint8_t)o;
-    }
-    start[k] = st;
-    kind[k] = kd;                                          // a packet without the sync byte is skipped (more(), player.cpp:476-479)
+    const EfTsPacket r = ef_ts_read(ts + k * 188);
+    const bool audio = r.sync && (r.pid == 0x101 || r.pid == 0x102) && r.payload;
+    start[k] = audio && r.start < 188 ? (uint8_t)r.start : 0;
+    kind[k] = audio && r.pusi ? (r.pts_prefix ? 1 : 2) : 0;  // 0 continuation, 1 PES start with PTS, 2 PES start without
 }
 
 // One thread per file walks its packets in order (a few thousand): byte offsets of the payloads that reach push_audio().

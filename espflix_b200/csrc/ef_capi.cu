@@ -2414,13 +2414,12 @@ uint64_t trick_video_es(const uint8_t* ts, uint64_t pkt, uint64_t end, size_t ca
     uint64_t k = pkt;
     for (; k < end && es.size() < cap; k++) {
         const uint8_t* d = ts + k * 188;
-        if (d[0] != 0x47 || (((d[1] << 8) | d[2]) & 0x1FFF) != 0x100 || !(d[3] & 0x10)) continue;
-        int o = (d[3] & 0x20) ? 5 + d[4] : 4;
-        if ((d[1] & 0x40) && o + 14 <= 188) {
-            const int flags = (d[o + 6] << 8) | d[o + 7];
-            if (k == pkt && pts_ok) *pts_ok = (flags & 0x80) && (d[o + 9] & 0xF0) == ((flags >> 2) & 0x30);
-            o += 9 + d[o + 8];
-        }
+        const EfTsPacket r = ef_ts_read(d);
+        if (!r.sync || r.pid != 0x100 || !r.payload) continue;
+        if (k == pkt && pts_ok) *pts_ok = r.pts >= 0;
+        // the one difference from ef_ts_read's start (the device's ES): the PES header is skipped only when its first 14 bytes lie
+        // inside the packet, so a malformed one that leaves 9 to 13 bytes stays in the ES
+        const int o = r.pusi && r.pes + 14 > 188 ? r.pes : r.start;
         if (o < 188) es.insert(es.end(), d + o, d + 188);
     }
     return k;
@@ -2868,8 +2867,8 @@ int ef_trick_build(int device, const uint8_t* ts, const uint64_t* off, int n_fil
     for (const TrickSeg& s : segs) {                 // a first guess of the pictures per segment: its video PES starts
         uint64_t n = 1;
         for (uint64_t k = s.pkt0; k < s.pkt1; k++) {
-            const uint8_t* d = base + k * 188;
-            n += (d[1] & 0x40) && (((d[1] << 8) | d[2]) & 0x1FFF) == 0x100;
+            const EfTsPacket r = ef_ts_read(base + k * 188);
+            n += r.pusi && r.pid == 0x100;
         }
         max_pusi = std::max(max_pusi, n);
     }
@@ -3355,15 +3354,13 @@ extern "C" int ef_mux_audio(int device, const uint8_t* ts, const uint64_t* ts_of
         std::vector<std::pair<uint64_t, int64_t>> starts;                  // (packet, pts) of every video PES start
         for (uint64_t k = 0; k < n_pk; k++) {
             const uint8_t* d = d0 + k * 188;
-            const int pid = ((d[1] << 8) | d[2]) & 0x1FFF;
-            if (pid == 0x101 || pid == 0x102) return fail(EF_EINVAL, "title %d packet %llu is on audio PID 0x%x", t, (unsigned long long)k, pid);
-            if (pid != 0x100 || !(d[1] & 0x40) || !(d[3] & 0x10)) continue;     // more() demuxes only packets with a payload
-            const int o = (d[3] & 0x20) ? 5 + d[4] : 4;
+            const EfTsPacket r = ef_ts_read(d);
+            if (r.pid == 0x101 || r.pid == 0x102) return fail(EF_EINVAL, "title %d packet %llu is on audio PID 0x%x", t, (unsigned long long)k, r.pid);
+            if (r.pid != 0x100 || !r.pusi || !r.payload) continue;          // more() demuxes only packets with a payload
             // the PTS must parse as parse_pts() reads it (player.cpp:299): a malformed prefix nibble is no PTS to the decoder
-            if (o + 14 > 188 || d[o] || d[o + 1] || d[o + 2] != 1 || !(d[o + 7] & 0x80) || (d[o + 9] & 0xF0) != ((d[o + 7] >> 2) & 0x30))
+            if (r.pts < 0 || d[r.pes] || d[r.pes + 1] || d[r.pes + 2] != 1)
                 return fail(EF_EINVAL, "title %d packet %llu: a video PES start without a PTS", t, (unsigned long long)k);
-            const uint8_t* q = d + o + 9;
-            starts.push_back({ k, (int64_t)((q[0] >> 1) & 7) << 30 | (int64_t)q[1] << 22 | (int64_t)(q[2] >> 1) << 15 | (int64_t)q[3] << 7 | (q[4] >> 1) });
+            starts.push_back({ k, r.pts });
         }
         // a_k rises with k, so the first start with v_j >= a_k never moves back: one pass over the starts for all the PES
         uint64_t pk = n_pk;
@@ -3391,20 +3388,8 @@ extern "C" int ef_mux_audio(int device, const uint8_t* ts, const uint64_t* ts_of
         for (uint64_t k = 0; k <= n_pk; k++) {
             for (; e < plan[t].size() && plan[t][e].before == k; e++) {  // the audio PES that go before input packet k
                 const Pes& a = plan[t][e];
-                const uint64_t pay = a.n * fbytes, len = 14 + pay;
-                uint8_t h[14] = { 0, 0, 1, 0xBD, (uint8_t)((8 + pay) >> 8), (uint8_t)(8 + pay), 0x80, 0x80, 5 };
-                const uint64_t v = (uint64_t)a.pts;
-                h[9] = (uint8_t)(0x21 | ((v >> 29) & 0x0E)); h[10] = (uint8_t)(v >> 22); h[11] = (uint8_t)(0x01 | ((v >> 14) & 0xFE));
-                h[12] = (uint8_t)(v >> 7); h[13] = (uint8_t)(0x01 | ((v << 1) & 0xFE));
-                for (uint64_t pos = 0; pos < len; pos += 184, cc++, o += 188) {
-                    const uint64_t left = len - pos, af = left >= 184 ? 0 : 184 - left;
-                    o[0] = 0x47; o[1] = (uint8_t)((pos ? 0 : 0x40) | 0x01); o[2] = 0x02; o[3] = (uint8_t)((af ? 0x30 : 0x10) | (cc & 15));
-                    if (af) { o[4] = (uint8_t)(af - 1); if (af > 1) { o[5] = 0; memset(o + 6, 0xFF, af - 2); } }
-                    for (uint64_t b = 4 + af; b < 188; b++) {
-                        const uint64_t x = pos + b - 4 - af;
-                        o[b] = x < 14 ? h[x] : a0[a.frame * fbytes + x - 14];
-                    }
-                }
+                const uint32_t pay = (uint32_t)(a.n * fbytes);
+                for (uint32_t j = 0; j < a.pkts; j++, cc++, o += 188) ef_pes_packet(o, 0, 1, j, 0x102, 0xBD, 8 + pay, a.pts, cc, a0 + a.frame * fbytes, pay);
             }
             if (k < n_pk) { memcpy(o, d0 + k * 188, 188); o += 188; }
         }

@@ -353,6 +353,85 @@ static inline __host__ __device__ int ef_strips_to_tiled(int b)
     return ef_chroma_offset(r >> 3, x - EF_W, (row >> 4) * 8 + (r & 7));
 }
 
+// ---- 188-byte transport-stream packets and their PES headers (ISO 13818-1) ---------------------------------------------------------
+// The 33-bit PTS of the 5 PTS bytes of a PES header (marker bits and prefix nibble ignored)
+static inline __host__ __device__ int64_t ef_pts_decode(const uint8_t* q)
+{
+    return (int64_t)(q[0] & 0x0E) << 29 | (int64_t)q[1] << 22 | (int64_t)(q[2] >> 1) << 15 | (int64_t)q[3] << 7 | (q[4] >> 1);
+}
+
+// What one packet holds, read as more() / demux() read it (player.cpp:381-493), with no read outside its 188 bytes. It decides nothing:
+// each caller applies its own rule to the fields (DESIGN.md §4, K0 index kernels).
+struct EfTsPacket {
+    bool sync, pusi, payload;      // sync byte 0x47, payload_unit_start, adaptation_field_control 1 or 3
+    int pid;
+    int pes;                       // the byte after the adaptation field (past the packet when the field runs past it)
+    int start;                     // the first ES byte, 188 = none: pes, or on pusi the byte after the 9 + header_data_length PES bytes
+    bool pts_prefix;               // pusi, PTS flag set, first PTS byte inside the packet and parse_pts()'s prefix nibble (player.cpp:299)
+    int64_t pts;                   // the PTS when pts_prefix holds and all 5 of its bytes are inside the packet, else -1
+};
+
+static inline __host__ __device__ EfTsPacket ef_ts_read(const uint8_t* d)
+{
+    EfTsPacket r;
+    r.sync = d[0] == 0x47;
+    r.pusi = (d[1] & 0x40) != 0;
+    r.payload = (d[3] & 0x10) != 0;
+    r.pid = ((d[1] << 8) | d[2]) & 0x1FFF;
+    r.pes = (d[3] & 0x20) ? 5 + d[4] : 4;
+    r.start = r.pes < 188 ? r.pes : 188;
+    r.pts_prefix = false;
+    r.pts = -1;
+    if (r.pusi) {                                              // the PES header: 9 bytes and header_data_length more
+        const int o = r.pes, e = o + 9;
+        r.start = 188;
+        if (e <= 188) {
+            const int flags = d[o + 7];                        // PTS_DTS_flags in bits 6-7
+            if (e + d[o + 8] < 188) r.start = e + d[o + 8];
+            r.pts_prefix = (flags & 0x80) && e < 188 && (d[e] & 0xF0) == ((flags >> 2) & 0x30);   // '0010' PTS only, '0011' with DTS
+            if (r.pts_prefix && e + 5 <= 188) r.pts = ef_pts_decode(d + e);
+        }
+    }
+    return r;
+}
+
+// Writes bytes first, first + step, ... of packet j of one PES in the muxes' layout (efs_wrap_ts's): the packet header with the
+// continuity counter cc, the last packet's stuffing adaptation field, then the PES: a 14-byte header (stream_id, PES_packet_length
+// `length`, flags 80 80 05 and the PTS with prefix '0010') and the n payload bytes, 184 PES bytes to a full packet. A warp writes a
+// packet with first = lane and step = 32, the host with 0 and 1. The payload bytes take a loop of their own, which on the host is a
+// plain copy: a test per byte made ef_mux_audio slower.
+static inline __host__ __device__ void ef_pes_packet(uint8_t* pkt, uint32_t first, uint32_t step, uint32_t j, int pid, int stream_id,
+                                                     uint32_t length, int64_t pts, uint32_t cc, const uint8_t* payload, uint32_t n)
+{
+    const uint32_t left = 14 + n - j * 184, af = left >= 184 ? 0 : 184 - left;    // adaptation field bytes, its length byte included
+    const uint32_t p0 = (j ? 4 : 18) + af;                                          // the packet's first payload byte
+    const uint64_t v = (uint64_t)pts;
+    auto head = [&](uint32_t t) -> uint8_t {
+        if (t == 0) return 0x47;
+        if (t == 1) return (uint8_t)((j ? 0 : 0x40) | pid >> 8);
+        if (t == 2) return (uint8_t)pid;
+        if (t == 3) return (uint8_t)((af ? 0x30 : 0x10) | (cc & 15));
+        if (t < 4 + af) return t == 4 ? (uint8_t)(af - 1) : t == 5 ? 0 : 0xFF;
+        switch (t - 4 - af) {                                                       // the PES header, in packet 0
+        case 2: return 1;
+        case 3: return (uint8_t)stream_id;
+        case 4: return (uint8_t)(length >> 8);
+        case 5: return (uint8_t)length;
+        case 6: case 7: return 0x80;
+        case 8: return 5;
+        case 9: return (uint8_t)(0x21 | ((v >> 29) & 0x0E));
+        case 10: return (uint8_t)(v >> 22);
+        case 11: return (uint8_t)(0x01 | ((v >> 14) & 0xFE));
+        case 12: return (uint8_t)(v >> 7);
+        case 13: return (uint8_t)(0x01 | ((v << 1) & 0xFE));
+        default: return 0;
+        }
+    };
+    uint32_t t = first;
+    for (; t < p0; t += step) pkt[t] = head(t);
+    for (; t < 188; t += step) pkt[t] = payload[j * 184 + t - 18 - af];
+}
+
 #ifdef __CUDACC__    // device code only: ef_tables.cpp reads this header through the host compiler
 // Integer prefix sums over one CTA of a 1-D launch (lane = threadIdx.x & 31).
 // Lane i of a full warp gets x_0 + ... + x_i; all 32 lanes must call it.

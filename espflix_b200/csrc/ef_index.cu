@@ -316,29 +316,16 @@ ef_fill_kernel(EfDev* __restrict__ Dp)
 }
 
 // ---- TS -> ES compaction -------------------------------------------------------------------------
-// One thread per 188-byte packet: payload start/length for PID 0x100 following more()/demux()
-// (player.cpp:381-493): sync byte, adaptation field, PES header skipped on payload_unit_start.
-__device__ __forceinline__ void ts_payload(const uint8_t* d, int& start, int& n)
-{
-    start = 188; n = 0;
-    if (d[0] != 0x47) return;
-    const int pid = ((d[1] << 8) | d[2]) & 0x1FFF;
-    if (pid != 0x100 || !(d[3] & 0x10)) return;
-    int o = 4;
-    if (d[3] & 0x20) o = 5 + d[4];
-    if (d[1] & 0x40) { if (o + 9 > 188) return; o = o + 9 + d[o + 8]; }      // payload = d + 6 + 3 + header_data_length
-    if (o < 188) { start = o; n = 188 - o; }
-}
-
-// pass 1: per-packet payload length; pass 2: exclusive scan of the lengths INSIDE every stream (one CTA per stream,
-// streams are independent) + the stream totals; pass 3: scan of the totals -> ES offset of every stream; pass 4: copy.
+// A packet's ES bytes are the payload of PID 0x100 from ef_ts_read's start, as more()/demux() take them (player.cpp:381-493); a
+// packet without the sync byte or the payload flag has none. pass 1: per-packet payload length, one thread per packet; pass 2:
+// exclusive scan of the lengths INSIDE every stream (one CTA per stream, streams are independent) + the stream totals; pass 3: scan
+// of the totals -> ES offset of every stream; pass 4: copy.
 __global__ void ef_ts_len_kernel(const uint8_t* __restrict__ ts, uint64_t n_packets, uint32_t* __restrict__ out_len)
 {
     const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_packets) return;
-    int start, n;
-    ts_payload(ts + k * 188, start, n);
-    out_len[k] = (uint32_t)n;
+    const EfTsPacket r = ef_ts_read(ts + k * 188);
+    out_len[k] = r.sync && r.pid == 0x100 && r.payload ? 188 - r.start : 0;
 }
 
 // one warp per packet: lanes copy the payload bytes to es_off[stream] + offset inside the stream
@@ -349,10 +336,10 @@ __global__ void ef_ts_copy_kernel(const uint8_t* __restrict__ ts, uint64_t n_pac
     const int lane = threadIdx.x & 31;
     if (k >= n_packets) return;
     const uint8_t* d = ts + k * 188;
-    int start, n;
-    ts_payload(d, start, n);
+    const EfTsPacket r = ef_ts_read(d);
+    if (!r.sync || r.pid != 0x100 || !r.payload) return;
     uint8_t* dst = es + es_off[pkt_stream[k]] + local_off[k];
-    for (int i = lane; i < n; i += 32) dst[i] = d[start + i];
+    for (int i = r.start + lane; i < 188; i += 32) dst[i - r.start] = d[i];
 }
 
 // exclusive scan of the payload lengths of ONE stream's packets per CTA (grid = n_streams)
@@ -461,26 +448,11 @@ ef_carry_restart_kernel(const uint8_t* __restrict__ ops, int first, int count, E
 // and the 2 bytes after it. Hence: pts(picture) = PTS of the last valid video PES start whose first payload byte lies at ES
 // offset <= code byte + 2, else the value carried from earlier submits (-1 if none; reset() does not clear _pts).
 
-// PTS of a video (PID 0x100) packet that starts a PES with a non-empty payload and a PTS with the right prefix; -1 otherwise
-__device__ __forceinline__ int64_t ts_video_pes_pts(const uint8_t* d)
-{
-    if (d[0] != 0x47 || !(d[1] & 0x40) || !(d[3] & 0x10)) return -1;
-    if ((((d[1] << 8) | d[2]) & 0x1FFF) != 0x100) return -1;
-    const int o = (d[3] & 0x20) ? 5 + d[4] : 4;
-    if (o + 9 > 188 || o + 9 + d[o + 8] >= 188) return -1;        // no PES payload reaches the ES (as ts_payload())
-    const int flags = (d[o + 6] << 8) | d[o + 7];
-    if (!(flags & 0x0080) || o + 14 > 188) return -1;             // PES_PTS
-    const uint8_t* q = d + o + 9;
-    if ((q[0] & 0xF0) != ((flags >> 2) & 0x30)) return -1;        // parse_pts(): '0010' for PTS only, '0011' with DTS
-    int64_t n = ((int64_t)(q[0] & 0x0E)) << 29;
-    n += (int64_t)((((uint32_t)q[1] << 8) | q[2]) >> 1) << 15;
-    return n + ((((uint32_t)q[3] << 8) | q[4]) >> 1);
-}
-
-// Packet pass, one CTA per stream, one thread per packet: the stream's video PES starts with a valid PTS, in packet order, as
-// (stream-local ES offset of the first payload byte, pts) at list_*[first packet of the stream ...]; span[s] = (that index, count).
-// local_off comes from ef_ts_scan_kernel. The lists belong to one ES buffer: the shared packet tables are overwritten by the next
-// submit while the compute stream may still resolve this one.
+// Packet pass, one CTA per stream, one thread per packet: the stream's video PES starts whose payload reaches the ES (as in
+// ef_ts_len_kernel) and that carry a PTS (ef_ts_read's pts), in packet order, as (stream-local ES offset of the first payload byte,
+// pts) at list_*[first packet of the stream ...]; span[s] = (that index, count). local_off comes from ef_ts_scan_kernel. The lists
+// belong to one ES buffer: the shared packet tables are overwritten by the next submit while the compute stream may still resolve
+// this one.
 __global__ void __launch_bounds__(256)
 ef_pts_packet_kernel(const uint8_t* __restrict__ ts, const uint64_t* __restrict__ ts_off, const uint32_t* __restrict__ local_off,
                      uint32_t* __restrict__ list_off, int64_t* __restrict__ list_pts, uint2* __restrict__ span)
@@ -491,7 +463,11 @@ ef_pts_packet_kernel(const uint8_t* __restrict__ ts, const uint64_t* __restrict_
     scan.init();
     for (uint64_t base = p0; base < p1; base += 256) {
         const uint64_t k = base + threadIdx.x;
-        const int64_t pts = k < p1 ? ts_video_pes_pts(ts + k * 188) : -1;
+        int64_t pts = -1;
+        if (k < p1) {
+            const EfTsPacket r = ef_ts_read(ts + k * 188);
+            if (r.sync && r.pid == 0x100 && r.payload && r.pusi && r.start < 188) pts = r.pts;
+        }
         const uint64_t j = p0 + scan.exclusive(pts >= 0);
         if (pts >= 0) {
             list_off[j] = local_off[k];

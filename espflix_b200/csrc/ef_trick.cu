@@ -31,37 +31,7 @@ __global__ void ef_trick_mux_kernel(const uint8_t* __restrict__ es, const EfTric
     while (lo < hi) { const int m = (lo + hi + 1) >> 1; if (pics[m].pkt_first <= k) lo = m; else hi = m - 1; }
     const EfTrickPic d = pics[lo];
     const uint32_t j = (uint32_t)(k - d.pkt_first);
-    const uint32_t pes_len = 14 + d.es_len, pos = j * 184, left = pes_len - pos;
-    const uint32_t af = left >= 184 ? 0 : 184 - left;                   // adaptation field bytes, its length byte included
-    const uint64_t pts = (uint64_t)d.pts & ((1ull << 33) - 1);
-    uint8_t* pkt = out + k * 188;
-    for (int t = lane; t < 188; t += 32) {
-        uint8_t v;
-        if (t == 0) v = 0x47;
-        else if (t == 1) v = (uint8_t)((j == 0 ? 0x40 : 0) | 0x01);
-        else if (t == 2) v = 0x00;
-        else if (t == 3) v = (uint8_t)((af ? 0x30 : 0x10) | ((d.cc0 + j) & 15));
-        else if ((uint32_t)t < 4 + af) v = t == 4 ? (uint8_t)(af - 1) : t == 5 ? 0 : 0xFF;
-        else {
-            const uint32_t b = pos + (uint32_t)t - 4 - af;             // byte of the PES
-            if (b >= 14) v = es[d.es_off + b - 14];
-            else {
-                switch (b) {
-                case 2: v = 1; break;
-                case 3: v = 0xE0; break;
-                case 6: case 7: v = 0x80; break;
-                case 8: v = 5; break;
-                case 9: v = (uint8_t)(0x21 | ((pts >> 29) & 0x0E)); break;
-                case 10: v = (uint8_t)(pts >> 22); break;
-                case 11: v = (uint8_t)(0x01 | ((pts >> 14) & 0xFE)); break;
-                case 12: v = (uint8_t)(pts >> 7); break;
-                case 13: v = (uint8_t)(0x01 | ((pts << 1) & 0xFE)); break;
-                default: v = 0;
-                }
-            }
-        }
-        pkt[t] = v;
-    }
+    ef_pes_packet(out + k * 188, lane, 32, j, 0x100, 0xE0, 0, d.pts, d.cc0 + j, es + d.es_off, d.es_len);
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------------------------
