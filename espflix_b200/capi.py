@@ -108,6 +108,7 @@ _SIGNATURES = {
     "ef_library_add_poster": (_I, [_VP, _I, _VP, ctypes.c_uint64]),
     "ef_library_nv_read": (_I, [_VP, _I, _I, _I, _VP]),
     "ef_library_nv_write": (_I, [_VP, _I, _I, _I, _VP]),
+    "ef_library_keys": (_I, [_VP, _VP, _VP, _VP]),
     "ef_encode_build": (_I, [_I, _VP, _VP, _I, _VP, _VP, ctypes.c_uint64, _VP]),
     "ef_encode_stage_ms": (_I, [ctypes.POINTER(ctypes.c_float)] * 5),
     "ef_encode_build_rate": (_I, [_I, _VP, _VP, _I, _VP, _VP, _VP, ctypes.c_uint64, _VP, _VP, _VP]),
@@ -120,6 +121,9 @@ _SIGNATURES = {
 LIB_PLAY_AT, LIB_PLAY, LIB_SKIP, LIB_FAST_FORWARD, LIB_REWIND, LIB_PAUSE, LIB_RESUME, LIB_STOP, LIB_NAV, LIB_NAV_STEP, LIB_MENU = range(11)
 LIB_IDLE, LIB_PLAYING, LIB_PAUSED, LIB_STOPPED, LIB_ENDED, LIB_POSTER = range(6)
 LIB_POSTER_FILE = 3              # ef_library_status.file of a stream on its poster, ef_library_read's part for poster.ts
+# ef_library_keys: the remote's keys (the HID codes of the reference's key_event()) and the done codes it reports
+KEY_MENU, KEY_PLAY, KEY_SELECT, KEY_RIGHT, KEY_LEFT, KEY_DOWN, KEY_UP = 16, 19, 40, 79, 80, 81, 82
+KEY_DONE_NOTHING, KEY_DONE_ENDED = 0x0F, 0x10
 LIBRARY_STATUS = np.dtype([("title", "<i4"), ("speed", "<i4"), ("state", "<i4"), ("file", "<i4"), ("cursor", "<u8"), ("pos", "<i8")])
 
 
@@ -596,6 +600,27 @@ class Context:
         ps = None if per_stream is None else np.ascontiguousarray(np.broadcast_to(per_stream, (self.n_streams,)), dtype=np.uint32)
         st = getattr(stream, "cuda_stream", stream)
         self._check(self.lib.ef_library_submit(self._h, int(packets), _ptr(ps), st))
+
+    def library_keys(self, keys, done=None, stream=0):
+        """ef_library_keys: one iteration of the reference's loop() on every stream with keys[s] (KEY_*, 0 none), enqueued on `stream`
+        (a torch.cuda.Stream or a raw handle). keys: n_streams bytes, a numpy array or a CUDA torch.uint8 tensor (a producer on the
+        device); done: None or a CUDA torch.uint8 tensor of n_streams that receives each stream's done code. Returns done."""
+        n = self.n_streams
+        if isinstance(keys, np.ndarray) or not hasattr(keys, "data_ptr"):
+            keys = np.ascontiguousarray(np.broadcast_to(keys, (n,)), dtype=np.uint8)
+            kp = keys.ctypes.data
+        else:
+            import torch
+            if not (keys.is_cuda and keys.dtype == torch.uint8 and keys.is_contiguous() and keys.numel() == n):
+                raise TypeError("keys must be a contiguous CUDA torch.uint8 tensor of n_streams")
+            kp = keys.data_ptr()
+        if done is not None:
+            import torch
+            if not (done.is_cuda and done.dtype == torch.uint8 and done.is_contiguous() and done.numel() == n):
+                raise TypeError("done must be a contiguous CUDA torch.uint8 tensor of n_streams")
+        st = getattr(stream, "cuda_stream", stream)
+        self._check(self.lib.ef_library_keys(self._h, kp, None if done is None else done.data_ptr(), st))
+        return done
 
     def library_info(self, first=0, count=None):
         """ef_library_info -> LIBRARY_STATUS rows (title, speed, state, file, cursor, pos) of streams [first, first + count)"""

@@ -102,6 +102,8 @@ cudaError_t ef_launch_library_resolve(EfLibStream* ls, const EfLibTitle* titles,
 cudaError_t ef_launch_library_gather(EfLibStream* ls, const EfLibTitle* titles, const uint32_t* budget, uint32_t packets, int n_streams,
                                      const uint8_t** src, uint64_t* off, uint8_t* end, const uint8_t* mode, uint8_t* smode, uint8_t* dst,
                                      uint64_t max_bytes, cudaStream_t st, uint64_t* launches);
+cudaError_t ef_launch_library_keys(EfLibStream* ls, const EfLibTitle* titles, const int64_t* pts_last, const uint8_t* keys, uint8_t* done, uint8_t* ops,
+                                   uint8_t* mode, int64_t* nv, int n_streams, int n_titles, EfOverlayState* ovl, EfClockState* clk, cudaStream_t st);
 static_assert(sizeof(idx_hdr) == 104, "video.idx header: the reference's idx_hdr");
 static_assert(sizeof(EfLibStream) == sizeof(ef_library_status), "EfLibStream mirrors ef_library_status");
 static_assert(sizeof(EfPaceOut) == sizeof(ef_present_info), "EfPaceOut mirrors ef_present_info");
@@ -409,6 +411,12 @@ struct ef_ctx {
     uint8_t* d_lib_mode = nullptr;                // [n_streams] the scroll mode of every stream's latest nav
     uint8_t* d_lib_smode = nullptr;               // [n_streams] the modes a library submit carries (its posters that end in it)
     uint8_t* d_lib_mode2[2] = { nullptr, nullptr };   // per ES buffer: the modes its submit carries, 0 for a submit of the host
+    // the remote (ef_library_keys), allocated by its first call: the keys, the restart op of every stream, and ev_keys after the
+    // call's last kernel, which the asynchronous calls that follow wait for on their streams
+    uint8_t* d_keys = nullptr;                    // [n_streams] the keys of a call made with host keys
+    uint8_t* d_keys_ops = nullptr;                // [n_streams]
+    std::vector<uint8_t> h_keys;                  // pageable: the copy takes the keys before the call returns
+    cudaEvent_t ev_keys = nullptr;
 };
 
 namespace {
@@ -685,6 +693,7 @@ int ef_reset(ef_ctx* c)
     TRY(wait_frames_read(c));
     TRY(audio_resolve(c));
     TRY(pace_resolve(c));
+    if (c->ev_keys) CK(cudaEventSynchronize(c->ev_keys));   // its restart may still write the states reset below
     CK(cudaMemset(c->h.frames, 0, (size_t)c->cfg.n_streams * 2 * EF_FRAME + 1024));     // Frame::init zero-fills (player.cpp:25)
     ef_reset_seq_kernel<<<(c->cfg.n_streams + 127) / 128, 128>>>(c->d);
     CK(cudaGetLastError());
@@ -728,7 +737,32 @@ static int restart_ready(ef_ctx* c, const char* what)
     return EF_OK;
 }
 
-// The restart itself (ops checked, restart_ready passed): ef_restart_streams and ef_library_command
+// The restart kernels on `st` for streams [first, first + count) from the device ops d_ops[count]: ef_restart_kernel, then with
+// `audio` the end of the demux gates of the streams it marks, with `carry` ef_carry_restart_kernel. Streams with op 0 do not change.
+static int restart_launch(ef_ctx* c, int first, int count, const uint8_t* d_ops, bool audio, bool carry, cudaStream_t st)
+{
+    const int n = c->cfg.n_streams, p = c->pending;
+    ef_restart_kernel<<<(count + 127) / 128, 128, 0, st>>>(d_ops, first, count, c->paced ? c->d_pace : nullptr, c->pts ? c->d_pts_last : nullptr,
+                                                           audio ? c->d_aud_state : nullptr, audio ? c->d_ended : nullptr);
+    CK(cudaGetLastError());
+    c->launches++;
+    if (audio) {                                          // the demux gates: the current one, and that of a submit queued behind it
+        CK(ef_launch_audio_end(c->d_ended, n, c->d_gate2[c->active], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
+                               p >= 0 && c->aud_ts[p], nullptr, st));
+        c->launches++;
+    }
+    if (carry) {                                          // MpegDecoder::reset() clears the bit reader (player.cpp:446-447)
+        ef_carry_restart_kernel<<<(count * 32 + 127) / 128, 128, 0, st>>>(d_ops, first, count, carry_args(c, c->active), c->pts ? c->d_pts_carry : nullptr,
+                                                                          p >= 0 ? c->d_es2[p] : nullptr, p >= 0 ? c->d_es_off2[p] : nullptr,
+                                                                          p >= 0 ? c->d_held_in2[p] : nullptr);
+        CK(cudaGetLastError());
+        c->launches++;
+    }
+    return EF_OK;
+}
+
+// The restart itself (ops checked, restart_ready passed): ef_restart_streams and ef_library_command. Synchronous; the subsystems
+// of op 1 run only when some stream has it.
 static int restart_apply(ef_ctx* c, int first, int count, const uint8_t* ops)
 {
     const int n = c->cfg.n_streams;
@@ -740,25 +774,15 @@ static int restart_apply(ef_ctx* c, int first, int count, const uint8_t* ops)
     if (!c->d_restart_ops) TRY(dev_alloc(c, &c->d_restart_ops, (size_t)n));
     CK(cudaMemcpy(c->d_restart_ops, ops, (size_t)count, cudaMemcpyHostToDevice));
     if (audio) CK(cudaMemset(c->d_ended, 0, (size_t)n));
-    ef_restart_kernel<<<(count + 127) / 128, 128>>>(c->d_restart_ops, first, count, c->paced ? c->d_pace : nullptr, c->pts ? c->d_pts_last : nullptr,
-                                                     audio ? c->d_aud_state : nullptr, audio ? c->d_ended : nullptr);
-    CK(cudaGetLastError());
-    c->launches++;
-    if (audio) {                                          // the demux gates: the current one, and that of a submit queued behind it
-        const int p = c->pending;
-        CK(ef_launch_audio_end(c->d_ended, n, c->d_gate2[c->active], p >= 0 ? c->d_gate2[p] : nullptr, p >= 0 ? c->d_skip2[p] : nullptr,
-                               p >= 0 && c->aud_ts[p], nullptr, 0));
-        c->launches++;
-    }
-    if (c->carry && any_reset) {                          // MpegDecoder::reset() clears the bit reader (player.cpp:446-447)
-        const int p = c->pending;
-        ef_carry_restart_kernel<<<(count * 32 + 127) / 128, 128>>>(c->d_restart_ops, first, count, carry_args(c, c->active), c->pts ? c->d_pts_carry : nullptr,
-                                                                   p >= 0 ? c->d_es2[p] : nullptr, p >= 0 ? c->d_es_off2[p] : nullptr,
-                                                                   p >= 0 ? c->d_held_in2[p] : nullptr);
-        CK(cudaGetLastError());
-        c->launches++;
-    }
+    TRY(restart_launch(c, first, count, c->d_restart_ops, audio, c->carry && any_reset, 0));
     CK(cudaDeviceSynchronize());
+    return EF_OK;
+}
+
+// The asynchronous calls on `st` that follow an ef_library_keys run after it (the synchronous ones wait for the device)
+static int keys_order(ef_ctx* c, cudaStream_t st)
+{
+    if (c->ev_keys) CK(cudaStreamWaitEvent(st, c->ev_keys, 0));
     return EF_OK;
 }
 
@@ -801,6 +825,7 @@ static int submit_common(ef_ctx* c, const uint8_t* src, const uint64_t* off, boo
         CK(cudaStreamWaitEvent(up, c->ev_user, 0));
     }
     CK(cudaStreamWaitEvent(up, c->ev_buf_free[b], 0));    // kernels of the submit that last used this buffer are done
+    TRY(keys_order(c, up));                               // a restart of ef_library_keys may still rewrite a queued submit
     if (c->audio) CK(cudaStreamWaitEvent(up, c->ev_aud_done, 0));   // and the last audio call: it reads this buffer's audio, or
                                                                      // shuts demux gates the demux below reads
     uint8_t* d_es = c->d_es2[b];
@@ -929,6 +954,7 @@ int ef_index(ef_ctx* c, void* stream)
         c->d = c->dd[c->active];
         c->aud_unconsumed = c->audio && c->aud_ts[c->active];
     }                                            // else: index the front buffer again (same input, next GOP period)
+    TRY(keys_order(c, st));
     if (c->profiling) { CK(cudaEventRecord(c->ev_prof[0], st)); c->prof_index = true; }
     CK(cudaMemsetAsync(c->h.info, 0, 32, st));
     const EfCarryArgs carry = c->carry ? carry_args(c, c->active) : EfCarryArgs{};
@@ -1685,6 +1711,7 @@ static int audio_assemble(ef_ctx* c, const uint8_t* end_of_stream, cudaStream_t 
     CK(cudaStreamWaitEvent(cs, c->ev_up_done[a], 0));        // the demux of the current submit has finished
     if (p >= 0) CK(cudaStreamWaitEvent(cs, c->ev_up_done[p], 0));   // and that of a submit queued behind it (ef_audio_end_kernel)
     CK(cudaStreamWaitEvent(cs, c->ev_aud_done, 0));
+    TRY(keys_order(c, cs));                                  // its restart wrote the audio states, the gates and d_ended
     CK(cudaMemcpyAsync(c->d_ended, c->h_ended, (size_t)n, cudaMemcpyHostToDevice, cs));
     CK(cudaEventRecord(c->ev_ended_free, cs));
     const uint64_t* new_off = c->aud_unconsumed ? c->d_aud_off2[a] : nullptr;
@@ -1860,6 +1887,7 @@ int ef_present_format(ef_ctx* c, int format)
 static int present_schedule(ef_ctx* c, int pic, const uint8_t* modes, const uint32_t* idle_n, void* pinned, cudaStream_t st)
 {
     const int n = c->cfg.n_streams;
+    TRY(keys_order(c, st));
     if (pic >= 0 && modes) memcpy(pinned, modes, (size_t)n);
     if (pic < 0) memcpy(pinned, idle_n, (size_t)n * 4);
     const bool arg = pic < 0 || modes;
@@ -2297,6 +2325,7 @@ int ef_library_submit(ef_ctx* c, uint32_t packets, const uint32_t* per_stream, v
         return fail(EF_ENOMEM, "a library submit of up to %llu packets exceeds es_capacity %zu", (unsigned long long)bound, c->cfg.es_capacity);
     cudaStream_t st = (cudaStream_t)stream;
     CK(cudaStreamWaitEvent(st, c->ev_lib_staged, 0));   // the upload of the previous library submit has copied the staging buffer
+    TRY(keys_order(c, st));                               // the keys have moved the cursors
     if (per_stream) CK(cudaMemcpyAsync(c->d_lib_budget, per_stream, (size_t)n * 4, cudaMemcpyHostToDevice, st));
     CK(ef_launch_library_gather(c->d_lib, c->d_lib_titles, per_stream ? c->d_lib_budget : nullptr, packets, n, c->d_lib_src, c->d_lib_off,
                                 c->d_lib_end, c->d_lib_mode, c->d_lib_smode, c->d_lib_stage, bound * 188, st, &c->launches));
@@ -2319,6 +2348,43 @@ int ef_library_info(ef_ctx* c, int first, int count, ef_library_status* status)
     if (!count) return EF_OK;
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(status, c->d_lib + first, (size_t)count * sizeof(EfLibStream), cudaMemcpyDeviceToHost));
+    return EF_OK;
+}
+
+// ---- the remote: one ESPFlix::loop() iteration (espflix.cpp:886-1010) per stream, with the key it was given ---------------------
+int ef_library_keys(ef_ctx* c, const uint8_t* keys, uint8_t* done, void* stream)
+{
+    DeviceScope scope_(c ? c->cfg.device : -1);
+    if (!c) return fail(EF_EINVAL, "null context");
+    TRY(library_ready(c, "ef_library_keys"));
+    if (!keys) return fail(EF_EINVAL, "null keys");
+    if (done && !is_device_ptr(done)) return fail(EF_EINVAL, "ef_library_keys takes device memory for done");
+    TRY(restart_ready(c, "ef_library_keys"));
+    const int n = c->cfg.n_streams;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!c->d_keys_ops) {
+        TRY(dev_alloc(c, &c->d_keys, (size_t)n)); TRY(dev_alloc(c, &c->d_keys_ops, (size_t)n));
+        c->h_keys.resize((size_t)n);
+    }
+    // after what the keys read and the restart rewrites: the last library submit's gather (its upload recorded ev_lib_staged after
+    // it), the last ef_index (the PTS and held bytes), the demux of a queued submit, the last audio call and the previous keys
+    CK(cudaStreamWaitEvent(st, c->ev_lib_staged, 0));
+    CK(cudaStreamWaitEvent(st, c->ev_buf_free[c->active], 0));
+    CK(cudaStreamWaitEvent(st, c->ev_scanned, 0));
+    if (c->pending >= 0) CK(cudaStreamWaitEvent(st, c->ev_up_done[c->pending], 0));
+    if (c->audio) CK(cudaStreamWaitEvent(st, c->ev_aud_done, 0));
+    TRY(keys_order(c, st));
+    if (!is_device_ptr(keys)) {
+        memcpy(c->h_keys.data(), keys, (size_t)n);
+        CK(cudaMemcpyAsync(c->d_keys, c->h_keys.data(), (size_t)n, cudaMemcpyHostToDevice, st));
+        keys = c->d_keys;
+    }
+    CK(ef_launch_library_keys(c->d_lib, c->d_lib_titles, c->d_pts_last, keys, done, c->d_keys_ops, c->d_lib_mode, c->d_lib_nv, n,
+                              (int)c->lib_titles.size(), c->paced ? c->d_ovl : nullptr, c->paced ? c->d_clk : nullptr, st));
+    c->launches++;
+    TRY(restart_launch(c, 0, n, c->d_keys_ops, c->audio, true, st));
+    if (!c->ev_keys) TRY(event(c, &c->ev_keys));
+    CK(cudaEventRecord(c->ev_keys, st));
     return EF_OK;
 }
 

@@ -116,6 +116,112 @@ __global__ void ef_library_resolve_kernel(EfLibStream* __restrict__ ls, const Ef
     ls[s] = v;
 }
 
+// One thread per stream: one iteration of ESPFlix::loop() (espflix.cpp:886-1010) with keys[s] (0: none). First the pause branch of a
+// stream whose title ended (_pending == DONE): nav(s, title) as EF_LIB_MENU does on ENDED; a title without a poster stays ENDED and
+// ignores the key. Then the key on the state that left, its pending action resolved at once (the library pauses at the submit
+// boundary): the EF_LIB_* command it runs as, by the rules of ef_library_resolve_kernel. A command ef_library_command would refuse
+// (a missing trick file, no poster at the target) does nothing. done[s] (may be NULL) = that command or EF_KEY_DONE_NOTHING, with
+// EF_KEY_DONE_ENDED when the DONE branch ran; ops[s] = the restart op of the iteration. ovl (NULL off a presenting context): the blend
+// play(), the pause, the resume and nav() leave, staged as ef_present_overlay stages it. clk (NULL before ef_present_clock): on a
+// stream whose clock is on, speed and the paused bit follow the stream, _last_seconds = 0 where play_pause() and the pause zero it
+// (espflix.cpp:819, 935), and a nav to another title writes that title's records.
+__global__ void ef_library_keys_kernel(EfLibStream* __restrict__ ls, const EfLibTitle* __restrict__ titles, const int64_t* __restrict__ pts_last,
+                                       const uint8_t* __restrict__ keys, uint8_t* __restrict__ done, uint8_t* __restrict__ ops, uint8_t* __restrict__ mode,
+                                       int64_t* __restrict__ nv, int n_streams, int n_titles, EfOverlayState* __restrict__ ovl, EfClockState* __restrict__ clk)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_streams) return;
+    EfLibStream v = ls[s];
+    const int key = keys[s], title0 = v.title;
+    uint32_t d = EF_KEY_DONE_NOTHING;
+    int op = 0, blend = -2;                                             // -2: no blend of its own staged
+    bool zero_seconds = false;
+    if (v.state != EF_LIB_IDLE && !(v.state == EF_LIB_ENDED && !titles[v.title].ts[EF_LIB_POSTER_FILE])) {
+        if (v.state == EF_LIB_ENDED) {                                  // the DONE branch: set_state(NAV)
+            lib_nav(v, s, v.title, mode, nv, n_streams, ovl);
+            d |= EF_KEY_DONE_ENDED;
+            op = 1;
+        }
+        const bool play = key == EF_KEY_PLAY || key == EF_KEY_SELECT, side = key == EF_KEY_RIGHT || key == EF_KEY_LEFT;
+        const bool vert = key == EF_KEY_UP || key == EF_KEY_DOWN;
+        const int sign = key == EF_KEY_RIGHT || key == EF_KEY_UP ? 1 : -1;
+        int cmd = -1, arg = 0;
+        if (v.state == EF_LIB_POSTER) {
+            if (play) cmd = EF_LIB_PLAY;                                // play_pause() from NAV
+            else if (side) { cmd = EF_LIB_NAV_STEP; arg = sign; }       // nav(_nav +- 1)
+            zero_seconds = play;
+        } else if (v.state == EF_LIB_PLAYING) {                         // the key pauses with _pending set; the pause branch
+            if (key == EF_KEY_MENU) cmd = EF_LIB_MENU;
+            else if (v.speed && (play || side || vert)) cmd = EF_LIB_PLAY;   // trick mode: play_pause() from NAV
+            else if (play) cmd = EF_LIB_PAUSE;
+            else if (side) cmd = sign > 0 ? EF_LIB_FAST_FORWARD : EF_LIB_REWIND;
+            else if (vert) { cmd = EF_LIB_SKIP; arg = 30 * sign; }
+            zero_seconds = cmd >= 0 && (play || v.speed);               // play_pause(), or the NONE case of the pause branch
+        } else if (v.state == EF_LIB_PAUSED) {
+            if (key == EF_KEY_MENU) cmd = EF_LIB_MENU;
+            else if (play) cmd = EF_LIB_RESUME;
+            else if (side) cmd = sign > 0 ? EF_LIB_FAST_FORWARD : EF_LIB_REWIND;
+            zero_seconds = play;
+        } else if (v.state == EF_LIB_STOPPED) {
+            if (key == EF_KEY_MENU) cmd = EF_LIB_MENU;
+            zero_seconds = play;                                        // play_pause() does nothing else there
+        }
+        const EfLibTitle& t = titles[v.title];
+        int nav_to = -1;                                                // the title whose poster the command shows
+        if (cmd == EF_LIB_NAV_STEP) {
+            nav_to = v.title + arg;
+            if (nav_to < 0 || nav_to >= n_titles) cmd = -1;             // nav()'s early return
+        } else if (cmd == EF_LIB_MENU && !(v.state == EF_LIB_PLAYING && v.speed)) nav_to = v.title;
+        if (cmd >= 0 && nav_to >= 0 && !titles[nav_to].ts[EF_LIB_POSTER_FILE]) cmd = -1;
+        if ((cmd == EF_LIB_FAST_FORWARD && !t.ts[2]) || (cmd == EF_LIB_REWIND && !t.ts[0])) cmd = -1;
+        if (cmd >= 0) {
+            if (cmd != EF_LIB_RESUME && v.state == EF_LIB_PLAYING) v.pos = ef_lib_pts2pts(t, pts_last[s], v.speed);   // save_pos
+            d = (d & ~0xFu) | (uint32_t)cmd;
+            switch (cmd) {
+            case EF_LIB_PLAY: lib_play(v, t, 0); break;
+            case EF_LIB_SKIP:
+                v.pos += (int32_t)((uint32_t)arg * 90000u);
+                lib_play(v, t, 0);
+                break;
+            case EF_LIB_FAST_FORWARD: lib_play(v, t, 1); break;
+            case EF_LIB_REWIND: lib_play(v, t, -1); break;
+            case EF_LIB_PAUSE: v.state = EF_LIB_PAUSED; blend = 180; break;    // show_progress(), then video_pause(1)
+            case EF_LIB_RESUME: v.state = EF_LIB_PLAYING; blend = 180; op = 2; break;
+            case EF_LIB_NAV_STEP: lib_nav(v, s, nav_to, mode, nv, n_streams, ovl); op = 1; break;
+            default:                                                    // MENU
+                if (v.state == EF_LIB_PLAYING) {                        // save_pos(pts, true)
+                    nv[(size_t)v.title * n_streams + s] = v.pos;
+                    if (v.speed) { lib_play(v, t, 0); break; }
+                }
+                lib_nav(v, s, v.title, mode, nv, n_streams, ovl);
+                op = 1;
+                break;
+            }
+            if (v.state == EF_LIB_PLAYING && cmd != EF_LIB_RESUME) {     // play(): show_progress(speed == 0 ? 180 : -1)
+                blend = v.speed == 0 ? 180 : -1;
+                op = 1;
+            }
+        }
+        if (ovl && blend != -2) {
+            ovl[s].p_blend = blend;
+            ovl[s].pending |= 2u;
+        }
+        if (clk && (clk[s].flags & 1u)) {
+            EfClockState& k = clk[s];
+            k.speed = v.speed;
+            k.flags = (k.flags & ~2u) | (v.state == EF_LIB_PAUSED ? 2u : 0u);
+            if (zero_seconds) k.last_seconds = 0;
+            if (v.title != title0) {
+                const EfLibTitle& u = titles[v.title];
+                k.v_first = u.v_first; k.v_last = u.v_last; k.f_first = u.f_first; k.f_last = u.f_last; k.r_first = u.r_first; k.r_last = u.r_last;
+            }
+        }
+        ls[s] = v;
+    }
+    if (done) done[s] = (uint8_t)d;
+    ops[s] = (uint8_t)op;
+}
+
 // One CTA: every PLAYING stream, and every POSTER stream with poster bytes left, takes min(its budget, packets left in its file)
 // packets from its cursor; the exclusive prefix of the run lengths gives each stream's place in the submit (off[n_streams + 1],
 // EfBlockScan). A stream whose cursor reaches the end of its file ends with this submit: end[s] = 1. A PLAYING stream becomes ENDED
@@ -217,6 +323,13 @@ cudaError_t ef_launch_library_resolve(EfLibStream* ls, const EfLibTitle* titles,
                                       int64_t arg, uint8_t* mode, int64_t* nv, int n_streams, int n_titles, EfOverlayState* ovl)
 {
     ef_library_resolve_kernel<<<(count + 127) / 128, 128>>>(ls, titles, pts_last, first, count, cmd, title, arg, mode, nv, n_streams, n_titles, ovl);
+    return cudaGetLastError();
+}
+
+cudaError_t ef_launch_library_keys(EfLibStream* ls, const EfLibTitle* titles, const int64_t* pts_last, const uint8_t* keys, uint8_t* done, uint8_t* ops,
+                                   uint8_t* mode, int64_t* nv, int n_streams, int n_titles, EfOverlayState* ovl, EfClockState* clk, cudaStream_t st)
+{
+    ef_library_keys_kernel<<<(n_streams + 127) / 128, 128, 0, st>>>(ls, titles, pts_last, keys, done, ops, mode, nv, n_streams, n_titles, ovl, clk);
     return cudaGetLastError();
 }
 

@@ -727,6 +727,49 @@ int ef_library_add_poster(ef_ctx* ctx, int title, const uint8_t* ts, uint64_t by
 int ef_library_nv_read(ef_ctx* ctx, int title, int first, int count, int64_t* pos);
 int ef_library_nv_write(ef_ctx* ctx, int title, int first, int count, const int64_t* pos);
 
+/* ---- the remote: one iteration of ESPFlix::loop() (espflix.cpp:886-1010) for every stream ----------------------------------------
+ * ef_library_keys     keys[s] = stream s's key for this iteration (the HID codes key_event() produces, espflix.cpp:1020-1040; 0 = none,
+ *                     any other code is ignored as loop()'s default: ignores it): n_streams bytes in host memory (read before the call
+ *                     returns) or device memory (a producer on the device, ordered by `stream`). Every stream runs, in the reference's
+ *                     order:
+ *                     1. the pause branch of a title that ended (_pending == DONE): an ENDED stream navs to its title's poster as
+ *                        EF_LIB_MENU does on ENDED, also with key 0. A title without a poster stays ENDED and ignores the key.
+ *                     2. the key, on the state step 1 left; the pending branch resolves at once (the library pauses at the submit
+ *                        boundary), get_pts() being ef_picture_pts's last_pts, so each key runs as one command of ef_library_command:
+ *                          key             POSTER            PLAYING speed 0        PLAYING speed +-1   PAUSED              STOPPED
+ *                          MENU            nothing           EF_LIB_MENU            EF_LIB_MENU         EF_LIB_MENU         EF_LIB_MENU
+ *                          PLAY / SELECT   EF_LIB_PLAY       EF_LIB_PAUSE           EF_LIB_PLAY         EF_LIB_RESUME       nothing
+ *                          RIGHT / LEFT    NAV_STEP +1 / -1  FAST_FORWARD / REWIND  EF_LIB_PLAY         FAST_FORWARD / REW  nothing
+ *                          UP / DOWN       nothing           EF_LIB_SKIP +30 / -30  EF_LIB_PLAY         nothing             nothing
+ *                        IDLE streams ignore every key. A command ef_library_command would refuse with EF_EINVAL (a missing trick
+ *                        file, no poster at the target) does nothing; a step outside the row does nothing (nav()'s early return).
+ *                     done (device memory, n_streams bytes, or NULL): the low nibble = the EF_LIB_* command the key ran as, or
+ *                     EF_KEY_DONE_NOTHING; bit 4 (EF_KEY_DONE_ENDED) = step 1 ran. The restart op of the commands runs as
+ *                     ef_library_command runs it (op 1 when either step restarts). On a presenting context each stream also gets the
+ *                     blend loop() leaves, staged as ef_present_overlay stages it: 0 after a nav (hide_progress()), 180 after a play at
+ *                     speed 0, a pause or a resume (show_progress()), -1 after a play at speed +-1. On a stream whose clock is on
+ *                     (ef_present_clock flag bit 0) the clock's speed and paused bit follow the stream, _last_seconds becomes 0 where
+ *                     play_pause() or the pause zero it (espflix.cpp:819, 935: PLAY / SELECT on a stream that takes keys, and every
+ *                     key that acts at speed +-1), and a nav to another title writes that title's video.idx records.
+ *                     Asynchronous: enqueued on `stream`, no wait for the device and no read-back. The keys act between the current
+ *                     submit and the next one, where ef_library_command acts; the next ef_library_submit, submit, ef_index, present and
+ *                     audio call are ordered after it on the device through an event (the synchronous calls wait for the device).
+ *                     Launches per call: the keys kernel, ef_restart_kernel, ef_carry_restart_kernel and, on an audio context, the
+ *                     audio end kernel; a context that never calls it launches what it launched before. EF_ESTATE: the cases of
+ *                     ef_library_command (no title, no PTS or carry) and of ef_restart_streams (unpresented pictures, unconsumed
+ *                     audio; an outstanding async present chain or audio call is waited for first). EF_EINVAL: keys NULL, or done in
+ *                     host memory. */
+#define EF_KEY_MENU   16
+#define EF_KEY_PLAY   19
+#define EF_KEY_SELECT 40
+#define EF_KEY_RIGHT  79
+#define EF_KEY_LEFT   80
+#define EF_KEY_DOWN   81
+#define EF_KEY_UP     82
+#define EF_KEY_DONE_NOTHING 0x0F  /* done[s]: the key ran no command */
+#define EF_KEY_DONE_ENDED   0x10  /* done[s]: the title had ended and the DONE branch ran first */
+int ef_library_keys(ef_ctx* ctx, const uint8_t* keys, uint8_t* done, void* stream);
+
 /* ---- experiment, NOT on the decode path (north_star: "the 8x8 IDCT ... batched onto tensor cores") ------------
  * The linearised IDCT of MpegDecoder::idct() (player.cpp:922-996) as a [n_blocks x 64] x [64 x 64] TF32 GEMM on
  * Hopper wgmma with register accumulators and TMA-fed operand tiles (csrc/ef_idct_tc.cu). coefs: n_blocks x 64 prescaled
